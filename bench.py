@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - env-steps/s of the vid2player3d rollout hot path on B200 (BASELINE.json metric).
+"""bench.py - env-steps/s of the vid2player3d rollout hot path on H100 (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--envs 8192] [--impl b200|reference] [--legs all|none|amass,dual,ppo,tables]
+                  [--dump-outputs DIR]
   torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...        (one rank per GPU, NCCL)
 
 PRIMARY WORKLOAD (value / ms_per_step / roofline / e2e): BASELINE config 3, "vid2player federer single-player": 8192 envs per GPU,
@@ -10,7 +11,7 @@ env step), ball launcher pool + racket / ground contact, reward return_w_estimat
 length 300.  One "step" = one high-level `PhysicsMVAEController.step(actions)`:
     motion generator (resident kinematic target stream + the MVAE mixture-of-experts decoder forward, random weights of the
     reference's shapes) -> SMPL FK targets -> 734-d imitation obs -> low-level policy MLP 734-1024-1024-512-75 (random weights,
-    tcgen05 layers) -> PD targets + articulated step + ball (one physics launch) -> state views -> high-level obs / reward /
+    wgmma layers) -> PD targets + articulated step + ball (one physics launch) -> state views -> high-level obs / reward /
     reset FSM,
 followed by `reset(done ids)` like the rl_games loop does every step.  The whole step is ONE CUDA-graph replay, the reset a
 second one.  Random high-level policy: actions ~ clamp(N(0,1), -5, 5), [N, 35].
@@ -22,6 +23,12 @@ every 2 ms during the timed region.
 SECONDARY LEGS (flat top-level keys, every N): config 2 (embodied_pose amass_im at 8192 envs), config 5 (dual 2 x 8192 paired envs
 over the box, sharded 16384 / N per GPU), config 4 (djokovic_im PPO: horizon-32 rollouts + minibatch updates with the gradient
 all-reduce inside the timed region).
+
+--dump-outputs DIR: what the last timed step handed its caller - the high-level observation, reward and reset flags that `env.step`
+returned (copied on the device before `reset_done` resets the finished envs and clears their flags) and the physics state the next step
+starts from (after that reset) - as DIR/<name>.npy (float32), written after the timed region.  ~3 KB per env (~25 MB at 8192 envs); above
+64 MB in all, a fixed seeded sample of env rows is written instead, with its row indices in DIR/env_index.npy.  Inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 
 --impl reference: the CPU restatement of the SAME primary workload (oracle/, "kind": "port": Isaac Gym cannot be installed) on the
 host cores, all 8192 envs, honouring --steps / --warmup.
@@ -55,11 +62,12 @@ def parse():
     p.add_argument("--legs", default="all", help="secondary legs: all | none | comma list of amass,dual,ppo,tables")
     p.add_argument("--cpu-sample-envs", type=int, default=1024, help="envs of the in-line cpu_baseline sample (N=1 b200 arm)")
     p.add_argument("--no-cpu-baseline", action="store_true")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy")
     return p.parse_args()
 
 
-PHYS_KERNEL_NAME = {"tmem": "step_kernel_tmem (56 envs per SM, lane-private body fields in tensor memory: one round for 8192 envs)",
-                    "packed": "step_kernel_packed<split> (28 envs per SM, two rounds)", "packed3": "step_kernel_packed3", "lane": "step_kernel"}
+PHYS_KERNEL_NAME = {"tmem": "step_kernel_tmem (56 envs per SM, lane-private body fields in thread-local memory)",
+                    "packed": "step_kernel_packed<split> (28 envs per SM)", "packed3": "step_kernel_packed3", "lane": "step_kernel"}
 
 
 def peaks():
@@ -68,7 +76,7 @@ def peaks():
             d = json.load(f)
             return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3 3.35 TB/s), not measured"
 
 
 class ClockSampler:
@@ -153,6 +161,27 @@ def amass_task(envs, device_index, seed, asset="smpl_mesh_humanoid_amass_v1"):
     torch.manual_seed(seed)
     task = HumanoidSMPLIM(im_cfg(envs, flat, episodeLength=300, asset=f"mjcf/{asset}.xml"), SIM_PARAMS, 1, "cuda", device_index, True)
     return model, flat, task
+
+
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(d, step_out, task, n_envs):
+    """step_out: obs / rew / reset as env.step returned them in the last timed step; task: the physics state after it -> d/<name>.npy
+    (float32, one row per env), a seeded sample of env rows when the whole would exceed DUMP_LIMIT_BYTES"""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    arrays = dict(step_out, root_states=task._root_states, dof_state=task._dof_state, rigid_body_state=task._rigid_body_state)
+    arrays = {k: t.detach().float().reshape(n_envs, -1) for k, t in arrays.items()}
+    per_env = sum(t.shape[1] * 4 for t in arrays.values())
+    if per_env * n_envs > DUMP_LIMIT_BYTES:
+        idx = np.sort(np.random.default_rng(0).choice(n_envs, (DUMP_LIMIT_BYTES - (1 << 20)) // (per_env + 8), replace=False))   # 1 MB for headers; 8 B per index
+        np.save(os.path.join(d, "env_index.npy"), idx)
+        sel = torch.from_numpy(idx).to(next(iter(arrays.values())).device)
+        arrays = {k: t.index_select(0, sel) for k, t in arrays.items()}
+    for name, t in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), t.cpu().numpy())
 
 
 def timed_steps(step_fn, K, flush, sampler=None):
@@ -607,7 +636,13 @@ def main():
     def step(i):
         env.step(pool[i % len(pool)])                              # one graph replay
         env.reset_done()                                           # reset(finished envs) from the device flags: mask + one graph replay
-        # (step + reset captured as ONE graph measured 1.4 % slower than the two replays, profiles/r2z_notes.md: not kept)
+    step_out = {}
+
+    def timed_step(i):
+        env.step(pool[i % len(pool)])
+        if args.dump_outputs and i == K - 1:                       # what step() hands its caller, before reset_done clears the flags
+            step_out.update(obs=env.obs_buf.clone(), rew=env.rew_buf.clone(), reset=env.reset_buf.clone())
+        env.reset_done()
     for i in range(4):
         step_ids(i)
     env.enable_cuda_graph(count_nodes=True)
@@ -629,12 +664,14 @@ def main():
     prof = os.environ.get("B200_BENCH_PROFILE") == "1"      # tools/federer_launches.sh: ncu --profile-from-start off sees the timed loop only
     if prof:
         torch.cuda.cudart().cudaProfilerStart()
-    step_ms = timed_steps(step, K, flush, sampler)
+    step_ms = timed_steps(timed_step, K, flush, sampler)
     barrier()
     if prof:
         torch.cuda.cudart().cudaProfilerStop()
     wall = time.perf_counter() - t_wall
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, step_out, task, N)
     total_ms = sum(step_ms)
     # the physics launch alone (dominant kernel): the SAME rollout continued for 10 steps with the step run eagerly (an event pair
     # inside b200env_step cannot live in a graph), L2 flushed before every step as in the timed loop
@@ -786,10 +823,7 @@ def main():
         "gpu_launches": int((graph_nodes + (reset_nodes or 0) + 1) * K) if graph_nodes else int(step_launches),
         "gpu_launches_note": "kernel nodes of the step graph + the reset graph (+ the mask kernel) x timed steps, counted from the graphs' DOT dumps; "
                              "our own kernels among them per step: 22 (step graph) + 7 (reset graph)",
-        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": {"tmem": 17394176, "packed": 8026112}.get(kform),
-                     "traffic_note": "from_profile: dram__bytes_read.sum + dram__bytes_write.sum of ONE physics launch (the dominant kernel) in the "
-                                     "ncu --set full captures profiles/r2i_step_kernel_ncu.md (step_kernel_packed) / profiles/r2t_tmem.md "
-                                     "(step_kernel_tmem, capture r2ac_c3: 17.4 MB); not measured by this run",
+        "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "kernel": "one env step = one CUDA graph (motion targets, FK, 734-d obs, decoder + policy GEMMs, physics, post step); dominant launch "
                                + PHYS_KERNEL_NAME[kform], "kernel_ms": ms_step, "algorithmic_bytes_per_env_step": ALGO_BYTES_CFG3,
                      "dominant_kernel": {"name": PHYS_KERNEL_NAME[kform] + " (12 substeps + ball)", "ms": phys_ms, "launches_timed": 10,

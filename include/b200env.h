@@ -1,4 +1,4 @@
-/* b200env.h - C ABI of the B200-native vectorised humanoid(+ball) environment step.
+/* b200env.h - C ABI of the H100-native vectorised humanoid(+ball) environment step.
  *
  * This is the drop-in boundary under the reference's Task surface (SURVEY.md 8b, "Level A").
  * The reference has no C ABI of its own: its tasks talk to Isaac Gym through pybind
@@ -234,7 +234,7 @@ int b200env_set_env_slice(b200env_handle h, int32_t env_first, int32_t env_strid
 int b200env_set_hull_faces(b200env_handle h, const float* planes, const uint8_t* tris, const int32_t* ntris, int32_t tmax);
 
 /* Which form of the physics launch this handle uses: 0 lane-per-body kernel, 1 step_kernel_packed (28 envs per SM, two rounds for 8192
- * envs), 2 packed3 (A/B builds only), 3 step_kernel_tmem (56 envs per SM, lane-private fields in tensor memory: one round).  Chosen at
+ * envs), 2 packed3 (A/B builds only), 3 step_kernel_tmem (56 envs per SM, lane-private fields in thread-local memory).  Chosen at
  * b200env_create from the model's tree and the environment variable B200ENV_KERNEL (lane | packed | tmem; default: see DESIGN.md 5). */
 int32_t b200env_kernel_form(b200env_handle h);
 

@@ -1,5 +1,5 @@
 /* b200nn.h - C ABI of libb200nn.so: the two network forwards that sit on either side of the physics in the vid2player
- * rollout step (SURVEY.md 8f-1), as hand-written sm_100a GEMMs (tcgen05.mma, TMEM accumulators, TMA operand loads).
+ * rollout step (SURVEY.md 8f-1), as hand-written sm_90a GEMMs (wgmma.mma_async, register accumulators, TMA operand loads).
  *
  * What it replaces in the reference (Python / PyTorch, no C ABI there):
  *   - the low-level policy forward of ImitatorPlayer.run_one_step (vid2player/players/im_player.py:187-202 ->
@@ -8,7 +8,7 @@
  *   - the MVAE mixture-of-experts decoder MixedDecoder.forward (vid2player/motion_vae/model.py:237-252), called once per
  *     env step by MVAEPlayer.step (players/mvae_player.py:184-199) under autocast (motion_vae/base.py:390-406):
  *     y = sum_e c_e (x W_e + b_e) per layer, c = softmax(gate(z, c)).  The reference materialises a blended weight matrix
- *     PER ENV (2.7 GB per layer at 8192 envs); here the E expert products of an output tile are E accumulators in TMEM and the
+ *     PER ENV (2.7 GB per layer at 8192 envs); here the E expert products of an output tile are E register accumulators and the
  *     blend is the epilogue.
  *
  * One `linear` object = one launch: out[:, col0 : col0 + N] = act( sum_e coef[:, e] * (A W_e^T + bias_e) ).

@@ -16,7 +16,7 @@ thread_local int emu_lane = 0;
 #else
 #include "../../vid2player3d_b200/csrc/packed.cuh"
 #ifdef EMU_PACKEDT
-#include "../../vid2player3d_b200/csrc/packed_t.cuh"   // one-wave form: private fields in a per-lane array here (PrivMem), tensor memory on the GPU
+#include "../../vid2player3d_b200/csrc/packed_t.cuh"   // one-wave form: private fields in a per-lane array here (PrivMem), a thread-local array on the GPU
 #endif
 #define EMU_EPW EPW
 #define EMU_LPE PK_LANES_PER_ENV

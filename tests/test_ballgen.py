@@ -126,7 +126,7 @@ def test_full_size_tables_properties():
     assert bool(torch.isfinite(tx).all()) and bool((tx[:, 0] == 0).all()) and bool((ty[:, 0] == 0).all())
     # A ball that is still above its launch height after the 2 s of flight has its drop columns EXTRAPOLATED from the last two
     # samples (the reference does the same, :101-110): meaningless values, non-finite when the two heights coincide (14 of the
-    # 8.25 M rows on B200).  Balls launched flat or downwards without back-spin (whose lift exceeds gravity at 60 m/s) come down at
+    # 8.25 M rows on the GPU).  Balls launched flat or downwards without back-spin (whose lift exceeds gravity at 60 m/s) come down at
     # once: there every column is an interpolation.
     down = torch.from_numpy((vv <= 0) & (vs >= 0)).to(ty.device)
     assert bool(torch.isfinite(ty[down]).all())

@@ -274,7 +274,7 @@ def _pt_tables(ms):
 @pytest.mark.parametrize("asset", ["smpl_mesh_humanoid_amass_v1", "smpl_mesh_humanoid_federer", "smpl_mesh_humanoid_djokovic", "smpl_mesh_humanoid_nadal"])
 def test_owner_slot_tables_of_the_one_wave_form(asset):
     """csrc/dyn_common.cuh::build_pt_tables: every dynamic body has one (block, slot) of its own; the bodies of a tree depth share a block
-    (one warp-uniform TMEM address per level pass) and sit in different slots; a welded body has a lane at its depth but no block; the
+    (one warp-uniform private-store column block per level pass) and sit in different slots; a welded body has a lane at its depth but no block; the
     mailbox rank of a body is its rank among the dynamic bodies of its depth"""
     mod = model_compiler.canonical_racket_last(model_compiler.load_compiled(asset))
     ms, _ = abi.pack_model(mod, float(mod["mass"].sum()) / 90.0)

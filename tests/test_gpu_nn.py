@@ -1,4 +1,4 @@
-"""GPU tests of libb200nn.so (tcgen05 GEMM layers, include/b200nn.h) through its C ABI.
+"""GPU tests of libb200nn.so (wgmma GEMM layers, include/b200nn.h) through its C ABI.
 
 Tolerances.  Operands are bf16 (8 significant bits), accumulation fp32.  Against a torch computation that rounds the SAME
 operands to bf16 the kernel must agree to accumulation-order noise (`TIGHT`); against the fp32 reference module (the

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): CUDA path through the C ABI vs the oracles.
+"""GPU parity tests (run on an H100): CUDA path through the C ABI vs the oracles.
 
 Chain of trust: reference functions -> golden fixtures -> numpy oracle (tests/test_oracle_golden.py)
 -> these tests.  The physics half compares against oracle/physics_ref.c (float64 restatement of OUR
@@ -137,7 +137,7 @@ def test_physics_f32_random_one_step(model, small_lib):
           f"contact force max {np.abs(o[4]).max():.0f} N")
     assert np.abs(o[4]).max() > 50.0
     assert eq.max() < 1e-4
-    assert np.quantile(ev, 0.95) < 5e-4 and ev.max() < 2e-3     # measured on B200 (round 2): p95 5.5e-5, max 2.1e-4
+    assert np.quantile(ev, 0.95) < 5e-4 and ev.max() < 2e-3
 
 
 def test_motion_state_golden():

@@ -1,4 +1,4 @@
-"""step_kernel_tmem (csrc/packed_t.cuh: 56 envs per SM, the lane-private fields of the bodies in tensor memory) against
+"""step_kernel_tmem (csrc/packed_t.cuh: 56 envs per SM, the lane-private fields of the bodies in thread-local memory) against
 step_kernel_packed (28 envs per SM, everything in shared-memory records): the same arithmetic in the same order, so the two kernels
 are held to EXACT equality - physics only (b200env_physics_only), the embodied_pose task step and the vid2player controller step.
 The float64 parity of this form against oracle/physics_ref.c is checked on the CPU lane emulator (tests/test_emu_packed.py, variant

@@ -401,7 +401,7 @@ def test_racket_hit_is_detected():
 
 def test_controller_cuda_graph_matches_eager():
     """the captured high-level step replays EXACTLY the eager path: with the deterministic motion player (resident stream + MVAE decoder
-    GEMMs), the tcgen05 policy and the counter-based random walk nothing in a step draws from torch's generator, so after 6 steps +
+    GEMMs), the wgmma policy and the counter-based random walk nothing in a step draws from torch's generator, so after 6 steps +
     resets every state tensor, observation, reward and flag must be bit-identical between eager launches and graph replays"""
     from helpers import SIM_PARAMS, v2p_cfg
     from vid2player3d_b200.tasks import PhysicsMVAEController

@@ -1,63 +1,25 @@
-"""Caller-side proof of the boundary (SURVEY.md 8b, VERDICT r1 item 6): the REFERENCE's own rl_games-facing code -
-`VecTaskPythonWrapper` (embodied_pose/env/tasks/vec_task.py:16-63,120-138, vec_task_wrappers.py:22-28) and `RLGPUEnv.step/reset`
-(embodied_pose/run.py:93-137) - is imported unchanged through the isaacgym shim and driven over a task object.
+"""Caller-side proof of the boundary (SURVEY.md 8b): the REFERENCE's own rl_games-facing code - `VecTaskPythonWrapper`
+(embodied_pose/env/tasks/vec_task.py:16-63,120-138, vec_task_wrappers.py:22-28) and `RLGPUEnv.step/reset` (embodied_pose/run.py:93-137).
 
-  * CPU part (runs where /root/reference exists, i.e. in the build container): the reference classes drive a recording stand-in with
-    CPU buffers; every attribute / method they touch on the task must be provided by the B200 task classes.
-  * GPU part (needs a CUDA device AND the reference checkout; the driver's GPU box has no /root/reference, so it runs only on a
-    machine that has both): the same reference classes drive `vid2player3d_b200.tasks.HumanoidSMPLIM` for 32 steps, and the
-    reference's `compute_humanoid_observations_imitation` evaluated on the live GPU buffers matches `b200env_obs_imitation`.
-Both run in a subprocess so the mocked third-party modules never leak into this interpreter."""
+  * CPU part: tests/golden/reference_callers.json records what those reference classes touch on a task object when they drive it
+    (tests/golden/make_golden_callers.py runs them unchanged over a recording stand-in); every attribute / method they touch must be
+    provided by the task classes.
+  * GPU part: the same call sequence (reset, steps with the wrapper's action / observation clamps, resets of the finished envs) drives
+    `vid2player3d_b200.tasks.HumanoidSMPLIM` for 32 steps, and the imitation observation computed on the live GPU buffers matches
+    oracle/ref_port.py's restatement of the reference's `compute_humanoid_observations_imitation` (pinned by test_oracle_golden.py)."""
 import json
 import os
 import re
-import subprocess
-import sys
 
+import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.environ.get("V2P_REFERENCE", "/root/reference")
-needs_ref = pytest.mark.skipif(not os.path.isdir(os.path.join(REF, "embodied_pose")), reason="reference checkout not present")
-
-PRELUDE = r'''
-import json, os, sys
-sys.path.insert(0, os.path.join(%(root)r, "tests", "golden")); sys.path.insert(0, %(root)r)
-import _refenv
-_refenv.setup("embodied_pose")
-import torch, types
-import numpy as _np
-if not hasattr(_np, 'Inf'):
-    _np.Inf = _np.inf          # the reference targets numpy < 2 (vec_task.py:28-30)
-for _pkg in ("agents", "players", "models", "learning"):          # the reference's top-level packages (no __init__.py): make sure they
-    _m = types.ModuleType(_pkg)                                  # are not shadowed by same-named site-packages
-    _m.__path__ = [os.path.join(_refenv.REF, "embodied_pose", _pkg)]
-    sys.modules[_pkg] = _m
-import rl_games.common                                             # mocked (rl_games 1.1.4 is not installed); RLGPUEnv needs a real base class
-_ve = types.ModuleType("rl_games.common.vecenv")
-class _IVecEnv: pass
-_ve.IVecEnv, _ve.register = _IVecEnv, (lambda *a, **k: None)
-rl_games.common.vecenv = sys.modules["rl_games.common.vecenv"] = _ve
-from env.tasks.vec_task_wrappers import VecTaskPythonWrapper      # the reference's classes, unchanged
-import run as ref_run
-
-def make_rlgpu(env):
-    e = ref_run.RLGPUEnv.__new__(ref_run.RLGPUEnv)     # __init__ only looks the env creator up in rl_games' registry
-    e.env, e.use_global_obs, e.full_state = env, env.num_states > 0, {}
-    e.full_state["obs"] = e.reset()
-    return e
-'''
-
-
-def _run(code):
-    r = subprocess.run([sys.executable, "-c", PRELUDE % {"root": ROOT} + code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    return json.loads(r.stdout.strip().splitlines()[-1])
 
 
 def _provided_names():
-    """attributes the B200 task classes define: class members + every `self.<name> =` of their sources (no CUDA needed)"""
+    """attributes the task classes define: class members + every `self.<name> =` of their sources (no CUDA needed)"""
     from vid2player3d_b200.tasks import base_task, humanoid_smpl_im
     names = set(dir(humanoid_smpl_im.HumanoidSMPLIM))
     for mod in (base_task, humanoid_smpl_im):
@@ -66,74 +28,42 @@ def _provided_names():
     return names
 
 
-@needs_ref
 def test_reference_vec_task_and_rlgpu_env_touch_only_what_the_b200_task_provides():
-    out = _run(r'''
-class Recorder:
-    """stand-in with the buffer contract of BaseTask (base_task.py:62-74); records what the reference code touches"""
-    def __init__(self):
-        object.__setattr__(self, "touched", set())
-        d = dict(num_envs=6, num_obs=461, num_states=0, num_actions=75, obs_buf=torch.randn(6, 461) * 9, states_buf=torch.zeros(6, 0),
-                 rew_buf=torch.rand(6), reset_buf=torch.zeros(6, dtype=torch.long), progress_buf=torch.zeros(6, dtype=torch.long),
-                 extras={"terminate": torch.zeros(6, dtype=torch.long)}, steps=[])
-        object.__setattr__(self, "d", d)
-    def __getattr__(self, k):
-        self.touched.add(k)
-        if k == "step":
-            return lambda a: self.d["steps"].append(tuple(a.shape))
-        if k == "reset":
-            return lambda ids=None: self.d["steps"].append(("reset", None if ids is None else len(ids)))
-        return self.d[k]
-
-t = Recorder()
-vec = VecTaskPythonWrapper(t, "cpu", 5.0, 1.0)
-env = make_rlgpu(vec)
-obs = env.reset()
-for _ in range(3):
-    obs, rew, done, info = env.step(torch.randn(6, 75) * 3)
-env.reset(torch.tensor([1, 4]))
-info_d = env.get_env_info()
-print(json.dumps({"touched": sorted(t.touched), "steps": t.d["steps"], "obs_max": float(obs.abs().max()),
-                  "n_agents": env.get_number_of_agents(), "info_keys": sorted(info_d)}))
-''')
+    with open(os.path.join(ROOT, "tests", "golden", "reference_callers.json")) as f:
+        out = json.load(f)
     provided = _provided_names()
     missing = [n for n in out["touched"] if n not in provided]
-    assert not missing, f"the reference's callers touch task attributes the B200 task does not define: {missing}"
+    assert not missing, f"the reference's callers touch task attributes the task does not define: {missing}"
     assert out["obs_max"] <= 5.0 and out["n_agents"] == 1 and out["info_keys"] == ["action_space", "observation_space"]
     assert out["steps"][0] == ["reset", None] and out["steps"][-1] == ["reset", 2] and out["steps"].count([6, 75]) == 3
 
 
-@needs_ref
 @pytest.mark.gpu
 def test_reference_callers_drive_the_b200_task_on_the_gpu():
-    if not torch.cuda.is_available():
-        pytest.skip("needs a CUDA device")
-    out = _run(r'''
-from env.tasks import humanoid_smpl_im as H                        # the reference task module (its jit functions)
-from vid2player3d_b200 import model_compiler, motion_lib
-from vid2player3d_b200.configs import SIM_PARAMS, im_cfg
-from vid2player3d_b200.tasks import HumanoidSMPLIM
-model = model_compiler.load_compiled("smpl_mesh_humanoid_amass_v1")
-flat = motion_lib.synthetic(model, num_motions=6, num_frames=60, seed=3)
-torch.manual_seed(0)
-task = HumanoidSMPLIM(im_cfg(64, flat), SIM_PARAMS, 1, "cuda", 0, True)
-vec = VecTaskPythonWrapper(task, "cuda:0", 5.0, 1.0)
-env = make_rlgpu(vec)
-finite, worst = True, 0.0
-for i in range(32):
-    obs, rew, done, info = env.step(torch.rand(64, 75, device="cuda:0") * 2 - 1)
-    finite &= bool(torch.isfinite(obs).all() and torch.isfinite(rew).all())
-    rbs = task._rigid_body_state.view(64, -1, 13)
-    c = lambda x: x.contiguous()
-    args = (c(rbs[..., 0:3]), c(rbs[..., 3:7]), task._target_rb_pos, task._target_rb_rot, c(task._dof_pos), c(task._dof_vel),
-            task._target_dof_pos, c(rbs[..., 7:10]), c(rbs[..., 10:13]), task._reset_ref_motion_bodies)
-    ref = H.compute_humanoid_observations_imitation(*args, True, True)           # reference function on the live GPU buffers
-    ours = task.compute_imitation_obs(*args, True, True)
-    worst = max(worst, float((ref - ours).abs().max()))
-    ids = done.nonzero(as_tuple=False).flatten()
-    if len(ids):
-        env.reset(ids)
-print(json.dumps({"finite": finite, "worst": worst, "obs_shape": list(obs.shape), "terminate": "terminate" in info}))
-''')
-    assert out["finite"] and out["obs_shape"] == [64, 461] and out["terminate"]
-    assert out["worst"] < 1e-5, out["worst"]
+    from oracle import ref_port as R
+    from vid2player3d_b200 import model_compiler, motion_lib
+    from vid2player3d_b200.configs import SIM_PARAMS, im_cfg
+    from vid2player3d_b200.tasks import HumanoidSMPLIM
+    model = model_compiler.load_compiled("smpl_mesh_humanoid_amass_v1")
+    flat = motion_lib.synthetic(model, num_motions=6, num_frames=60, seed=3)
+    torch.manual_seed(0)
+    task = HumanoidSMPLIM(im_cfg(64, flat), SIM_PARAMS, 1, "cuda", 0, True)
+    task.reset()
+    finite, worst = True, 0.0
+    c = lambda x: x.contiguous()  # noqa: E731
+    g = lambda x: x.detach().cpu().numpy()  # noqa: E731   float32, as the reference evaluates it
+    for i in range(32):
+        task.step(torch.clamp(torch.rand(64, 75, device="cuda:0") * 2 - 1, -1.0, 1.0))     # VecTaskPythonWrapper: clip_actions = 1
+        obs = torch.clamp(task.obs_buf, -5.0, 5.0)                                         # clip_obs = 5
+        finite &= bool(torch.isfinite(obs).all() and torch.isfinite(task.rew_buf).all())
+        rbs = task._rigid_body_state.view(64, -1, 13)
+        args = (c(rbs[..., 0:3]), c(rbs[..., 3:7]), task._target_rb_pos, task._target_rb_rot, c(task._dof_pos), c(task._dof_vel),
+                task._target_dof_pos, c(rbs[..., 7:10]), c(rbs[..., 10:13]), task._reset_ref_motion_bodies)
+        ours = task.compute_imitation_obs(*args, True, True)
+        ref = R.compute_humanoid_observations_imitation(*[g(a) for a in args], True, True)
+        worst = max(worst, float(np.abs(ref - g(ours)).max()))
+        ids = task.reset_buf.nonzero(as_tuple=False).flatten()
+        if len(ids):
+            task.reset(ids)
+    assert finite and list(obs.shape) == [64, 461] and "terminate" in task.extras
+    assert worst < 1e-5, worst

@@ -9,7 +9,7 @@
 cd "$(dirname "$0")/.."
 D=$PWD/vid2player3d_b200/lib
 if [ "$1" = "build" ]; then
-  FL="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550"
+  FL="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550"
   /usr/local/cuda/bin/nvcc $FL -DPK_CONTACT_COMPACT=0 ${EXTRA} -o $D/ab_nocc.so vid2player3d_b200/csrc/b200env.cu vid2player3d_b200/csrc/b200env_v2p.cu
   /usr/local/cuda/bin/nvcc $FL -DB200ENV_WITH_PACKED3=1 ${EXTRA} -o $D/ab_p3.so vid2player3d_b200/csrc/b200env.cu vid2player3d_b200/csrc/b200env_v2p.cu
   ls -la $D

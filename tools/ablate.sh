@@ -6,7 +6,7 @@ cd "$(dirname "$0")/.."
 D=vid2player3d_b200/lib
 if [ "$1" = "build" ]; then
   for v in ${ABLS:-1 2 3 4 5}; do
-    /usr/local/cuda/bin/nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550 \
+    /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550 \
       -DABL=$v ${EXTRA} -o $D/abl_$v.so vid2player3d_b200/csrc/b200env.cu vid2player3d_b200/csrc/b200env_v2p.cu &
   done
   wait

@@ -1,6 +1,5 @@
 """Ground-contact load of a falling humanoid, step by step (CPU only: float64 restatement): bodies in contact per env and penetrating hull
-vertices per body - the length of the serial vertex loop that decides when the LAST warp of the one-wave physics launch finishes
-(profiles/r2aa_transient.md).   python tools/impact_load.py"""
+vertices per body - the length of the serial vertex loop that decides when the LAST warp of the one-wave physics launch finishes.   python tools/impact_load.py"""
 import sys
 import os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

@@ -1,4 +1,4 @@
-"""Timing of the tcgen05 layers against cuBLAS on the same box (not the bench contract): python tools/perf_nn.py [envs]
+"""Timing of the wgmma layers against cuBLAS on the same box (not the bench contract): python tools/perf_nn.py [envs]
 Every variant is captured into a CUDA graph and replayed (that is how the step uses it); times are CUDA events over 50 replays."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -34,7 +34,7 @@ def graph_ms(fn, reps=50):
 net = nn.PolicyMLP.random(M, dev)
 obs = torch.randn(M, 734, device=dev)
 ms = graph_ms(lambda: net(obs))
-print(f"PolicyMLP b200nn (cast + 4 tcgen05 launches): {ms * 1e3:.1f} us  {net.flops / ms / 1e9:.1f} TFLOP/s")
+print(f"PolicyMLP b200nn (cast + 4 wgmma launches): {ms * 1e3:.1f} us  {net.flops / ms / 1e9:.1f} TFLOP/s")
 for i, l in enumerate(net.layers):
     t = graph_ms(l.run)
     print(f"   layer {i}: {t * 1e3:.1f} us  {l.flops / t / 1e9:.1f} TFLOP/s")

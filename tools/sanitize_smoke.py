@@ -49,7 +49,7 @@ for _ in range(2):
     dual._reset_envs_masked(m)
 torch.cuda.synchronize()
 print("dual masked reset done", bool(torch.isfinite(dual.obs_buf).all()))
-# round 2: the tcgen05 layers and the fused step glue (policy + decoder in the step, masked reset through reset_done)
+# the wgmma layers and the fused step glue (policy + decoder in the step, masked reset through reset_done)
 cfg = v2p_cfg(40)
 cfg["env"]["motion_player"], cfg["env"]["low_level_policy"] = "stream+decoder", "b200nn"
 env2 = PhysicsMVAEController(cfg, SIM_PARAMS, 1, "cuda", 0, True)

@@ -5,7 +5,7 @@
 cd "$(dirname "$0")/.."
 D=$PWD/vid2player3d_b200/lib
 if [ "$1" = "build" ]; then
-  FL="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550"
+  FL="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 --shared -Xcompiler -fPIC -diag-suppress 177,550"
   S="vid2player3d_b200/csrc/b200env.cu vid2player3d_b200/csrc/b200env_v2p.cu"
   for w in 5 6 7; do
     /usr/local/cuda/bin/nvcc $FL -DPK_WARPS=$w -DPK_BOUND_WARPS=14 -o $D/ab_w${w}_r128.so $S &

@@ -1,6 +1,6 @@
 // packed3.cuh - "2 envs per warp, 3 lanes per body in the backward pass" form of the articulated control step.
 //
-// Why (profiles/r1h_step_kernel_packed_ncu.md): the 4-envs-per-warp kernel is bound by one warp's dependent instruction stream - 7
+// Why: the 4-envs-per-warp kernel is bound by one warp's dependent instruction stream - 7
 // warps per SM keep 38 % of the issue slots busy, and shared memory (7.2 KB of records per env) does not allow more envs in flight.
 // The same 28 envs per SM can be spread over 14 warps if a warp carries 2 envs, which pays only if the stream per warp gets
 // shorter.  Here lane = (env g = lane / 16, body slot s = (lane % 16) / 3, column c = lane % 3), lane 15 of each half-warp carries

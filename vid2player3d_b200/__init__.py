@@ -1,4 +1,4 @@
-"""vid2player3d_b200 - B200-native rollout hot path behind the vid2player3d Task surface.
+"""vid2player3d_b200 - H100-native rollout hot path behind the vid2player3d Task surface.
 
 Package contents (only what the hot path needs; SURVEY.md 8):
   csrc/            CUDA kernels + C ABI (include/b200env.h)

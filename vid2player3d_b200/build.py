@@ -1,5 +1,5 @@
-"""In-tree build of the CUDA extension (libb200env.so) for sm_100a.  nvcc cross-compiles
-without a GPU; the built .so travels to the GPU box with the repo snapshot."""
+"""In-tree build of the CUDA extensions (libb200env.so, libb200nn.so) for sm_90a (H100).  nvcc cross-compiles
+without a GPU."""
 import os
 import subprocess
 
@@ -8,12 +8,12 @@ SRCS = [os.path.join(HERE, "csrc", "b200env.cu"), os.path.join(HERE, "csrc", "b2
 HDRS = [os.path.join(os.path.dirname(HERE), "include", h) for h in ("b200env.h", "b200env_v2p.h", "b200ball.h")] + [os.path.join(HERE, "csrc", f) for f in ("packed.cuh", "packed_t.cuh", "ballgen.cuh", "dyn_common.cuh")]
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.environ.get("B200ENV_LIB", os.path.join(LIB_DIR, "libb200env.so"))  # override: A/B kernel variants
-# the network forwards of SURVEY.md 8f-1 (tcgen05 GEMMs): a library of their own, include/b200nn.h
+# the network forwards of SURVEY.md 8f-1 (wgmma GEMMs): a library of their own, include/b200nn.h
 SRCS_NN = [os.path.join(HERE, "csrc", "b200nn.cu")]
 HDRS_NN = [os.path.join(os.path.dirname(HERE), "include", "b200nn.h")]
 LIB_NN = os.environ.get("B200NN_LIB", os.path.join(LIB_DIR, "libb200nn.so"))
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "--shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--shared",
               "-Xcompiler", "-fPIC", "-diag-suppress", "177,550"]
 
 
@@ -38,7 +38,7 @@ def _nvcc(lib, srcs, verbose):
 
 
 def build(force=False, verbose=False):
-    """libb200env.so and libb200nn.so, both for sm_100a, in-tree"""
+    """libb200env.so and libb200nn.so, both for sm_90a, in-tree"""
     if force or needs_build():
         _nvcc(LIB, SRCS, verbose)
     if force or needs_build(LIB_NN, SRCS_NN + HDRS_NN):

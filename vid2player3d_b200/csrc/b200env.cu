@@ -1,4 +1,4 @@
-// b200env.cu - B200 (sm_100a) kernels + C ABI of the vectorised humanoid environment step.
+// b200env.cu - H100 (sm_90a) kernels + C ABI of the vectorised humanoid environment step.
 //
 // One warp per env, one lane per rigid body.  Per-asset constants (tree tables, inertias, PD
 // gains, convex-hull vertices) are staged once per CTA into shared memory with a TMA bulk copy
@@ -28,7 +28,7 @@
 #include "dyn_common.cuh"
 
 #ifndef WARPS_PER_CTA
-#define WARPS_PER_CTA 8  // A/B on B200 (profiles/r1_notes.md): 8 warps x 2 CTAs/SM, barrier per substep
+#define WARPS_PER_CTA 8  // 8 warps x 2 CTAs/SM, barrier per substep
 #endif
 #ifndef PT_STEP_SYNC
 #define PT_STEP_SYNC 1   // step_kernel_tmem: CTA barrier at every substep (keeps the 14 warps on the same instruction-cache lines)
@@ -70,7 +70,7 @@ struct b200env {
   int32_t *d_bin, *d_perm;             // [num_envs]
   uint32_t *d_pos, *d_cnt;             // [num_envs], [SORT_BINS]
   int packed3;                         // 1: the physics launch is step_kernel_packed3 (B200ENV_KERNEL=packed3)
-  int tmem;                            // 1: the physics launch is step_kernel_tmem (one wave, private fields in tensor memory; B200ENV_KERNEL=tmem|packed)
+  int tmem;                            // 1: the physics launch is step_kernel_tmem (56 envs per SM, private fields in thread-local memory; B200ENV_KERNEL=tmem)
   int split;                           // 1: three launches (pre / physics / post), 0: one fused launch.  env B200ENV_SPLIT=0|1
   int env_first = 0, env_stride = 1;   // b200env_set_env_slice: local env i = row env_first + env_stride * i of the bound tensors
   int step_grid;
@@ -428,7 +428,7 @@ __device__ __forceinline__ void control_step(const DevBlob& B, const float* vert
 #include "packed.cuh"
 #include "packed_t.cuh"
 // A/B variants that lost their measurements live outside the product build (VERDICT r1 item 10): -DB200ENV_WITH_PACKED3=1 compiles the
-// 2-envs-per-warp / 3-lanes-per-body kernel of tools/variants/packed3.cuh back in (B200ENV_KERNEL=packed3; 16 % slower, profiles/r1j, r2a)
+// 2-envs-per-warp / 3-lanes-per-body kernel of tools/variants/packed3.cuh back in (B200ENV_KERNEL=packed3)
 #ifndef B200ENV_WITH_PACKED3
 #define B200ENV_WITH_PACKED3 0
 #endif
@@ -1176,7 +1176,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
     if (ABL != 1) control_step_packed<float>(B, verts, pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
 #if POST_SYNC
     // fused form only: re-aligns the warps before the long straight-line epilogue (I-cache).  The split form's epilogue is a
-    // state write-back; without the barrier it measured 295.3 vs 298.3 us per 8192-env step (profiles/r1h_ab.log).
+    // state write-back and goes without it.
     if (!SPLIT && full_batch) group_sync();
 #endif
     if (cfg.has_ball && valid && s == BALL_SLOT && !shadow) ball_writeback(bf, erow_g, ball);
@@ -1200,44 +1200,28 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 
 // ------------------------------------------------------------------------------------------
 // One-wave form of the middle launch (pre_kernel -> this -> post_kernel): csrc/packed_t.cuh.  14 warps x 4 envs = 56 envs per CTA
-// (3.5 KB of shared memory per env + the constant block = 220 KB), the lane-private fields of the bodies in tensor memory: warp w owns
-// the 32 TMEM lanes of quadrant w % 4 and the 128 columns starting at 128 * (w / 4).  8192 envs = 147 CTAs: ONE round on 148 SMs.
+// (3.5 KB of shared memory per env + the constant block = 220 KB), the lane-private fields of the bodies in a per-thread array of
+// PT_WARP_COLS floats in local memory.
 #ifndef PT_WARPS
 #define PT_WARPS 14
 #endif
-__device__ __forceinline__ uint32_t pt_tmem_alloc(uint32_t* holder, int warp) {
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(holder)), "r"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  return *holder;
-}
-__device__ __forceinline__ void pt_tmem_free(uint32_t base, int warp) {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(512) : "memory");
-}
 
 __global__ void __launch_bounds__(PT_WARPS * 32, 1)
 step_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf, int num_envs,
                  unsigned long long* __restrict__ ticket, int env_first, int env_stride, const float* __restrict__ ext_wrench) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t s_tmem;
   load_blob(smem, gblob, blob_bytes, &mbar);
   const DevBlob& B = *reinterpret_cast<const DevBlob*>(smem);
   const b200_model_t& M = B.m;
   const float* verts = reinterpret_cast<const float*>(smem + sizeof(DevBlob));
-  const int warp = __shfl_sync(FULL, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // the shuffle tells the compiler that warp is warp-uniform: the
-                                                                                          // window addresses of the private store stay in uniform registers
+  const int warp = __shfl_sync(FULL, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // the shuffle tells the compiler that warp is warp-uniform
   float* wrec = reinterpret_cast<float*>(smem + ((blob_bytes + 15) & ~15u)) + (size_t)warp * EPW * PT_ENV_STRIDE;
   __shared__ b200_cfg_t s_cfg;
   for (int k = threadIdx.x; k < (int)(sizeof(b200_cfg_t) / 4); k += blockDim.x) reinterpret_cast<uint32_t*>(&s_cfg)[k] = reinterpret_cast<const uint32_t*>(gcfg)[k];
-  const uint32_t tbase = pt_tmem_alloc(&s_tmem, warp);   // has a __syncthreads: s_cfg is complete behind it
-  const PrivTmem ps{tbase + (((uint32_t)(warp & 3) * 32u) << 16) + (uint32_t)(warp >> 2) * PT_WARP_COLS};
+  __syncthreads();   // s_cfg complete
+  float priv[PT_WARP_COLS];
+  const PrivMem<float> ps{priv};
   const b200_cfg_t& cfg = s_cfg;
   LaneConst lc = lane_const(M, lane);
   if (lc.active) lc.rix = B.t.rix[lane];
@@ -1323,11 +1307,10 @@ step_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b
     }
     __syncwarp();
   }
-  pt_tmem_free(tbase, warp);
 }
 
-// the test entry of the same device code (b200env_physics_only with the handle in tmem mode): float only - the private store of the
-// double instantiation does not fit the tensor memory; float64 parity of this form is checked on the CPU lane emulator (tests/emu)
+// the test entry of the same device code (b200env_physics_only with the handle in tmem mode): float only; float64 parity of this form
+// is checked on the CPU lane emulator (tests/emu)
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, int n, int n_steps,
@@ -1336,15 +1319,14 @@ physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
   typedef float T;
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
-  __shared__ uint32_t s_tmem;
   load_blob(smem, gblob, blob_bytes, &mbar);
   const DevBlob& B = *reinterpret_cast<const DevBlob*>(smem);
   const b200_model_t& M = B.m;
   const float* verts = reinterpret_cast<const float*>(smem + sizeof(DevBlob));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   T* wrec = reinterpret_cast<T*>(smem + ((blob_bytes + 15) & ~15u)) + (size_t)warp * EPW * PT_ENV_STRIDE;
-  const uint32_t tbase = pt_tmem_alloc(&s_tmem, warp);
-  const PrivTmem ps{tbase + (((uint32_t)(warp & 3) * 32u) << 16) + (uint32_t)(warp >> 2) * PT_WARP_COLS};
+  T priv[PT_WARP_COLS];
+  const PrivMem<T> ps{priv};
   const int64_t eb = ((int64_t)blockIdx.x * WARPS + warp) * EPW;
   if (eb < n) {
     LaneConst lc = lane_const(M, lane);
@@ -1420,7 +1402,6 @@ physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
       if (hits) hits[e] = ball.hits;
     }
   }
-  pt_tmem_free(tbase, warp);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2059,7 +2040,7 @@ int b200env_create(const b200_model_t* model, const float* verts, const b200_cfg
   const char* sv = getenv("B200ENV_SPLIT");
   h->split = h->packed && !(sv && strcmp(sv, "0") == 0);
   // packed3 (2 envs per warp, 3 lanes per body in the backward pass; csrc/packed3.cuh): needs the split form and at most 5 bodies
-  // per tree depth.  B200ENV_KERNEL=packed3 selects it (A/B against the 4-envs-per-warp kernel, profiles/).
+  // per tree depth.  B200ENV_KERNEL=packed3 selects it (A/B against the 4-envs-per-warp kernel).
 #if B200ENV_WITH_PACKED3
   int wide = 0;
   for (int d = 0; d < MAX_LEVELS; d++) if (hb.t.lvl_all[d][SLOTS3] >= 0) wide = 1;
@@ -2070,9 +2051,10 @@ int b200env_create(const b200_model_t* model, const float* verts, const b200_cfg
   const char* so = getenv("B200ENV_SORT");
   h->sort = h->split && !h->packed3 && so && strcmp(so, "1") == 0;
   // one-wave form (csrc/packed_t.cuh): needs the split form and a tree that fits 3 column blocks x 8 owner slots
-  // It is the default where it applies (round 2: -8 % per config-2 step, -6 % per config-3 step, profiles/r2t_tmem.md);
-  // B200ENV_KERNEL=packed keeps the two-round kernel for A/B.
-  h->tmem = h->split && !h->packed3 && !h->sort && hb.t.pt_ok && hb.t.pt_nmbox <= PT_MBOX_MAX && !(kv && strcmp(kv, "packed") == 0);
+  // B200ENV_KERNEL=tmem selects it.  Not the default: on an H100 SXM (700 W power limit) the primary workload at 8192 envs measured
+  // 1.69 ms per step with it against 1.25 ms with step_kernel_packed (physics launch 1.24 vs 0.80 ms) - the private store spills out
+  // of L1, which the shared-memory records of step_kernel_packed leave room for.
+  h->tmem = h->split && !h->packed3 && !h->sort && hb.t.pt_ok && hb.t.pt_nmbox <= PT_MBOX_MAX && kv && strcmp(kv, "tmem") == 0;
   if (cfg->has_ball && cfg->ball_body_contact && !h->packed) {
     delete h;
     return fail(-2, "b200env_create: ball_body_contact needs the packed kernels (the lane-per-body kernel does not have it)%s");
@@ -2204,7 +2186,7 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
       if (h->tmem) {
         CUDA_OK(cudaFuncSetAttribute(step_kernel_tmem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_tmem, PT_WARPS * 32, psmem));
-        if (per_sm > 1) per_sm = 1;   // the CTA takes the SM's whole tensor memory
+        if (per_sm > 1) per_sm = 1;   // one CTA per SM: its 56 envs take nearly all of the shared memory
       } else
 #if B200ENV_WITH_PACKED3
       if (h->packed3) {
@@ -2395,7 +2377,7 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
   if (h->packed) {
     const size_t bsm = (h->blob_bytes + 15) & ~(size_t)15;
     if (prec == 0 && h->tmem) {
-      constexpr int W = 6;   // more than 4 warps: windows in two column ranges of the tensor memory
+      constexpr int W = 6;   // more than 4 warps: several CTA batches of the test kernel in small tests
       const size_t sm = bsm + (size_t)W * EPW * PT_ENV_STRIDE * sizeof(float);
       CUDA_OK(cudaFuncSetAttribute(physics_kernel_tmem<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
       physics_kernel_tmem<W><<<(n + W * EPW - 1) / (W * EPW), W * 32, sm, (cudaStream_t)stream>>>(

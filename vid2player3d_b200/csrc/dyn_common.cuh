@@ -33,8 +33,8 @@ struct DevTree {
   const unsigned char* face_tris;
   int32_t face_tmax, face_pad_[3];
   int32_t ntris[B200_MAX_BODIES];
-  // packed_t.cuh (one-wave kernel: lane-private fields in tensor memory): every dynamic body has a fixed owner lane slot and one of
-  // three column blocks of its lane; the bodies of one tree depth share a block (one warp-uniform TMEM address per level pass)
+  // packed_t.cuh (one-wave kernel: lane-private fields in thread-local memory): every dynamic body has a fixed owner lane slot and one
+  // of three column blocks of its lane's private store; the bodies of one tree depth share a block (one warp-uniform block per level pass)
   int8_t pt_blk[B200_MAX_BODIES];             // column block of a dynamic body, -1: welded
   int8_t pt_slot[B200_MAX_BODIES];            // lane slot of the body in every pass
   int8_t pt_body[3][PK_SLOTS];                // body pass: the dynamic body of (block, slot), -1 padded
@@ -44,8 +44,8 @@ struct DevTree {
   int32_t pt_ok, pt_nmbox, pt_pad_[4];        // pt_ok: the tree fits (3 blocks x 8 slots); pt_nmbox: mailbox entries per env
   // ball-body contact: bounding sphere of every hull about the centroid of its vertices (body frame: centre xyz, radius) - the reach
   // test in front of the exact hull query.  The sphere about the body ORIGIN (b200_model_t::radius, what the ground contact uses) is
-  // up to a limb's length for a hull that starts at its joint; a ball near a lying player passed it for ten bodies at a time
-  // (profiles/r2ad_pt_prof.log).  Pruning only: a ball outside this sphere + its radius is outside the hull + its radius.
+  // up to a limb's length for a hull that starts at its joint; a ball near a lying player passed it for ten bodies at a time.
+  // Pruning only: a ball outside this sphere + its radius is outside the hull + its radius.
   float bs[B200_MAX_BODIES][4];
 };
 struct DevBlob {
@@ -663,8 +663,7 @@ template <typename T>
 __device__ __forceinline__ bool hull_sphere(const float* vb, int vmax, const float* pl, const unsigned char* tr, int nt, const T* c, T R, T& pen,
                                             T* nl) {
   // The planes and triangles live in global memory (L2): four faces per iteration, their loads issued together, so that a lane pays one
-  // memory latency per four faces instead of one per face (the face loop of ONE lane decides when a one-wave launch ends,
-  // profiles/r2aa_transient.md).  Faces are still examined in ascending order: same separating test, same maximum, same closest point.
+  // memory latency per four faces instead of one per face (the face loop of ONE lane decides when a one-wave launch ends).  Faces are still examined in ascending order: same separating test, same maximum, same closest point.
   T smax = T(-1e30);
   int imax = 0;
   for (int t = 0; t < nt; t += 4) {
@@ -721,7 +720,7 @@ __device__ __forceinline__ bool hull_sphere(const float* vb, int vmax, const flo
 
 
 // hull_sphere with the faces of ONE body spread over the 8 lanes of an env's group (lane slot s takes the faces s, s + 8, s + 16, ...,
-// four of them per iteration): what bounds a launch is the longest serial face walk of a single lane (profiles/r2aa_transient.md) -
+// four of them per iteration): what bounds a launch is the longest serial face walk of a single lane -
 // ~2 x 100 dependent L2 round trips when one lane does a whole hull.  Every lane of the WARP calls this together (the exchanges are
 // warp shuffles); act: this lane's group has a body to test (its arguments are the same on the 8 lanes).  The outcome is the serial
 // function's bit for bit: the same per-face values, the maximum / the minimum taken with the serial loop's tie rule (the lowest face).

@@ -1,6 +1,6 @@
 // packed.cuh - "4 envs per warp" variant of the articulated control step (included by b200env.cu).
 //
-// Why: ncu of the lane-per-body kernel (profiles/r1a_step_kernel_ncu.md) shows the three tree passes running with 2-8 of 32
+// Why: in the lane-per-body kernel the three tree passes run with 2-8 of 32
 // lanes active - at most 5 bodies share a tree depth.  Here a warp owns EPW = 4 envs; lane = (env slot g = lane/8, body slot
 // s = lane%8) and at every tree level slot s handles the s-th body of that depth (host table DevTree::lvl_*), so the level
 // loops run on up to 20 lanes and are executed once for 4 envs.  Bodies change lanes from level to level, therefore the
@@ -9,11 +9,11 @@
 #pragma once
 
 #ifndef PK_CONTACT_COMPACT
-#define PK_CONTACT_COMPACT 1   // 1: per-vertex ground contact as a compacted phase of its own (pk_contact_phase); bit-identical, 291.9 -> 283.8 us
-                               // per 8192-env step on B200 (profiles/r2a_ab.md); 0 keeps the in-place form for A/B
+#define PK_CONTACT_COMPACT 1   // 1: per-vertex ground contact as a compacted phase of its own (pk_contact_phase); bit-identical;
+                               // 0 keeps the in-place form for A/B
 #endif
 #ifndef PK_SYNC_EVERY
-#define PK_SYNC_EVERY 1   // CTA barrier every n-th substep (keeps the CTA's warps on the same instruction-cache lines); A/B in profiles/r2n
+#define PK_SYNC_EVERY 1   // CTA barrier every n-th substep (keeps the CTA's warps on the same instruction-cache lines)
 #endif
 #ifndef PK_WARPS
 #define PK_WARPS 7          // 7 warps x 4 envs x 7.2 KB records + 20 KB constants = 227 KB of shared memory: one CTA per SM
@@ -565,7 +565,7 @@ __device__ __forceinline__ void pk_ball_contacts_extra(const DevBlob& B, const f
 // against the bounding sphere); the cheap shapes - the racket handle capsule, bodies of a model without hull faces - are finished
 // right there; (2) the bodies with a convex hull that passed the reach test are taken one after the other, in ascending body order, by
 // the WHOLE group (hull_sphere_coop: the hull's faces over 8 lanes).  The first version walked a hull's ~100 faces twice on one lane,
-// one dependent L2 round trip per face, and that one lane decided when a one-wave launch ended (profiles/r2aa_transient.md).  The
+// one dependent L2 round trip per face, and that one lane decided when a one-wave launch ended.  The
 // deepest contact wins (ties: the lower body index, as in the serial loop of the restatement) and the ball's lane applies it.
 template <typename T, int RS = REC>   // RS: record stride (packed_t.cuh has its own record layout; the pose run is the same)
 __device__ __forceinline__ void pk_ball_contacts_group(const DevBlob& B, const float* verts, const PhysCfg<T>& c, const T* env, int lane, bool valid,

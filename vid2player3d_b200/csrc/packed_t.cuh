@@ -1,14 +1,13 @@
 // packed_t.cuh - the "one wave" form of the packed articulated step (included by b200env.cu after packed.cuh).
 //
-// Why: step_kernel_packed keeps a 72-float record per body in shared memory, 7.2 KB per env, so an SM holds 28 envs (7 warps) and
-// 8192 envs take TWO rounds of 148 CTAs; the launch is latency-bound on one warp's dependent instruction stream and the issue slots
-// are 39 % busy (profiles/r2i_step_kernel_ncu.md).  56 resident envs per SM (8192 <= 148 x 56: ONE round, 14 warps) need <= 3.7 KB
-// per env, but the fields that lanes hand to each other are already 4.0 KB (profiles/r2a_ab.md).  Here
+// Why: step_kernel_packed keeps a 72-float record per body in shared memory, 7.2 KB per env, so an SM holds 28 envs (7 warps); the
+// launch is latency-bound on one warp's dependent instruction stream.  56 resident envs per SM (14 warps) need <= 3.7 KB per env of
+// shared memory, but the fields that lanes hand to each other are already 4.0 KB.  Here
 //   * every dynamic body has ONE owner lane for all passes (DevTree::pt_slot: the bodies of a tree depth sit in different slots of
 //     the env's 8 lanes), so the fields only the owner touches - joint state, PD target, r / zeta, joint-space bias, E / D^-1 and the
-//     C / bn / bf part of the articulated inertia: 40 floats per body - move out of shared memory into TENSOR MEMORY: 128 columns per
-//     lane, three 40-column blocks (DevTree::pt_blk), read and written with tcgen05.ld / tcgen05.st 32x32b (lane-private rows; the
-//     bodies of one depth share a block, so the address of a level pass is warp-uniform as the instruction requires);
+//     C / bn / bf part of the articulated inertia: 40 floats per body - move out of shared memory into a LANE-PRIVATE store: 128
+//     values per lane, three 40-value blocks (DevTree::pt_blk); on the GPU a per-thread array in local memory (interleaved by the
+//     hardware, so a warp's access to one column is one coalesced transaction, cached in L1 / L2);
 //   * child -> parent hand-over of the articulated inertia goes through a small per-env mailbox (one entry per body of a depth)
 //     instead of read-modify-write on the parent's record; the parent adds its children in rank order (same order, same bits);
 //   * what stays in shared memory per body is the pose / velocity of its origin (13 floats, read by children, the ball, contacts)
@@ -17,8 +16,8 @@
 //   * ground contact: masks in the body pass, the bodies in contact of an env compacted into exchange entries carved out of the mailbox
 //     (idle between two backward passes) and applied by the env's 8 lanes, 8 bodies per chunk.
 // The arithmetic is that of packed.cuh, operation for operation (tests/test_gpu_tmem.py holds the two kernels to exact equality in a
-// -fmad=false build; tests/test_emu_packed.py in float32 emulation).  PS is the private store: PrivTmem (device, float) or PrivMem
-// (plain memory: CPU lane emulator, double).  Measurements: profiles/r2t_tmem.md, r2aa_transient.md, r2ad_pt_prof.md.
+// -fmad=false build; tests/test_emu_packed.py in float32 emulation).  PS is the private store, PrivMem: the thread's local array on
+// the GPU (float), one row of a plain array per lane in the CPU lane emulator (double).
 #pragma once
 
 enum { PT_Q = 0, PT_P = 4, PT_W = 7, PT_V = 10, PT_A = 13, PT_BM = 19, PT_REC = 28 };
@@ -59,7 +58,7 @@ static_assert(PT_CX * PT_CXS <= PT_MBOX_MAX * PT_MB && PT_CX <= 8, "exchange ent
 #ifndef PT_ABL
 #define PT_ABL 0   // ablation of the phases (timing / register-pressure experiments only): 1 body pass, 2 backward, 3 forward, 4 root / ball, 5 no ground contact
 #endif
-#define PT_WARP_COLS 128    // tensor-memory columns of one warp (14 warps: at most 4 per lane quadrant -> 4 x 128 = 512)
+#define PT_WARP_COLS 128    // values of one lane's private store
 #define PT_XMASK (PT_BLOCKS * PT_COLS)   // columns 120..125 of a lane: penetration masks (2 words per block) of bodies waiting for a later contact chunk
 
 // private store as plain memory: one array of PT_BLOCKS * PT_COLS values per lane
@@ -79,77 +78,6 @@ template <typename T> struct PrivMem {
   __device__ __forceinline__ void wait_st() const {}
 };
 
-#if defined(__CUDA_ARCH__) || defined(__CUDACC__)
-// private store in tensor memory.  Every call is a warp-wide collective (.sync.aligned): all 32 lanes execute it, with the same
-// address; lanes without a body of their own load and store back whatever their cells hold.
-template <int N> __device__ __forceinline__ void tm_ld(uint32_t a, float* r);
-template <int N> __device__ __forceinline__ void tm_st(uint32_t a, const float* r);
-template <> __device__ __forceinline__ void tm_ld<1>(uint32_t a, float* r) {
-  uint32_t x;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(x) : "r"(a));
-  r[0] = __uint_as_float(x);
-}
-template <> __device__ __forceinline__ void tm_ld<2>(uint32_t a, float* r) {
-  uint32_t x, y;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(x), "=r"(y) : "r"(a));
-  r[0] = __uint_as_float(x); r[1] = __uint_as_float(y);
-}
-template <> __device__ __forceinline__ void tm_ld<4>(uint32_t a, float* r) {
-  uint32_t x[4];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(x[0]), "=r"(x[1]), "=r"(x[2]), "=r"(x[3]) : "r"(a));
-#pragma unroll
-  for (int k = 0; k < 4; k++) r[k] = __uint_as_float(x[k]);
-}
-template <> __device__ __forceinline__ void tm_ld<8>(uint32_t a, float* r) {
-  uint32_t x[8];
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(x[0]), "=r"(x[1]), "=r"(x[2]), "=r"(x[3]), "=r"(x[4]), "=r"(x[5]), "=r"(x[6]), "=r"(x[7]) : "r"(a));
-#pragma unroll
-  for (int k = 0; k < 8; k++) r[k] = __uint_as_float(x[k]);
-}
-template <> __device__ __forceinline__ void tm_st<1>(uint32_t a, const float* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(a), "r"(__float_as_uint(r[0])) : "memory");
-}
-template <> __device__ __forceinline__ void tm_st<2>(uint32_t a, const float* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(a), "r"(__float_as_uint(r[0])), "r"(__float_as_uint(r[1])) : "memory");
-}
-template <> __device__ __forceinline__ void tm_st<4>(uint32_t a, const float* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(__float_as_uint(r[0])), "r"(__float_as_uint(r[1])),
-               "r"(__float_as_uint(r[2])), "r"(__float_as_uint(r[3])) : "memory");
-}
-template <> __device__ __forceinline__ void tm_st<8>(uint32_t a, const float* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(a), "r"(__float_as_uint(r[0])),
-               "r"(__float_as_uint(r[1])), "r"(__float_as_uint(r[2])), "r"(__float_as_uint(r[3])), "r"(__float_as_uint(r[4])),
-               "r"(__float_as_uint(r[5])), "r"(__float_as_uint(r[6])), "r"(__float_as_uint(r[7])) : "memory");
-}
-// run of N columns from the compile-time offset OFF of a block: widest shapes whose column offset is a multiple of their width
-// (block bases are multiples of 8 columns)
-template <int OFF, int N, int K> __device__ __forceinline__ void tm_ld_run(uint32_t a, float* r) {
-  if constexpr (K < N) {
-    if constexpr ((OFF + K) % 8 == 0 && N - K >= 8) { tm_ld<8>(a + K, r + K); tm_ld_run<OFF, N, K + 8>(a, r); }
-    else if constexpr ((OFF + K) % 4 == 0 && N - K >= 4) { tm_ld<4>(a + K, r + K); tm_ld_run<OFF, N, K + 4>(a, r); }
-    else if constexpr ((OFF + K) % 2 == 0 && N - K >= 2) { tm_ld<2>(a + K, r + K); tm_ld_run<OFF, N, K + 2>(a, r); }
-    else { tm_ld<1>(a + K, r + K); tm_ld_run<OFF, N, K + 1>(a, r); }
-  }
-}
-template <int OFF, int N, int K> __device__ __forceinline__ void tm_st_run(uint32_t a, const float* r) {
-  if constexpr (K < N) {
-    if constexpr ((OFF + K) % 8 == 0 && N - K >= 8) { tm_st<8>(a + K, r + K); tm_st_run<OFF, N, K + 8>(a, r); }
-    else if constexpr ((OFF + K) % 4 == 0 && N - K >= 4) { tm_st<4>(a + K, r + K); tm_st_run<OFF, N, K + 4>(a, r); }
-    else if constexpr ((OFF + K) % 2 == 0 && N - K >= 2) { tm_st<2>(a + K, r + K); tm_st_run<OFF, N, K + 2>(a, r); }
-    else { tm_st<1>(a + K, r + K); tm_st_run<OFF, N, K + 1>(a, r); }
-  }
-}
-struct PrivTmem {
-  uint32_t base;   // tensor-memory address of the warp's window: (32 * (warp % 4)) << 16 | first column
-  template <int OFF, int N> __device__ __forceinline__ void ld(int blk, float* r) const { tm_ld_run<OFF, N, 0>(base + blk * PT_COLS + OFF, r); }
-  template <int OFF, int N> __device__ __forceinline__ void st(int blk, const float* r) const { tm_st_run<OFF, N, 0>(base + blk * PT_COLS + OFF, r); }
-  __device__ __forceinline__ void ld2(int col, float* r) const { tm_ld<2>(base + col, r); }
-  __device__ __forceinline__ void st2(int col, const float* r) const { tm_st<2>(base + col, r); }
-  __device__ __forceinline__ void wait_ld() const { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-  __device__ __forceinline__ void wait_st() const { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-};
-#endif
 
 // the barrier at the top of a substep: the whole CTA, or (PT_SYNC_GROUPS = 2) the even and the odd warps among themselves - half as many
 // warps to wait for, two instruction streams in the instruction cache

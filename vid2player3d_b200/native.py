@@ -22,7 +22,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB):
             raise RuntimeError(f"{LIB} not built - run `python -c 'import __graft_entry__ as g; g.build()'` "
-                               "(the B200 environment has no CPU fallback)")
+                               "(the environment has no CPU fallback)")
         L = C.CDLL(LIB)
         L.b200env_last_error.restype = C.c_char_p
         L.b200env_launch_count.restype = C.c_int64

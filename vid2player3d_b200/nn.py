@@ -1,5 +1,5 @@
 """Host side of libb200nn.so (C ABI: include/b200nn.h): the low-level policy MLP and the MVAE mixture-of-experts decoder as
-chains of hand-written sm_100a GEMM launches (csrc/b200nn.cu).  Mirrors, by name and argument meaning,
+chains of hand-written sm_90a GEMM launches (csrc/b200nn.cu).  Mirrors, by name and argument meaning,
 
   * the actor of the reference's imitation network (embodied_pose/models/im_network_builder.py:191-230: RunningMeanStd
     normalisation, `actor_mlp` 734 -> 1024 -> 1024 -> 512 with ReLU, linear `mu`) as run by ImitatorPlayer.run_one_step
@@ -189,7 +189,7 @@ class MixedDecoder:
     `weights[i]` [E, in_i, out_i], `biases[i]` [E, out_i] for the three decoder layers (input of every layer = cat(z, previous
     output)), `gate` = [(weight [out, in], bias [out])] x 3 (nn.Linear layout, ELU between).  The reference blends the expert weight
     matrices per env and runs a batched GEMV; here every layer is one launch: the E expert products of a 128 x 64 output tile are E
-    TMEM accumulators, the softmax coefficients blend them in the epilogue."""
+    register accumulators, the softmax coefficients blend them in the epilogue."""
 
     def __init__(self, weights, biases, gate, num_envs, device, latent_size=32):
         self.rows, self.device, self.L = num_envs, torch.device(device), latent_size

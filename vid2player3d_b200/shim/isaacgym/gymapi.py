@@ -2,7 +2,7 @@
 
 Only what the reference's config / task modules touch at import or config-parse time
 (SURVEY.md §8b Level B).  `acquire_gym()` returns an object whose every method raises:
-with the Level-A boundary the B200 task classes never call gym.* (create_sim is stubbed).
+with the Level-A boundary the task classes never call gym.* (create_sim is stubbed).
 """
 
 SIM_PHYSX = 1
@@ -125,7 +125,7 @@ class _NoGym:
     def __getattr__(self, name):
         def _raise(*a, **k):
             raise RuntimeError(
-                f"isaacgym shim: gym.{name}() is not available - physics runs in the B200 CUDA "
+                f"isaacgym shim: gym.{name}() is not available - physics runs in the CUDA "
                 "extension behind the Task surface (include/b200env.h), not through gymapi")
         return _raise
 

@@ -12,7 +12,7 @@ class BaseTask:
         self.device_type = cfg.get("device_type", "cuda")
         self.device_id = cfg.get("device_id", 0)
         if self.device_type not in ("cuda", "GPU"):
-            raise RuntimeError("the B200 environment runs on a CUDA device only (no CPU pipeline); "
+            raise RuntimeError("the environment runs on a CUDA device only (no CPU pipeline); "
                                f"got device_type={self.device_type!r}")
         self.device = "cuda:" + str(self.device_id)
         self.headless = cfg["headless"]

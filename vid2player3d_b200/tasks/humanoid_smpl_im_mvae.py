@@ -108,8 +108,7 @@ class HumanoidSMPLIMMVAE(BaseTask):
         ball["ball_mu_ground"] = 0.5 * (env.get("plane", {}).get("dynamicFriction", 1.0) + v2p.get("ball_friction", 0.2))
         # the ball also collides with the humanoid's bodies and the racket handle, as it does in the reference's PhysX scene (ball
         # collision filter 0, :436-442); include/b200env.h `ball_body_contact`, exact against the bodies' convex hulls
-        # (b200env_set_hull_faces).  On by default since round 2 (the body loop runs on the
-        # 8 lanes of the env's group: +59 us per 8192-env step of config 3 without the any-contact skip, profiles/r2m_ball_body.md);
+        # (b200env_set_hull_faces).  On by default (the body loop runs on the 8 lanes of the env's group);
         # vid2player.ball_body_contact: False switches it off
         if v2p.get("ball_body_contact", True):
             ball["ball_body_contact"] = 1

@@ -191,7 +191,7 @@ class StreamMotionPlayer:
 class DecoderStreamPlayer(StreamMotionPlayer):
     """StreamMotionPlayer + the MVAE decoder forward of MVAEPlayer.step (vid2player/players/mvae_player.py:184-199) executed every
     step with parameters of the reference's shapes (random: the trained checkpoints are unreleased, README.md:13): the 32-d latent
-    action and the 288-d condition go through `nn.MixedDecoder` (gate + three mixture-of-experts layers, tcgen05 GEMMs,
+    action and the 288-d condition go through `nn.MixedDecoder` (gate + three mixture-of-experts layers, wgmma GEMMs,
     include/b200nn.h), the predicted frame becomes the next condition like `_update_mvae_state` (:201-204, autoregressive, kept in
     the normalised range), the two extra outputs are the phase prediction (`_phase_decoded`).  The kinematic TARGETS still come from
     the resident stream - a random-weight decoder produces noise poses - so this measures the decoder where it runs (inside the
@@ -231,7 +231,7 @@ class PhysicsMVAEController:
         self.cfg_v2p = env["vid2player"]
         cfg["device_type"], cfg["device_id"], cfg["headless"] = device_type, device_id, headless
         if device_type not in ("cuda", "GPU"):
-            raise RuntimeError("the B200 environment runs on a CUDA device only (no CPU pipeline)")
+            raise RuntimeError("the environment runs on a CUDA device only (no CPU pipeline)")
         self._max_episode_length = env["episodeLength"]
         self._enable_early_termination = env.get("enableEarlyTermination", False)
         self._is_train = env.get("is_train", True)
@@ -311,7 +311,7 @@ class PhysicsMVAEController:
             w_pos=float(weights.get('pos', 1.0 if rtype == 'reach' else 0.0)), w_ball_pos=float(weights.get('ball_pos', 0.0)),
             court_min=self._court_min.tolist(), court_max=self._court_max.tolist(), est_params=self._est_params, dual=0,
             use_history=int(self._use_history))
-        # fused step glue (B200): action handling of pre_physics_step as one launch; trajectory roll + step counters inside the post launch
+        # fused step glue: action handling of pre_physics_step as one launch; trajectory roll + step counters inside the post launch
         self._fused_pre = bool(self.cfg.get("b200_fused_glue", True)) and not self.cfg_v2p.get('add_residual_root')
         self._fused_post = bool(self.cfg.get("b200_fused_glue", True))
         self._mvae_actions = f(N, self._num_mvae_action)
@@ -341,7 +341,7 @@ class PhysicsMVAEController:
             zeros = torch.zeros(self.num_envs, task.num_actions, device=self.device)
             policy = lambda obs: zeros  # noqa: E731  (zero residual: PD targets = kinematic targets)
         elif policy == "b200nn":     # the reference's actor shape (734 -> 1024 -> 1024 -> 512 -> 75, ReLU) with random weights, as
-            from .. import nn        # tcgen05 layers; obs clamp and action clamp of run_one_step are folded into its first / last launch
+            from .. import nn        # wgmma layers; obs clamp and action clamp of run_one_step are folded into its first / last launch
             policy = nn.PolicyMLP.random(self.num_envs, self.device, in_dim=task.num_obs, out_dim=task.num_actions,
                                          seed=self.cfg.get("seed", 10), clamp_obs=5.0, clamp_actions=1.0,
                                          out_gain=float(env.get("low_level_policy_gain", 0.1)))
@@ -401,7 +401,7 @@ class PhysicsMVAEController:
         return True
 
     def reset_done(self):
-        """B200 addition: `reset(reset_buf.nonzero())` without the id list - the mask of the finished envs is taken from the device
+        """Addition: `reset(reset_buf.nonzero())` without the id list - the mask of the finished envs is taken from the device
         flags and the whole reset is one replay of the reset graph: no host synchronisation between steps.  Needs enable_cuda_graph()."""
         if getattr(self, "_reset_graph", None) is None:
             self.reset(self.reset_buf.nonzero(as_tuple=False).flatten())

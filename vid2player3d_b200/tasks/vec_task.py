@@ -70,7 +70,7 @@ class VecTaskPython(VecTask):
                 self.task.rew_buf.to(self.rl_device), self.task.reset_buf.to(self.rl_device), self.task.extras)
 
     def enable_cuda_graph(self, actions=None, warmup=3):
-        """B200 addition (not in the reference): capture `clamp(actions) -> task.step -> clamp(obs)` - 1 memset + 5 kernels - into
+        """Addition (not in the reference): capture `clamp(actions) -> task.step -> clamp(obs)` - 1 memset + 5 kernels - into
         one CUDA graph; `step()` then costs one graph launch on the host instead of ~8 launches through PyTorch and ctypes.
         `actions`: the device tensor the caller will keep passing (its storage becomes the graph's input; any other tensor is
         copied into it first).  The returned observation tensor is a fixed buffer, overwritten by the next step (the reference
