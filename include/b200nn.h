@@ -16,6 +16,9 @@
  * Shapes are padded by the caller (the Python binding does it): rows of A / out to a multiple of 128, K and the leading
  * dimensions to a multiple of 64 elements with zero padding, rows of W_e to a multiple of the output tile (128, or 32 when E > 1).
  * Functions return 0 on success; b200nn_last_error() describes the last failure.  No allocation and no host sync in `run`.
+ *
+ * Non-finite values propagate as in torch: ReLU, the output clamp and the cast clamp keep a NaN a NaN (torch.relu / torch.clamp
+ * semantics), so an env whose observation blew up yields NaN actions instead of plausible clamped ones.
  */
 #ifndef B200NN_H
 #define B200NN_H
@@ -53,7 +56,10 @@ typedef struct b200nn_linear_desc {
 int b200nn_abi_version(void);
 const char* b200nn_last_error(void);
 
-/* builds the TMA tensor maps of the operands (host side, once); the device buffers must stay where they are */
+/* builds the TMA tensor maps of the operands (host side, once); the device buffers must stay where they are.  Returns -2 (before any
+ * driver call) for a descriptor the kernel cannot run: num_experts outside 1..6, K / lda / ldw not padded to 64, n_padded not a
+ * multiple of the tile or n outside 1..n_padded, rows < 1, bf16 ldo / out_col0 not multiples of 8, operands not 16-byte aligned,
+ * out_col0 < 0, ldo < out_col0 + n, an unknown act. */
 int b200nn_linear_create(const b200nn_linear_desc_t* desc, int32_t device, b200nn_linear_handle* out);
 int b200nn_linear_destroy(b200nn_linear_handle h);
 /* one launch on `stream` (CUDA-graph capturable) */

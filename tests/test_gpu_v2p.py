@@ -867,3 +867,62 @@ def test_obs_imitation_rows_matches_gathered_inputs():
     want = torch.clamp((ref - mean) * rstd, -5, 5).to(torch.bfloat16)
     assert torch.equal(op[:96, :734], want) and float(op[96:].abs().max()) == 0 and float(op[:, 734:].abs().max()) == 0
 
+
+
+def test_obs_operand_row_propagates_nan():
+    """the bf16 operand row written with the observation keeps a NaN feature NaN (torch.clamp semantics) instead of clamping it to a
+    bound: an env whose state blew up must not get a plausible action"""
+    from vid2player3d_b200.tasks import PhysicsMVAEController
+    torch.manual_seed(3)
+    env = PhysicsMVAEController(v2p_cfg(96), SIM_PARAMS, 1, "cuda", 0, True)
+    env.reset()
+    env.step(torch.clamp(torch.randn(96, env.num_actions, device=DEV), -5, 5))
+    task = env._physics_player.task
+    task._dof_vel[5, 3] = float("nan")
+    out = torch.zeros_like(task.obs_buf)
+    op = torch.zeros(128, 768, device=DEV, dtype=torch.bfloat16)
+    mean, rstd = torch.randn(734, device=DEV) * 0.1, torch.rand(734, device=DEV) + 0.5
+    task._env.obs_imitation_rows(96, task._rigid_body_state, 26, task._dof_state, task._target_rb_pos, task._target_rb_rot, task._target_dof_pos,
+                                 task._reset_ref_motion_bodies, True, True, out, obs_bf16=op, mean=mean, rstd=rstd, clamp=5.0)
+    torch.cuda.synchronize()
+    nan = torch.isnan(out)
+    assert bool(nan[5].any()) and not bool(nan[torch.arange(96, device=DEV) != 5].any())
+    want = torch.clamp((out - mean) * rstd, -5, 5).to(torch.bfloat16)
+    got = op[:96, :734]
+    assert torch.equal(torch.isnan(got.float()), nan), "NaN features of the observation must stay NaN in the policy operand"
+    assert torch.equal(got[~nan], want[~nan])
+
+
+def test_low_level_policy_fused_and_unfused_agree():
+    """run_one_step's two branches give the same actions: the fused one (the observation kernel writes the policy's normalised,
+    clamped operand row) and the unfused one (any callable policy, here the same network behind a lambda) both hand the policy the raw
+    observation, as the reference does (clip_obs = inf, player_builder.py:40); the only clamp is the policy's own after its
+    normalisation.  Same weights, same physics state; the raw observation has features beyond +-5."""
+    from vid2player3d_b200 import nn
+    from vid2player3d_b200.tasks import PhysicsMVAEController
+    N, steps = 64, 3
+    g = torch.Generator().manual_seed(8)
+    mean, var = torch.randn(734, generator=g) * 0.5, torch.rand(734, generator=g) * 4 + 0.25
+    runs = []
+    for fused in (True, False):
+        net = nn.PolicyMLP.random(N, DEV, seed=3, out_gain=1.0, obs_mean=mean, obs_var=var, clamp_obs=5.0, clamp_actions=1.0)
+        torch.manual_seed(4)
+        cfg = v2p_cfg(N)
+        cfg["env"]["low_level_policy"] = net if fused else (lambda obs, net=net: net(obs))
+        env = PhysicsMVAEController(cfg, SIM_PARAMS, 1, "cuda", 0, True)
+        task = env._physics_player.task
+        assert (task._obs_operand is not None) == fused and task.num_obs == 734 and task.num_actions == 75
+        env.reset()
+        gen = torch.Generator(device=DEV).manual_seed(9)
+        rec = []
+        for _ in range(steps):
+            env.step(torch.clamp(torch.randn(N, env.num_actions, device=DEV, generator=gen), -5, 5))
+            torch.cuda.synchronize()
+            rec.append((task.obs_buf.clone(), net.out.clone(), task._dof_state.clone()))
+        runs.append(rec)
+    assert float(runs[0][-1][0].abs().max()) > 5.0, "the state must carry raw observation features beyond +-5"
+    for i, ((o0, a0, s0), (o1, a1, s1)) in enumerate(zip(*runs)):
+        assert torch.equal(o0, o1), f"step {i}: observations differ"
+        d = (a0 - a1).abs()
+        assert torch.equal(a0, a1), f"step {i}: fused and unfused actions differ by up to {float(d.max()):.3g} on {int((d > 0).sum())} entries"
+        assert torch.equal(s0, s1), f"step {i}: physics state differs"

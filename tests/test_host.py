@@ -291,6 +291,64 @@ def test_nn_library_exports_and_layout(tmp_path):
             nn.Linear(torch.zeros(128, 64, dtype=torch.bfloat16), torch.zeros(8, 64), torch.zeros(8), torch.zeros(128, 64, dtype=torch.bfloat16), 4)
 
 
+def test_nn_linear_create_rejects_bad_descriptors():
+    """b200nn_linear_create validates the descriptor before it looks up the driver, so fake (aligned, non-null, never dereferenced)
+    pointers reach every rule on a machine without a GPU: each malformed descriptor returns -2 with its own message; a valid one
+    gets past validation (-3 without a CUDA driver, 0 with one)."""
+    from vid2player3d_b200 import build, nn
+    build.build()
+    L = nn.lib()
+
+    def desc(**kw):
+        d = dict(a=0x10000, lda=128, w=0x20000, ldw=128, bias=0x30000, coef=0x40000, out=0x50000, ldo=256, out_col0=0, rows=200, n=100,
+                 n_padded=128, k_padded=128, num_experts=1, act=1, out_bf16=1, out_min=0.0, out_max=0.0)
+        d.update(kw)
+        return nn.LinearDesc(**d)
+
+    def create(d):
+        h = C.c_void_p()
+        rc = L.b200nn_linear_create(C.byref(d), C.c_int32(0), C.byref(h))
+        if h:
+            L.b200nn_linear_destroy(h)
+        return rc, L.b200nn_last_error().decode()
+
+    bad = [
+        (dict(num_experts=0), "num_experts must be 1..6"),
+        (dict(num_experts=7), "num_experts must be 1..6"),
+        (dict(k_padded=96), "padded to multiples of 64"),
+        (dict(k_padded=0), "padded to multiples of 64"),
+        (dict(lda=96), "padded to multiples of 64"),
+        (dict(ldw=64), "padded to multiples of 64"),              # ldw < k_padded
+        (dict(n_padded=96), "n_padded must be a multiple"),
+        (dict(n=0), "n_padded must be a multiple"),
+        (dict(n=129), "n_padded must be a multiple"),
+        (dict(num_experts=2, n_padded=48, n=40), "n_padded must be a multiple"),
+        (dict(rows=0), "rows < 1"),
+        (dict(ldo=252), "multiples of 8"),
+        (dict(out_col0=4), "multiples of 8"),
+        (dict(a=0x10008), "16-byte aligned"),
+        (dict(w=0x20004), "16-byte aligned"),
+        (dict(out=0x50002), "16-byte aligned"),
+        (dict(out_col0=-8), "out_col0 < 0"),
+        (dict(out_bf16=0, out_col0=-1), "out_col0 < 0"),
+        (dict(ldo=96), "ldo < out_col0 \\+ n"),
+        (dict(out_col0=160), "ldo < out_col0 \\+ n"),
+        (dict(out_bf16=0, ldo=103, out_col0=5, n=99), "ldo < out_col0 \\+ n"),
+        (dict(act=3), "unknown activation"),
+        (dict(act=-1), "unknown activation"),
+    ]
+    for kw, msg in bad:
+        rc, err = create(desc(**kw))
+        assert rc == -2 and re.search(msg, err), (kw, rc, err)
+    rc, err = create(desc(num_experts=2, n_padded=32, n=32, coef=None))
+    assert rc == -1 and "coefficient" in err                      # a mixture layer without its coefficients
+    want = 0 if torch.cuda.is_available() else -3
+    for kw in (dict(), dict(num_experts=6, n_padded=64, n=33, act=2), dict(out_bf16=0, ldo=103, out_col0=3, n=100, act=0),
+               dict(out_col0=32, ldo=136, n=100, out_min=-1.0, out_max=1.0)):
+        rc, err = create(desc(**kw))
+        assert rc == want, (kw, rc, err)
+
+
 def test_v2p_glue_struct_layouts(tmp_path):
     from vid2player3d_b200 import abi
     src = tmp_path / "sz.c"

@@ -1915,8 +1915,9 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
         x0 = (x0 - __ldg(ob.mean + k)) * __ldg(ob.rstd + k);
         if (k + 1 < W) x1 = (x1 - __ldg(ob.mean + k + 1)) * __ldg(ob.rstd + k + 1);
       }
-      x0 = fminf(fmaxf(x0, -ob.clamp), ob.clamp);
-      x1 = fminf(fmaxf(x1, -ob.clamp), ob.clamp);
+      // torch.clamp semantics: a NaN feature stays NaN in the operand (fminf / fmaxf would hide a blown-up env behind -clamp)
+      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x0) : "f"(ob.clamp), "f"(-ob.clamp));
+      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x1) : "f"(ob.clamp), "f"(-ob.clamp));
       if (k + 1 < W) *reinterpret_cast<__nv_bfloat162*>(brow + k) = __floats2bfloat162_rn(x0, x1);   // ld is a multiple of 64: 4-byte aligned
       else brow[k] = __float2bfloat16_rn(x0);
     }

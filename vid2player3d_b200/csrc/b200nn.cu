@@ -129,8 +129,14 @@ template <> __device__ __forceinline__ void wgmma_bf16<64>(float* d, uint64_t ad
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
+// min / max that return NaN when an input is NaN (torch.relu / torch.clamp semantics; fminf / fmaxf would turn a NaN into the other
+// operand and hide a blown-up env behind a plausible value).  One instruction each, like fminf / fmaxf; equal to them otherwise.
+__device__ __forceinline__ float fmax_nan(float a, float b) { float r; asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+__device__ __forceinline__ float fmin_nan(float a, float b) { float r; asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b)); return r; }
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) { return fmin_nan(fmax_nan(x, lo), hi); }
+
 __device__ __forceinline__ float apply_act(float x, int act) {
-  if (act == B200NN_ACT_RELU) return fmaxf(x, 0.f);
+  if (act == B200NN_ACT_RELU) return fmax_nan(x, 0.f);
   if (act == B200NN_ACT_ELU) return x > 0.f ? x : expm1f(x);   // F.elu, alpha = 1
   return x;
 }
@@ -160,7 +166,7 @@ struct LinearParams {
 
 __device__ __forceinline__ float finish(float x, const LinearParams& p) {
   x = apply_act(x, p.act);
-  return p.out_min < p.out_max ? fminf(fmaxf(x, p.out_min), p.out_max) : x;
+  return p.out_min < p.out_max ? clamp_nan(x, p.out_min, p.out_max) : x;
 }
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -314,7 +320,7 @@ __global__ void cast_rows_kernel(const float* __restrict__ src, int ld_src, __nv
     for (int c = threadIdx.x; c < cols; c += blockDim.x) {
       float x = s[c];
       if (mean) x = (x - __ldg(mean + c)) * __ldg(rstd + c);
-      const __nv_bfloat16 v = __float2bfloat16_rn(fminf(fmaxf(x, lo), hi));
+      const __nv_bfloat16 v = __float2bfloat16_rn(clamp_nan(x, lo, hi));
       dst[o + c] = v;
       if (dst2) dst2[o + c] = v;
       if (dst3) dst3[o + c] = v;
@@ -420,6 +426,9 @@ int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_l
   if (d->n_padded < bn || d->n_padded % bn || d->n < 1 || d->n > d->n_padded) return fail(-2, "b200nn_linear_create: n_padded must be a multiple of the output tile");
   if (d->rows < 1) return fail(-2, "b200nn_linear_create: rows < 1");
   if (d->out_bf16 && (d->ldo % 8 || d->out_col0 % 8)) return fail(-2, "b200nn_linear_create: bf16 output needs ldo and out_col0 multiples of 8");
+  if (d->out_col0 < 0) return fail(-2, "b200nn_linear_create: out_col0 < 0");
+  if ((int64_t)d->ldo < (int64_t)d->out_col0 + d->n) return fail(-2, "b200nn_linear_create: ldo < out_col0 + n");
+  if (d->act != B200NN_ACT_NONE && d->act != B200NN_ACT_RELU && d->act != B200NN_ACT_ELU) return fail(-2, "b200nn_linear_create: unknown activation");
   if (((uintptr_t)d->a | (uintptr_t)d->w | (uintptr_t)d->out) & 15) return fail(-2, "b200nn_linear_create: operands must be 16-byte aligned");
   encode_tiled_fn enc = get_encode();
   if (!enc) return fail(-3, "b200nn_linear_create: cuTensorMapEncodeTiled not available (no CUDA driver)");

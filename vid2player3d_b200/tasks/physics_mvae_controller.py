@@ -351,11 +351,14 @@ class PhysicsMVAEController:
             task._obs_operand = (policy.x, policy.mean, policy.rstd, policy.clamp_obs)
 
         def run_one_step():   # ImitatorPlayer.run_one_step (players/im_player.py:187-202)
+            # The reference clamps the raw observation to env.clip_obs, which player_builder.py:40 reads from `clip_observations`
+            # (default inf; no imitation config sets it): the only observation clamp is the policy's own, after its running-mean-std
+            # normalisation.  Both branches give the policy the raw observation.
             with torch.no_grad():
                 if fused:
                     task.step(self._low_level_policy.forward_prepared())
                 else:
-                    action = self._low_level_policy(torch.clamp(task.obs_buf, -5.0, 5.0))
+                    action = self._low_level_policy(task.obs_buf)
                     task.step(torch.clamp(action, -1.0, 1.0))
         self._physics_player = SimpleNamespace(task=task, run_one_step=run_one_step)
         player = env.get("motion_player", None)
