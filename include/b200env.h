@@ -233,8 +233,8 @@ int b200env_set_env_slice(b200env_handle h, int32_t env_first, int32_t env_strid
  * uses the approximation. */
 int b200env_set_hull_faces(b200env_handle h, const float* planes, const uint8_t* tris, const int32_t* ntris, int32_t tmax);
 
-/* Which form of the physics launch this handle uses: 0 lane-per-body kernel, 1 step_kernel_packed (28 envs per SM, two rounds for 8192
- * envs), 2 packed3 (A/B builds only), 3 step_kernel_tmem (56 envs per SM, lane-private fields in thread-local memory).  Chosen at
+/* Which form of the physics launch this handle uses: 0 lane-per-body kernel, 1 step_kernel_packed (32 envs per SM in the split form:
+ * two rounds for 8192 envs on 132 SMs), 2 packed3 (A/B builds only), 3 step_kernel_tmem (56 envs per SM, lane-private fields in thread-local memory).  Chosen at
  * b200env_create from the model's tree and the environment variable B200ENV_KERNEL (lane | packed | tmem; default: see DESIGN.md 5). */
 int32_t b200env_kernel_form(b200env_handle h);
 

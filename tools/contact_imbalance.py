@@ -3,7 +3,7 @@
 Rolls N humanoids forward with a random policy until they lie on the ground (the state the bench workload is in: 92 % of the envs),
 then counts, per env and body, the hull vertices below the ground plane - the per-vertex loop of contact_hull is the part of the
 body pass whose cost differs between lanes.  Reports, for the packed kernel's lane mapping (body b of env g is handled by lane
-(g, b % 8) in round b / 8; a warp = 4 consecutive envs; a CTA batch = 7 warps):
+(g, b % 8) in round b / 8; a warp = 4 consecutive envs; a CTA batch = 8 warps, the split form's step_kernel_packed):
   * penetrating vertices per env (mean, p90, max),
   * executed vs useful iterations of the vertex loop: a warp runs max-over-lanes iterations per round,
   * the spread of the per-warp totals inside a CTA batch (what the batch barrier waits for)."""
@@ -58,15 +58,15 @@ def main(n=224, steps=45, seed=0):
     warp_tot = np.array(warp_tot)
     print(f"vertex-loop iterations per control-step substep: useful {useful}, executed in lock step {executed} -> lanes busy {useful / executed * 100:.0f} %")
     print(f"serial vertex iterations per warp and substep (sum over the 3 rounds of the max over lanes): mean {warp_tot.mean():.1f}, max {warp_tot.max()}")
-    nbatch = len(warp_tot) // 7
-    b = warp_tot[:nbatch * 7].reshape(nbatch, 7)
-    print(f"inside a CTA batch of 7 warps: mean of max {b.max(1).mean():.1f} vs mean {b.mean():.1f} -> the slowest warp has "
+    nbatch = len(warp_tot) // 8
+    b = warp_tot[:nbatch * 8].reshape(nbatch, 8)
+    print(f"inside a CTA batch of 8 warps: mean of max {b.max(1).mean():.1f} vs mean {b.mean():.1f} -> the slowest warp has "
           f"{(b.max(1).mean() / b.mean() - 1) * 100:.0f} % more vertex iterations than the average one (~70 instructions each)")
     def layout(order):
         """serial vertex iterations per warp / per batch when the envs are handed out in `order`"""
         P = pen[order]
         wt = np.array([sum(P[w0:w0 + 4, r * 8:(r + 1) * 8].max() for r in range(3)) for w0 in range(0, n - 3, 4)])
-        bt = wt[:len(wt) // 7 * 7].reshape(-1, 7)
+        bt = wt[:len(wt) // 8 * 8].reshape(-1, 8)
         return wt.mean(), bt.max(1).mean()
     env_serial = np.array([sum(pen[e, r * 8:(r + 1) * 8].max() for r in range(3)) for e in range(n)])
     print("hand-out order of the envs -> (mean serial iterations per warp, mean over batches of the slowest warp):")

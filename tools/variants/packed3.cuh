@@ -1,8 +1,8 @@
 // packed3.cuh - "2 envs per warp, 3 lanes per body in the backward pass" form of the articulated control step.
 //
 // Why: the 4-envs-per-warp kernel is bound by one warp's dependent instruction stream - 7
-// warps per SM keep 38 % of the issue slots busy, and shared memory (7.2 KB of records per env) does not allow more envs in flight.
-// The same 28 envs per SM can be spread over 14 warps if a warp carries 2 envs, which pays only if the stream per warp gets
+// warps per SM keep 38 % of the issue slots busy, and shared memory (then 7.2 KB of records per env) did not allow more envs in flight.
+// The same 28 envs per SM could be spread over 14 warps if a warp carries 2 envs, which pays only if the stream per warp gets
 // shorter.  Here lane = (env g = lane / 16, body slot s = (lane % 16) / 3, column c = lane % 3), lane 15 of each half-warp carries
 // the ball.  The backward step of a body - the longest block of a tree level - is done by its 3 column lanes: each owns one column
 // of the 3x3 blocks (G = D^-1 A, K = D^-1 B, the articulated A / B / C, the shifted blocks) and one component of the bias
@@ -33,8 +33,8 @@ template <typename T>
 __device__ __forceinline__ void pk_backward3(const DevBlob& B, T* env, int b, bool live, int c, int l1, int l2, T* oA, T* oB, T* oC, T& obn,
                                              T& obf) {
   T* rec = env + RIX(B, b) * REC;
-  T ab[28], rzu[12], E[6];   // A[6] Bm[9] C[6] bn[3] bf[3] pad | r[3] zeta_a[3] zeta_l[3] u[3]
-  ldr<R_A, 28>(rec, ab); ldr<R_R, 12>(rec, rzu); ldr<R_E, 6>(rec, E);
+  T ab[R_AB], rzu[12], E[6];   // A[6] Bm[9] C[6] bn[3] bf[3] | r[3] zeta_a[3] zeta_l[3] u[3]
+  ldr<R_A, R_AB>(rec, ab); ldr<R_R, 12>(rec, rzu); ldr<R_E, 6>(rec, E);
   const T *A = ab, *Bm = ab + 6, *C = ab + 15, *bn = ab + 21, *bf = ab + 24, *r = rzu, *za = rzu + 3, *zl = rzu + 6;
   T D[6], Dinv[6], ub[3];
 #pragma unroll
@@ -125,6 +125,8 @@ __device__ __forceinline__ void control_step_packed3(const DevBlob& B, const flo
   const int l1 = (base + (col == 2 ? 0 : col + 1)) & 31, l2 = (base + (col == 0 ? 2 : col - 1)) & 31;
   T* env = wrec + g * ENV_STRIDE;
   const int nb = M.nb;
+  T pd[PK_PD_SLOTS][3];   // PD targets of my body-pass bodies (b = rr * 16 + u, rr = 0, 1)
+  pk_pd_take<T, LPE3>(B, env, u, valid, pd);
   for (int d = 1; d <= M.max_depth; d++) {
     const int b = lead ? B.t.lvl_all[d][s] : -1;
     if (b >= 0) pk_fk<T, true>(B, env, b);
@@ -143,7 +145,11 @@ __device__ __forceinline__ void control_step_packed3(const DevBlob& B, const flo
       // 1. per-body inertia / bias / contacts / joint drive: one lane per body, 16 lanes per env
       for (int rr = 0; rr * LPE3 < nb; rr++) {
         const int b = rr * LPE3 + u;
-        if (valid && b < nb && !M.fixed[b]) pk_body<T>(B, verts, c, env, b, sim == 0);
+        if (valid && b < nb && !M.fixed[b]) {
+          T pdb[3];
+          pk_pd_pick<T>(pd, rr, pdb);
+          pk_body<T>(B, verts, c, env, b, sim == 0, pdb);
+        }
       }
       __syncwarp();
       // 2. articulated inertia, leaves -> root: 3 lanes per body
@@ -197,4 +203,5 @@ __device__ __forceinline__ void control_step_packed3(const DevBlob& B, const flo
       }
     }
   }
+  pk_pd_park<T, LPE3>(B, env, u, valid, pd);
 }

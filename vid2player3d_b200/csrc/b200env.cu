@@ -1033,41 +1033,48 @@ post_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gc
 }
 
 // ------------------------------------------------------------------------------------------
-// packed variant of the fused step: 4 envs per warp in the physics (packed.cuh), lane-per-body prologue / epilogue per env
-#ifndef PK_WARPS
-#define PK_WARPS 7          // 7 warps x 4 envs x 7.2 KB records + 20 KB constants = 227 KB of shared memory: one CTA per SM
-#endif
+// packed variant of the fused step: 4 envs per warp in the physics (packed.cuh), lane-per-body prologue / epilogue per env.
+// Warps per CTA (packed.cuh): PK_WARPS = 8 for the split form, 8 x 4 envs x 6,848 B of records + the 7,312 B DevBlob header =
+// 226,448 B of shared memory; PK_WARPS_FUSED = 7 for the fused form, which also carries PK_SCRATCH floats of prologue scratch per
+// warp.  One CTA per SM either way.  The hull vertices behind the header are read from global memory (L1), not staged: with them
+// the split form's 32 envs would not fit, and at 28 envs per SM 8192 envs take 3 rounds of batches on 132 SMs instead of 2.
 #define PK_SCRATCH 232
-// PK_SHADOW=1 (experiment, tools/shadow.sh): launch 2 x PK_WARPS warps; warps PK_WARPS.. are "shadows" that run the instruction stream
-// of warp - PK_WARPS on the same records with every store suppressed: what would 14 resident warps cost (issue slots, shared-memory
-// bandwidth, 128 registers)?  Results of the real warps are unchanged.
+// PK_SHADOW=1 (experiment, tools/shadow.sh): launch twice the warps; the second half are "shadows" that run the instruction stream
+// of their twin in the first half on the same records with every store suppressed: what would twice the resident warps cost (issue
+// slots, shared-memory bandwidth, registers)?  Results of the real warps are unchanged.
 #ifndef PK_SHADOW
 #define PK_SHADOW 0
 #endif
-#define PK_LAUNCH_WARPS (PK_WARPS * (PK_SHADOW ? 2 : 1))
-#ifndef PK_BOUND_WARPS
-#define PK_BOUND_WARPS PK_LAUNCH_WARPS    // A/B: a larger bound = the register budget of that many warps at the product's warp count
+__host__ __device__ constexpr int pk_warps(bool split) { return split ? PK_WARPS : PK_WARPS_FUSED; }
+__host__ __device__ constexpr int pk_launch_warps(bool split) { return pk_warps(split) * (PK_SHADOW ? 2 : 1); }
+#ifdef PK_BOUND_WARPS
+#define PK_BOUND(split) (PK_BOUND_WARPS)   // A/B: a larger bound = the register budget of that many warps at the product's warp count
+#else
+#define PK_BOUND(split) pk_launch_warps(split)
 #endif
 
 // SPLIT = false: the whole env step in this launch.  SPLIT = true: the middle launch of pre_kernel -> this -> post_kernel; here only
 // the state rows / PD targets / residual wrench are read and the state rows written (the once-per-step task logic runs in the two
-// high-occupancy kernels, where its memory latency is covered by 48+ warps per SM instead of the 7 this kernel can hold).
+// high-occupancy kernels, where its memory latency is covered by 48+ warps per SM instead of the 8 this kernel can hold).
 template <bool SPLIT>
-__global__ void __launch_bounds__(PK_BOUND_WARPS * 32, 1)
+__global__ void __launch_bounds__(PK_BOUND(SPLIT) * 32, 1)
 step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf,
                    b200_motion_lib_t ml, const float* __restrict__ actions, int num_envs, unsigned long long* __restrict__ ticket,
                    int env_first, int env_stride, const float* __restrict__ ext_wrench, const int32_t* __restrict__ perm) {
+  constexpr int PK_WARPS_K = pk_warps(SPLIT);
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
-  load_blob(smem, gblob, blob_bytes, &mbar);
+  static_assert(sizeof(DevBlob) % 16 == 0, "the bulk copy of the header moves whole 16-byte units");
+  (void)blob_bytes;
+  load_blob(smem, gblob, (uint32_t)sizeof(DevBlob), &mbar);   // the header only; the vertices stay in global memory
   const DevBlob& B = *reinterpret_cast<const DevBlob*>(smem);
   const b200_model_t& M = B.m;
-  const float* verts = reinterpret_cast<const float*>(smem + sizeof(DevBlob));
-  float* scratch_all = reinterpret_cast<float*>(smem + ((blob_bytes + 15) & ~15u));
-  const int warp = (threadIdx.x >> 5) % PK_WARPS, lane = threadIdx.x & 31;
-  const bool shadow = PK_SHADOW && (int)threadIdx.x >= PK_WARPS * 32;
+  const float* __restrict__ verts = reinterpret_cast<const float*>(gblob + 1);   // SoA [nb][3][vmax] behind the header, read-only
+  float* scratch_all = reinterpret_cast<float*>(smem + sizeof(DevBlob));
+  const int warp = (threadIdx.x >> 5) % PK_WARPS_K, lane = threadIdx.x & 31;
+  const bool shadow = PK_SHADOW && (int)threadIdx.x >= PK_WARPS_K * 32;
   float* scr = scratch_all + warp * PK_SCRATCH;   // prologue / epilogue scratch of the fused form; the split form has none
-  float* wrec = scratch_all + (SPLIT ? 0 : PK_WARPS * PK_SCRATCH) + (size_t)warp * EPW * ENV_STRIDE;
+  float* wrec = scratch_all + (SPLIT ? 0 : PK_WARPS_K * PK_SCRATCH) + (size_t)warp * EPW * ENV_STRIDE;
   __shared__ b200_cfg_t s_cfg;  // constants in shared memory: no global (long-scoreboard) reloads inside the substep loop
   for (int k = threadIdx.x; k < (int)(sizeof(b200_cfg_t) / 4); k += blockDim.x) reinterpret_cast<uint32_t*>(&s_cfg)[k] = reinterpret_cast<const uint32_t*>(gcfg)[k];
   __syncthreads();
@@ -1084,9 +1091,9 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #ifndef PK_GROUPS
 #define PK_GROUPS 1   // 2 measured 1.5 % slower (343 vs 338 us): mixing the phases costs more I-cache than it hides latency
 #endif
-  constexpr int G0 = PK_GROUPS == 1 ? PK_WARPS : (PK_WARPS + 1) / 2;       // warps in group 0
+  constexpr int G0 = PK_GROUPS == 1 ? PK_WARPS_K : (PK_WARPS_K + 1) / 2;   // warps in group 0
   const int grp = warp < G0 ? 0 : 1;
-  const int gw0 = grp == 0 ? 0 : G0, gwn = grp == 0 ? G0 : PK_WARPS - G0;     // first warp / number of warps of my group
+  const int gw0 = grp == 0 ? 0 : G0, gwn = grp == 0 ? G0 : PK_WARPS_K - G0;   // first warp / number of warps of my group
   const int BATCH = gwn * EPW;
   const int gthreads = gwn * 32 * (PK_SHADOW ? 2 : 1);
   auto group_sync = [&]() { asm volatile("bar.sync %0, %1;" ::"r"(grp + 1), "r"(gthreads) : "memory"); };
@@ -1454,7 +1461,7 @@ __global__ void sort_perm_kernel(int num_envs, const int32_t* __restrict__ bin, 
 // ------------------------------------------------------------------------------------------
 #if B200ENV_WITH_PACKED3
 // packed3 form of the middle launch (pre_kernel -> this -> post_kernel): 2 envs per warp, 14 warps per CTA (csrc/packed3.cuh).
-// Same shared-memory footprint and the same 28 envs per CTA batch as step_kernel_packed<split>; twice the warps.
+// 28 envs per CTA batch, the batch step_kernel_packed<split> had at 7 warps; twice the warps.
 #ifndef PK3_WARPS
 #define PK3_WARPS 14
 #endif
@@ -2173,10 +2180,18 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
   if (!h->bound || (!h->has_ml && h->cfg.task_mode == 0)) return fail(-4, "b200env_step: bind buffers and a motion lib first%s");
   cudaSetDevice(h->device);
   if (h->packed) {
+    // step_kernel_packed stages the DevBlob header only (its vertices stay in global memory); the other forms stage the whole blob
     const size_t psmem = h->tmem ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float)
-                                 : ((h->blob_bytes + 15) & ~(size_t)15) + (h->split ? 0 : PK_WARPS * PK_SCRATCH * sizeof(float)) +
-                                       (size_t)PK_WARPS * EPW * ENV_STRIDE * sizeof(float);
-    const int batch = (h->tmem ? PT_WARPS : PK_WARPS) * EPW;
+#if B200ENV_WITH_PACKED3
+                         : h->packed3 ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PK3_WARPS * EPW3 * ENV_STRIDE * sizeof(float)
+#endif
+                                 : sizeof(DevBlob) + (h->split ? 0 : PK_WARPS_FUSED * PK_SCRATCH * sizeof(float)) +
+                                       (size_t)pk_warps(h->split) * EPW * ENV_STRIDE * sizeof(float);
+    const int batch = h->tmem ? PT_WARPS * EPW :
+#if B200ENV_WITH_PACKED3
+                      h->packed3 ? PK3_WARPS * EPW3 :
+#endif
+                      pk_warps(h->split) * EPW;
     const int need = (h->num_envs + batch - 1) / batch;
     if (h->step_grid == 0) {
       if (!h->tmem) {
@@ -2195,8 +2210,8 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed3, PK3_WARPS * 32, psmem));
       } else
 #endif
-      if (h->split) { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true>, PK_LAUNCH_WARPS * 32, psmem)); }
-      else { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<false>, PK_LAUNCH_WARPS * 32, psmem)); }
+      if (h->split) { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true>, pk_launch_warps(true) * 32, psmem)); }
+      else { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<false>, pk_launch_warps(false) * 32, psmem)); }
       CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
       h->step_grid = per_sm * sms < need ? per_sm * sms : need;
       if (h->step_grid < 1) return fail(-5, "b200env_step: step_kernel_packed does not fit on this device%s");
@@ -2237,7 +2252,7 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
       else
 #endif
-        step_kernel_packed<true><<<h->step_grid, PK_LAUNCH_WARPS * 32, psmem, (cudaStream_t)stream>>>(
+        step_kernel_packed<true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first,
             h->env_stride, h->d_ext, h->sort ? h->d_perm : nullptr);
       if (tv0) { cudaEventRecord(tv1, (cudaStream_t)stream); h->tev->push_back(tv0); h->tev->push_back(tv1); }
@@ -2248,7 +2263,7 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
       h->launches += h->cfg.task_mode == 0 ? 3 : 2;
       return 0;
     }
-    step_kernel_packed<false><<<h->step_grid, PK_LAUNCH_WARPS * 32, psmem, (cudaStream_t)stream>>>(
+    step_kernel_packed<false><<<h->step_grid, pk_launch_warps(false) * 32, psmem, (cudaStream_t)stream>>>(
         (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first,
         h->env_stride, nullptr, nullptr);
     CUDA_OK(cudaGetLastError());

@@ -16,7 +16,10 @@
 #define PK_SYNC_EVERY 1   // CTA barrier every n-th substep (keeps the CTA's warps on the same instruction-cache lines)
 #endif
 #ifndef PK_WARPS
-#define PK_WARPS 7          // 7 warps x 4 envs x 7.2 KB records + 20 KB constants = 227 KB of shared memory: one CTA per SM
+#define PK_WARPS 8          // split form: 8 warps x 4 envs x 6.7 KB records + the 7.1 KB DevBlob header = 221 KB of shared memory: one CTA per SM
+#endif
+#ifndef PK_WARPS_FUSED
+#define PK_WARPS_FUSED 7    // fused form: its 0.9 KB of prologue scratch per warp leaves room for 7 warps only
 #endif
 #ifndef PK_SHADOW
 #define PK_SHADOW 0         // experiment (b200env.cu): twice the warps, the second half running store-less copies of the first
@@ -29,17 +32,23 @@
 // read / written together form runs that start on 4-float boundaries, so that a run moves with LDS.128 / STS.128 instead of one
 // 32-bit access per float (ncu r1g: 21 M of the 97 M warp instructions of a launch were scalar LDS / STS).  Body b lives in
 // record B.t.rix[b] = its rank in breadth-first order: the bodies of one tree depth are handled by neighbouring lanes at the
-// same time, and consecutive records are 18 float4 apart -> different bank groups for the 8 lanes of a quarter-warp phase
+// same time, and consecutive records are 17 float4 apart -> 8 different bank groups for the 8 lanes of a quarter-warp phase
 // (the SMPL numbering itself puts siblings 4 bodies apart = the same bank group).
+// 68 floats hold everything the substep has live at once (71 at peak, minus the PD target, which a lane keeps in registers
+// through the control step - pk_pd_take - and no padding): 32 envs of records fit next to the constant block, so one CTA of
+// 8 warps carries 32 envs per SM.
 enum {
   R_Q = 0, R_P = 4, R_W = 7, R_V = 10, R_WT = 13,          // [0,16)  world pose / velocity of the body origin, joint velocity
-  R_QJ = 16, R_PD = 20, R_CFX = 23,                        // [16,24) joint rotation, PD target, contact force x
-  R_R = 24, R_ZETA = 27, R_U = 33,                         // [24,36) p - p_parent, velocity-product terms, joint-space bias
-  R_A = 36, R_BM = 42, R_C = 51, R_BN = 57, R_BF = 60, R_PAD = 63,  // [36,64) articulated inertia + bias (27 contiguous + 1 pad)
-  R_E = 64,                                                // [64,70) E_w, then D^-1
-  R_CFY = 70, R_CFZ = 71, REC = 72
+  R_QJ = 16,                                               // [16,20) joint rotation
+  R_R = 20, R_ZETA = 23, R_U = 29,                         // [20,32) p - p_parent, velocity-product terms, joint-space bias
+  R_A = 32, R_BM = 38, R_C = 47, R_BN = 53, R_BF = 56,     // [32,59) articulated inertia + bias (27 contiguous)
+  R_CFX = 59,                                              // contact force x
+  R_E = 60,                                                // [60,66) E_w, then D^-1
+  R_CFY = 66, R_CFZ = 67, REC = 68
 };
-#define R_ACC 56   // (alpha, a) of the body after the backward pass: aliases C[5], bn, bf[0..1] (dead by then); v4 + v2
+#define R_AB 27    // length of the run A[6] Bm[9] C[6] bn[3] bf[3] at R_A
+#define R_PD R_U   // between control steps a body's PD target is parked in its U slot (dead there; pk_pd_take / pk_pd_park)
+#define R_ACC 52   // (alpha, a) of the body after the backward pass: aliases C[5], bn, bf[0..1] (dead by then); v4 + v2
 #define B200_MAX_BODIES_PK 25
 #define ENV_EXT (B200_MAX_BODIES_PK * REC)  // per-env extras: extF[3] extT[3] reactF[3] reactX[3]
 #define ENV_STRIDE (ENV_EXT + 12)
@@ -78,7 +87,7 @@ template <int OFF, int N, int K> __device__ __forceinline__ void str_f(float* re
 }
 template <int OFF, int N> __device__ __forceinline__ void ldr(const float* rec, float* r) { ldr_f<OFF, N, 0>(rec, r); }
 #if defined(PK_SHADOW) && PK_SHADOW && defined(__CUDA_ARCH__)
-#define PK_IS_SHADOW ((int)threadIdx.x >= PK_WARPS * 32)
+#define PK_IS_SHADOW ((int)threadIdx.x >= (int)blockDim.x / 2)
 #else
 #define PK_IS_SHADOW false
 #endif
@@ -90,6 +99,48 @@ template <int OFF, int N> __device__ __forceinline__ void ldr(const double* rec,
 template <int OFF, int N> __device__ __forceinline__ void str(double* rec, const double* r) {
 #pragma unroll
   for (int k = 0; k < N; k++) rec[OFF + k] = r[k];
+}
+
+// PD targets.  pk_store_state parks a body's target in the U slot of its record (R_PD), which the substep does not use between
+// control steps.  At the start of a control step each lane takes the targets of the bodies it runs in the body pass
+// (b = rr * LPE + s) into registers, pd[rr % 3]: with LPE = 8 and at most 25 bodies, rr = 3 only occurs for b = 24 on slot 0, whose
+// rr = 0 body is the root (no target).  At the end it parks them again (U is dead once the last forward pass has read it), so that
+// the records hold them for the next control step of a multi-step launch.
+#define PK_PD_SLOTS 3
+static_assert(B200_MAX_BODIES_PK <= PK_PD_SLOTS * SLOTS + 1, "pd[rr % 3] needs at most 3 body-pass rounds per lane besides the root");
+// the target of the body of round rr (selects, not an indexed access: pd stays in registers)
+template <typename T> __device__ __forceinline__ void pk_pd_pick(const T (&pd)[PK_PD_SLOTS][3], int rr, T* out) {
+#pragma unroll
+  for (int k = 0; k < 3; k++) out[k] = rr == 1 ? pd[1][k] : (rr == 2 ? pd[2][k] : pd[0][k]);
+}
+template <typename T, int LPE = SLOTS>
+__device__ __forceinline__ void pk_pd_take(const DevBlob& B, const T* env, int s, bool valid, T (&pd)[PK_PD_SLOTS][3]) {
+  const b200_model_t& M = B.m;
+#pragma unroll
+  for (int i = 0; i < PK_PD_SLOTS; i++) pd[i][0] = pd[i][1] = pd[i][2] = T(0);
+  for (int rr = 0; rr * LPE < M.nb; rr++) {
+    const int b = rr * LPE + s;
+    if (!valid || b == 0 || b >= M.nb || M.fixed[b]) continue;
+    T t[3];
+    ldr<R_PD, 3>(env + RIX(B, b) * REC, t);
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+      if (rr == 1) pd[1][k] = t[k];
+      else if (rr == 2) pd[2][k] = t[k];
+      else pd[0][k] = t[k];
+    }
+  }
+}
+template <typename T, int LPE = SLOTS>
+__device__ __forceinline__ void pk_pd_park(const DevBlob& B, T* env, int s, bool valid, const T (&pd)[PK_PD_SLOTS][3]) {
+  const b200_model_t& M = B.m;
+  for (int rr = 0; rr * LPE < M.nb; rr++) {
+    const int b = rr * LPE + s;
+    if (!valid || b == 0 || b >= M.nb || M.fixed[b]) continue;
+    T t[3];
+    pk_pd_pick<T>(pd, rr, t);
+    str<R_PD, 3>(env + RIX(B, b) * REC, t);
+  }
 }
 
 // kinematics of one body from its parent's record.  JOINT_IN_REGS: the caller (forward pass) just produced the body's joint
@@ -152,19 +203,20 @@ template <> __device__ __forceinline__ double pk_bits_to_slot<double>(uint32_t x
 __device__ __forceinline__ uint32_t pk_slot_to_bits(float f) { uint32_t x; memcpy(&x, &f, 4); return x; }
 __device__ __forceinline__ uint32_t pk_slot_to_bits(double d) { return (uint32_t)d; }
 
+// pd: the body's PD target (from the lane's registers, pk_pd_pick)
 template <typename T, bool DEFER_CONTACT = false>
-__device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c, T* env, int b, bool ext_on) {
+__device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c, T* env, int b, bool ext_on,
+                                        const T* pd) {
   const b200_model_t& M = B.m;
   T* rec = env + RIX(B, b) * REC;
   T own[16], R[9];   // Q[4] p[3] w[3] v[3] wt[3]
   ldr<R_Q, 16>(rec, own);
   const T *Q = own, *p = own + 4, *w = own + 7, *v = own + 10;
   qmat(Q, R);
-  T ab[28];          // A[6] Bm[9] C[6] bn[3] bf[3] pad: one run of the record
+  T ab[R_AB];        // A[6] Bm[9] C[6] bn[3] bf[3]: one run of the record
   T *A = ab, *Bm = ab + 6, *C = ab + 15, *bn = ab + 21, *bf = ab + 24, cf[3] = {0, 0, 0};
 #pragma unroll
   for (int k = 6; k < 21; k++) ab[k] = T(0);
-  ab[27] = T(0);
   const T ms = T(M.mass[b]);
   T cl[3] = {T(M.com[b][0]), T(M.com[b][1]), T(M.com[b][2])}, cw[3];
   mv3(R, cl, cw);
@@ -221,14 +273,14 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
   } else if (nv > 0 && p[2] - T(M.radius[b]) < T(0)) {
     contact_hull<T>(verts + (size_t)b * M.vmax * 3, M.vmax, nv, c, R, p, v, w, A, Bm, C, bn, bf, cf);
   }
-  str<R_A, 28>(rec, ab);
+  str<R_A, R_AB>(rec, ab);
   if (!PK_IS_SHADOW) rec[R_CFX] = cf[0];
   str<R_CFY, 2>(rec, cf + 1);
   if (b > 0) {
     const int d0 = M.dof_of_body[b];
-    T jp[8], q[3], tau[3], e[3], u[3], E[6];   // qj[4] pd[3] (cf x)
-    ldr<R_QJ, 8>(rec, jp);
-    const T *qj = jp, *pd = jp + 4, *wt = own + 13;
+    T qj[4], q[3], tau[3], e[3], u[3], E[6];
+    ldr<R_QJ, 4>(rec, qj);
+    const T* wt = own + 13;
     qlog(qj, q);
 #pragma unroll
     for (int k = 0; k < 3; k++) {
@@ -254,8 +306,8 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
 template <typename T>
 __device__ __forceinline__ void pk_backward(const DevBlob& B, T* env, int b, T* out) {
   T* rec = env + RIX(B, b) * REC;
-  T ab[28], rzu[12], E[6];   // A[6] Bm[9] C[6] bn[3] bf[3] pad | r[3] zeta[6] u[3]
-  ldr<R_A, 28>(rec, ab); ldr<R_R, 12>(rec, rzu); ldr<R_E, 6>(rec, E);
+  T ab[R_AB], rzu[12], E[6];   // A[6] Bm[9] C[6] bn[3] bf[3] | r[3] zeta[6] u[3]
+  ldr<R_A, R_AB>(rec, ab); ldr<R_R, 12>(rec, rzu); ldr<R_E, 6>(rec, E);
   const T *A = ab, *Bm = ab + 6, *C = ab + 15, *bn = ab + 21, *bf = ab + 24, *r = rzu, *zeta = rzu + 3;
   T u[3] = {rzu[9], rzu[10], rzu[11]};
   T D[6], Dinv[6];
@@ -335,13 +387,12 @@ __device__ __forceinline__ void pk_backward(const DevBlob& B, T* env, int b, T* 
   cross3(r, af, rxf);
 #pragma unroll
   for (int k = 0; k < 3; k++) { out[21 + k] = an[k] + rxf[k]; out[24 + k] = af[k]; }
-  out[27] = T(0);
 }
 
 template <typename T> __device__ __forceinline__ void pk_root(const PhysCfg<T>& c, T* env) {
   T* rec = env;   // the root is record 0
-  T ab[28], acc[6];
-  ldr<R_A, 28>(rec, ab);
+  T ab[R_AB], acc[6];
+  ldr<R_A, R_AB>(rec, ab);
   const T *A = ab, *Bm = ab + 6, *C = ab + 15, *bn = ab + 21, *bf = ab + 24;
   T Ci[6], Cif[9], BC[9], S[6], Si[6], rhs[3], t[3];
   sym_inv(C, Ci);
@@ -464,14 +515,14 @@ __device__ __forceinline__ void pk_contact_phase(const DevBlob& B, const float* 
     if (idx < n) {
       const int b = pk_nth_set_bit(word, idx);        // = rr*8 + slot = the body index
       T* rec = env + RIX(B, b) * REC;
-      T own[13], R[9], ab[28], cf[3];
+      T own[13], R[9], ab[R_AB], cf[3];
       ldr<R_Q, 13>(rec, own);
-      ldr<R_A, 28>(rec, ab);
+      ldr<R_A, R_AB>(rec, ab);
       const unsigned long long mask = (unsigned long long)pk_slot_to_bits(rec[R_CFY]) | ((unsigned long long)pk_slot_to_bits(rec[R_CFZ]) << 32);
       cf[0] = rec[R_CFX]; cf[1] = T(0); cf[2] = T(0);
       qmat(own, R);
       contact_apply<T>(verts + (size_t)b * M.vmax * 3, M.vmax, mask, c, R, own + 4, own + 10, own + 7, ab, ab + 6, ab + 15, ab + 21, ab + 24, cf);
-      str<R_A, 28>(rec, ab);
+      str<R_A, R_AB>(rec, ab);
       if (!PK_IS_SHADOW) rec[R_CFX] = cf[0];
       str<R_CFY, 2>(rec, cf + 1);
     }
@@ -714,6 +765,8 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
   const int g = lane >> 3, s = lane & 7;
   T* env = wrec + g * ENV_STRIDE;
   const int nb = M.nb;
+  T pd[PK_PD_SLOTS][3];   // PD targets of my body-pass bodies
+  pk_pd_take<T>(B, env, s, valid, pd);
   // kinematics of the start state, root -> leaves; every later FK is fused into the forward pass of the substep before it
   for (int d = 1; d <= M.max_depth; d++) {
     const int b = valid ? B.t.lvl_all[d][s] : -1;
@@ -734,7 +787,11 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
       // 1. per-body inertia / bias / contacts / joint drive
       for (int rr = 0; rr * SLOTS < (ABL == 8 ? 0 : nb); rr++) {
         const int b = rr * SLOTS + s;
-        if (valid && b < nb && !M.fixed[b]) pk_body<T, PK_CONTACT_COMPACT != 0>(B, verts, c, env, b, sim == 0);
+        if (valid && b < nb && !M.fixed[b]) {
+          T pdb[3];
+          pk_pd_pick<T>(pd, rr, pdb);
+          pk_body<T, PK_CONTACT_COMPACT != 0>(B, verts, c, env, b, sim == 0, pdb);
+        }
       }
       __syncwarp();
 #if PK_CONTACT_COMPACT
@@ -744,17 +801,17 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
       // 2. articulated inertia, leaves -> root
       for (int d = (ABL == 9 ? 0 : M.max_depth); d >= 1; d--) {
         const int b = valid ? B.t.lvl_dyn[d][s] : -1;
-        T out[28];
+        T out[R_AB];
         if (b >= 0) pk_backward<T>(B, env, b, out);
         const int rounds = B.t.maxch[d - 1];
         for (int cr = 0; cr < rounds; cr++) {
           if (b >= 0 && B.t.child_rank[b] == cr) {
             T* pr = env + RIX(B, M.parent[b]) * REC;
-            T acc[28];
-            ldr<R_A, 28>(pr, acc);
+            T acc[R_AB];
+            ldr<R_A, R_AB>(pr, acc);
 #pragma unroll
-            for (int k = 0; k < 28; k++) acc[k] += out[k];
-            str<R_A, 28>(pr, acc);
+            for (int k = 0; k < R_AB; k++) acc[k] += out[k];
+            str<R_A, R_AB>(pr, acc);
           }
           __syncwarp();
         }
@@ -800,6 +857,7 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
       }
     }
   }
+  pk_pd_park<T>(B, env, s, valid, pd);
 }
 
 // state of one env between the lane-per-body prologue / epilogue (lane = body) and the records
@@ -815,12 +873,8 @@ template <typename T> __device__ __forceinline__ void pk_store_state(T* env, con
       for (int k = 0; k < 3; k++) { o[4 + k] = L.p[k]; o[7 + k] = L.w[k]; o[10 + k] = L.v[k]; }
       str<R_Q, 13>(rec, o);
     } else if (lc.dyn) {
-      T o[7];
-#pragma unroll
-      for (int k = 0; k < 4; k++) o[k] = L.qj[k];
-#pragma unroll
-      for (int k = 0; k < 3; k++) o[4 + k] = pd[k];
-      str<R_QJ, 7>(rec, o);
+      str<R_QJ, 4>(rec, L.qj);
+      str<R_PD, 3>(rec, pd);
       str<R_WT, 3>(rec, L.wt);
     }
   }

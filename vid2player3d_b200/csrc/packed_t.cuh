@@ -1,6 +1,6 @@
 // packed_t.cuh - the "one wave" form of the packed articulated step (included by b200env.cu after packed.cuh).
 //
-// Why: step_kernel_packed keeps a 72-float record per body in shared memory, 7.2 KB per env, so an SM holds 28 envs (7 warps); the
+// Why: step_kernel_packed keeps a 68-float record per body in shared memory, 6.7 KB per env, so an SM holds 32 envs (8 warps); the
 // launch is latency-bound on one warp's dependent instruction stream.  56 resident envs per SM (14 warps) need <= 3.7 KB per env of
 // shared memory, but the fields that lanes hand to each other are already 4.0 KB.  Here
 //   * every dynamic body has ONE owner lane for all passes (DevTree::pt_slot: the bodies of a tree depth sit in different slots of
