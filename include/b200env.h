@@ -203,8 +203,10 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
                                int32_t local_root_obs, int32_t root_height_obs, float* obs, void* obs_bf16, int32_t ld_bf16, const float* mean,
                                const float* rstd, float clamp, void* stream);
 
-/* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1):
- * the same device code as b200env_step's physics, exposed so tests can compare it with the
+/* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1): a separate test launch
+ * (physics_kernel_packed; physics_kernel_tmem / physics_kernel for the other forms) that shares the control step
+ * (control_step_packed) with b200env_step's physics launch, but not that launch's persistent hand-out of env batches,
+ * its state-row loads and stores or its shared-memory layout.  Exposed so tests can compare the control step with the
  * float64 CPU restatement (oracle/physics_ref.c).  root [n,13], dof_pos/dof_vel/pd_tar [n,nd],
  * ext_wrench [n,6] (force, torque on body 0, world frame, first sim step only),
  * rb_out [n,nb,13], contact_out [n,nb,3].  n_steps control steps are run back to back.
@@ -237,6 +239,12 @@ int b200env_set_hull_faces(b200env_handle h, const float* planes, const uint8_t*
  * two rounds for 8192 envs on 132 SMs), 2 packed3 (A/B builds only), 3 step_kernel_tmem (56 envs per SM, lane-private fields in thread-local memory).  Chosen at
  * b200env_create from the model's tree and the environment variable B200ENV_KERNEL (lane | packed | tmem; default: see DESIGN.md 5). */
 int32_t b200env_kernel_form(b200env_handle h);
+
+/* Shape of b200env_step's physics launch for this handle: *envs_per_batch = envs a CTA takes per ticket (32 for the split
+ * step_kernel_packed, 28 for the fused form, 56 for step_kernel_tmem, 8 for the lane-per-body kernel), *grid = resident CTA slots
+ * of the persistent launch (CTAs per SM x SMs).  A step of n envs runs min(*grid, ceil(n / *envs_per_batch)) CTAs, so batch b of
+ * the env order runs in round b / *grid.  Computed from the same expressions b200env_step uses; needs the device, not a bind. */
+int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int32_t* grid);
 
 /* number of kernels launched by this handle so far (bench.py "gpu_launches") */
 int64_t b200env_launch_count(b200env_handle h);

@@ -73,7 +73,8 @@ struct b200env {
   int tmem;                            // 1: the physics launch is step_kernel_tmem (56 envs per SM, private fields in thread-local memory; B200ENV_KERNEL=tmem)
   int split;                           // 1: three launches (pre / physics / post), 0: one fused launch.  env B200ENV_SPLIT=0|1
   int env_first = 0, env_stride = 1;   // b200env_set_env_slice: local env i = row env_first + env_stride * i of the bound tensors
-  int step_grid;
+  int step_slots;                      // resident CTA slots of the persistent physics launch (0 = not computed yet)
+  int step_grid;                       // CTAs of the physics launch: min(step_slots, batches of num_envs)
   int packed;        // 1: 4-envs-per-warp kernels (packed.cuh); 0: lane-per-body kernels.  env B200ENV_KERNEL=lane|packed
   int packed_ok;     // tree fits the packed layout (<= 8 bodies per depth, <= 25 bodies)
   int64_t launches;
@@ -2175,35 +2176,41 @@ int b200env_set_motion_lib(b200env_handle h, const b200_motion_lib_t* ml) {
 static int need_ctas(const b200env* h) { return (h->num_envs + WARPS_PER_CTA - 1) / WARPS_PER_CTA; }
 static size_t step_smem(const b200env* h) { return ((h->blob_bytes + 15) & ~(size_t)15) + WARPS_PER_CTA * SCRATCH_FLOATS * sizeof(float); }
 
-int b200env_step(b200env_handle h, const float* actions, void* stream) {
-  if (!h || !actions) return fail(-1, "b200env_step: null argument%s");
-  if (!h->bound || (!h->has_ml && h->cfg.task_mode == 0)) return fail(-4, "b200env_step: bind buffers and a motion lib first%s");
-  cudaSetDevice(h->device);
+// Shape of the physics launch of b200env_step: dynamic shared memory, envs per CTA batch and the persistent grid.  The grid's
+// resident CTA slots (per SM x SMs) are computed on the first call and kept; a launch of num_envs envs runs
+// min(slots, ceil(num_envs / batch)) CTAs (h->step_grid).
+static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out) {
+  size_t psmem;
+  int batch;
   if (h->packed) {
     // step_kernel_packed stages the DevBlob header only (its vertices stay in global memory); the other forms stage the whole blob
-    const size_t psmem = h->tmem ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float)
+    psmem = h->tmem ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float)
 #if B200ENV_WITH_PACKED3
-                         : h->packed3 ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PK3_WARPS * EPW3 * ENV_STRIDE * sizeof(float)
+            : h->packed3 ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PK3_WARPS * EPW3 * ENV_STRIDE * sizeof(float)
 #endif
-                                 : sizeof(DevBlob) + (h->split ? 0 : PK_WARPS_FUSED * PK_SCRATCH * sizeof(float)) +
-                                       (size_t)pk_warps(h->split) * EPW * ENV_STRIDE * sizeof(float);
-    const int batch = h->tmem ? PT_WARPS * EPW :
+                    : sizeof(DevBlob) + (h->split ? 0 : PK_WARPS_FUSED * PK_SCRATCH * sizeof(float)) +
+                          (size_t)pk_warps(h->split) * EPW * ENV_STRIDE * sizeof(float);
+    batch = h->tmem ? PT_WARPS * EPW :
 #if B200ENV_WITH_PACKED3
-                      h->packed3 ? PK3_WARPS * EPW3 :
+            h->packed3 ? PK3_WARPS * EPW3 :
 #endif
-                      pk_warps(h->split) * EPW;
-    const int need = (h->num_envs + batch - 1) / batch;
-    if (h->step_grid == 0) {
-      if (!h->tmem) {
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-      }
-      int per_sm = 0, sms = 0;
-      if (h->tmem) {
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_tmem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_tmem, PT_WARPS * 32, psmem));
-        if (per_sm > 1) per_sm = 1;   // one CTA per SM: its 56 envs take nearly all of the shared memory
-      } else
+            pk_warps(h->split) * EPW;
+  } else {
+    psmem = step_smem(h);
+    batch = WARPS_PER_CTA;
+  }
+  if (h->step_slots == 0) {
+    int per_sm = 0, sms = 0;
+    if (!h->packed) {
+      CUDA_OK(cudaFuncSetAttribute(step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, WARPS_PER_CTA * 32, psmem));
+    } else if (h->tmem) {
+      CUDA_OK(cudaFuncSetAttribute(step_kernel_tmem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_tmem, PT_WARPS * 32, psmem));
+      if (per_sm > 1) per_sm = 1;   // one CTA per SM: its 56 envs take nearly all of the shared memory
+    } else {
+      CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+      CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
 #if B200ENV_WITH_PACKED3
       if (h->packed3) {
         CUDA_OK(cudaFuncSetAttribute(step_kernel_packed3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
@@ -2212,10 +2219,40 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
 #endif
       if (h->split) { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true>, pk_launch_warps(true) * 32, psmem)); }
       else { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<false>, pk_launch_warps(false) * 32, psmem)); }
-      CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-      h->step_grid = per_sm * sms < need ? per_sm * sms : need;
-      if (h->step_grid < 1) return fail(-5, "b200env_step: step_kernel_packed does not fit on this device%s");
     }
+    CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    if (per_sm * sms < 1) return fail(-5, h->packed ? "b200env_step: step_kernel_packed does not fit on this device%s"
+                                                     : "b200env_step: step_kernel does not fit on this device%s");
+    h->step_slots = per_sm * sms;
+    const int need = (h->num_envs + batch - 1) / batch;
+    h->step_grid = h->step_slots < need ? h->step_slots : need;
+  }
+  *psmem_out = psmem;
+  *batch_out = batch;
+  return 0;
+}
+
+int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int32_t* grid) {
+  if (!h || !envs_per_batch || !grid) return fail(-1, "b200env_physics_launch_shape: null argument%s");
+  CUDA_OK(cudaSetDevice(h->device));
+  size_t psmem;
+  int batch;
+  const int rc = physics_launch_config(h, &psmem, &batch);
+  if (rc) return rc;
+  *envs_per_batch = batch;
+  *grid = h->step_slots;
+  return 0;
+}
+
+int b200env_step(b200env_handle h, const float* actions, void* stream) {
+  if (!h || !actions) return fail(-1, "b200env_step: null argument%s");
+  if (!h->bound || (!h->has_ml && h->cfg.task_mode == 0)) return fail(-4, "b200env_step: bind buffers and a motion lib first%s");
+  cudaSetDevice(h->device);
+  size_t psmem;
+  int batch;
+  const int rc = physics_launch_config(h, &psmem, &batch);
+  if (rc) return rc;
+  if (h->packed) {
     // the ticket counter is re-zeroed on the stream before every launch: nothing in the launch depends on host-side
     // history, so a step can be captured into a CUDA graph and replayed
     if (!h->split) CUDA_OK(cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned long long), (cudaStream_t)stream));   // split form: pre_kernel zeroes it
@@ -2270,18 +2307,8 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
     h->launches++;
     return 0;
   }
-  const size_t smem = step_smem(h);
-  if (h->step_grid == 0) {
-    CUDA_OK(cudaFuncSetAttribute(step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0, sms = 0;
-    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, WARPS_PER_CTA * 32, smem));
-    CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-    const int need = need_ctas(h);
-    h->step_grid = per_sm * sms < need ? per_sm * sms : need;
-    if (h->step_grid < 1) return fail(-5, "b200env_step: step_kernel does not fit on this device%s");
-  }
   CUDA_OK(cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned long long), (cudaStream_t)stream));
-  step_kernel<<<h->step_grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes,
+  step_kernel<<<h->step_grid, WARPS_PER_CTA * 32, psmem, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes,
                                                                                  h->d_cfg, h->bufs, h->ml, actions, h->num_envs,
                                                                                  h->d_ticket, h->env_first, h->env_stride);
   CUDA_OK(cudaGetLastError());

@@ -14,7 +14,8 @@ _lib = None
 SYMBOLS = ["b200env_abi_version", "b200env_last_error", "b200env_create", "b200env_destroy", "b200env_bind",
            "b200env_set_motion_lib", "b200env_step", "b200env_reset", "b200env_motion_state", "b200env_obs_imitation",
            "b200env_physics_only", "b200env_launch_count", "b200env_set_env_slice", "b200env_motion_context", "b200env_set_kernel_timing",
-           "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form"]
+           "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form",
+           "b200env_physics_launch_shape"]
 
 
 def lib():
@@ -171,6 +172,14 @@ class Env:
     def kernel_form(self):
         """'lane' | 'packed' | 'packed3' | 'tmem' (include/b200env.h: b200env_kernel_form)"""
         return ("lane", "packed", "packed3", "tmem")[int(lib().b200env_kernel_form(self._h))]
+
+    @property
+    def physics_launch_shape(self):
+        """(envs per CTA batch, resident CTA slots of the persistent grid) of the step's physics launch (include/b200env.h:
+        b200env_physics_launch_shape); a step of n envs runs batch b in round b // grid"""
+        b, g = C.c_int32(0), C.c_int32(0)
+        _check(lib().b200env_physics_launch_shape(self._h, C.byref(b), C.byref(g)))
+        return b.value, g.value
 
     @property
     def launch_count(self):
