@@ -503,7 +503,10 @@ __device__ __forceinline__ void ref_exp_map_to_quat(const float* e, float* q) { 
   q[0] /= qn; q[1] /= qn; q[2] /= qn; q[3] /= qn;
 }
 __device__ __forceinline__ void ref_slerp(const float* q0, const float* q1in, float t, float* o) {  // :168-190
-  float c = q0[0] * q1in[0] + q0[1] * q1in[1] + q0[2] * q1in[2] + q0[3] * q1in[3];
+  // sum(q0 * q1) as the reference rounds it: products first, added left to right, no fma.  Near c = 1 the weights below divide by
+  // sqrt(1 - c c), so one ulp of c moves the slerp by up to ~1e-5 (sin(half) = 0.047 already gives 1.2e-5).
+  float c = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(q0[0], q1in[0]), __fmul_rn(q0[1], q1in[1])), __fmul_rn(q0[2], q1in[2])),
+                      __fmul_rn(q0[3], q1in[3]));
   float sg = c < 0.f ? -1.f : 1.f;
   float q1[4] = {sg * q1in[0], sg * q1in[1], sg * q1in[2], sg * q1in[3]};
   c = fabsf(c);
