@@ -61,7 +61,8 @@ typedef struct b200v2p_ctrl {
       max_episode_length, est_nx, est_ny;
   int32_t obs_only; /* 1: refresh obs_buf only (the _compute_observations call of _reset_envs :200-201), touch nothing else */
   int32_t dual;     /* 1: reset FSM of PhysicsMVAEControllerDual._compute_reset (env/tasks/physics_mvae_controller_dual.py:92-120):
-                       envs (2k, 2k+1) are opponents; reset_buf is only ever SET, terminate_buf is not written */
+                       envs (2k, 2k+1) are opponents, so n must be even; reset_buf is only ever SET, terminate_buf is not written.
+                       num_obs must equal 225 + 3 * obs_traj_len (+ 2 with use_target): the NaN test sees exactly these columns */
   int32_t use_history; /* cfg use_history_ball_obs (:348-351): the task observation is the HISTORY of ball positions (ball_obs)
                           instead of the future trajectory window (ball_traj) */
   int32_t advance;     /* 1 (ignored with obs_only): first do the tail of physics_step and the head of post_physics_step (:364-366,

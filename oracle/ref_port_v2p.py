@@ -257,6 +257,17 @@ def in_court(p):
     return (p[:, 0] > COURT_MIN[0]) & (p[:, 0] < COURT_MAX[0]) & (p[:, 1] > COURT_MIN[1]) & (p[:, 1] < COURT_MAX[1])
 
 
+def est_round(v):
+    """torch.round: half to even"""
+    return np.round(v)
+
+
+def net_crossing_x(b):
+    """x where the outgoing ball crosses the net (utils/tennis_ball_out_estimator.py:172): tensor ops, every product rounded"""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return b[:, 0] + b[:, 7] * np.abs(b[:, 1] / b[:, 8])
+
+
 def estimator_estimate(ball_states, est_x, est_y, params):
     """TennisBallOutEstimator.estimate (utils/tennis_ball_out_estimator.py:164-205) with index math :126-162.
     params rows: VEL_X, VEL_Y, VSPIN, TRAJ_X, TRAJ_Y ranges (lo, hi, step).  Returns per-row
@@ -265,8 +276,7 @@ def estimator_estimate(ball_states, est_x, est_y, params):
     VX, VY, VS, TX, TY = [tuple(float(v) for v in r) for r in params]
     b = ball_states
     valid = (b[:, 8] > VX[0]) & (b[:, 9] > VY[0]) & (b[:, 9] < VY[1]) & (b[:, 2] < TY[1])
-    with np.errstate(divide="ignore", invalid="ignore"):
-        x_net = b[:, 0] + b[:, 7] * np.abs(b[:, 1] / b[:, 8])
+    x_net = net_crossing_x(b)
     valid &= (x_net > -4) & (x_net < 4)
     n = len(b)
     bounce_pos, bounce_time, max_h = np.zeros((n, 2), b.dtype), np.zeros(n, b.dtype), np.zeros(n, b.dtype)
@@ -278,7 +288,7 @@ def estimator_estimate(ball_states, est_x, est_y, params):
 
         def idx(v, rng):
             v = np.clip(v, f(rng[0]), f(rng[1] - rng[2]))
-            return np.round((v - f(rng[0])) / f(rng[2]))
+            return est_round((v - f(rng[0])) / f(rng[2]))
         dim = ((VX[1] - VX[0]) / VX[2], (VY[1] - VY[0]) / VY[2], (VS[1] - VS[0]) / VS[2])
         ti = (idx(vel_x, VX) * f(dim[1]) * f(dim[2]) + idx(vel_y, VY) * f(dim[2]) + idx(vspin, VS)).astype(np.int64)
         tx, ty = est_x[ti], est_y[ti]
@@ -320,6 +330,245 @@ def controller_reset(root_pos, court_min, court_max, obs_has_nan, progress, max_
     recovery = recovery & ~terminate
     reaction = reaction | reset.astype(bool)
     return reset, terminate_buf, reaction, recovery
+
+
+# --------------------------------------------------------------------------- a14-a16 as one step (b200v2p_controller_post)
+REWARD_NAMES = ("reach", "return", "return_w_estimate")
+
+
+def advance_counters(s):
+    """tail of physics_step (:364-366) + head of post_physics_step (:441-442): the trajectory window rolls by one frame with a zero
+    last frame, the reaction timer and the episode progress count one step"""
+    tr = s["ball_traj"]
+    s["ball_traj"] = np.concatenate([tr[:, 1:], np.zeros_like(tr[:, :1])], 1)
+    s["tar_time"] = s["tar_time"] + 1
+    s["progress"] = s["progress"] + 1
+
+
+def history_rows(s, cfg):
+    """rows whose ball history _compute_task_obs rolls (:345-346): every row in a step; in an observation refresh (_reset_envs
+    :200-201, dual :64-66) the rows being reset"""
+    if not cfg.get("obs_only"):
+        return np.ones(len(s["root_pos"]), bool)
+    return s["reset_reaction"] | (s["reset_recovery"] & (not cfg.get("dual")))
+
+
+def controller_post(s, cfg):
+    """One b200v2p_controller_post launch on the numpy state `s` (dict of per-env arrays, returned updated in a copy):
+    post_physics_step (:440-452) = [advance] -> _update_state (:271-314) -> _compute_reward (:368-406) -> _compute_observations
+    (:316-360, ball history rolled) -> _compute_reset (:408-436), or the dual FSM (physics_mvae_controller_dual.py:92-120).
+    cfg keys: obs_traj_len, use_target, reward_type (REWARD_NAMES), early_termination, max_len, court_min, court_max, scales, weights,
+    est (est_x, est_y, params) or None, and the launch flags advance / obs_only / dual / use_history.  obs_only: the observation refresh
+    of _reset_envs; with s["touch_mask"] (the humanoids just reset) the rows neither in it nor flagged for a task reset are not
+    touched and the task flags of the rows in it are cleared afterwards (:176-177)."""
+    s = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in s.items()}
+    n = len(s["root_pos"])
+    f = np.float32
+    obs_only, dual, L = bool(cfg.get("obs_only")), bool(cfg.get("dual")), int(cfg["obs_traj_len"])
+    touch = s.get("touch_mask")
+    rows = np.ones(n, bool)
+    if obs_only and touch is not None:
+        rows = touch | s["reset_reaction"] | s["reset_recovery"]
+    if cfg.get("advance") and not obs_only:
+        advance_counters(s)
+    if not obs_only:
+        upd = (s["tar_action"] == 0) & s["has_bounce_now"]
+        s["bounce_in"] = np.where(upd, in_court(s["bounce_pos"]), s["bounce_in"])
+        est = cfg.get("est")
+        if est is not None and s["has_contact_now"].any():
+            ids = np.flatnonzero(s["has_contact_now"])
+            valid, bp, bt, mh = estimator_estimate(s["ball_states"][ids, :13], est[0], est[1], est[2])
+            ids = ids[valid]
+            s["est_bounce_pos"][ids, :2] = bp[valid]
+            s["est_bounce_time"][ids] = bt[valid]
+            s["est_max_height"][ids] = mh[valid]
+            s["est_bounce_in"][ids] = in_court(s["est_bounce_pos"][ids])
+        rt, sc, w = cfg["reward_type"], cfg["scales"], cfg["weights"]
+        if rt == "reach":
+            rew, sub = reward_reach(s["phase"], s["tar_action"], s["racket_pos"], s["ball_pos"], s["swing_type"], sc, w)
+            sub = np.concatenate([sub, np.zeros_like(sub)], 1)
+        elif rt == "return":
+            rew, sub = reward_return(s["phase"], s["racket_pos"], s["ball_pos"], s["has_contact"], s["has_bounce"], s["bounce_pos"],
+                                     s["target_bounce_pos"], s["swing_type"], sc, w)
+        else:
+            rew, sub = reward_return_w_estimate(s["racket_pos"], s["phase"], s["swing_type_cycle"], s["ball_pos"], s["has_contact"],
+                                                s["est_bounce_pos"], s["est_bounce_time"], s["est_bounce_in"], s["target_bounce_pos"], sc, w)
+        s["rew"], s["sub"] = rew.astype(f), sub.astype(f)
+    roll = history_rows(s, cfg) & rows
+    if s.get("ball_obs") is not None and L > 0:
+        s["ball_obs"] = roll_ball_obs(s["ball_obs"], s["ball_pos"], np.flatnonzero(roll))
+    r = np.flatnonzero(rows)
+    if len(r):
+        hist = s["ball_obs"][r] if cfg.get("use_history") else None
+        s["obs"][r] = controller_obs(s["rbs"][r, :25], s["root_pos"][r], s["root_vel"][r], s["racket_normal"][r], s["ball_traj"][r],
+                                     s["target_bounce_pos"][r], L, bool(cfg["use_target"]), hist)
+    if not obs_only:
+        has_nan = np.isnan(s["obs"]).any(1)
+        if dual:
+            s["reset"], rea, rec, s["distance"] = dual_controller_reset(s["tar_action"], s["has_contact"], s["has_bounce"], s["ball_pos"],
+                                                                        s["root_pos"], s["root_vel"], s["bounce_in"], s["distance"],
+                                                                        s["reset"])
+        else:
+            s["distance"] = (s["distance"] + np.sqrt((s["root_vel"][:, :2] ** 2).sum(-1))).astype(f)
+            s["reset"], s["terminate"], rea, rec = controller_reset(
+                s["root_pos"], np.asarray(cfg["court_min"], f), np.asarray(cfg["court_max"], f), has_nan, s["progress"], cfg["max_len"],
+                s["tar_time"], s["tar_time_total"], s["tar_action"], s["has_contact"], s["ball_pos"], s["est_bounce_in"],
+                bool(cfg["early_termination"]), rt == "return_w_estimate")
+        s["reset_reaction"], s["reset_recovery"] = rea.astype(bool), rec.astype(bool)
+    elif touch is not None:
+        s["reset_reaction"] = s["reset_reaction"] & ~touch
+        s["reset_recovery"] = s["reset_recovery"] & ~touch
+    return s
+
+
+# --------------------------------------------------------------------------- task resets (b200v2p_task_reset)
+def pool_index(ball_pos, pool_rand, side_rand, pool_size):
+    """TennisBallGeneratorOffline.generate with start_pos (utils/tennis_ball.py:436-444): a ball coming back from the other side
+    (y > 0) is drawn near its x: ((x + 4) / 8 * P) truncated, + side_rand, clamped to the pool; otherwise pool_rand"""
+    f = np.float32
+    x = ball_pos[:, 0].astype(f)
+    near = (((x + f(4)) / f(8) * f(pool_size)).astype(np.int64) + side_rand).clip(0, pool_size - 1)
+    return np.where(ball_pos[:, 1] > 0, near, pool_rand)
+
+
+def task_reset(s, cfg, draws):
+    """_reset_envs (:173-201) task part for the reset masks in s: _reset_balls (:503-524) of the reaction envs, _reset_recovery_tasks
+    (:242-245), _reset_reaction_tasks (:203-240).  draws: pool_rand, side_rand, frame_rand, target_seed (3 floats: continuous, n: discrete).
+    s["rbs"] ball row = the last body of each env.  Returns an updated copy."""
+    s = {k: (v.copy() if isinstance(v, np.ndarray) else v) for k, v in s.items()}
+    f = np.float32
+    rea, rec = np.flatnonzero(s["reset_reaction"]), np.flatnonzero(s["reset_recovery"])
+    if len(rea):
+        pool = cfg["pool"]
+        idx = pool_index(s["ball_pos"][rea], draws["pool_rand"][rea], draws["side_rand"][rea], len(pool))
+        traj, pos, vel, w = ball_reset(pool, idx)
+        if s.get("ball_obs") is not None:
+            s["ball_obs"][rea] = pos[:, None, :]
+        else:
+            s["ball_traj"][rea] = traj
+        for key in ("ball_states", "rbs_ball"):
+            s[key][rea, 0:3], s[key][rea, 7:10], s[key][rea, 10:13] = pos, vel, w
+        s["ball_pos"][rea], s["ball_vel"][rea], s["bounce_pos"][rea] = pos, vel, 0
+        s["has_bounce"][rea], s["has_contact"][rea] = False, False
+    s["tar_action"][rec] = 0
+    s["has_bounce"][rec] = False
+    s["bounce_pos"][rec] = 0
+    if len(rea):
+        s["tar_time"][rea] = 0
+        s["tar_action"][rea] = 1
+        s["num_reset_reaction"][rea] += 1
+        s["bounce_in"][rea], s["est_bounce_in"][rea] = False, False
+        s["est_bounce_pos"][rea], s["est_bounce_time"][rea], s["est_max_height"][rea] = 0, 0, 0
+        s["swing_type_cycle"][rea] = -1
+        s["tar_time_total"][rea] = cfg["reaction_nframes"] + draws["frame_rand"][rea]
+        seed = np.asarray(draws["target_seed"], f)
+        tmin, tmax = np.asarray(cfg["target_min"], f), np.asarray(cfg["target_max"], f)
+        if cfg["target_mode"] == "continuous":
+            s["target_bounce_pos"][rea] = seed * (tmax - tmin) + tmin
+        elif cfg["target_mode"] == "discrete":
+            sd = seed[rea]
+            s["target_bounce_pos"][rea, 0] = np.where(sd < f(0.33), f(-3), np.where(sd > f(0.67), f(3), f(0)))
+            s["target_bounce_pos"][rea, 1:] = (10, 0)
+    return s
+
+
+def quat_rotate(q, v):
+    """isaacgym.torch_utils.quat_rotate (xyzw): v (2w^2 - 1) + 2 w (q x v) + 2 q (q . v)"""
+    f = q.dtype.type
+    w, u = q[..., 3:4], q[..., :3]
+    return v * (f(2) * w * w - f(1)) + np.cross(u, v) * w * f(2) + u * (u * v).sum(-1, keepdims=True) * f(2)
+
+
+def actor_reset(s, src, ids, cfg):
+    """HumanoidSMPLIMMVAE._reset_actors + _set_env_state (humanoid_smpl_im_mvae.py:463-501) + the humanoid part of _reset_env_tensors
+    (:562-581) for the env ids: the FK pose src (root_pos, root_rot, dof_pos, rb_pos [N,24,3], rb_rot [N,24,4], velocities zero) is
+    written into the sim state.  The welded racket row (cfg racket_body >= 0) is not in the reference, which gets it from the simulator's
+    forward kinematics: here it is the parent body's pose with the racket offset rotated by the parent (quat_rotate); in dual mode odd
+    envs use the second player's parent and offset."""
+    s = {k: v.copy() for k, v in s.items()}
+    ids = np.asarray(ids)
+    rbs, nd = s["rbs"], s["dof_state"].shape[1]
+    rbs[ids, :24, 0:3], rbs[ids, :24, 3:7], rbs[ids, :24, 7:13] = src["rb_pos"][ids], src["rb_rot"][ids], 0
+    s["prev_target_rb_rot"][ids] = src["rb_rot"][ids]
+    if cfg["racket_body"] >= 0:
+        second = (ids % 2 == 1) & bool(cfg.get("dual"))
+        par = np.where(second, cfg.get("racket_parent2", cfg["racket_parent"]), cfg["racket_parent"])
+        off = np.where(second[:, None], np.asarray(cfg.get("racket_offset2", cfg["racket_offset"]), np.float32),
+                       np.asarray(cfg["racket_offset"], np.float32)).astype(np.float32)
+        q = src["rb_rot"][ids, par]
+        rbs[ids, cfg["racket_body"], 0:3] = src["rb_pos"][ids, par] + quat_rotate(q, off)
+        rbs[ids, cfg["racket_body"], 3:7], rbs[ids, cfg["racket_body"], 7:13] = q, 0
+    s["dof_state"][ids, :, 0], s["dof_state"][ids, :, 1] = src["dof_pos"][ids, :nd], 0
+    s["pd_target_dof_pos"][ids] = src["dof_pos"][ids, :nd]
+    rs = s["root_states"]
+    rs[ids, 0:3], rs[ids, 3:7], rs[ids, 7:13] = src["root_pos"][ids], src["root_rot"][ids], 0
+    for k in ("prev_target_root_pos", "root_pos", "target_root_pos"):
+        s[k][ids] = src["root_pos"][ids]
+    s["root_vel"][ids] = 0
+    for k in ("progress", "reset", "terminate"):
+        s[k][ids] = 0
+    return s
+
+
+def ctrl_reset(s, mask):
+    """PhysicsMVAEController._reset_env_tensors (:200-208) + num_reset += 1 for the envs in mask"""
+    s = {k: v.copy() for k, v in s.items()}
+    for k in ("progress", "reset", "terminate", "num_reset_reaction"):
+        s[k][mask] = 0
+    s["distance"][mask] = 0
+    s["num_reset"][mask] += 1
+    return s
+
+
+# --------------------------------------------------------------------------- counter-based normals and the target stream
+# Project contracts, not reference behaviour: their specification is the comment of include/b200env_v2p.h and b200env_v2p.cu.
+M64 = (1 << 64) - 1
+
+
+def splitmix64(x):
+    x = np.asarray(x, np.uint64) + np.uint64(0x9E3779B97F4A7C15)
+    x = (x ^ (x >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    x = (x ^ (x >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return x ^ (x >> np.uint64(31))
+
+
+def counter_hash(seed, step, idx):
+    """splitmix64(splitmix64(seed ^ step * 0xD1B54A32D192ED03) + idx), all mod 2^64"""
+    with np.errstate(over="ignore"):
+        h0 = splitmix64(np.uint64(seed) ^ np.uint64((int(step) * 0xD1B54A32D192ED03) & M64))
+        return splitmix64(h0 + np.asarray(idx, np.uint64))
+
+
+def counter_normal(seed, step, idx):
+    """Box-Muller from the 24-bit halves of the hash: u1 in (0, 1], u2 in [0, 1); float32 like the kernel"""
+    f = np.float32
+    h = counter_hash(seed, step, idx)
+    u1 = ((h >> np.uint64(40)).astype(np.uint32) + np.uint32(1)).astype(f) * f(1.0 / 16777217.0)
+    u2 = ((h >> np.uint64(8)) & np.uint64(0xFFFFFF)).astype(f) * f(1.0 / 16777216.0)
+    return (np.sqrt(f(-2) * np.log(u1)) * np.cos(f(6.283185307179586) * u2)).astype(f)
+
+
+def pre_step(actions, tar_action, step, cfg):
+    """b200v2p_pre_step: (mvae_actions, res_dof_actions); element i = e * (latent + res) + k draws counter_normal(seed, step, i)"""
+    f = np.float32
+    n, nl, nr = len(actions), cfg["num_latent"], cfg["num_res_dof"]
+    lat = (actions[:, :nl] * f(cfg["vae_action_scale"])).astype(f)
+    if cfg["random_walk_in_recovery"]:
+        i = np.arange(n)[:, None] * (nl + nr) + np.arange(nl)[None]
+        rnd = np.clip(counter_normal(cfg["seed"], step, i), f(-5), f(5))
+        lat = np.where((tar_action == 0)[:, None], rnd, lat)
+    return lat, (actions[:, nl:nl + nr] * f(cfg["residual_dof_scale"])).astype(f)
+
+
+def stream_frames(clock, advance, offset, frames, n, seed=0, reseed_mask=None):
+    """b200v2p_stream_gather: (frame per env, new offsets).  t = clock + advance; a reseeded env draws offset = hash(seed, t, e) % frames;
+    env e reads frame (t + offset[e]) mod frames (non-negative)"""
+    t = int(clock) + int(advance)
+    off = np.asarray(offset, np.int64).copy()
+    if reseed_mask is not None:
+        e = np.flatnonzero(reseed_mask)
+        off[e] = (counter_hash(seed, t, e) % np.uint64(frames)).astype(np.int64)
+    return np.mod(t + off, frames), off
 
 
 # --------------------------------------------------------------------------- a13b: head look-at correction

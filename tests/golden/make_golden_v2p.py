@@ -10,6 +10,8 @@ through fake `self` objects.  Run in the build container only:  python tests/gol
                         PhysicsMVAEControllerDual._compute_reset (physics_mvae_controller_dual.py:92-120)
   v2p_controller.npz    actor/task obs (:333-360), rewards (:493-602), check_out_of_court, _update_state + estimator
                         (:271-314, tennis_ball_out_estimator.py:164-205), _compute_reset (:408-436)          (a14-a16)
+  v2p_task_reset.npz    TennisBallGeneratorOffline.generate with start_pos (tennis_ball.py:436-444), the controller's
+                        _reset_recovery_tasks / _reset_reaction_tasks (physics_mvae_controller.py:203-245), both target modes
 """
 import os
 import sys
@@ -489,7 +491,92 @@ def dual():
     npz("v2p_dual.npz", **rec)
 
 
+def task_reset():
+    """the pool index rule with start_pos, the recovery / reaction task resets; the torch draws are recorded in call order"""
+    P, N = 997, 96
+    rng = np.random.default_rng(8)
+    pool = rng.normal(0, 5, (P, 307)).astype(np.float32)
+    path = os.path.join("/tmp", "v2p_pool_tr.npy")
+    np.save(path, pool)
+    gen = TennisBallGeneratorOffline(traj_file=path, sample_random=True, num_envs=N)
+    start = np.stack([rng.uniform(-5, 5, N), rng.uniform(-3, 3, N), np.ones(N)], -1).astype(np.float32)
+    start[:10, 0] = [-4, np.nextafter(np.float32(-4), np.float32(0)), 4, np.nextafter(np.float32(4), np.float32(0)), -4 - 8 / P, -5, 5, 0,
+                     -4 + 8 / P, 4 - 8 / P]
+    start[:10, 1] = 1.0
+    start[10:13, 1] = [0.0, np.nextafter(np.float32(0), np.float32(1)), np.nextafter(np.float32(0), np.float32(-1))]
+    draws, randint = [], torch.randint
+
+    def rec_randint(*a, **k):
+        draws.append(randint(*a, **k))
+        return draws[-1]
+    torch.manual_seed(4)
+    torch.randint = rec_randint
+    try:
+        _, launch_pos, _, _ = gen.generate(N, need_init_state=True, start_pos=torch.from_numpy(start))
+    finally:
+        torch.randint = randint
+    index = np.array([int(np.flatnonzero((pool[:, 0:3] == p).all(1))[0]) for p in launch_pos.numpy()])
+    side = np.zeros(N, np.int64)
+    side[start[:, 1] > 0] = draws[1].numpy()
+    out = dict(tr_pool_size=P, tr_start=start, tr_pool_rand=draws[0].numpy(), tr_side_rand=side, tr_index=index)
+    # _reset_recovery_tasks / _reset_reaction_tasks through a fake controller
+    for mode in ("continuous", "discrete"):
+        c = SimpleNamespace(device='cpu', cfg_v2p={'use_history_ball_obs': True, 'reset_reaction_nframes': 70, 'use_random_ball_target': mode},
+                            _obs_ball_traj_length=10)
+        c._ball_obs, c._ball_pos = torch.randn(N, 10, 3), torch.randn(N, 3)
+        c._tar_time, c._tar_action, c._num_reset_reaction = torch.randint(0, 80, (N,)), torch.randint(0, 2, (N,)), torch.randint(0, 5, (N,))
+        c._bounce_in, c._est_bounce_in = torch.rand(N) < 0.5, torch.rand(N) < 0.5
+        c._est_bounce_pos, c._est_bounce_time, c._est_max_height = torch.randn(N, 3), torch.rand(N), torch.rand(N)
+        c._mvae_player = SimpleNamespace(_swing_type_cycle=torch.randint(-1, 4, (N,)))
+        c._tar_time_total, c._target_bounce_pos = torch.randint(60, 80, (N,)), torch.randn(N, 3)
+        c._target_bounce_min, c._target_bounce_max = torch.tensor([-3.0, 9.0, 0.0]), torch.tensor([3.0, 11.0, 0.0])
+        c._physics_player = SimpleNamespace(task=SimpleNamespace(_has_bounce=torch.rand(N) < 0.5, _bounce_pos=torch.randn(N, 3)))
+        names = ("_ball_obs", "_ball_pos", "_tar_time", "_tar_action", "_num_reset_reaction", "_bounce_in", "_est_bounce_in", "_est_bounce_pos",
+                 "_est_bounce_time", "_est_max_height", "_tar_time_total", "_target_bounce_pos")
+        for k in names:
+            out[f"{mode}_in{k}"] = getattr(c, k).clone()
+        out[f"{mode}_in_cycle"] = c._mvae_player._swing_type_cycle.clone()
+        out[f"{mode}_in_has_bounce"] = c._physics_player.task._has_bounce.clone()
+        out[f"{mode}_in_bounce_pos"] = c._physics_player.task._bounce_pos.clone()
+        rec_ids, rea_ids = torch.tensor([1, 4, 9, 33, 70]), torch.tensor([0, 4, 17, 33, 50, 51, 95])
+        C.PhysicsMVAEController._reset_recovery_tasks(c, rec_ids)
+        rd, rand = [], torch.rand
+        torch.manual_seed(5)
+        torch.randint = rec_randint
+        torch.rand = lambda *a, **k: rd.append(rand(*a, **k)) or rd[-1]
+        try:
+            draws.clear()
+            C.PhysicsMVAEController._reset_reaction_tasks(c, rea_ids)
+        finally:
+            torch.randint, torch.rand = randint, rand
+        if mode == "discrete":
+            rd[0][:3] = torch.tensor([0.33, 0.67, float(np.nextafter(np.float32(0.33), np.float32(1)))])
+            torch.manual_seed(5)   # replay with the edge seeds written into the draw
+            seeds = rd[0].clone()
+            torch.randint = lambda *a, **k: draws[0]
+            torch.rand = lambda *a, **k: seeds
+            try:
+                for k in names:
+                    getattr(c, k).copy_(out[f"{mode}_in{k}"])
+                c._mvae_player._swing_type_cycle.copy_(out[f"{mode}_in_cycle"])
+                c._physics_player.task._has_bounce.copy_(out[f"{mode}_in_has_bounce"])
+                c._physics_player.task._bounce_pos.copy_(out[f"{mode}_in_bounce_pos"])
+                C.PhysicsMVAEController._reset_recovery_tasks(c, rec_ids)
+                C.PhysicsMVAEController._reset_reaction_tasks(c, rea_ids)
+            finally:
+                torch.randint, torch.rand = randint, rand
+        out.update({f"{mode}_rec_ids": rec_ids, f"{mode}_rea_ids": rea_ids, f"{mode}_frame_rand": draws[0], f"{mode}_seed": rd[0],
+                    f"{mode}_out_cycle": c._mvae_player._swing_type_cycle, f"{mode}_out_has_bounce": c._physics_player.task._has_bounce,
+                    f"{mode}_out_bounce_pos": c._physics_player.task._bounce_pos})
+        for k in names:
+            out[f"{mode}_out{k}"] = getattr(c, k).clone()
+    npz("v2p_task_reset.npz", **out)
+
+
 if __name__ == "__main__":
+    if sys.argv[1:] == ["task_reset"]:
+        task_reset()
+        sys.exit(0)
     dual()
     fix_head()
     smpl_to_sim()

@@ -152,3 +152,45 @@ def test_history_ball_obs_variant():
         assert np.array_equal(h, g[f"hist_after_full{k}"])
         close(V.controller_obs(*args, ball_obs=h), g[f"hist_obs_full{k}"], 2e-6)
 
+
+
+def test_task_reset():
+    """pool_index against TennisBallGeneratorOffline.generate with start_pos (x edges at -4, 4, +-8 / P, outside the court; ball_y at 0
+    and +-1 ulp), and task_reset's recovery / reaction bookkeeping against _reset_recovery_tasks / _reset_reaction_tasks in both
+    target modes (discrete seeds at 0.33 and 0.67), history rows included; the fixture's recorded draws are fed back in"""
+    g = golden("v2p_task_reset.npz")
+    P = int(g["tr_pool_size"])
+    got = V.pool_index(g["tr_start"], g["tr_pool_rand"], g["tr_side_rand"], P)
+    assert np.array_equal(got, g["tr_index"]), np.flatnonzero(got != g["tr_index"])
+    for mode in ("continuous", "discrete"):
+        i = lambda k: g[f"{mode}_in_{k}"].copy()  # noqa: E731
+        n = len(i("ball_pos"))
+        rea, rec = np.zeros(n, bool), np.zeros(n, bool)
+        rea[g[f"{mode}_rea_ids"]], rec[g[f"{mode}_rec_ids"]] = True, True
+        # a pool whose row e is env e's ball position: the launch position the reaction rows' history is reset to
+        pool = np.zeros((n, 307), np.float32)
+        pool[:, 0:3] = i("ball_pos")
+        ball_pos = i("ball_pos")
+        ball_pos[:, 1] = -1          # near side: the draw pool_rand (= the env) picks the row
+        s = dict(ball_pos=ball_pos, ball_vel=np.zeros((n, 3), np.float32), bounce_pos=i("bounce_pos"), ball_traj=np.zeros((n, 100, 3), np.float32),
+                 est_bounce_pos=i("est_bounce_pos"), est_bounce_time=i("est_bounce_time"), est_max_height=i("est_max_height"),
+                 target_bounce_pos=i("target_bounce_pos"), ball_states=np.zeros((n, 13), np.float32), rbs_ball=np.zeros((n, 13), np.float32),
+                 has_bounce=i("has_bounce"), has_contact=np.zeros(n, bool), bounce_in=i("bounce_in"), est_bounce_in=i("est_bounce_in"),
+                 tar_time=i("tar_time"), tar_time_total=i("tar_time_total"), tar_action=i("tar_action"), num_reset_reaction=i("num_reset_reaction"),
+                 swing_type_cycle=i("cycle"), reset_reaction=rea, reset_recovery=rec, ball_obs=i("ball_obs"))
+        frame = np.zeros(n, np.int64)
+        frame[g[f"{mode}_rea_ids"]] = g[f"{mode}_frame_rand"]
+        seed = g[f"{mode}_seed"]
+        if mode == "discrete":
+            seed = np.zeros(n, np.float32)
+            seed[g[f"{mode}_rea_ids"]] = g[f"{mode}_seed"]
+        out = V.task_reset(s, dict(pool=pool, reaction_nframes=70, target_mode=mode, target_min=(-3, 9, 0), target_max=(3, 11, 0)),
+                           dict(pool_rand=np.arange(n), side_rand=np.zeros(n, np.int64), frame_rand=frame, target_seed=seed))
+        for k, gk in (("ball_obs", "ball_obs"), ("tar_time", "tar_time"), ("tar_action", "tar_action"), ("num_reset_reaction", "num_reset_reaction"),
+                      ("bounce_in", "bounce_in"), ("est_bounce_in", "est_bounce_in"), ("est_bounce_pos", "est_bounce_pos"),
+                      ("est_bounce_time", "est_bounce_time"), ("est_max_height", "est_max_height"), ("tar_time_total", "tar_time_total"),
+                      ("target_bounce_pos", "target_bounce_pos"), ("swing_type_cycle", "cycle")):
+            assert np.array_equal(out[k], g[f"{mode}_out_{gk}"]), (mode, k)
+        # has_bounce / bounce_pos: the reference's _reset_balls (not in this fixture) clears them for the reaction rows too
+        for k in ("has_bounce", "bounce_pos"):
+            assert np.array_equal(out[k][~rea], g[f"{mode}_out_{k}"][~rea]), (mode, k)

@@ -68,7 +68,8 @@ __device__ __forceinline__ void quat_wxyz_to_angle_axis(const float* q, float* a
 }
 // quaternion (given in the converter's WXYZ slot order) -> rotation matrix (konia_transform.py:474-555)
 __device__ __forceinline__ void quat_wxyz_to_rotmat(const float* qi, float* m) {
-  const float n = fmaxf(sqrtf(qi[0] * qi[0] + qi[1] * qi[1] + qi[2] * qi[2] + qi[3] * qi[3]), 1e-12f);
+  const float n0 = sqrtf(qi[0] * qi[0] + qi[1] * qi[1] + qi[2] * qi[2] + qi[3] * qi[3]);
+  const float n = n0 < 1e-12f ? 1e-12f : n0;   // clamp_min that keeps a NaN (fmaxf would drop it): a NaN quaternion gives a NaN matrix
   const float w = qi[0] / n, x = qi[1] / n, y = qi[2] / n, z = qi[3] / n;
   const float tx = 2.0f * x, ty = 2.0f * y, tz = 2.0f * z;
   const float twx = tx * w, twy = ty * w, twz = tz * w, txx = tx * x, txy = ty * x, txz = tz * x, tyy = ty * y, tyz = tz * y, tzz = tz * z;
@@ -301,7 +302,7 @@ __global__ void ball_reset_kernel(int n, const int64_t* __restrict__ env_ids, co
     const float v[3] = {row[3], row[4], row[5]};
     // ang vel = vspin * 2pi * normalize(v x (0,0,-1))   (:508-509)
     float c[3] = {-v[1], v[0], 0.0f};
-    const float nn = fmaxf(sqrtf(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]), 1e-12f);
+    const float nn = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(c[0], c[0]), __fmul_rn(c[1], c[1])), __fmul_rn(c[2], c[2]))), 1e-12f);
     const float s = row[6] * 3.141592653589793f * 2.0f;
 #pragma unroll
     for (int k = 0; k < 3; k++) { b[k] = row[k]; b[7 + k] = v[k]; b[10 + k] = s * (c[k] / nn); ball_pos[e * 3 + k] = row[k]; ball_vel[e * 3 + k] = v[k]; bounce_pos[e * 3 + k] = 0.0f; }
@@ -382,12 +383,14 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
     if (c.has_contact_now[e] && c.est_x) {
       const float* b = c.ball_states + e * c.ball_stride;
       const float *VX = c.est_params, *VY = c.est_params + 3, *VS = c.est_params + 6, *TX = c.est_params + 9, *TY = c.est_params + 12;
+      // x_net, vel_x and vspin round every product like the reference's tensor ops (no fma contraction): one rounding flips the
+      // x_net = +-4 validity test or the table row at a cell edge
       bool valid = (b[8] > VX[0]) && (b[9] > VY[0]) && (b[9] < VY[1]) && (b[2] < TY[1]);
-      const float x_net = b[0] + b[7] * fabsf(b[1] / b[8]);
+      const float x_net = __fadd_rn(b[0], __fmul_rn(b[7], fabsf(b[1] / b[8])));
       valid = valid && (x_net > -4.0f) && (x_net < 4.0f);
       if (valid) {
-        const float vel_x = sqrtf(b[7] * b[7] + b[8] * b[8]);
-        const float vspin = sqrtf(b[10] * b[10] + b[11] * b[11] + b[12] * b[12]) / 6.283185307179586f;
+        const float vel_x = sqrtf(__fadd_rn(__fmul_rn(b[7], b[7]), __fmul_rn(b[8], b[8])));
+        const float vspin = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(b[10], b[10]), __fmul_rn(b[11], b[11])), __fmul_rn(b[12], b[12]))) / 6.283185307179586f;
         const float d1 = (VY[1] - VY[0]) / VY[2], d2 = (VS[1] - VS[0]) / VS[2];
         const int64_t ti = (int64_t)(est_index(vel_x, VX) * d1 * d2 + est_index(b[9], VY) * d2 + est_index(vspin, VS));
         const float* tx = c.est_x + ti * c.est_nx;
@@ -428,7 +431,8 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
         const float* src = c.has_bounce[e] ? (c.bounce_pos + e * 3) : bp;
 #pragma unroll
         for (int k = 0; k < 3; k++) err += (src[k] - tp[k]) * (src[k] - tp[k]);
-        s1 = (has_contact ? 1.0f : 0.0f) * fminf(fmaxf((400.0f - err) / 400.0f, 0.0f), 1.0f);
+        const float r = (400.0f - err) / 400.0f;
+        s1 = (has_contact ? 1.0f : 0.0f) * (r < 0.0f ? 0.0f : (r > 1.0f ? 1.0f : r));   // torch.clamp keeps a NaN
       } else {  // return_w_estimate
         float err = 0.0f;
 #pragma unroll
@@ -603,7 +607,8 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) task_reset_kernel(b200v2p_tres
       float* rb = r.rigid_body_state + (e * r.bodies_per_env + r.bodies_per_env - 1) * 13;
       const float v[3] = {row[3], row[4], row[5]};
       const float c[3] = {-v[1], v[0], 0.0f};
-      const float nn = fmaxf(sqrtf(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]), 1e-12f);
+      // F.normalize and the target below: every product rounded on its own, like the reference's tensor ops (no fma contraction)
+      const float nn = fmaxf(sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(c[0], c[0]), __fmul_rn(c[1], c[1])), __fmul_rn(c[2], c[2]))), 1e-12f);
       const float sp = row[6] * 3.141592653589793f * 2.0f;
 #pragma unroll
       for (int k = 0; k < 3; k++) {
@@ -634,7 +639,8 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) task_reset_kernel(b200v2p_tres
     r.tar_time_total[e] = (int64_t)r.reaction_nframes + r.frame_rand[e];
     if (r.target_mode == 1) {        // 'continuous': one target shared by the envs reset in this call (:226-229)
 #pragma unroll
-      for (int k = 0; k < 3; k++) r.target_bounce_pos[e * 3 + k] = r.target_seed[k] * (r.target_max[k] - r.target_min[k]) + r.target_min[k];
+      for (int k = 0; k < 3; k++)
+        r.target_bounce_pos[e * 3 + k] = __fadd_rn(__fmul_rn(r.target_seed[k], r.target_max[k] - r.target_min[k]), r.target_min[k]);
     } else if (r.target_mode == 2) { // left / middle / right (:230-237)
       const float sd = r.target_seed[e];
       r.target_bounce_pos[e * 3] = sd < 0.33f ? -3.0f : (sd > 0.67f ? 3.0f : 0.0f);
@@ -915,8 +921,11 @@ int b200v2p_stream_gather(const b200v2p_stream_t* s, void* stream) {
 int b200v2p_controller_post(const b200v2p_ctrl_t* c, void* stream) {
   if (!c) return vfail(-1, "b200v2p_controller_post: null");
   if (c->n == 0) return 0;
-  if (c->obs_traj_len < 0 || c->obs_traj_len > 100 || c->num_obs < 225 + 3 * c->obs_traj_len + (c->use_target ? 2 : 0))
+  if (c->n < 0) return vfail(-1, "b200v2p_controller_post: bad arguments");
+  // the NaN test of the reset FSM covers the columns the launch writes: a wider row would carry columns it never checks
+  if (c->obs_traj_len < 0 || c->obs_traj_len > 100 || c->num_obs != 225 + 3 * c->obs_traj_len + (c->use_target ? 2 : 0))
     return vfail(-2, "b200v2p_controller_post: observation width / trajectory length mismatch");
+  if (c->dual && (c->n & 1)) return vfail(-2, "b200v2p_controller_post: dual mode needs an even number of envs (pairs 2k, 2k+1)");
   if (c->reward_type < 0 || c->reward_type > 2) return vfail(-2, "b200v2p_controller_post: reward_type must be 0 (reach), 1 (return) or 2 (return_w_estimate)");
   if (c->use_history && !c->ball_obs) return vfail(-2, "b200v2p_controller_post: use_history needs the ball_obs buffer");
   controller_post_kernel<<<(c->n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*c);

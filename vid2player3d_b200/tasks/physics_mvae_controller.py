@@ -505,7 +505,7 @@ class PhysicsMVAEController:
         if len(reaction_ids) > 0:
             self._reset_reaction_tasks(reaction_ids)
         if len(all_ids) > 0:
-            self._compute_observations()
+            self._compute_observations(all_ids)
         self._has_init = True
 
     def _reset_reaction_tasks(self, env_ids):
@@ -602,15 +602,15 @@ class PhysicsMVAEController:
         if not self._is_train:
             self._joint_rot = t._joint_rot          # :274-275
 
-    def _compute_observations(self, env_ids=None):
-        """used on reset: the observation rows are refreshed by the same kernel (reward / reset flags of a reset env are rewritten
-        by the next step before anyone reads them)"""
-        keep = (self.rew_buf.clone(), self.reset_buf.clone(), self._terminate_buf.clone(), self._reset_reaction_buf.clone(),
-                self._reset_recovery_buf.clone(), self._distance.clone(), self._sub_rewards.clone())
-        self._compute_post()
-        self.rew_buf.copy_(keep[0]); self.reset_buf.copy_(keep[1]); self._terminate_buf.copy_(keep[2])
-        self._reset_reaction_buf.copy_(keep[3]); self._reset_recovery_buf.copy_(keep[4]); self._distance.copy_(keep[5])
-        self._sub_rewards.copy_(keep[6])
+    def _compute_observations(self, env_ids):
+        """_compute_observations(env_ids) (:316-360) on reset: the observation-only form of the post kernel refreshes the rows of
+        env_ids and rolls their ball history (:345-346), and writes nothing else.  The rows are passed as a reaction mask with an
+        empty touch mask, so every other row is skipped and no flag is cleared."""
+        rows = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        rows[env_ids] = True
+        t = self._tensors()
+        t.update(reset_reaction=rows, reset_recovery=torch.zeros_like(rows), touch_mask=torch.zeros_like(rows))
+        native_v2p.controller_post(dict(self._post_cfg, obs_only=1), t)
 
     def step(self, actions):
         if self._graph is not None:
