@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 5
+#define B200_ABI_VERSION 6
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:
@@ -245,6 +245,31 @@ int32_t b200env_kernel_form(b200env_handle h);
  * of the persistent launch (CTAs per SM x SMs).  A step of n envs runs min(*grid, ceil(n / *envs_per_batch)) CTAs, so batch b of
  * the env order runs in round b / *grid.  Computed from the same expressions b200env_step uses; needs the device, not a bind. */
 int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int32_t* grid);
+
+/* Several assets of one topology in one handle (replaces the per-env actors of HumanoidSMPLIM._create_envs, each built from its
+ * motion's body: embodied_pose/env/tasks/humanoid_smpl_im.py:231-351, PD gains scaled by that actor's mass :356-389).  models [num_assets]
+ * and verts [num_assets] (verts[a]: [nb][models[a].vmax][3]) are HOST arrays; env e is simulated with asset env_asset[e] for the
+ * handle's lifetime.  Every asset must have asset 0's topology (nb, nd, max_depth, parent, depth, fixed, dof_of_body); vmax, the
+ * vertices and every numeric field may differ.  The physics launch hands out the batches of b200env_plan_assets (at most 32 envs of
+ * one asset each) and re-stages the asset's header in shared memory when a CTA moves to a batch of another asset; every other launch
+ * reads the topology only.  Not supported with several assets (refused with an error): cfg.has_ball, the non-default kernel forms
+ * (B200ENV_KERNEL=lane|tmem|packed3, B200ENV_SPLIT=0, B200ENV_SORT=1), b200env_set_env_slice, b200env_set_hull_faces and
+ * b200env_physics_only. */
+int b200env_create_assets(const b200_model_t* models, const float* const* verts, int32_t num_assets, const int32_t* env_asset,
+                          const b200_cfg_t* cfg, int32_t num_envs, int32_t device, b200env_handle* out);
+
+/* The batch plan of b200env_create_assets, host only (no device needed): rows [num_envs] = the envs grouped by asset (ascending env
+ * index inside an asset), then one batch per up to envs_per_batch consecutive rows of one asset: batch i covers rows
+ * [batch_first[i], batch_first[i] + batch_count[i]) of asset batch_asset[i].  Asset a gets ceil(n_a / envs_per_batch) batches (none
+ * when n_a = 0), in ascending asset order.  The batch arrays need room for num_envs entries; *num_batches receives their number. */
+int b200env_plan_assets(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t envs_per_batch, int32_t* rows,
+                        int32_t* batch_asset, int32_t* batch_first, int32_t* batch_count, int32_t* num_batches);
+
+/* The plan a handle of b200env_create_assets runs (batch b runs in round b / grid of b200env_physics_launch_shape).  Array
+ * arguments may be NULL (query the sizes first: rows has num_envs entries, the batch arrays *num_batches).  Fails on a handle of
+ * b200env_create. */
+int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batches, int32_t* rows, int32_t* batch_asset,
+                       int32_t* batch_first, int32_t* batch_count);
 
 /* number of kernels launched by this handle so far (bench.py "gpu_launches") */
 int64_t b200env_launch_count(b200env_handle h);

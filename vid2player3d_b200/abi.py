@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 
 class Model(C.Structure):

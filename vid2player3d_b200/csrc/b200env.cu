@@ -22,6 +22,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "../../include/b200env.h"
@@ -80,6 +81,15 @@ struct b200env {
   int64_t launches;
   int timing;                          // b200env_set_kernel_timing: event pairs around the physics launch
   std::vector<cudaEvent_t>* tev;       // recorded (start, stop) pairs
+  // b200env_create_assets: several assets of one topology (0 = a b200env_create handle).  d_blob holds asset 0 (what every launch but
+  // the physics launch reads: topology only); the physics launch step_kernel_packed<true, true> hands out the batches of the plan.
+  int num_assets;
+  void* d_assets;                      // every asset's DevBlob header + SoA vertices, back to back
+  const DevBlob** d_asset_ptr;         // [num_assets] into d_assets
+  int32_t* d_rows;                     // [num_envs] row order: envs grouped by asset
+  int4* d_batches;                     // [num_batches] {asset, first position in d_rows, count, 0}
+  int num_batches;
+  std::vector<int32_t>* plan;          // host copy: rows [num_envs] | asset, first, count [num_batches] each
 };
 
 static thread_local char g_err[512] = "";
@@ -438,15 +448,11 @@ __device__ __forceinline__ void control_step(const DevBlob& B, const float* vert
 #endif
 
 // ------------------------------------------------------------------------------------------
-// TMA bulk load of the constant block into shared memory (one elected thread issues it)
-__device__ __forceinline__ void load_blob(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* mbar) {
-  const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar);
-  const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smem_dst);
-  if (threadIdx.x == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mb));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
+// TMA bulk load of the constant block into shared memory (one elected thread issues it).  load_blob initialises the mbarrier and
+// completes its phase 0; reload_blob re-uses the initialised mbarrier for phase `parity` (1, 0, 1, ... for the 2nd, 3rd, 4th copy).
+// A reload overwrites data other threads read: every reader must be past a barrier before it is called.
+template <bool PHASE0>   // PHASE0: the first phase of a fresh mbarrier, parity 0 as an immediate
+__device__ __forceinline__ void bulk_copy_wait(uint32_t dst, const void* gsrc, uint32_t bytes, uint32_t mb, uint32_t parity) {
   if (threadIdx.x == 0) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(bytes) : "memory");
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
@@ -455,14 +461,36 @@ __device__ __forceinline__ void load_blob(void* smem_dst, const void* gsrc, uint
   }
   uint32_t done = 0;
   while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(mb)
-        : "memory");
+    if constexpr (PHASE0)
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\t"
+          "selp.u32 %0, 1, 0, p;\n\t}"
+          : "=r"(done)
+          : "r"(mb)
+          : "memory");
+    else
+      asm volatile(
+          "{\n\t.reg .pred p;\n\t"
+          "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+          "selp.u32 %0, 1, 0, p;\n\t}"
+          : "=r"(done)
+          : "r"(mb), "r"(parity)
+          : "memory");
   }
+}
+__device__ __forceinline__ void load_blob(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* mbar) {
+  const uint32_t mb = (uint32_t)__cvta_generic_to_shared(mbar);
+  const uint32_t dst = (uint32_t)__cvta_generic_to_shared(smem_dst);
+  if (threadIdx.x == 0) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mb));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  bulk_copy_wait<true>(dst, gsrc, bytes, mb, 0);
+}
+__device__ __forceinline__ void reload_blob(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* mbar, uint32_t parity) {
+  bulk_copy_wait<false>((uint32_t)__cvta_generic_to_shared(smem_dst), gsrc, bytes, (uint32_t)__cvta_generic_to_shared(mbar), parity);
 }
 
 
@@ -1060,11 +1088,15 @@ __host__ __device__ constexpr int pk_launch_warps(bool split) { return pk_warps(
 // SPLIT = false: the whole env step in this launch.  SPLIT = true: the middle launch of pre_kernel -> this -> post_kernel; here only
 // the state rows / PD targets / residual wrench are read and the state rows written (the once-per-step task logic runs in the two
 // high-occupancy kernels, where its memory latency is covered by 48+ warps per SM instead of the 8 this kernel can hold).
-template <bool SPLIT>
+// MULTI = true (split form only): several assets of one topology in the launch (b200env_create_assets).  The ticket hands out
+// entries of the batch table `batches` ({asset, first position in the row order `perm`, count <= BATCH, 0}); a CTA whose batch has
+// another asset than the header in its shared memory copies that asset's header (assets[asset]) over it first.  gblob = assets[0].
+template <bool SPLIT, bool MULTI = false>
 __global__ void __launch_bounds__(PK_BOUND(SPLIT) * 32, 1)
 step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf,
                    b200_motion_lib_t ml, const float* __restrict__ actions, int num_envs, unsigned long long* __restrict__ ticket,
-                   int env_first, int env_stride, const float* __restrict__ ext_wrench, const int32_t* __restrict__ perm) {
+                   int env_first, int env_stride, const float* __restrict__ ext_wrench, const int32_t* __restrict__ perm,
+                   const DevBlob* const* __restrict__ assets = nullptr, const int4* __restrict__ batches = nullptr, int num_batches = 0) {
   constexpr int PK_WARPS_K = pk_warps(SPLIT);
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
@@ -1074,6 +1106,8 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
   const DevBlob& B = *reinterpret_cast<const DevBlob*>(smem);
   const b200_model_t& M = B.m;
   const float* __restrict__ verts = reinterpret_cast<const float*>(gblob + 1);   // SoA [nb][3][vmax] behind the header, read-only
+  int cur_asset = 0;            // MULTI: asset of the header in shared memory
+  uint32_t blob_parity = 0;     // MULTI: phase of the last completed header copy
   float* scratch_all = reinterpret_cast<float*>(smem + sizeof(DevBlob));
   const int warp = (threadIdx.x >> 5) % PK_WARPS_K, lane = threadIdx.x & 31;
   const bool shadow = PK_SHADOW && (int)threadIdx.x >= PK_WARPS_K * 32;
@@ -1095,6 +1129,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #ifndef PK_GROUPS
 #define PK_GROUPS 1   // 2 measured 1.5 % slower (343 vs 338 us): mixing the phases costs more I-cache than it hides latency
 #endif
+  static_assert(!MULTI || (SPLIT && PK_GROUPS == 1 && !PK_WARP_TICKETS), "several assets: split form, one group of warps per CTA");
   constexpr int G0 = PK_GROUPS == 1 ? PK_WARPS_K : (PK_WARPS_K + 1) / 2;   // warps in group 0
   const int grp = warp < G0 ? 0 : 1;
   const int gw0 = grp == 0 ? 0 : G0, gwn = grp == 0 ? G0 : PK_WARPS_K - G0;   // first warp / number of warps of my group
@@ -1110,19 +1145,32 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
     unsigned long long tk = 0;
     if (lane == 0) tk = atomicAdd(ticket, (unsigned long long)EPW);
     tk = __shfl_sync(FULL, tk, 0);
-    const int64_t eb = (int64_t)tk;
-    if (eb >= num_envs) break;
+    const int64_t eb = (int64_t)tk, end = num_envs;
+    if (eb >= end) break;
     const bool full_batch = false;
     (void)s_tk; (void)BATCH; (void)group_sync;
 #else
     group_sync();
-    if ((int)threadIdx.x == gw0 * 32) s_tk[grp] = atomicAdd(ticket, (unsigned long long)BATCH);
+    if ((int)threadIdx.x == gw0 * 32) s_tk[grp] = atomicAdd(ticket, MULTI ? 1ull : (unsigned long long)BATCH);
     group_sync();
-    const int64_t e0 = (int64_t)s_tk[grp];
-    if (e0 >= num_envs) break;
-    const bool full_batch = e0 + BATCH <= num_envs;
+    int64_t e0 = (int64_t)s_tk[grp], end = num_envs;   // positions [e0, end) of the hand-out order, at most BATCH of them taken
+    if (MULTI) {
+      if (e0 >= num_batches) break;
+      const int4 bt = batches[e0];
+      if (bt.x != cur_asset) {   // every warp of the CTA is past the group barrier: nothing reads the old header any more
+        cur_asset = bt.x;
+        const DevBlob* ga = assets[cur_asset];
+        blob_parity ^= 1u;
+        reload_blob(smem, ga, (uint32_t)sizeof(DevBlob), &mbar, blob_parity);
+        verts = reinterpret_cast<const float*>(ga + 1);
+      }
+      e0 = bt.y;
+      end = (int64_t)bt.y + bt.z;
+    }
+    if (e0 >= end) break;
+    const bool full_batch = e0 + BATCH <= end;
     const int64_t eb = e0 + (int64_t)(warp - gw0) * EPW;
-    if (!full_batch && eb >= num_envs) continue;
+    if (!full_batch && eb >= end) continue;
 #endif
 
     if (SPLIT) {
@@ -1131,7 +1179,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
       const int nd = M.nd;
 #pragma unroll
       for (int k = 0; k < EPW; k++) {
-        const int64_t ek = eb + k < num_envs ? eb + k : (int64_t)num_envs - 1;   // ragged tail: re-read the last env, never stored
+        const int64_t ek = eb + k < end ? eb + k : end - 1;   // ragged tail: re-read the last env, never stored
         const int64_t e = row(ek);
         if (lc.dyn && lane > 0) {
           const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
@@ -1142,7 +1190,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
       }
 #pragma unroll
       for (int k = 0; k < EPW; k++) {
-        if (eb + k >= num_envs) break;
+        if (eb + k >= end) break;
         Lane<float> L;
         float pdtar[3] = {0.f, 0.f, 0.f}, extF[3] = {0.f, 0.f, 0.f}, extT[3] = {0.f, 0.f, 0.f};
 #pragma unroll
@@ -1169,7 +1217,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
       }
     } else {
     for (int k = 0; k < EPW; k++) {
-      if (eb + k >= num_envs) break;
+      if (eb + k >= end) break;
       const int64_t e = env_first + (int64_t)env_stride * (eb + k);  // row in the bound tensors (env slice)
       Lane<float> L;
       float pdtar[3], extF[3], extT[3];
@@ -1179,7 +1227,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
     }
     }
     __syncwarp();
-    const bool valid = eb + g < num_envs;
+    const bool valid = eb + g < end;
     Ball<float> ball;
     ball_clear(ball);
     const int64_t erow_g = SPLIT ? row(valid ? eb + g : eb) : env_first + (int64_t)env_stride * (eb + g);
@@ -1192,7 +1240,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #endif
     if (cfg.has_ball && valid && s == BALL_SLOT && !shadow) ball_writeback(bf, erow_g, ball);
     for (int k = 0; k < EPW; k++) {
-      if (eb + k >= num_envs || shadow) break;
+      if (eb + k >= end || shadow) break;
       const int64_t e = SPLIT ? row(eb + k) : env_first + (int64_t)env_stride * (eb + k);
       Lane<float> L;
       float cf[3];
@@ -2104,14 +2152,140 @@ int b200env_destroy(b200env_handle h) {
   cudaFree(h->d_ticket);
   cudaFree(h->d_ext);
   cudaFree(h->d_bin); cudaFree(h->d_perm); cudaFree(h->d_pos); cudaFree(h->d_cnt);
+  cudaFree(h->d_assets); cudaFree(h->d_asset_ptr); cudaFree(h->d_rows); cudaFree(h->d_batches);
+  delete h->plan;
   if (h->tev) { for (cudaEvent_t e : *h->tev) cudaEventDestroy(e); delete h->tev; }
   delete h;
+  return 0;
+}
+
+int b200env_plan_assets(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t envs_per_batch, int32_t* rows,
+                        int32_t* batch_asset, int32_t* batch_first, int32_t* batch_count, int32_t* num_batches) {
+  if (!env_asset || !rows || !batch_asset || !batch_first || !batch_count || !num_batches) return fail(-1, "b200env_plan_assets: null argument%s");
+  if (num_envs < 1) return fail(-2, "b200env_plan_assets: num_envs must be positive%s");
+  if (num_assets < 1) return fail(-2, "b200env_plan_assets: num_assets must be at least 1%s");
+  if (envs_per_batch < 1) return fail(-2, "b200env_plan_assets: envs_per_batch must be positive%s");
+  std::vector<int32_t> start(num_assets + 1, 0);
+  for (int e = 0; e < num_envs; e++) {
+    if (env_asset[e] < 0 || env_asset[e] >= num_assets) return fail(-2, "b200env_plan_assets: env_asset out of range [0, num_assets)%s");
+    start[env_asset[e] + 1]++;
+  }
+  for (int a = 0; a < num_assets; a++) start[a + 1] += start[a];
+  std::vector<int32_t> next(start.begin(), start.end() - 1);
+  for (int e = 0; e < num_envs; e++) rows[next[env_asset[e]]++] = e;   // stable: ascending env index inside an asset
+  int nbat = 0;
+  for (int a = 0; a < num_assets; a++)
+    for (int p = start[a]; p < start[a + 1]; p += envs_per_batch) {
+      batch_asset[nbat] = a;
+      batch_first[nbat] = p;
+      batch_count[nbat] = start[a + 1] - p < envs_per_batch ? start[a + 1] - p : envs_per_batch;
+      nbat++;
+    }
+  *num_batches = nbat;
+  return 0;
+}
+
+int b200env_create_assets(const b200_model_t* models, const float* const* verts, int32_t num_assets, const int32_t* env_asset,
+                          const b200_cfg_t* cfg, int32_t num_envs, int32_t device, b200env_handle* out) {
+  if (!models || !verts || !env_asset || !cfg || !out) return fail(-1, "b200env_create_assets: null argument%s");
+  if (num_assets < 1) return fail(-2, "b200env_create_assets: num_assets must be at least 1%s");
+  if (num_envs < 1) return fail(-2, "b200env_create_assets: num_envs must be positive%s");
+  const b200_model_t& m0 = models[0];
+  for (int a = 0; a < num_assets; a++) {
+    const b200_model_t& m = models[a];
+    if (!verts[a]) return fail(-1, "b200env_create_assets: null vertex array%s");
+    if (m.nb != m0.nb || m.nd != m0.nd || m.max_depth != m0.max_depth)
+      return fail(-2, "b200env_create_assets: every asset must have the topology of asset 0 (nb, nd, max_depth differ)%s");
+    if (m0.nb < 1 || m0.nb > B200_MAX_BODIES) return fail(-2, "b200env_create: model dimensions out of range%s");
+    for (int b = 0; b < m0.nb; b++)
+      if (m.parent[b] != m0.parent[b] || m.depth[b] != m0.depth[b] || m.fixed[b] != m0.fixed[b] || m.dof_of_body[b] != m0.dof_of_body[b])
+        return fail(-2, "b200env_create_assets: every asset must have the topology of asset 0 (parent, depth, fixed or dof_of_body differ)%s");
+    if (m.vmax % 4) return fail(-2, "b200env_create: vmax must be a multiple of 4%s");
+    for (int b = 0; b < m.nb; b++)
+      if (m.nverts[b] < 0 || m.nverts[b] > 64 || m.nverts[b] > m.vmax)
+        return fail(-2, "b200env_create: at most 64 hull vertices per body (contact_hull keeps a 64-bit penetration mask)%s");
+  }
+  for (int e = 0; e < num_envs; e++)
+    if (env_asset[e] < 0 || env_asset[e] >= num_assets) return fail(-2, "b200env_create_assets: env_asset out of range [0, num_assets)%s");
+  if (cfg->has_ball) return fail(-2, "b200env_create_assets: has_ball is not supported with several assets (the racket constants are per player)%s");
+  const char* kv = getenv("B200ENV_KERNEL");
+  const char* sv = getenv("B200ENV_SPLIT");
+  const char* so = getenv("B200ENV_SORT");
+  if ((kv && strcmp(kv, "packed") != 0) || (sv && strcmp(sv, "0") == 0) || (so && strcmp(so, "1") == 0))
+    return fail(-2, "b200env_create_assets: several assets run in the default kernel form only (unset B200ENV_KERNEL, B200ENV_SPLIT, B200ENV_SORT)%s");
+  // the planner and its outputs: rows | asset | first | count (at most one batch per env)
+  std::vector<int32_t>* plan = new std::vector<int32_t>((size_t)num_envs * 4);
+  int32_t nbat = 0;
+  int32_t* P = plan->data();
+  const int batch = pk_warps(true) * EPW;
+  int rc = b200env_plan_assets(env_asset, num_envs, num_assets, batch, P, P + num_envs, P + 2 * (size_t)num_envs, P + 3 * (size_t)num_envs, &nbat);
+  if (rc) { delete plan; return rc; }
+  std::vector<int4> bt(nbat);
+  for (int i = 0; i < nbat; i++) bt[i] = make_int4(P[num_envs + i], P[2 * num_envs + i], P[3 * num_envs + i], 0);
+  // compact to rows | asset [nbat] | first [nbat] | count [nbat]
+  std::copy(P + 2 * (size_t)num_envs, P + 2 * (size_t)num_envs + nbat, P + num_envs + nbat);
+  std::copy(P + 3 * (size_t)num_envs, P + 3 * (size_t)num_envs + nbat, P + num_envs + 2 * nbat);
+  plan->resize((size_t)num_envs + 3 * nbat);
+  P = plan->data();
+  // asset 0 through the one-asset path: validation, kernel form, d_blob / d_cfg / ticket
+  b200env_handle h = nullptr;
+  rc = b200env_create(&models[0], verts[0], cfg, num_envs, device, &h);
+  if (rc) { delete plan; return rc; }
+  h->plan = plan;
+  h->num_assets = num_assets;
+  h->num_batches = nbat;
+  if (!h->packed || !h->split || h->sort || h->tmem || h->packed3) {
+    b200env_destroy(h);
+    return fail(-2, "b200env_create_assets: several assets need the packed split form of the physics launch%s");
+  }
+  std::vector<size_t> off(num_assets + 1, 0);
+  for (int a = 0; a < num_assets; a++)
+    off[a + 1] = off[a] + sizeof(DevBlob) + (((size_t)models[a].nb * models[a].vmax * 3 * sizeof(float) + 15) & ~(size_t)15);
+  std::vector<unsigned char> host(off[num_assets], 0);
+  for (int a = 0; a < num_assets; a++) {
+    DevBlob hb;
+    int slots_ok = 1;
+    build_dev_blob(&models[a], hb, &slots_ok);   // same topology as asset 0, which b200env_create accepted
+    hull_vertex_radius(&models[a], verts[a], hb.t.vrho);
+    hull_bounding_spheres(&models[a], verts[a], hb.t.bs);
+    memcpy(host.data() + off[a], &hb, sizeof(hb));
+    verts_to_soa(&models[a], verts[a], reinterpret_cast<float*>(host.data() + off[a] + sizeof(DevBlob)));
+  }
+#define CUDA_OK_H(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200env_destroy(h); return fail(-10, "CUDA error: %s", cudaGetErrorString(_e)); } } while (0)
+  CUDA_OK_H(cudaMalloc(&h->d_assets, host.size()));
+  CUDA_OK_H(cudaMemcpy(h->d_assets, host.data(), host.size(), cudaMemcpyHostToDevice));
+  std::vector<const DevBlob*> ptr(num_assets);
+  for (int a = 0; a < num_assets; a++) ptr[a] = reinterpret_cast<const DevBlob*>(static_cast<unsigned char*>(h->d_assets) + off[a]);
+  CUDA_OK_H(cudaMalloc(&h->d_asset_ptr, sizeof(const DevBlob*) * num_assets));
+  CUDA_OK_H(cudaMemcpy(h->d_asset_ptr, ptr.data(), sizeof(const DevBlob*) * num_assets, cudaMemcpyHostToDevice));
+  CUDA_OK_H(cudaMalloc(&h->d_rows, sizeof(int32_t) * num_envs));
+  CUDA_OK_H(cudaMemcpy(h->d_rows, P, sizeof(int32_t) * num_envs, cudaMemcpyHostToDevice));
+  CUDA_OK_H(cudaMalloc(&h->d_batches, sizeof(int4) * nbat));
+  CUDA_OK_H(cudaMemcpy(h->d_batches, bt.data(), sizeof(int4) * nbat, cudaMemcpyHostToDevice));
+#undef CUDA_OK_H
+  *out = h;
+  return 0;
+}
+
+int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batches, int32_t* rows, int32_t* batch_asset, int32_t* batch_first,
+                       int32_t* batch_count) {
+  if (!h || !num_assets || !num_batches) return fail(-1, "b200env_asset_plan: null argument%s");
+  if (!h->num_assets) return fail(-2, "b200env_asset_plan: not a handle of b200env_create_assets%s");
+  *num_assets = h->num_assets;
+  *num_batches = h->num_batches;
+  const int32_t* P = h->plan->data();
+  const size_t n = h->num_envs, nb = h->num_batches;
+  if (rows) memcpy(rows, P, n * sizeof(int32_t));
+  if (batch_asset) memcpy(batch_asset, P + n, nb * sizeof(int32_t));
+  if (batch_first) memcpy(batch_first, P + n + nb, nb * sizeof(int32_t));
+  if (batch_count) memcpy(batch_count, P + n + 2 * nb, nb * sizeof(int32_t));
   return 0;
 }
 
 int b200env_set_hull_faces(b200env_handle h, const float* planes, const uint8_t* tris, const int32_t* ntris, int32_t tmax) {
   if (!h || !planes || !tris || !ntris) return fail(-1, "b200env_set_hull_faces: null argument%s");
   if (tmax < 1 || tmax > 255) return fail(-2, "b200env_set_hull_faces: tmax must be in 1..255%s");
+  if (h->num_assets) return fail(-2, "b200env_set_hull_faces: not supported on a handle of several assets (b200env_create_assets)%s");
   const int nb = h->model.nb;
   for (int b = 0; b < nb; b++) {
     if (ntris[b] < 0 || ntris[b] > tmax) return fail(-2, "b200env_set_hull_faces: ntris out of range%s");
@@ -2220,6 +2394,10 @@ static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out) 
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed3, PK3_WARPS * 32, psmem));
       } else
 #endif
+      if (h->num_assets) {
+        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true, true>, pk_launch_warps(true) * 32, psmem));
+      } else
       if (h->split) { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true>, pk_launch_warps(true) * 32, psmem)); }
       else { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<false>, pk_launch_warps(false) * 32, psmem)); }
     }
@@ -2227,7 +2405,7 @@ static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out) 
     if (per_sm * sms < 1) return fail(-5, h->packed ? "b200env_step: step_kernel_packed does not fit on this device%s"
                                                      : "b200env_step: step_kernel does not fit on this device%s");
     h->step_slots = per_sm * sms;
-    const int need = (h->num_envs + batch - 1) / batch;
+    const int need = h->num_assets ? h->num_batches : (h->num_envs + batch - 1) / batch;
     h->step_grid = h->step_slots < need ? h->step_slots : need;
   }
   *psmem_out = psmem;
@@ -2292,6 +2470,11 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
       else
 #endif
+      if (h->num_assets)
+        step_kernel_packed<true, true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
+            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext,
+            h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);
+      else
         step_kernel_packed<true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first,
             h->env_stride, h->d_ext, h->sort ? h->d_perm : nullptr);
@@ -2419,6 +2602,7 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
                          void* stream) {
   if (!h || !root || !dof_pos || !dof_vel || !pd_tar || !rb_out) return fail(-1, "b200env_physics_only: null argument%s");
   if (n <= 0 || n_steps <= 0) return fail(-2, "b200env_physics_only: n and n_steps must be positive%s");
+  if (h->num_assets) return fail(-2, "b200env_physics_only: not supported on a handle of several assets (b200env_create_assets)%s");
   cudaSetDevice(h->device);
   if (h->packed) {
     const size_t bsm = (h->blob_bytes + 15) & ~(size_t)15;
@@ -2511,6 +2695,7 @@ int b200env_kernel_ms(b200env_handle h, double* mean_ms, int32_t* count) {
 int b200env_set_env_slice(b200env_handle h, int32_t env_first, int32_t env_stride) {
   if (!h) return fail(-1, "b200env_set_env_slice: null handle%s");
   if (env_first < 0 || env_stride < 1) return fail(-2, "b200env_set_env_slice: env_first >= 0 and env_stride >= 1 required%s");
+  if (h->num_assets) return fail(-2, "b200env_set_env_slice: not supported on a handle of several assets (b200env_create_assets)%s");
   h->env_first = env_first;
   h->env_stride = env_stride;
   return 0;

@@ -15,7 +15,9 @@ SYMBOLS = ["b200env_abi_version", "b200env_last_error", "b200env_create", "b200e
            "b200env_set_motion_lib", "b200env_step", "b200env_reset", "b200env_motion_state", "b200env_obs_imitation",
            "b200env_physics_only", "b200env_launch_count", "b200env_set_env_slice", "b200env_motion_context", "b200env_set_kernel_timing",
            "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form",
-           "b200env_physics_launch_shape"]
+           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan"]
+
+ENVS_PER_BATCH = 32   # envs per CTA batch of the default physics launch (step_kernel_packed<true>): the batch size of the asset plan
 
 
 def lib():
@@ -50,16 +52,45 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-class Env:
-    """Owns one b200env handle.  All tensors passed in must live on `device` and be contiguous."""
+def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH):
+    """the batch plan of a handle of several assets (include/b200env.h: b200env_plan_assets; host only): (rows [N] = envs grouped by
+    asset, batches [num_batches, 3] of (asset, first row, count))"""
+    import numpy as np
+    ea = np.ascontiguousarray(env_asset, np.int32)
+    n = len(ea)
+    rows, ba, bf, bc = (np.zeros(max(n, 1), np.int32) for _ in range(4))
+    nb = C.c_int32(0)
+    p = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+    _check(lib().b200env_plan_assets(p(ea), C.c_int32(n), C.c_int32(int(num_assets)), C.c_int32(int(envs_per_batch)), p(rows), p(ba), p(bf),
+                                     p(bc), C.byref(nb)))
+    k = nb.value
+    return rows[:n], np.stack([ba[:k], bf[:k], bc[:k]], 1)
 
-    def __init__(self, model_struct, verts, cfg_struct, num_envs, device_index):
+
+class Env:
+    """Owns one b200env handle.  All tensors passed in must live on `device` and be contiguous.
+
+    One asset: Env(model_struct, verts, cfg, N, dev).  Several assets of one topology (include/b200env.h: b200env_create_assets):
+    Env([model_struct, ...], [verts, ...], cfg, N, dev, env_asset=[asset of env 0, ...])."""
+
+    def __init__(self, model_struct, verts, cfg_struct, num_envs, device_index, env_asset=None):
         self._h = C.c_void_p()
         self._keep = []
         import numpy as np
-        verts = np.ascontiguousarray(verts, np.float32)
-        _check(lib().b200env_create(C.byref(model_struct), verts.ctypes.data_as(C.c_void_p), C.byref(cfg_struct),
-                                    C.c_int32(num_envs), C.c_int32(device_index), C.byref(self._h)))
+        if env_asset is None:
+            verts = np.ascontiguousarray(verts, np.float32)
+            _check(lib().b200env_create(C.byref(model_struct), verts.ctypes.data_as(C.c_void_p), C.byref(cfg_struct),
+                                        C.c_int32(num_envs), C.c_int32(device_index), C.byref(self._h)))
+        else:
+            models, vs = list(model_struct), [np.ascontiguousarray(v, np.float32) for v in verts]
+            ea = np.ascontiguousarray(env_asset, np.int32)
+            if len(models) != len(vs) or len(ea) != num_envs:
+                raise ValueError(f"{len(models)} models, {len(vs)} vertex arrays and {len(ea)} env_asset entries for {num_envs} envs")
+            marr = (abi.Model * len(models))(*models)
+            varr = (C.c_void_p * len(vs))(*[v.ctypes.data for v in vs])
+            _check(lib().b200env_create_assets(marr, varr, C.c_int32(len(models)), ea.ctypes.data_as(C.c_void_p), C.byref(cfg_struct),
+                                               C.c_int32(num_envs), C.c_int32(device_index), C.byref(self._h)))
+            model_struct = models[0]
         self.model, self.cfg, self.num_envs = model_struct, cfg_struct, num_envs
 
     def close(self):
@@ -180,6 +211,19 @@ class Env:
         b, g = C.c_int32(0), C.c_int32(0)
         _check(lib().b200env_physics_launch_shape(self._h, C.byref(b), C.byref(g)))
         return b.value, g.value
+
+    @property
+    def asset_plan(self):
+        """(num_assets, rows [N], batches [num_batches, 3] of (asset, first row, count)) of a handle of several assets
+        (include/b200env.h: b200env_asset_plan): batch b of rows[first:first + count] runs in round b // grid"""
+        import numpy as np
+        na, nb = C.c_int32(0), C.c_int32(0)
+        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), None, None, None, None))
+        rows = np.zeros(self.num_envs, np.int32)
+        b = np.zeros((3, max(nb.value, 1)), np.int32)
+        p = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
+        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), p(rows), p(b[0]), p(b[1]), p(b[2])))
+        return na.value, rows, b[:, :nb.value].T.copy()
 
     @property
     def launch_count(self):

@@ -139,15 +139,51 @@ class HumanoidSMPLIM(BaseTask):
     def get_action_size(self):
         return self._num_actions
 
+    def _pack(self, model):
+        """pack_model with the PD gains scaled by the model's own mass (:376-383)"""
+        pd_scale = float(model["mass"].sum()) / self.cfg["env"].get('default_humanoid_mass', 90.0)
+        return abi.pack_model(model, pd_scale * self.kp_scale, pd_scale * self.kd_scale)
+
+    def _motion_asset_models(self):
+        """cfg.env.motion_assets: one entry per motion of the library - an asset file name (resolved like asset.assetFileName) or a
+        compiled model dict - as (compiled models of the distinct assets, asset index of every motion).  Identical compiled assets
+        (same packed constants and vertices) are one asset."""
+        entries = self.cfg["env"]["motion_assets"]
+        if len(entries) != self._motion_lib.num_motions():
+            raise ValueError(f"motion_assets has {len(entries)} entries for {self._motion_lib.num_motions()} motions")
+        models, keys, of_motion = [], {}, []
+        for entry in entries:
+            if isinstance(entry, (str, os.PathLike)):
+                entry = model_compiler.load_compiled(os.path.splitext(os.path.basename(str(entry)))[0])
+            ms, verts = self._pack(entry)
+            key = bytes(ms) + verts.tobytes()
+            if key not in keys:
+                keys[key] = len(models)
+                models.append(entry)
+            of_motion.append(keys[key])
+        return models, np.asarray(of_motion, np.int64)
+
     def create_sim(self):
-        """Stub of BaseTask.create_sim/_create_envs (humanoid_smpl_im.py:231-351): all N envs are
-        instances of one compiled model - O(1) host work, no per-env Python loop."""
+        """Stub of BaseTask.create_sim/_create_envs (humanoid_smpl_im.py:231-351): all N envs are instances of one compiled model -
+        O(1) host work, no per-env Python loop.  With cfg.env.motion_assets, env e is simulated with the asset of its motion
+        _reset_ref_motion_ids[e] (one handle of several assets: the motion ids are sampled here, before the handle exists)."""
         env = self.cfg["env"]
-        pd_scale = self.humanoid_mass / env.get('default_humanoid_mass', 90.0)  # :376-383
-        self._model_struct, self._verts = abi.pack_model(self._model, pd_scale * self.kp_scale, pd_scale * self.kd_scale)
+        self._model_struct, self._verts = self._pack(self._model)
+        structs = None
+        if "motion_assets" in env:
+            self._reset_ref_motion_ids = self._sample_motion_ids()
+            models, of_motion = self._motion_asset_models()
+            self._env_asset = of_motion[self._reset_ref_motion_ids.cpu().numpy()]
+            self._asset_models = models
+            packed = [self._pack(m) for m in models]
+            structs, verts = [p[0] for p in packed], [p[1] for p in packed]
+            self.humanoid_masses = np.array([float(m["mass"].sum()) for m in models])[self._env_asset]     # :370-371
+            self._model_struct, self._verts = structs[self._env_asset[-1]], verts[self._env_asset[-1]]  # the last env's, as the loop leaves them
+            lim = models[self._env_asset[0]]["limits"]                                                    # env 0's (:340-349)
+        else:
+            lim = self._model["limits"]
         self.stiffness = torch.tensor(list(self._model_struct.kp)[:self.num_dof], device=self.device)
         self.damping = torch.tensor(list(self._model_struct.kd)[:self.num_dof], device=self.device)
-        lim = self._model["limits"]
         self.dof_limits_lower = torch.tensor(np.minimum(lim[:, 0], lim[:, 1]), device=self.device, dtype=torch.float)
         self.dof_limits_upper = torch.tensor(np.maximum(lim[:, 0], lim[:, 1]), device=self.device, dtype=torch.float)
         physx = self.cfg.get("b200_physics", {})
@@ -161,7 +197,10 @@ class HumanoidSMPLIM(BaseTask):
             key_bodies=tuple(env["keyBodies"]), body_pos_weights=env.get('body_pos_weights', None),
             reward_specs=env.get('reward_specs', None), shape_dim=self._motion_lib.motion_bodies.shape[-1],
             ground_tolerance=self.ground_tolerance, friction_mu=env["plane"]["dynamicFriction"], **physx)
-        self._env = native.Env(self._model_struct, self._verts, self._cfg_struct, self.num_envs, self.device_id)
+        if structs is None:
+            self._env = native.Env(self._model_struct, self._verts, self._cfg_struct, self.num_envs, self.device_id)
+        else:
+            self._env = native.Env(structs, verts, self._cfg_struct, self.num_envs, self.device_id, env_asset=self._env_asset)
         self._key_body_ids = torch.tensor(list(self._cfg_struct.key_body)[:self._cfg_struct.num_key], device=self.device)
         self._contact_body_ids = torch.tensor([i for i in range(self.num_bodies) if self._cfg_struct.contact_body[i]],
                                               device=self.device)
@@ -190,7 +229,8 @@ class HumanoidSMPLIM(BaseTask):
         self._contact_forces = self._contact_force_tensor.view(N, B, 3)
         self.dof_force_tensor = f(N, D)
         K, S = self._cfg_struct.num_key, self._cfg_struct.shape_dim
-        self._reset_ref_motion_ids = self._sample_motion_ids()
+        if "motion_assets" not in self.cfg["env"]:   # with motion_assets create_sim sampled them
+            self._reset_ref_motion_ids = self._sample_motion_ids()
         self._reset_ref_motion_bodies = self._ml_t["motion_bodies"][self._reset_ref_motion_ids].contiguous()
         self._cur_ref_motion_times = f(N)
         self._reset_ref_motion_times = f(N)
