@@ -568,9 +568,12 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) ball_in_estimate_kernel(int n,
     float* so = s_out + i * 13;
     const float vin[2] = {__fmul_rn(-vx, dx), __fmul_rn(-vx, dy)};
     const float sp = __fmul_rn(__fmul_rn(vs, 3.141592653589793f), 2.0f);
-    // omega = vspin * 2 pi * normalize(v x (0,0,-1)) = (-v_y, v_x, 0) / |.|
-    const float nn = fmaxf(sqrtf(__fadd_rn(__fmul_rn(vin[1], vin[1]), __fmul_rn(vin[0], vin[0]))), 1e-12f);
-    const float wi[3] = {__fmul_rn(sp, __fdiv_rn(-vin[1], nn)), __fmul_rn(sp, __fdiv_rn(vin[0], nn)), 0.0f};
+    // omega = vspin * 2 pi * normalize(v x (0,0,-1)) = (-v_y, v_x, 0) / |.|.  The clamp keeps a NaN like F.normalize's clamp_min:
+    // at v_xy = 0 the direction is NaN, and so is every component of omega, z included (0 / NaN)
+    const float n0 = sqrtf(__fadd_rn(__fmul_rn(vin[1], vin[1]), __fmul_rn(vin[0], vin[0])));
+    const float nn = n0 < 1e-12f ? 1e-12f : n0;
+    const float wz = __fmul_rn(sp, __fdiv_rn(0.0f, nn));
+    const float wi[3] = {__fmul_rn(sp, __fdiv_rn(-vin[1], nn)), __fmul_rn(sp, __fdiv_rn(vin[0], nn)), wz};
     si[0] = -b[0]; si[1] = -b[1]; si[2] = height;
     so[0] = b[0];  so[1] = b[1];  so[2] = height;
 #pragma unroll
@@ -578,7 +581,7 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) ball_in_estimate_kernel(int n,
     si[7] = vin[0]; si[8] = vin[1]; si[9] = vy;
     so[7] = -vin[0]; so[8] = -vin[1]; so[9] = vy;
 #pragma unroll
-    for (int k = 0; k < 3; k++) { si[10 + k] = wi[k]; so[10 + k] = k < 2 ? -wi[k] : 0.0f; }
+    for (int k = 0; k < 3; k++) { si[10 + k] = wi[k]; so[10 + k] = k < 2 ? -wi[k] : wz; }
   }
 }
 
@@ -830,7 +833,8 @@ int b200v2p_ball_reset(int32_t n, const int64_t* env_ids, const int64_t* pool_in
                        float* ball_pos, float* ball_vel, uint8_t* has_bounce, float* bounce_pos, uint8_t* has_contact, float* traj,
                        void* stream) {
   if (n == 0) return 0;
-  if (n < 0 || !env_ids || !pool_index || !pool || !ball_states || !ball_pos || !ball_vel || !has_bounce || !bounce_pos || !has_contact || !traj)
+  if (n < 0 || !env_ids || !pool_index || !pool || !ball_states || !ball_pos || !ball_vel || !has_bounce || !bounce_pos || !has_contact || !traj ||
+      stride < 13)
     return vfail(-1, "b200v2p_ball_reset: bad arguments");
   ball_reset_kernel<<<n, 64, 0, (cudaStream_t)stream>>>(n, env_ids, pool_index, pool, ball_states, stride, ball_pos, ball_vel, has_bounce,
                                                         bounce_pos, has_contact, traj);
@@ -841,8 +845,10 @@ int b200v2p_ball_reset(int32_t n, const int64_t* env_ids, const int64_t* pool_in
 int b200v2p_ball_in_estimate(int32_t n, const int64_t* contact_ids, const float* ball_states, int32_t stride, const float* table,
                              int64_t table_rows, const double* params, float* traj, float* states_in, float* states_out, void* stream) {
   if (n == 0) return 0;
-  if (n < 0 || !contact_ids || !ball_states || !table || table_rows < 1 || !params || !traj || !states_in || !states_out)
+  if (n < 0 || !contact_ids || !ball_states || !table || table_rows < 1 || !params || !traj || !states_in || !states_out || stride < 13)
     return vfail(-1, "b200v2p_ball_in_estimate: bad arguments");
+  for (int k = 0; k < 4; k++)
+    if (!(params[k * 3 + 2] > 0)) return vfail(-2, "b200v2p_ball_in_estimate: grid steps must be positive");
   InParams P;
   double dim[4];
   for (int k = 0; k < 4; k++) {   // python-double arithmetic of the reference, then the float32 cast torch applies to scalars
@@ -860,6 +866,14 @@ int b200v2p_ball_in_estimate(int32_t n, const int64_t* contact_ids, const float*
 int b200v2p_update_state(const b200v2p_state_t* s, void* stream) {
   if (!s) return vfail(-1, "b200v2p_update_state: null");
   if (s->n == 0) return 0;
+  const int B = s->bodies_per_env;
+  const auto body_ok = [B](int b) { return b >= 0 && b < B; };
+  if (s->n < 0 || !s->rigid_body_state || !s->root_states || !s->ball_states || !s->has_contact || !s->has_contact_now || !s->root_pos ||
+      !s->root_vel || !s->racket_pos || !s->racket_vel || !s->racket_normal || !s->ball_pos || !s->ball_vel || !s->ball_vspin ||
+      s->ball_stride < 13 || s->root_stride < 13)
+    return vfail(-1, "b200v2p_update_state: bad arguments");
+  if (!body_ok(s->racket_body) || !body_ok(s->wrist_body) || (s->dual && (!body_ok(s->racket_body2) || !body_ok(s->wrist_body2))))
+    return vfail(-2, "b200v2p_update_state: racket and wrist bodies must lie in [0, bodies_per_env)");
   update_state_kernel<<<(s->n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*s);
   V_CUDA_OK();
   return 0;
