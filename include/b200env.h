@@ -176,6 +176,22 @@ int b200env_step(b200env_handle h, const float* actions, void* stream);
  * (sampled by the host like MotionLib.sample_time). */
 int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_times, int32_t n, void* stream);
 
+/* HumanoidSMPLIM._reset_actors + _init_context (humanoid_smpl_im.py:470-563) for every env e < num_envs with mask[e] != 0, driven by
+ * the device mask instead of an id list: no host synchronisation, two launches, replayable inside a CUDA graph.
+ * Draws: u_k = (bits(seed, *counter, 2e + k) >> 40) * 2^-24 with bits = splitmix64(splitmix64(seed ^ counter * 0xD1B54A32D192ED03) + idx).
+ * u_1 < ref_prob: ref-state init at t = 0 (sample_time 0) or t = u_0 * max(motion_length - truncate, 0) in float32 (sample_time 1,
+ * MotionLib.sample_time); the rows are written exactly as b200env_reset writes them at (e, t), reset_times[e] = t, and the
+ * context window exactly as b200env_motion_context writes it for (e, motion_ids[e], t, num_frames, first_frame, dt).
+ * Otherwise default init (_reset_default :482-487): root row = init_root[e] ([N,13]), dof pos / vel = init_dof_pos[e] /
+ * init_dof_vel[e] ([N,nd]), progress / reset / terminate = 0, raw obs from the new dofs and the rigid-body rows as they stand;
+ * init_* may be NULL when ref_prob >= 1.  Rows whose mask is clear are not touched.
+ * counter: [1] int64 device, advanced by 1 by every call; work: [num_envs + 2] int32 device, zero before the first call (each call
+ * leaves its counters zero). */
+int b200env_reset_masked(b200env_handle h, const uint8_t* mask, int32_t sample_time, float truncate, float ref_prob, uint64_t seed,
+                         int64_t* counter, const float* init_root, const float* init_dof_pos, const float* init_dof_vel, float* reset_times,
+                         int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, int32_t* work,
+                         void* stream);
+
 /* replaces MotionLib.get_motion_state(..., return_rigid_body=True, adjust_height=True)
  * (motion_lib.py:164-266) for arbitrary (id, time) pairs, e.g. _init_context
  * (humanoid_smpl_im.py:530-563).  Any output pointer may be NULL. */

@@ -5,7 +5,7 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRCS = [os.path.join(HERE, "csrc", "b200env.cu"), os.path.join(HERE, "csrc", "b200env_v2p.cu")]
-HDRS = [os.path.join(os.path.dirname(HERE), "include", h) for h in ("b200env.h", "b200env_v2p.h", "b200ball.h")] + [os.path.join(HERE, "csrc", f) for f in ("packed.cuh", "packed_t.cuh", "ballgen.cuh", "dyn_common.cuh")]
+HDRS = [os.path.join(os.path.dirname(HERE), "include", h) for h in ("b200env.h", "b200env_v2p.h", "b200ball.h")] + [os.path.join(HERE, "csrc", f) for f in ("packed.cuh", "packed_t.cuh", "ballgen.cuh", "dyn_common.cuh", "counter_rng.cuh")]
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.environ.get("B200ENV_LIB", os.path.join(LIB_DIR, "libb200env.so"))  # override: A/B kernel variants
 # the network forwards of SURVEY.md 8f-1 (wgmma GEMMs): a library of their own, include/b200nn.h

@@ -27,6 +27,7 @@
 
 #include "../../include/b200env.h"
 #include "dyn_common.cuh"
+#include "counter_rng.cuh"
 
 #ifndef WARPS_PER_CTA
 #define WARPS_PER_CTA 8  // 8 warps x 2 CTAs/SM, barrier per substep
@@ -1713,17 +1714,12 @@ physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, co
 }
 
 // ------------------------------------------------------------------------------------------
-// reset: ref-state init from the MoCap buffer (_reset_ref_state_init :489-528, _set_env_state :741-755)
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
-reset_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf, b200_motion_lib_t ml,
-             const int64_t* __restrict__ env_ids, const float* __restrict__ times, int n) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int i = blockIdx.x * WARPS_PER_CTA + warp;
-  if (i >= n) return;
+// reset: ref-state init from the MoCap buffer (_reset_ref_state_init :489-528, _set_env_state :741-755) of env e at motion time t;
+// one warp, lane = body.  reset_kernel (id list) and reset_masked_kernel (device mask) both write their rows through it.
+__device__ __forceinline__ void reset_row(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_buffers_t& bf,
+                                          const b200_motion_lib_t& ml, int64_t e, float t, int lane) {
   const b200_model_t& M = gblob->m;
   const b200_cfg_t& cfg = *gcfg;
-  const int64_t e = env_ids[i];
-  const float t = times[i];
   const int64_t mid = bf.motion_ids[e];
   const int nd = M.nd, nbl = ml.num_lib_bodies;
   const int dof0 = lane < M.nb ? M.dof_of_body[lane] : -1;
@@ -1768,6 +1764,73 @@ reset_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ g
                 bf.motion_bodies + e * cfg.shape_dim);
 }
 
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf, b200_motion_lib_t ml,
+             const int64_t* __restrict__ env_ids, const float* __restrict__ times, int n) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int i = blockIdx.x * WARPS_PER_CTA + warp;
+  if (i >= n) return;
+  reset_row(gblob, gcfg, bf, ml, env_ids[i], times[i], lane);
+}
+
+// default init of env e (_reset_default :482-487 + humanoid_smpl.py:161-173): root row and dofs from the initial buffers, flags
+// cleared, and the raw obs of the new dofs with the rigid-body rows as they stand (the reset does not write those)
+__device__ __forceinline__ void reset_default_row(const b200_model_t& M, const b200_cfg_t& cfg, const b200_buffers_t& bf, int nbl,
+                                                  const float* __restrict__ init_root, const float* __restrict__ init_dof_pos,
+                                                  const float* __restrict__ init_dof_vel, int64_t e, int lane) {
+  const int nd = M.nd;
+  if (lane < 13) bf.root_states[e * bf.actors_per_env * 13 + lane] = init_root[e * 13 + lane];
+  for (int k = lane; k < nd; k += 32) {
+    bf.dof_state[(e * nd + k) * 2] = init_dof_pos[e * nd + k];
+    bf.dof_state[(e * nd + k) * 2 + 1] = init_dof_vel[e * nd + k];
+  }
+  if (lane == 0) { bf.progress_buf[e] = 0; bf.reset_buf[e] = 0; bf.terminate_buf[e] = 0; }
+  const bool is_body = lane < nbl;
+  const int dof0 = lane < M.nb ? M.dof_of_body[lane] : -1;
+  float rb[13] = {0.f}, dq[3] = {0.f, 0.f, 0.f}, dqd[3] = {0.f, 0.f, 0.f};
+  if (is_body) {
+    const float* row = bf.rigid_body_state + (e * bf.bodies_per_env + lane) * 13;
+#pragma unroll
+    for (int k = 0; k < 13; k++) rb[k] = row[k];
+    if (dof0 >= 0) {
+#pragma unroll
+      for (int k = 0; k < 3; k++) { dq[k] = init_dof_pos[e * nd + dof0 + k]; dqd[k] = init_dof_vel[e * nd + dof0 + k]; }
+    }
+  }
+  store_obs_raw(bf.obs_buf + e * bf.num_obs, nbl, nd, cfg.shape_dim, lane, is_body, dof0, rb, rb + 3, rb + 7, rb + 10, dq, dqd,
+                bf.motion_bodies + e * cfg.shape_dim);
+}
+
+// b200env_reset_masked, first launch: warp per env; the envs whose mask byte is set draw (counter_uniform) and are reset.  Draw 2e + 1
+// < ref_prob picks the ref-state init, at t = 0 or, with sample_time, t = u * max(length - truncate, 0) with u = draw 2e (MotionLib.
+// sample_time, motion_lib.py:138-159, in torch's float32 operation order); the other envs take the default init.  Every ref-init env
+// appends itself to the work list of the context launch.
+__device__ __forceinline__ float counter_uniform(uint64_t seed, uint64_t counter, uint64_t idx) {   // [0, 1) in 24 bits, like torch.rand
+  return (float)(uint32_t)(counter_bits(seed, counter, idx) >> 40) * (1.0f / 16777216.0f);
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_masked_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf, b200_motion_lib_t ml,
+                    int n, const uint8_t* __restrict__ mask, int sample_time, float truncate, float ref_prob, uint64_t seed,
+                    const int64_t* __restrict__ counter, const float* __restrict__ init_root, const float* __restrict__ init_dof_pos,
+                    const float* __restrict__ init_dof_vel, float* __restrict__ reset_times, int32_t* __restrict__ work) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t e = (int64_t)blockIdx.x * WARPS_PER_CTA + warp;
+  if (e >= n || !mask[e]) return;
+  const uint64_t c = (uint64_t)counter[0];
+  if (counter_uniform(seed, c, 2 * (uint64_t)e + 1) < ref_prob) {
+    float t = 0.0f;
+    if (sample_time)
+      t = __fmul_rn(counter_uniform(seed, c, 2 * (uint64_t)e), fmaxf(__fsub_rn(ml.motion_lengths[bf.motion_ids[e]], truncate), 0.0f));
+    reset_row(gblob, gcfg, bf, ml, e, t, lane);
+    if (lane == 0) {
+      reset_times[e] = t;
+      work[2 + atomicAdd(&work[0], 1)] = (int32_t)e;
+    }
+  } else {
+    reset_default_row(gblob->m, *gcfg, bf, ml.num_lib_bodies, init_root, init_dof_pos, init_dof_vel, e, lane);
+  }
+}
+
 // MotionLib.get_motion_state for arbitrary (id, time) pairs
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
 motion_state_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
@@ -1801,25 +1864,17 @@ motion_state_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restr
   if (dof_vel) for (int k = lane; k < nd; k += 32) dof_vel[i * nd + k] = ml.dvs[s.f0 * nd + k];
 }
 
-// _init_context (humanoid_smpl_im.py:530-563): the P-frame MoCap window of each listed env written straight into
-// context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos and context_mask[row, j]; warp per (env, frame).
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
-motion_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
-                      const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids, const float* __restrict__ times, int n, int P,
-                      int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp;
-  if (w >= (int64_t)n * P) return;
-  const int64_t i = w / P;
-  const int j = (int)(w - i * P);
+// _init_context (humanoid_smpl_im.py:530-563): frame j of the P-frame MoCap window of motion mid starting at motion time time0, written
+// straight into context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos and context_mask[row, j]; one warp.
+__device__ __forceinline__ void context_frame(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_motion_lib_t& ml,
+                                              int64_t mid, float time0, int64_t row, int j, int P, int first, float dt, float two_dt,
+                                              float* __restrict__ feat, uint8_t* __restrict__ mask, int lane) {
   const b200_model_t& M = gblob->m;
   const int nd = M.nd, nbl = ml.num_lib_bodies;
   const int dof0 = lane < M.nb ? M.dof_of_body[lane] : -1;
-  const int64_t mid = ids[i];
   // torch: (motion_times + dt).unsqueeze(-1) + dt * arange(first, first + P), all float32, op by op
-  const float t = __fadd_rn(__fadd_rn(times[i], dt), __fmul_rn((float)(first + j), dt));
+  const float t = __fadd_rn(__fadd_rn(time0, dt), __fmul_rn((float)(first + j), dt));
   const MotionSample s = sample_motion(ml, M, mid, t, lane, gcfg->ground_tolerance);
-  const int64_t row = env_ids ? env_ids[i] : i;
   const int W = nbl * 3 + nbl * 4 + nd + nbl * 3 + nd;
   float* o = feat + (row * P + j) * W;
   if (lane < nbl) {
@@ -1833,6 +1888,41 @@ motion_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __res
     }
   }
   if (lane == 0) mask[row * P + j] = t <= __fadd_rn(ml.motion_lengths[mid], two_dt) ? 1 : 0;
+}
+
+// the window of each listed env; warp per (env, frame)
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+motion_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                      const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids, const float* __restrict__ times, int n, int P,
+                      int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp;
+  if (w >= (int64_t)n * P) return;
+  const int64_t i = w / P;
+  const int j = (int)(w - i * P);
+  context_frame(gblob, gcfg, ml, ids[i], times[i], env_ids ? env_ids[i] : i, j, P, first, dt, two_dt, feat, mask, lane);
+}
+
+// b200env_reset_masked, second launch: the window of every env on the work list of reset_masked_kernel at its drawn time, warp per
+// (env, frame) over a grid of fixed size (the list's length is only known on the device).  The last block to finish clears the list
+// and advances the launch counter, so the pair of launches replays inside a CUDA graph with fresh draws every time.
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                     const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
+                     int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t total = (int64_t)work[0] * P;
+  for (int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp; w < total; w += (int64_t)gridDim.x * WARPS_PER_CTA) {
+    const int64_t i = w / P;
+    const int j = (int)(w - i * P);
+    const int64_t e = work[2 + i];
+    context_frame(gblob, gcfg, ml, motion_ids[e], reset_times[e], e, j, P, first, dt, two_dt, feat, mask, lane);
+  }
+  __shared__ bool last;
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(reinterpret_cast<unsigned int*>(&work[1]), 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (last && threadIdx.x == 0) { counter[0] += 1; work[0] = 0; work[1] = 0; __threadfence(); }
 }
 
 // compute_humanoid_observations_imitation (humanoid_smpl_im.py:773-850): warp per env, lane per body
@@ -2513,6 +2603,34 @@ int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_
                                                                       motion_times, n);
   CUDA_OK(cudaGetLastError());
   h->launches++;
+  return 0;
+}
+
+int b200env_reset_masked(b200env_handle h, const uint8_t* mask, int32_t sample_time, float truncate, float ref_prob, uint64_t seed,
+                         int64_t* counter, const float* init_root, const float* init_dof_pos, const float* init_dof_vel, float* reset_times,
+                         int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, int32_t* work,
+                         void* stream) {
+  if (!h) return fail(-1, "b200env_reset_masked: null handle%s");
+  if (!mask || !counter || !reset_times || !context_feat || !context_mask || !work || num_frames < 1)
+    return fail(-1, "b200env_reset_masked: bad arguments%s");
+  if (ref_prob < 1.0f && (!init_root || !init_dof_pos || !init_dof_vel))
+    return fail(-1, "b200env_reset_masked: ref_prob < 1 needs the initial root and dof buffers%s");
+  if (!h->bound || !h->has_ml) return fail(-4, "b200env_reset_masked: bind buffers and a motion lib first%s");
+  cudaSetDevice(h->device);
+  const int n = h->num_envs;
+  reset_masked_kernel<<<(n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+      (const DevBlob*)h->d_blob, h->d_cfg, h->bufs, h->ml, n, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos,
+      init_dof_vel, reset_times, work);
+  CUDA_OK(cudaGetLastError());
+  int sms = 0;
+  CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+  const int64_t warps = (int64_t)n * num_frames;
+  const int grid = (int)std::min<int64_t>((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (int64_t)sms * 8);
+  reset_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
+                                                                              reset_times, work, counter, num_frames, first_frame, dt,
+                                                                              (float)(2.0 * (double)dt), context_feat, context_mask);
+  CUDA_OK(cudaGetLastError());
+  h->launches += 2;
   return 0;
 }
 

@@ -15,6 +15,7 @@
 #include <stdio.h>
 
 #include "../../include/b200env_v2p.h"
+#include "counter_rng.cuh"
 
 #define FULL 0xffffffffu
 #define V2P_WARPS 4
@@ -720,14 +721,8 @@ __global__ void ctrl_reset_kernel(int n, const uint8_t* __restrict__ mask, int64
 // by residual_dof_scale.  The normal deviates come from a counter-based generator (splitmix64 of seed, step counter, element index +
 // Box-Muller) so that the step needs no separate RNG launch; the step counter lives on the device and is advanced by the last
 // block to finish, which keeps the launch replayable inside a CUDA graph.
-__device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
-  x += 0x9E3779B97F4A7C15ull;
-  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-  return x ^ (x >> 31);
-}
 __device__ __forceinline__ float counter_normal(uint64_t seed, uint64_t step, uint64_t idx) {
-  const uint64_t h = splitmix64(splitmix64(seed ^ (step * 0xD1B54A32D192ED03ull)) + idx);
+  const uint64_t h = counter_bits(seed, step, idx);
   const float u1 = ((uint32_t)(h >> 40) + 1u) * (1.0f / 16777217.0f);     // (0, 1)
   const float u2 = (uint32_t)((h >> 8) & 0xFFFFFFu) * (1.0f / 16777216.0f);
   return sqrtf(-2.0f * logf(u1)) * cosf(6.283185307179586f * u2);

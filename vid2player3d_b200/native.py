@@ -15,7 +15,7 @@ SYMBOLS = ["b200env_abi_version", "b200env_last_error", "b200env_create", "b200e
            "b200env_set_motion_lib", "b200env_step", "b200env_reset", "b200env_motion_state", "b200env_obs_imitation",
            "b200env_physics_only", "b200env_launch_count", "b200env_set_env_slice", "b200env_motion_context", "b200env_set_kernel_timing",
            "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form",
-           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan"]
+           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan", "b200env_reset_masked"]
 
 ENVS_PER_BATCH = 32   # envs per CTA batch of the default physics launch (step_kernel_packed<true>): the batch size of the asset plan
 
@@ -156,6 +156,20 @@ class Env:
         n = int(env_ids.shape[0])
         if n:
             _check(lib().b200env_reset(self._h, _ptr(env_ids), _ptr(motion_times), C.c_int32(n), _stream()))
+
+    def reset_masked(self, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos, init_dof_vel, reset_times,
+                     num_frames, first_frame, dt, feat, feat_mask, work):
+        """reset of the envs whose mask [N] bool is set, context window included (include/b200env.h: b200env_reset_masked)"""
+        import torch
+        assert mask.dtype == torch.bool and counter.dtype == torch.int64 and work.dtype == torch.int32
+        assert mask.shape[0] == self.num_envs and work.shape[0] >= self.num_envs + 2
+        for t in (mask, counter, init_root, init_dof_pos, init_dof_vel, reset_times, feat, feat_mask, work):
+            assert t is None or (t.is_cuda and t.is_contiguous())
+        _check(lib().b200env_reset_masked(self._h, _ptr(mask), C.c_int32(int(bool(sample_time))), C.c_float(float(truncate)),
+                                          C.c_float(float(ref_prob)), C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), _ptr(counter),
+                                          _ptr(init_root), _ptr(init_dof_pos), _ptr(init_dof_vel), _ptr(reset_times),
+                                          C.c_int32(int(num_frames)), C.c_int32(int(first_frame)), C.c_float(float(dt)), _ptr(feat),
+                                          _ptr(feat_mask), _ptr(work), _stream()))
 
     def motion_state(self, ids, times, out):
         """out: dict name -> tensor or None for root_pos, root_rot, dof_pos, root_vel, root_ang_vel, dof_vel, key_pos,

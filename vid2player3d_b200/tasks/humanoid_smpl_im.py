@@ -242,6 +242,11 @@ class HumanoidSMPLIM(BaseTask):
         self._prev_target_rb_pos, self._prev_target_rb_rot = f(N, nbl, 3), f(N, nbl, 4)
         self._pd_target_dof_pos = f(N, D)
         self.actions = f(N, self._num_actions)
+        # reset_masked / reset_done: draw counter, work list of the context launch, mask of the finished envs, captured reset graph
+        self._reset_rng = torch.zeros(1, device=dev, dtype=torch.long)
+        self._reset_work = torch.zeros(N + 2, device=dev, dtype=torch.int32)
+        self._reset_mask = torch.zeros(N, device=dev, dtype=torch.bool)
+        self._reset_graph = None
         t = dict(root_states=self._root_states, dof_state=self._dof_state, rigid_body_state=self._rigid_body_state,
                  contact_forces=self._contact_force_tensor, obs_buf=self.obs_buf, rew_buf=self.rew_buf,
                  sub_rewards=self._sub_rewards, reset_buf=self.reset_buf, progress_buf=self.progress_buf,
@@ -348,9 +353,65 @@ class HumanoidSMPLIM(BaseTask):
         self._reset_ref_env_ids = env_ids
         self._init_context(env_ids, motion_ids, motion_times)
 
-    def _init_context(self, env_ids, motion_ids, motion_times):
-        """:530-563: 48-frame MoCap window per env -> context_feat / context_mask (one launch)."""
-        n = len(env_ids)
+    def reset_masked(self, mask):
+        """Addition (not in the reference): `reset(mask.nonzero())` without the id list - the envs whose entry of `mask` ([num_envs]
+        bool, device) is set are reset by two launches (include/b200env.h: b200env_reset_masked) that make no host synchronisation,
+        so the call can be captured in a CUDA graph.  Same state init, rows and context window as `reset(env_ids)`; the motion
+        times and the Hybrid choice are drawn on the device from a counter-based generator seeded by cfg["seed"], a different stream
+        of the same distribution as the torch.rand / torch.bernoulli draws of `reset(env_ids)`.  Not with cfg.env.transform_specs
+        (its transforms of the window are torch ops on the reset rows): use `reset(env_ids)` there."""
+        if self._transform_specs is not None:
+            raise ValueError("reset_masked: cfg.env.transform_specs transforms the context window in torch - use reset(env_ids)")
+        modes = {"Start": (False, 1.0), "Random": (True, 1.0), "Hybrid": (True, min(float(self._hybrid_init_prob), 1.0)),
+                 "Default": (False, 0.0)}
+        if self._state_init not in modes:
+            raise ValueError(f"Unsupported state initialization strategy: {self._state_init}")
+        sample_time, ref_prob = modes[self._state_init]
+        truncate = self.context_length * self.dt if self.truncate_time else 0.0
+        self._context_buffers()
+        self._env.reset_masked(mask, sample_time, truncate, ref_prob, self.cfg.get("seed", 10), self._reset_rng,
+                               self._initial_humanoid_root_states, self._initial_dof_pos, self._initial_dof_vel, self._reset_ref_motion_times,
+                               self.context_length + self.context_padding * 2, -self.context_padding, self.dt, self.context_feat,
+                               self.context_mask, self._reset_work)
+        self._forward_context()
+
+    def reset_done(self):
+        """Addition: reset the envs whose reset_buf is set, from the device flags: the mask is taken with torch.ne and the reset is
+        one replay of the reset graph when one was captured (VecTaskPython.enable_cuda_graph(reset_graph=True)), else `reset_masked`.
+        No host synchronisation.  With cfg.env.transform_specs: `reset(reset_buf.nonzero())`."""
+        if self._transform_specs is not None:
+            self.reset(self.reset_buf.nonzero(as_tuple=False).flatten())
+            return
+        torch.ne(self.reset_buf, 0, out=self._reset_mask)
+        if self._reset_graph is not None:
+            self._reset_graph.replay()
+        else:
+            self.reset_masked(self._reset_mask)
+
+    def _capture_reset_graph(self, tail=None):
+        """capture `reset_masked(self._reset_mask)` and then `tail()` as the graph `reset_done` replays (warm-up: one eager call with an
+        empty mask, which only advances the draw counter); nothing with cfg.env.transform_specs.  Returns whether a graph was captured."""
+        if self._transform_specs is not None:
+            return False
+        self._reset_graph = None
+        self._reset_mask.zero_()
+        s = torch.cuda.Stream(device=self.device)
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            self.reset_masked(self._reset_mask)
+            if tail is not None:
+                tail()
+        torch.cuda.current_stream().wait_stream(s)
+        torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            self.reset_masked(self._reset_mask)
+            if tail is not None:
+                tail()
+        self._reset_graph = g
+        return True
+
+    def _context_buffers(self):
         P = self.context_length + self.context_padding * 2
         nbl, D = self._num_lib_bodies, self.num_dof
         W = 2 * (3 * nbl + D) + 4 * nbl
@@ -359,11 +420,19 @@ class HumanoidSMPLIM(BaseTask):
             self.context_feat = torch.zeros(self.num_envs, P, W + (nbl if with_conf else 0), device=self.device)
             self.context_mask = torch.zeros(self.num_envs, P, device=self.device, dtype=torch.bool)
             self._context_raw = torch.zeros(self.num_envs, P, W, device=self.device) if with_conf else self.context_feat
+        return P, with_conf
+
+    def _init_context(self, env_ids, motion_ids, motion_times):
+        """:530-563: 48-frame MoCap window per env -> context_feat / context_mask (one launch)."""
+        P, with_conf = self._context_buffers()
         env_ids = env_ids.to(self.device, dtype=torch.long).contiguous()
         self._env.motion_context(env_ids, motion_ids.contiguous(), motion_times.contiguous(),
                                  P, -self.context_padding, self.dt, self._context_raw, self.context_mask)
         if with_conf:
             self.context_feat[env_ids] = self._transform_target(self._context_raw[env_ids])
+        self._forward_context()
+
+    def _forward_context(self):
         if self.model is not None:
             if not self.is_env_dim_setup:
                 self.model.a2c_network.setup_env_named_dims(self.obs_names, self.obs_shapes, self.obs_dims,

@@ -69,14 +69,16 @@ class VecTaskPython(VecTask):
         return (torch.clamp(self.task.obs_buf, -self.clip_obs, self.clip_obs).to(self.rl_device),
                 self.task.rew_buf.to(self.rl_device), self.task.reset_buf.to(self.rl_device), self.task.extras)
 
-    def enable_cuda_graph(self, actions=None, warmup=3):
+    def enable_cuda_graph(self, actions=None, warmup=3, reset_graph=False):
         """Addition (not in the reference): capture `clamp(actions) -> task.step -> clamp(obs)` - 1 memset + 5 kernels - into
         one CUDA graph; `step()` then costs one graph launch on the host instead of ~8 launches through PyTorch and ctypes.
         `actions`: the device tensor the caller will keep passing (its storage becomes the graph's input; any other tensor is
         copied into it first).  The returned observation tensor is a fixed buffer, overwritten by the next step (the reference
         returns a fresh clamp() result; rl_games copies it into its own rollout storage before stepping again).
         Valid while rl_device == the task's device and the task's step makes no host synchronisation (true for the env step).
-        The warm-up runs a few real env steps: call it before the reset() that starts a rollout."""
+        The warm-up runs a few real env steps: call it before the reset() that starts a rollout.
+        reset_graph=True (tasks with `reset_masked`, e.g. HumanoidSMPLIM): also capture `task.reset_masked(mask of the finished envs)
+        -> clamp(obs)` as a second graph, which `reset_done()` replays (not with cfg.env.transform_specs: that reset stays eager)."""
         assert str(self.rl_device) == str(self.task.device), "graph capture needs rl_device == sim device"
         dev = self.task.device
         self._graph = None
@@ -95,6 +97,10 @@ class VecTaskPython(VecTask):
             self.task.step(torch.clamp(self._graph_actions, -self.clip_actions, self.clip_actions))
             torch.clamp(self.task.obs_buf, -self.clip_obs, self.clip_obs, out=self._graph_obs)
         self._graph = g
+        if reset_graph:
+            self._reset_obs = torch.empty_like(self.task.obs_buf)
+            self._reset_obs_in_graph = self.task._capture_reset_graph(
+                lambda: torch.clamp(self.task.obs_buf, -self.clip_obs, self.clip_obs, out=self._reset_obs))
         return self._graph_actions
 
     def reset(self):
@@ -111,3 +117,14 @@ class VecTaskPythonWrapper(VecTaskPython):
     def reset(self, env_ids=None):
         self.task.reset(env_ids)
         return torch.clamp(self.task.obs_buf, -self.clip_obs, self.clip_obs).to(self.rl_device)
+
+    def reset_done(self):
+        """Addition: `reset(reset_buf.nonzero())` from the device flags (task.reset_done: no host synchronisation unless the task has
+        cfg.env.transform_specs).  Returns the clamped observations in a fixed buffer, overwritten by the next reset_done(); with
+        enable_cuda_graph(reset_graph=True) the reset and the clamp are one graph replay after the mask launch."""
+        self.task.reset_done()
+        if not getattr(self, "_reset_obs_in_graph", False):
+            if getattr(self, "_reset_obs", None) is None:
+                self._reset_obs = torch.empty_like(self.task.obs_buf)
+            torch.clamp(self.task.obs_buf, -self.clip_obs, self.clip_obs, out=self._reset_obs)
+        return self._reset_obs
