@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 6
+#define B200_ABI_VERSION 7
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:
@@ -266,9 +266,14 @@ int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int3
  * motion's body: embodied_pose/env/tasks/humanoid_smpl_im.py:231-351, PD gains scaled by that actor's mass :356-389).  models [num_assets]
  * and verts [num_assets] (verts[a]: [nb][models[a].vmax][3]) are HOST arrays; env e is simulated with asset env_asset[e] for the
  * handle's lifetime.  Every asset must have asset 0's topology (nb, nd, max_depth, parent, depth, fixed, dof_of_body); vmax, the
- * vertices and every numeric field may differ.  The physics launch hands out the batches of b200env_plan_assets (at most 32 envs of
- * one asset each) and re-stages the asset's header in shared memory when a CTA moves to a batch of another asset; every other launch
- * reads the topology only.  Not supported with several assets (refused with an error): cfg.has_ball, the non-default kernel forms
+ * vertices and every numeric field may differ.  The physics launch runs one of two plans:
+ *  - grouped (b200env_plan_assets): batches of at most 32 envs of one asset each; a CTA re-stages the asset's header in shared memory
+ *    when it moves to a batch of another asset;
+ *  - mixed (b200env_plan_assets_mixed): batches of 32 consecutive envs whatever their assets; each env's lanes read the numeric
+ *    constants and hull vertices of its own asset from global memory.
+ * The mixed plan runs exactly when it takes fewer rounds of the persistent grid (b200env_choose_asset_plan with the grid of
+ * b200env_physics_launch_shape); the environment variable B200ENV_ASSET_PLAN=grouped|mixed overrides that rule for A/B measurements
+ * and tests.  The results of both plans are bit-identical.  Every other launch reads the topology only.  Not supported with several assets (refused with an error): cfg.has_ball, the non-default kernel forms
  * (B200ENV_KERNEL=lane|tmem|packed3, B200ENV_SPLIT=0, B200ENV_SORT=1), b200env_set_env_slice, b200env_set_hull_faces and
  * b200env_physics_only. */
 int b200env_create_assets(const b200_model_t* models, const float* const* verts, int32_t num_assets, const int32_t* env_asset,
@@ -281,11 +286,22 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
 int b200env_plan_assets(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t envs_per_batch, int32_t* rows,
                         int32_t* batch_asset, int32_t* batch_first, int32_t* batch_count, int32_t* num_batches);
 
-/* The plan a handle of b200env_create_assets runs (batch b runs in round b / grid of b200env_physics_launch_shape).  Array
- * arguments may be NULL (query the sizes first: rows has num_envs entries, the batch arrays *num_batches).  Fails on a handle of
- * b200env_create. */
+/* The mixed batch plan of b200env_create_assets, host only, same arguments and outputs as b200env_plan_assets: rows = 0 .. num_envs-1
+ * (ascending env index, whatever the asset), batch i covers rows [i * envs_per_batch, ...) up to envs_per_batch of them;
+ * batch_asset[i] = the asset of its envs when they all have one, else -1.  ceil(num_envs / envs_per_batch) batches. */
+int b200env_plan_assets_mixed(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t envs_per_batch, int32_t* rows,
+                              int32_t* batch_asset, int32_t* batch_first, int32_t* batch_count, int32_t* num_batches);
+
+/* The plan rule of b200env_create_assets, host only: *mixed = 1 when ceil(ceil(num_envs / B) / grid) < ceil(sum_a ceil(n_a / B) / grid),
+ * i.e. when the mixed plan takes fewer rounds of a persistent grid of `grid` CTAs than the grouped plan (B = 32 envs per batch in
+ * both, n_a = envs of asset a), else 0. */
+int b200env_choose_asset_plan(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t grid, int32_t* mixed);
+
+/* The plan a handle of b200env_create_assets runs (batch b runs in round b / grid of b200env_physics_launch_shape); *mixed = 1 for
+ * the mixed plan, 0 for the grouped one.  Array arguments and mixed may be NULL (query the sizes first: rows has num_envs entries,
+ * the batch arrays *num_batches).  Fails on a handle of b200env_create. */
 int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batches, int32_t* rows, int32_t* batch_asset,
-                       int32_t* batch_first, int32_t* batch_count);
+                       int32_t* batch_first, int32_t* batch_count, int32_t* mixed);
 
 /* number of kernels launched by this handle so far (bench.py "gpu_launches") */
 int64_t b200env_launch_count(b200env_handle h);

@@ -91,6 +91,10 @@ struct b200env {
   int4* d_batches;                     // [num_batches] {asset, first position in d_rows, count, 0}
   int num_batches;
   std::vector<int32_t>* plan;          // host copy: rows [num_envs] | asset, first, count [num_batches] each
+  // the mixed plan (b200env_plan_assets_mixed, chosen by asset_plan_choice): batches of consecutive envs whatever their assets, run
+  // by step_kernel_packed<true, false, true>; d_env_blob[e] = env e's asset header in d_assets (d_rows / d_batches stay unset)
+  int mixed;
+  const DevBlob** d_env_blob;
 };
 
 static thread_local char g_err[512] = "";
@@ -1092,7 +1096,12 @@ __host__ __device__ constexpr int pk_launch_warps(bool split) { return pk_warps(
 // MULTI = true (split form only): several assets of one topology in the launch (b200env_create_assets).  The ticket hands out
 // entries of the batch table `batches` ({asset, first position in the row order `perm`, count <= BATCH, 0}); a CTA whose batch has
 // another asset than the header in its shared memory copies that asset's header (assets[asset]) over it first.  gblob = assets[0].
-template <bool SPLIT, bool MULTI = false>
+// MIXED = true (split form only): a CTA batch may hold envs of different assets of one topology (the mixed plan of
+// b200env_create_assets).  Batches are handed out as in the one-asset launch (consecutive envs, identity order).  The header in shared
+// memory is asset 0's and only its topology is used; each lane reads the numeric constants and the hull vertices of its own env's
+// asset from that asset's header in global memory, assets[e] for env e, through L1.  The per-env rows stay out of shared memory because
+// they would not fit next to 32 envs of records (DESIGN.md 5).
+template <bool SPLIT, bool MULTI = false, bool MIXED = false>
 __global__ void __launch_bounds__(PK_BOUND(SPLIT) * 32, 1)
 step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf,
                    b200_motion_lib_t ml, const float* __restrict__ actions, int num_envs, unsigned long long* __restrict__ ticket,
@@ -1131,6 +1140,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #define PK_GROUPS 1   // 2 measured 1.5 % slower (343 vs 338 us): mixing the phases costs more I-cache than it hides latency
 #endif
   static_assert(!MULTI || (SPLIT && PK_GROUPS == 1 && !PK_WARP_TICKETS), "several assets: split form, one group of warps per CTA");
+  static_assert(!MIXED || (SPLIT && !MULTI && !PK_SHADOW), "mixed batches: split form, one plan");
   constexpr int G0 = PK_GROUPS == 1 ? PK_WARPS_K : (PK_WARPS_K + 1) / 2;   // warps in group 0
   const int grp = warp < G0 ? 0 : 1;
   const int gw0 = grp == 0 ? 0 : G0, gwn = grp == 0 ? G0 : PK_WARPS_K - G0;   // first warp / number of warps of my group
@@ -1233,7 +1243,12 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
     ball_clear(ball);
     const int64_t erow_g = SPLIT ? row(valid ? eb + g : eb) : env_first + (int64_t)env_stride * (eb + g);
     if (cfg.has_ball && valid && s == BALL_SLOT) ball_load(bf, erow_g, ball);
-    if (ABL != 1) control_step_packed<float>(B, verts, pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
+    if constexpr (MIXED) {
+      const DevBlob* an = assets[valid ? eb + g : eb];   // my env's asset (a lane without an env: the warp's first env's, never stored)
+      if (ABL != 1) control_step_packed<float>(B, an->m, reinterpret_cast<const float*>(an + 1), pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
+    } else {
+      if (ABL != 1) control_step_packed<float>(B, verts, pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
+    }
 #if POST_SYNC
     // fused form only: re-aligns the warps before the long straight-line epilogue (I-cache).  The split form's epilogue is a
     // state write-back and goes without it.
@@ -2242,7 +2257,7 @@ int b200env_destroy(b200env_handle h) {
   cudaFree(h->d_ticket);
   cudaFree(h->d_ext);
   cudaFree(h->d_bin); cudaFree(h->d_perm); cudaFree(h->d_pos); cudaFree(h->d_cnt);
-  cudaFree(h->d_assets); cudaFree(h->d_asset_ptr); cudaFree(h->d_rows); cudaFree(h->d_batches);
+  cudaFree(h->d_assets); cudaFree(h->d_asset_ptr); cudaFree(h->d_rows); cudaFree(h->d_batches); cudaFree(h->d_env_blob);
   delete h->plan;
   if (h->tev) { for (cudaEvent_t e : *h->tev) cudaEventDestroy(e); delete h->tev; }
   delete h;
@@ -2275,6 +2290,50 @@ int b200env_plan_assets(const int32_t* env_asset, int32_t num_envs, int32_t num_
   return 0;
 }
 
+int b200env_plan_assets_mixed(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t envs_per_batch, int32_t* rows,
+                              int32_t* batch_asset, int32_t* batch_first, int32_t* batch_count, int32_t* num_batches) {
+  if (!env_asset || !rows || !batch_asset || !batch_first || !batch_count || !num_batches) return fail(-1, "b200env_plan_assets_mixed: null argument%s");
+  if (num_envs < 1) return fail(-2, "b200env_plan_assets_mixed: num_envs must be positive%s");
+  if (num_assets < 1) return fail(-2, "b200env_plan_assets_mixed: num_assets must be at least 1%s");
+  if (envs_per_batch < 1) return fail(-2, "b200env_plan_assets_mixed: envs_per_batch must be positive%s");
+  for (int e = 0; e < num_envs; e++) {
+    if (env_asset[e] < 0 || env_asset[e] >= num_assets) return fail(-2, "b200env_plan_assets_mixed: env_asset out of range [0, num_assets)%s");
+    rows[e] = e;
+  }
+  int nbat = 0;
+  for (int p = 0; p < num_envs; p += envs_per_batch) {
+    const int cnt = num_envs - p < envs_per_batch ? num_envs - p : envs_per_batch;
+    int a = env_asset[p];
+    for (int e = p + 1; e < p + cnt; e++) if (env_asset[e] != a) a = -1;
+    batch_asset[nbat] = a;
+    batch_first[nbat] = p;
+    batch_count[nbat] = cnt;
+    nbat++;
+  }
+  *num_batches = nbat;
+  return 0;
+}
+
+int b200env_choose_asset_plan(const int32_t* env_asset, int32_t num_envs, int32_t num_assets, int32_t grid, int32_t* mixed) {
+  if (!env_asset || !mixed) return fail(-1, "b200env_choose_asset_plan: null argument%s");
+  if (num_envs < 1) return fail(-2, "b200env_choose_asset_plan: num_envs must be positive%s");
+  if (num_assets < 1) return fail(-2, "b200env_choose_asset_plan: num_assets must be at least 1%s");
+  if (grid < 1) return fail(-2, "b200env_choose_asset_plan: grid must be positive%s");
+  const int64_t batch = pk_warps(true) * EPW;   // both plans: the envs per CTA batch of step_kernel_packed<true, ...>
+  std::vector<int64_t> n_a(num_assets, 0);
+  for (int e = 0; e < num_envs; e++) {
+    if (env_asset[e] < 0 || env_asset[e] >= num_assets) return fail(-2, "b200env_choose_asset_plan: env_asset out of range [0, num_assets)%s");
+    n_a[env_asset[e]]++;
+  }
+  int64_t grouped = 0;   // the batch count of b200env_plan_assets
+  for (int a = 0; a < num_assets; a++) grouped += (n_a[a] + batch - 1) / batch;
+  const int64_t mixed_batches = (num_envs + batch - 1) / batch;
+  *mixed = (mixed_batches + grid - 1) / grid < (grouped + grid - 1) / grid ? 1 : 0;
+  return 0;
+}
+
+static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out);
+
 int b200env_create_assets(const b200_model_t* models, const float* const* verts, int32_t num_assets, const int32_t* env_asset,
                           const b200_cfg_t* cfg, int32_t num_envs, int32_t device, b200env_handle* out) {
   if (!models || !verts || !env_asset || !cfg || !out) return fail(-1, "b200env_create_assets: null argument%s");
@@ -2303,6 +2362,9 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   const char* so = getenv("B200ENV_SORT");
   if ((kv && strcmp(kv, "packed") != 0) || (sv && strcmp(sv, "0") == 0) || (so && strcmp(so, "1") == 0))
     return fail(-2, "b200env_create_assets: several assets run in the default kernel form only (unset B200ENV_KERNEL, B200ENV_SPLIT, B200ENV_SORT)%s");
+  const char* pv = getenv("B200ENV_ASSET_PLAN");   // A/B and tests: run this plan instead of the one the rule chooses
+  if (pv && strcmp(pv, "grouped") != 0 && strcmp(pv, "mixed") != 0)
+    return fail(-2, "b200env_create_assets: B200ENV_ASSET_PLAN must be grouped or mixed%s");
   // the planner and its outputs: rows | asset | first | count (at most one batch per env)
   std::vector<int32_t>* plan = new std::vector<int32_t>((size_t)num_envs * 4);
   int32_t nbat = 0;
@@ -2348,6 +2410,34 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   for (int a = 0; a < num_assets; a++) ptr[a] = reinterpret_cast<const DevBlob*>(static_cast<unsigned char*>(h->d_assets) + off[a]);
   CUDA_OK_H(cudaMalloc(&h->d_asset_ptr, sizeof(const DevBlob*) * num_assets));
   CUDA_OK_H(cudaMemcpy(h->d_asset_ptr, ptr.data(), sizeof(const DevBlob*) * num_assets, cudaMemcpyHostToDevice));
+  // the plan: the mixed one exactly when it takes fewer rounds of the persistent grid than the grouped one
+  int32_t mixed = pv ? strcmp(pv, "mixed") == 0 : 0;
+  if (!pv) {
+    size_t psmem;
+    int bsz;
+    CUDA_OK_H(cudaSetDevice(h->device));
+    rc = physics_launch_config(h, &psmem, &bsz);   // the grid (resident CTA slots); computed again below for the chosen plan
+    if (!rc) rc = b200env_choose_asset_plan(env_asset, num_envs, num_assets, h->step_slots, &mixed);
+    if (rc) { b200env_destroy(h); return rc; }
+    h->step_slots = 0;
+  }
+  if (mixed) {
+    plan->assign((size_t)num_envs * 4, 0);
+    P = plan->data();
+    rc = b200env_plan_assets_mixed(env_asset, num_envs, num_assets, batch, P, P + num_envs, P + 2 * (size_t)num_envs, P + 3 * (size_t)num_envs, &nbat);
+    if (rc) { b200env_destroy(h); return rc; }
+    std::copy(P + 2 * (size_t)num_envs, P + 2 * (size_t)num_envs + nbat, P + num_envs + nbat);
+    std::copy(P + 3 * (size_t)num_envs, P + 3 * (size_t)num_envs + nbat, P + num_envs + 2 * nbat);
+    plan->resize((size_t)num_envs + 3 * nbat);
+    h->num_batches = nbat;
+    h->mixed = 1;
+    std::vector<const DevBlob*> eb(num_envs);
+    for (int e = 0; e < num_envs; e++) eb[e] = ptr[env_asset[e]];
+    CUDA_OK_H(cudaMalloc(&h->d_env_blob, sizeof(const DevBlob*) * num_envs));
+    CUDA_OK_H(cudaMemcpy(h->d_env_blob, eb.data(), sizeof(const DevBlob*) * num_envs, cudaMemcpyHostToDevice));
+    *out = h;
+    return 0;
+  }
   CUDA_OK_H(cudaMalloc(&h->d_rows, sizeof(int32_t) * num_envs));
   CUDA_OK_H(cudaMemcpy(h->d_rows, P, sizeof(int32_t) * num_envs, cudaMemcpyHostToDevice));
   CUDA_OK_H(cudaMalloc(&h->d_batches, sizeof(int4) * nbat));
@@ -2358,9 +2448,10 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
 }
 
 int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batches, int32_t* rows, int32_t* batch_asset, int32_t* batch_first,
-                       int32_t* batch_count) {
+                       int32_t* batch_count, int32_t* mixed) {
   if (!h || !num_assets || !num_batches) return fail(-1, "b200env_asset_plan: null argument%s");
   if (!h->num_assets) return fail(-2, "b200env_asset_plan: not a handle of b200env_create_assets%s");
+  if (mixed) *mixed = h->mixed;
   *num_assets = h->num_assets;
   *num_batches = h->num_batches;
   const int32_t* P = h->plan->data();
@@ -2484,7 +2575,10 @@ static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out) 
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed3, PK3_WARPS * 32, psmem));
       } else
 #endif
-      if (h->num_assets) {
+      if (h->mixed) {
+        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
+        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true, false, true>, pk_launch_warps(true) * 32, psmem));
+      } else if (h->num_assets) {
         CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
         CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true, true>, pk_launch_warps(true) * 32, psmem));
       } else
@@ -2560,7 +2654,11 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
       else
 #endif
-      if (h->num_assets)
+      if (h->mixed)
+        step_kernel_packed<true, false, true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
+            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext,
+            nullptr, h->d_env_blob);
+      else if (h->num_assets)
         step_kernel_packed<true, true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
             (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext,
             h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);

@@ -145,15 +145,17 @@ __device__ __forceinline__ void pk_pd_park(const DevBlob& B, T* env, int s, bool
 
 // kinematics of one body from its parent's record.  JOINT_IN_REGS: the caller (forward pass) just produced the body's joint
 // rotation / velocity and hands them over in registers (they are already in the record, this only saves the reload).
+// B: the topology (tree tables, parent, fixed); MN: the model whose numeric constants (here the joint offset) the body uses - B.m
+// itself, or in a batch of mixed assets (step_kernel_packed<true, false, true>) the env's own asset.
 template <typename T, bool WITH_ZETA, bool JOINT_IN_REGS = false>
-__device__ __forceinline__ void pk_fk(const DevBlob& B, T* env, int b, const T* qj_in = nullptr, const T* wt_in = nullptr) {
+__device__ __forceinline__ void pk_fk(const DevBlob& B, const b200_model_t& MN, T* env, int b, const T* qj_in = nullptr, const T* wt_in = nullptr) {
   const b200_model_t& M = B.m;
   T* rec = env + RIX(B, b) * REC;
   const T* par = env + RIX(B, M.parent[b]) * REC;
   T ps[13];  // parent Q[4] p[3] w[3] v[3]
   ldr<R_Q, 13>(par, ps);
   const T *pQ = ps, *pp = ps + 4, *pw = ps + 7, *pv = ps + 10;
-  T off[3] = {T(M.offset[b][0]), T(M.offset[b][1]), T(M.offset[b][2])}, rr[3], wxr[3];
+  T off[3] = {T(MN.offset[b][0]), T(MN.offset[b][1]), T(MN.offset[b][2])}, rr[3], wxr[3];
   T o[16];   // own Q[4] p[3] w[3] v[3] wt[3]
   qrot(pQ, off, rr);
   cross3(pw, rr, wxr);
@@ -193,6 +195,10 @@ __device__ __forceinline__ void pk_fk(const DevBlob& B, T* env, int b, const T* 
     }
   }
 }
+template <typename T, bool WITH_ZETA, bool JOINT_IN_REGS = false>
+__device__ __forceinline__ void pk_fk(const DevBlob& B, T* env, int b, const T* qj_in = nullptr, const T* wt_in = nullptr) {
+  pk_fk<T, WITH_ZETA, JOINT_IN_REGS>(B, B.m, env, b, qj_in, wt_in);
+}
 
 // rigid-body inertia + bias + external / contact / joint-drive terms of one dynamic body -> record
 // DEFER_CONTACT (PK_CONTACT_COMPACT): only the penetration mask of the hull is computed here and left in the record (in the two
@@ -203,10 +209,11 @@ template <> __device__ __forceinline__ double pk_bits_to_slot<double>(uint32_t x
 __device__ __forceinline__ uint32_t pk_slot_to_bits(float f) { uint32_t x; memcpy(&x, &f, 4); return x; }
 __device__ __forceinline__ uint32_t pk_slot_to_bits(double d) { return (uint32_t)d; }
 
-// pd: the body's PD target (from the lane's registers, pk_pd_pick)
+// pd: the body's PD target (from the lane's registers, pk_pd_pick).  MN / verts: the numeric constants and hull vertices of the
+// body's model (see pk_fk); B: the topology.
 template <typename T, bool DEFER_CONTACT = false>
-__device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c, T* env, int b, bool ext_on,
-                                        const T* pd) {
+__device__ __forceinline__ void pk_body(const DevBlob& B, const b200_model_t& MN, const float* __restrict__ verts, const PhysCfg<T>& c, T* env,
+                                        int b, bool ext_on, const T* pd) {
   const b200_model_t& M = B.m;
   T* rec = env + RIX(B, b) * REC;
   T own[16], R[9];   // Q[4] p[3] w[3] v[3] wt[3]
@@ -217,13 +224,13 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
   T *A = ab, *Bm = ab + 6, *C = ab + 15, *bn = ab + 21, *bf = ab + 24, cf[3] = {0, 0, 0};
 #pragma unroll
   for (int k = 6; k < 21; k++) ab[k] = T(0);
-  const T ms = T(M.mass[b]);
-  T cl[3] = {T(M.com[b][0]), T(M.com[b][1]), T(M.com[b][2])}, cw[3];
+  const T ms = T(MN.mass[b]);
+  T cl[3] = {T(MN.com[b][0]), T(MN.com[b][1]), T(MN.com[b][2])}, cw[3];
   mv3(R, cl, cw);
   {
     T Ib[6], F[9], RF[9];
 #pragma unroll
-    for (int k = 0; k < 6; k++) Ib[k] = T(M.inertia[b][k]);
+    for (int k = 0; k < 6; k++) Ib[k] = T(MN.inertia[b][k]);
     sym_full(Ib, F);
 #pragma unroll
     for (int i = 0; i < 3; i++)
@@ -264,14 +271,14 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
 #pragma unroll
     for (int k = 0; k < 3; k++) { bn[k] -= ext[3 + k] + cxF[k]; bf[k] -= eF[k]; }
   }
-  const int nv = ABL == 6 ? 0 : M.nverts[b];
+  const int nv = ABL == 6 ? 0 : MN.nverts[b];
   if (DEFER_CONTACT) {
     unsigned long long mask = 0ull;
-    if (nv > 0 && p[2] - T(M.radius[b]) < T(0)) mask = contact_mask<T>(verts + (size_t)b * M.vmax * 3, M.vmax, nv, R, p);
+    if (nv > 0 && p[2] - T(MN.radius[b]) < T(0)) mask = contact_mask<T>(verts + (size_t)b * MN.vmax * 3, MN.vmax, nv, R, p);
     cf[1] = pk_bits_to_slot<T>((uint32_t)mask);
     cf[2] = pk_bits_to_slot<T>((uint32_t)(mask >> 32));
-  } else if (nv > 0 && p[2] - T(M.radius[b]) < T(0)) {
-    contact_hull<T>(verts + (size_t)b * M.vmax * 3, M.vmax, nv, c, R, p, v, w, A, Bm, C, bn, bf, cf);
+  } else if (nv > 0 && p[2] - T(MN.radius[b]) < T(0)) {
+    contact_hull<T>(verts + (size_t)b * MN.vmax * 3, MN.vmax, nv, c, R, p, v, w, A, Bm, C, bn, bf, cf);
   }
   str<R_A, R_AB>(rec, ab);
   if (!PK_IS_SHADOW) rec[R_CFX] = cf[0];
@@ -284,10 +291,10 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
     qlog(qj, q);
 #pragma unroll
     for (int k = 0; k < 3; k++) {
-      T kp = T(M.kp[d0 + k]), kd = T(M.kd[d0 + k]);
-      e[k] = T(M.armature[d0 + k]) + c.h * kd + c.h * c.h * kp;
+      T kp = T(MN.kp[d0 + k]), kd = T(MN.kd[d0 + k]);
+      e[k] = T(MN.armature[d0 + k]) + c.h * kd + c.h * c.h * kp;
       tau[k] = kp * (pd[k] - q[k] - c.h * wt[k]) - kd * wt[k];
-      T lo = T(M.lim_lo[d0 + k]), hi = T(M.lim_hi[d0 + k]);
+      T lo = T(MN.lim_lo[d0 + k]), hi = T(MN.lim_hi[d0 + k]);
       if (q[k] < lo) { tau[k] += c.limk * (lo - q[k] - c.h * wt[k]) - c.limc * wt[k]; e[k] += c.h * c.limc + c.h * c.h * c.limk; }
       else if (q[k] > hi) { tau[k] += c.limk * (hi - q[k] - c.h * wt[k]) - c.limc * wt[k]; e[k] += c.h * c.limc + c.h * c.h * c.limk; }
     }
@@ -300,6 +307,11 @@ __device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restric
     E[5] = R[3] * R[6] * e[0] + R[4] * R[7] * e[1] + R[5] * R[8] * e[2];
     str<R_E, 6>(rec, E); str<R_U, 3>(rec, u);
   }
+}
+template <typename T, bool DEFER_CONTACT = false>
+__device__ __forceinline__ void pk_body(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c, T* env, int b, bool ext_on,
+                                        const T* pd) {
+  pk_body<T, DEFER_CONTACT>(B, B.m, verts, c, env, b, ext_on, pd);
 }
 
 // backward step of one dynamic non-root body: D^-1, u, articulated inertia/bias shifted to the parent origin -> out[27]
@@ -493,7 +505,8 @@ __device__ __forceinline__ int pk_nth_set_bit(uint32_t w, int n) {   // position
 #endif
 }
 template <typename T>
-__device__ __forceinline__ void pk_contact_phase(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c, T* env, int lane, bool valid) {
+__device__ __forceinline__ void pk_contact_phase(const DevBlob& B, const b200_model_t& MN, const float* __restrict__ verts, const PhysCfg<T>& c, T* env,
+                                                 int lane, bool valid) {
   const b200_model_t& M = B.m;
   const int g = lane >> 3, s = lane & 7, nb = M.nb;
   // which of my bodies (rounds 0..2 of the body pass) have penetrating vertices
@@ -521,7 +534,7 @@ __device__ __forceinline__ void pk_contact_phase(const DevBlob& B, const float* 
       const unsigned long long mask = (unsigned long long)pk_slot_to_bits(rec[R_CFY]) | ((unsigned long long)pk_slot_to_bits(rec[R_CFZ]) << 32);
       cf[0] = rec[R_CFX]; cf[1] = T(0); cf[2] = T(0);
       qmat(own, R);
-      contact_apply<T>(verts + (size_t)b * M.vmax * 3, M.vmax, mask, c, R, own + 4, own + 10, own + 7, ab, ab + 6, ab + 15, ab + 21, ab + 24, cf);
+      contact_apply<T>(verts + (size_t)b * MN.vmax * 3, MN.vmax, mask, c, R, own + 4, own + 10, own + 7, ab, ab + 6, ab + 15, ab + 21, ab + 24, cf);
       str<R_A, R_AB>(rec, ab);
       if (!PK_IS_SHADOW) rec[R_CFX] = cf[0];
       str<R_CFY, 2>(rec, cf + 1);
@@ -758,9 +771,12 @@ __device__ __forceinline__ void pk_ball_contacts_group(const DevBlob& B, const f
 
 // One control step for the warp's EPW envs.  wrec: the warp's records; valid: this lane's env exists.
 // The ball of env g is carried by lane (g, BALL_SLOT) in registers.
+// B: the tree tables and topology every env of the warp shares; MN / verts: the numeric constants and hull vertices of this lane's
+// env (B.m and its vertices when the warp's envs are of one asset).  The ball paths read B only: a handle whose envs have different
+// assets has no ball (b200env_create_assets).
 template <typename T>
-__device__ __forceinline__ void control_step_packed(const DevBlob& B, const float* verts, const PhysCfg<T>& c, T* wrec, int lane, bool valid,
-                                                    Ball<T>& ball, bool cta_sync) {
+__device__ __forceinline__ void control_step_packed(const DevBlob& B, const b200_model_t& MN, const float* verts, const PhysCfg<T>& c, T* wrec,
+                                                    int lane, bool valid, Ball<T>& ball, bool cta_sync) {
   const b200_model_t& M = B.m;
   const int g = lane >> 3, s = lane & 7;
   T* env = wrec + g * ENV_STRIDE;
@@ -770,7 +786,7 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
   // kinematics of the start state, root -> leaves; every later FK is fused into the forward pass of the substep before it
   for (int d = 1; d <= M.max_depth; d++) {
     const int b = valid ? B.t.lvl_all[d][s] : -1;
-    if (b >= 0) pk_fk<T, true>(B, env, b);
+    if (b >= 0) pk_fk<T, true>(B, MN, env, b);
     __syncwarp();
   }
   for (int sim = 0; sim < c.cfi; sim++) {
@@ -790,12 +806,12 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
         if (valid && b < nb && !M.fixed[b]) {
           T pdb[3];
           pk_pd_pick<T>(pd, rr, pdb);
-          pk_body<T, PK_CONTACT_COMPACT != 0>(B, verts, c, env, b, sim == 0, pdb);
+          pk_body<T, PK_CONTACT_COMPACT != 0>(B, MN, verts, c, env, b, sim == 0, pdb);
         }
       }
       __syncwarp();
 #if PK_CONTACT_COMPACT
-      pk_contact_phase<T>(B, verts, c, env, lane, valid);
+      pk_contact_phase<T>(B, MN, verts, c, env, lane, valid);
       __syncwarp();
 #endif
       // 2. articulated inertia, leaves -> root
@@ -848,9 +864,9 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
           if (!M.fixed[b]) {
             T qn[4], wt[3];
             pk_forward<T>(B, c, env, b, qn, wt);
-            pk_fk<T, true, true>(B, env, b, qn, wt);
+            pk_fk<T, true, true>(B, MN, env, b, qn, wt);
           } else {
-            pk_fk<T, true>(B, env, b);
+            pk_fk<T, true>(B, MN, env, b);
           }
         }
         __syncwarp();
@@ -858,6 +874,11 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const floa
     }
   }
   pk_pd_park<T>(B, env, s, valid, pd);
+}
+template <typename T>
+__device__ __forceinline__ void control_step_packed(const DevBlob& B, const float* verts, const PhysCfg<T>& c, T* wrec, int lane, bool valid,
+                                                    Ball<T>& ball, bool cta_sync) {
+  control_step_packed<T>(B, B.m, verts, c, wrec, lane, valid, ball, cta_sync);
 }
 
 // state of one env between the lane-per-body prologue / epilogue (lane = body) and the records

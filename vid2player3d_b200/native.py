@@ -15,7 +15,8 @@ SYMBOLS = ["b200env_abi_version", "b200env_last_error", "b200env_create", "b200e
            "b200env_set_motion_lib", "b200env_step", "b200env_reset", "b200env_motion_state", "b200env_obs_imitation",
            "b200env_physics_only", "b200env_launch_count", "b200env_set_env_slice", "b200env_motion_context", "b200env_set_kernel_timing",
            "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form",
-           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan", "b200env_reset_masked"]
+           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan", "b200env_reset_masked",
+           "b200env_plan_assets_mixed", "b200env_choose_asset_plan"]
 
 ENVS_PER_BATCH = 32   # envs per CTA batch of the default physics launch (step_kernel_packed<true>): the batch size of the asset plan
 
@@ -52,19 +53,31 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH):
+def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):
     """the batch plan of a handle of several assets (include/b200env.h: b200env_plan_assets; host only): (rows [N] = envs grouped by
-    asset, batches [num_batches, 3] of (asset, first row, count))"""
+    asset, batches [num_batches, 3] of (asset, first row, count)).  mixed: the mixed plan (b200env_plan_assets_mixed): rows in env
+    order, batches of consecutive envs whatever their asset (asset -1 for a batch of several)"""
     import numpy as np
     ea = np.ascontiguousarray(env_asset, np.int32)
     n = len(ea)
     rows, ba, bf, bc = (np.zeros(max(n, 1), np.int32) for _ in range(4))
     nb = C.c_int32(0)
     p = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-    _check(lib().b200env_plan_assets(p(ea), C.c_int32(n), C.c_int32(int(num_assets)), C.c_int32(int(envs_per_batch)), p(rows), p(ba), p(bf),
-                                     p(bc), C.byref(nb)))
+    fn = lib().b200env_plan_assets_mixed if mixed else lib().b200env_plan_assets
+    _check(fn(p(ea), C.c_int32(n), C.c_int32(int(num_assets)), C.c_int32(int(envs_per_batch)), p(rows), p(ba), p(bf), p(bc), C.byref(nb)))
     k = nb.value
     return rows[:n], np.stack([ba[:k], bf[:k], bc[:k]], 1)
+
+
+def choose_asset_plan(env_asset, num_assets, grid):
+    """True when b200env_create_assets runs the mixed plan on a persistent grid of `grid` CTAs (include/b200env.h:
+    b200env_choose_asset_plan; host only)"""
+    import numpy as np
+    ea = np.ascontiguousarray(env_asset, np.int32)
+    m = C.c_int32(0)
+    _check(lib().b200env_choose_asset_plan(ea.ctypes.data_as(C.c_void_p), C.c_int32(len(ea)), C.c_int32(int(num_assets)), C.c_int32(int(grid)),
+                                           C.byref(m)))
+    return bool(m.value)
 
 
 class Env:
@@ -232,12 +245,20 @@ class Env:
         (include/b200env.h: b200env_asset_plan): batch b of rows[first:first + count] runs in round b // grid"""
         import numpy as np
         na, nb = C.c_int32(0), C.c_int32(0)
-        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), None, None, None, None))
+        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), None, None, None, None, None))
         rows = np.zeros(self.num_envs, np.int32)
         b = np.zeros((3, max(nb.value, 1)), np.int32)
         p = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
-        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), p(rows), p(b[0]), p(b[1]), p(b[2])))
+        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), p(rows), p(b[0]), p(b[1]), p(b[2]), None))
         return na.value, rows, b[:, :nb.value].T.copy()
+
+    @property
+    def asset_plan_mixed(self):
+        """True when a handle of several assets runs the mixed plan (batches of consecutive envs whatever their asset), False for the
+        grouped one (include/b200env.h: b200env_asset_plan)"""
+        na, nb, m = C.c_int32(0), C.c_int32(0), C.c_int32(0)
+        _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), None, None, None, None, C.byref(m)))
+        return bool(m.value)
 
     @property
     def launch_count(self):
