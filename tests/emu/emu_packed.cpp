@@ -12,7 +12,7 @@ thread_local int emu_lane = 0;
 #define EMU_EPW EPW3
 #define EMU_LPE LPE3
 #define EMU_BALL_SLOT BALL_SLOT3
-#define EMU_STEP control_step_packed3
+#define EMU_STEP(B, MN, ...) control_step_packed3<T>(B, __VA_ARGS__)   // one asset: MN is B.m
 #else
 #include "../../vid2player3d_b200/csrc/packed.cuh"
 #ifdef EMU_PACKEDT
@@ -21,24 +21,24 @@ thread_local int emu_lane = 0;
 #define EMU_EPW EPW
 #define EMU_LPE PK_LANES_PER_ENV
 #define EMU_BALL_SLOT BALL_SLOT
-#define EMU_STEP control_step_packed
+#define EMU_STEP(B, MN, ...) control_step_packed<T>(B, MN, __VA_ARGS__)
 #endif
 
 #include <vector>
 
 namespace {
 template <typename T> struct Job {
-  const DevBlob* B;
+  const DevBlob* B;                 // the model; envs of several assets (emu_mixed.cpp): asset 0's, whose tree tables they share
   const float* verts;
+  const DevBlob* const* env_blob;   // several assets: [n] the header of env e's asset (its numeric constants), else null
+  const float* const* env_verts;    // several assets: [n] its SoA hull vertices, else null
   const b200_cfg_t* cfg;
   int n, n_steps;
-  T *root, *dof_pos, *dof_vel;
-  const T *pd_tar, *ext;
-  T *rb_out, *contact_out, *ballio;
-  int32_t* hits;
+  EnvArrays<T> io;
 };
 
-// one warp = the body of physics_kernel_packed<double> (b200env.cu) for envs eb .. eb + EPW - 1
+// one warp = the body of physics_kernel_packed<double> (b200env.cu) for envs eb .. eb + EPW - 1; with several assets each lane steps
+// with its env's model, as step_kernel_packed<true, false, true> does
 template <typename T> void lane_main(EmuWarp* w, int lane, const Job<T>* J, int64_t eb, T* wrec) {
   emu_warp = w;
   emu_lane = lane;
@@ -48,55 +48,28 @@ template <typename T> void lane_main(EmuWarp* w, int lane, const Job<T>* J, int6
   LaneConst lc = lane_const(M, lane);
   if (lc.active) lc.rix = B.t.rix[lane];
   PhysCfg<T> pc = make_phys_cfg<T>(*J->cfg);
-  const bool with_ball = pc.has_ball && J->ballio != nullptr;
+  const bool with_ball = pc.has_ball && J->io.ball != nullptr;
   pc.has_ball = with_ball;
   const int g = lane / EMU_LPE, s = lane % EMU_LPE;
   for (int k = 0; k < EMU_EPW; k++) {
     const int64_t e = eb + k;
     if (e >= n) break;
     Lane<T> L;
-    for (int j = 0; j < 4; j++) { L.Q[j] = 0; L.qj[j] = 0; }
-    L.Q[3] = 1; L.qj[3] = 1;
-    for (int j = 0; j < 3; j++) { L.p[j] = 0; L.w[j] = 0; L.v[j] = 0; L.wt[j] = 0; }
-    T pdt[3] = {0, 0, 0}, eF[3] = {0, 0, 0}, eT[3] = {0, 0, 0};
-    if (lane == 0) {
-      const T* rs = J->root + e * 13;
-      for (int j = 0; j < 3; j++) { L.p[j] = rs[j]; L.v[j] = rs[7 + j]; L.w[j] = rs[10 + j]; }
-      for (int j = 0; j < 4; j++) L.Q[j] = rs[3 + j];
-      qnormalize(L.Q);
-      if (J->ext) for (int j = 0; j < 3; j++) { eF[j] = J->ext[e * 6 + j]; eT[j] = J->ext[e * 6 + 3 + j]; }
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      for (int j = 0; j < 3; j++) { q[j] = J->dof_pos[e * nd + lc.dof0 + j]; L.wt[j] = J->dof_vel[e * nd + lc.dof0 + j]; pdt[j] = J->pd_tar[e * nd + lc.dof0 + j]; }
-      qexp(q, L.qj);
-    }
+    T pdt[3], eF[3], eT[3];
+    env_arrays_load<T>(J->io, nd, lc, lane, e, L, pdt, eF, eT);
     pk_store_state<T>(wrec + k * ENV_STRIDE, lc, lane, L, pdt, eF, eT);
   }
   __syncwarp();
   const bool valid = g < EMU_EPW && eb + g < n;
+  const int64_t me = valid ? eb + g : eb;   // a lane without an env takes the warp's first env's model, as the kernel does
+  const b200_model_t& MN = J->env_blob ? J->env_blob[me]->m : M;
+  const float* verts = J->env_verts ? J->env_verts[me] : J->verts;
   Ball<T> ball;
   ball_clear(ball);
-  if (with_ball && valid && s == EMU_BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { ball.p[j] = J->ballio[e * 13 + j]; ball.v[j] = J->ballio[e * 13 + 7 + j]; ball.w[j] = J->ballio[e * 13 + 10 + j]; }
-  }
+  if (with_ball && valid && s == EMU_BALL_SLOT) env_arrays_load_ball<T>(J->io, eb + g, ball);
   for (int st_ = 0; st_ < J->n_steps; st_++) {
-    EMU_STEP<T>(B, J->verts, pc, wrec, lane, valid, ball, false);
-    if (st_ + 1 < J->n_steps) {
-      for (int k = 0; k < EMU_EPW; k++) {
-        if (eb + k >= n) break;
-        if (lc.dyn && lane > 0) {
-          T* rec = wrec + k * ENV_STRIDE + lc.rix * REC;
-          T qj[4], q[3];
-          ldr<R_QJ, 4>(rec, qj);
-          qlog(qj, q);
-          qexp(q, qj);
-          str<R_QJ, 4>(rec, qj);
-        }
-      }
-      __syncwarp();
-    }
+    EMU_STEP(B, MN, verts, pc, wrec, lane, valid, ball, false);
+    if (st_ + 1 < J->n_steps) pk_requantize<T, EMU_EPW>(wrec, lc, lane, eb, n);
   }
   for (int k = 0; k < EMU_EPW; k++) {
     const int64_t e = eb + k;
@@ -104,28 +77,9 @@ template <typename T> void lane_main(EmuWarp* w, int lane, const Job<T>* J, int6
     Lane<T> L;
     T cf[3];
     pk_load_state<T>(wrec + k * ENV_STRIDE, lc, lane, L, cf);
-    if (lane == 0) {
-      T* rs = J->root + e * 13;
-      for (int j = 0; j < 3; j++) { rs[j] = L.p[j]; rs[7 + j] = L.v[j]; rs[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rs[3 + j] = L.Q[j];
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      qlog(L.qj, q);
-      for (int j = 0; j < 3; j++) { J->dof_pos[e * nd + lc.dof0 + j] = q[j]; J->dof_vel[e * nd + lc.dof0 + j] = L.wt[j]; }
-    }
-    if (lc.active) {
-      T* rb = J->rb_out + (e * nb + lane) * 13;
-      for (int j = 0; j < 3; j++) { rb[j] = L.p[j]; rb[7 + j] = L.v[j]; rb[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rb[3 + j] = L.Q[j];
-      if (J->contact_out) for (int j = 0; j < 3; j++) J->contact_out[(e * nb + lane) * 3 + j] = cf[j];
-    }
+    env_arrays_store<T>(J->io, nb, nd, lc, lane, e, L, cf);
   }
-  if (with_ball && valid && s == EMU_BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { J->ballio[e * 13 + j] = ball.p[j]; J->ballio[e * 13 + 7 + j] = ball.v[j]; J->ballio[e * 13 + 10 + j] = ball.w[j]; }
-    if (J->hits) J->hits[e] = ball.hits;
-  }
+  if (with_ball && valid && s == EMU_BALL_SLOT) env_arrays_store_ball<T>(J->io, eb + g, ball);
 }
 
 #ifdef EMU_PACKEDT
@@ -139,7 +93,7 @@ template <typename T> void lane_main_t(EmuWarp* w, int lane, const Job<T>* J, in
   LaneConst lc = lane_const(M, lane);
   if (lc.active) lc.rix = B.t.rix[lane];
   PhysCfg<T> pc = make_phys_cfg<T>(*J->cfg);
-  const bool with_ball = pc.has_ball && J->ballio != nullptr;
+  const bool with_ball = pc.has_ball && J->io.ball != nullptr;
   pc.has_ball = with_ball;
   const int g = lane / EMU_LPE, s = lane % EMU_LPE;
   PrivMem<T> ps{priv + (size_t)lane * PT_WARP_COLS};
@@ -147,22 +101,8 @@ template <typename T> void lane_main_t(EmuWarp* w, int lane, const Job<T>* J, in
     const int64_t e = eb + k;
     if (e >= n) break;
     Lane<T> L;
-    for (int j = 0; j < 4; j++) { L.Q[j] = 0; L.qj[j] = 0; }
-    L.Q[3] = 1; L.qj[3] = 1;
-    for (int j = 0; j < 3; j++) { L.p[j] = 0; L.w[j] = 0; L.v[j] = 0; L.wt[j] = 0; }
-    T pdt[3] = {0, 0, 0}, eF[3] = {0, 0, 0}, eT[3] = {0, 0, 0};
-    if (lane == 0) {
-      const T* rs = J->root + e * 13;
-      for (int j = 0; j < 3; j++) { L.p[j] = rs[j]; L.v[j] = rs[7 + j]; L.w[j] = rs[10 + j]; }
-      for (int j = 0; j < 4; j++) L.Q[j] = rs[3 + j];
-      qnormalize(L.Q);
-      if (J->ext) for (int j = 0; j < 3; j++) { eF[j] = J->ext[e * 6 + j]; eT[j] = J->ext[e * 6 + 3 + j]; }
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      for (int j = 0; j < 3; j++) { q[j] = J->dof_pos[e * nd + lc.dof0 + j]; L.wt[j] = J->dof_vel[e * nd + lc.dof0 + j]; pdt[j] = J->pd_tar[e * nd + lc.dof0 + j]; }
-      qexp(q, L.qj);
-    }
+    T pdt[3], eF[3], eT[3];
+    env_arrays_load<T>(J->io, nd, lc, lane, e, L, pdt, eF, eT);
     pt_stage_in<T>(wrec + k * PT_ENV_STRIDE, lc, lane, L, pdt, eF, eT);
   }
   __syncwarp();
@@ -170,11 +110,8 @@ template <typename T> void lane_main_t(EmuWarp* w, int lane, const Job<T>* J, in
   pt_adopt<T>(B, wrec, lane, valid, ps);
   Ball<T> ball;
   ball_clear(ball);
-  if (with_ball && valid && s == EMU_BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { ball.p[j] = J->ballio[e * 13 + j]; ball.v[j] = J->ballio[e * 13 + 7 + j]; ball.w[j] = J->ballio[e * 13 + 10 + j]; }
-  }
-  T* cf_env = (valid && J->contact_out) ? J->contact_out + (eb + g) * nb * 3 : nullptr;
+  if (with_ball && valid && s == EMU_BALL_SLOT) env_arrays_load_ball<T>(J->io, eb + g, ball);
+  T* cf_env = (valid && J->io.contact_out) ? J->io.contact_out + (eb + g) * nb * 3 : nullptr;
   for (int st_ = 0; st_ < J->n_steps; st_++) {
     control_step_t<T>(B, J->verts, pc, wrec, lane, valid, ball, ps, cf_env, false);
     if (st_ + 1 < J->n_steps) pt_requantize<T>(B, lane, valid, ps);
@@ -186,30 +123,34 @@ template <typename T> void lane_main_t(EmuWarp* w, int lane, const Job<T>* J, in
     if (e >= n) break;
     Lane<T> L;
     pt_load_state<T>(wrec + k * PT_ENV_STRIDE, lc, lane, L);
-    if (lane == 0) {
-      T* rs = J->root + e * 13;
-      for (int j = 0; j < 3; j++) { rs[j] = L.p[j]; rs[7 + j] = L.v[j]; rs[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rs[3 + j] = L.Q[j];
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      qlog(L.qj, q);
-      for (int j = 0; j < 3; j++) { J->dof_pos[e * nd + lc.dof0 + j] = q[j]; J->dof_vel[e * nd + lc.dof0 + j] = L.wt[j]; }
-    }
-    if (lc.active) {
-      T* rb = J->rb_out + (e * nb + lane) * 13;
-      for (int j = 0; j < 3; j++) { rb[j] = L.p[j]; rb[7 + j] = L.v[j]; rb[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rb[3 + j] = L.Q[j];
-      if (J->contact_out && !lc.dyn) for (int j = 0; j < 3; j++) J->contact_out[(e * nb + lane) * 3 + j] = T(0);   // welded bodies carry no contact force of their own
-    }
+    env_arrays_store<T>(J->io, nb, nd, lc, lane, e, L, nullptr);
   }
-  if (with_ball && valid && s == EMU_BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { J->ballio[e * 13 + j] = ball.p[j]; J->ballio[e * 13 + 7 + j] = ball.v[j]; J->ballio[e * 13 + 10 + j] = ball.w[j]; }
-    if (J->hits) J->hits[e] = ball.hits;
-  }
+  if (with_ball && valid && s == EMU_BALL_SLOT) env_arrays_store_ball<T>(J->io, eb + g, ball);
 }
 #endif
+
+// the warps of J, one after the other (each warp: 32 host threads)
+template <typename T> int run_warps(const Job<T>& J) {
+#ifdef EMU_PACKEDT
+  if (!J.B->t.pt_ok) return -2;
+  std::vector<T> rec((size_t)EMU_EPW * PT_ENV_STRIDE + 8, T(0)), priv((size_t)32 * PT_WARP_COLS, T(0));
+#else
+  std::vector<T> rec((size_t)EMU_EPW * ENV_STRIDE + 8, T(0));
+#endif
+  T* wrec = rec.data();
+  while ((uintptr_t)wrec % 16) wrec++;   // the records are read with 128-bit accesses on the float path
+  for (int64_t eb = 0; eb < J.n; eb += EMU_EPW) {
+    EmuWarp w;
+    std::vector<std::thread> th;
+#ifdef EMU_PACKEDT
+    for (int lane = 0; lane < 32; lane++) th.emplace_back(lane_main_t<T>, &w, lane, &J, eb, wrec, priv.data());
+#else
+    for (int lane = 0; lane < 32; lane++) th.emplace_back(lane_main<T>, &w, lane, &J, eb, wrec);
+#endif
+    for (auto& t : th) t.join();
+  }
+  return 0;
+}
 }  // namespace
 
 // hull faces of the exact ball / hull query (b200env_set_hull_faces on the product side): host arrays kept by the caller
@@ -239,26 +180,7 @@ static int run(const b200_model_t* model, const float* verts, const b200_cfg_t* 
   float* sv = soa.data();
   while ((uintptr_t)sv % 16) sv++;   // contact_hull reads the vertices with 128-bit loads
   verts_to_soa(model, verts, sv);
-  Job<T> J{&hb, sv, cfg, n, n_steps, root, dof_pos, dof_vel, pd_tar, ext, rb_out, contact_out, ballio, hits};
-#ifdef EMU_PACKEDT
-  if (!hb.t.pt_ok) return -2;
-  std::vector<T> rec((size_t)EMU_EPW * PT_ENV_STRIDE + 8, T(0)), priv((size_t)32 * PT_WARP_COLS, T(0));
-#else
-  std::vector<T> rec((size_t)EMU_EPW * ENV_STRIDE + 8, T(0));
-#endif
-  T* wrec = rec.data();
-  while ((uintptr_t)wrec % 16) wrec++;   // the records are read with 128-bit accesses on the float path
-  for (int64_t eb = 0; eb < n; eb += EMU_EPW) {
-    EmuWarp w;
-    std::vector<std::thread> th;
-#ifdef EMU_PACKEDT
-    for (int lane = 0; lane < 32; lane++) th.emplace_back(lane_main_t<T>, &w, lane, &J, eb, wrec, priv.data());
-#else
-    for (int lane = 0; lane < 32; lane++) th.emplace_back(lane_main<T>, &w, lane, &J, eb, wrec);
-#endif
-    for (auto& t : th) t.join();
-  }
-  return 0;
+  return run_warps(Job<T>{&hb, sv, nullptr, nullptr, cfg, n, n_steps, {root, dof_pos, dof_vel, pd_tar, ext, rb_out, contact_out, ballio, hits}});
 }
 
 // float64: the parity instantiation (vs oracle/physics_ref.c to round-off); float32: the arithmetic the product kernel runs

@@ -734,11 +734,7 @@ __device__ __forceinline__ void step_prologue(const b200_buffers_t& bf, const b2
   }
   __syncwarp();
 
-#pragma unroll
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0.f; L.qj[k] = 0.f; }
-  L.Q[3] = 1.f; L.qj[3] = 1.f;
-#pragma unroll
-  for (int k = 0; k < 3; k++) { L.p[k] = 0.f; L.w[k] = 0.f; L.v[k] = 0.f; L.wt[k] = 0.f; }
+  lane_rest(L);
   pdtar[0] = pdtar[1] = pdtar[2] = 0.f;
   if (lane == 0) {
 #pragma unroll
@@ -986,32 +982,6 @@ step_kernel(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_c
 
 // ------------------------------------------------------------------------------------------
 // three-launch form of the env step (b200env_step with h->split): pre_kernel -> step_kernel_packed<true> -> post_kernel.
-// state of env row e as the physics wants it, from the rows the pre_kernel left behind (lane = body)
-__device__ __forceinline__ void load_state_rows(const b200_buffers_t& bf, const b200_model_t& M, const LaneConst& lc, int lane, int64_t e,
-                                                const float* __restrict__ ext_wrench, Lane<float>& L, float* pdtar, float* extF, float* extT) {
-  const int nd = M.nd;
-#pragma unroll
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0.f; L.qj[k] = 0.f; }
-  L.Q[3] = 1.f; L.qj[3] = 1.f;
-#pragma unroll
-  for (int k = 0; k < 3; k++) { L.p[k] = 0.f; L.w[k] = 0.f; L.v[k] = 0.f; L.wt[k] = 0.f; pdtar[k] = 0.f; extF[k] = 0.f; extT[k] = 0.f; }
-  if (lane == 0) {
-    const float* rs = bf.root_states + e * bf.actors_per_env * 13;
-#pragma unroll
-    for (int k = 0; k < 3; k++) { L.p[k] = rs[k]; L.v[k] = rs[7 + k]; L.w[k] = rs[10 + k]; extF[k] = ext_wrench[e * 6 + k]; extT[k] = ext_wrench[e * 6 + 3 + k]; }
-#pragma unroll
-    for (int k = 0; k < 4; k++) L.Q[k] = rs[3 + k];
-    qnormalize(L.Q);
-  }
-  if (lc.dyn && lane > 0) {
-    const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
-    float q[3];
-#pragma unroll
-    for (int k = 0; k < 3; k++) { q[k] = ds[2 * k]; L.wt[k] = ds[2 * k + 1]; pdtar[k] = bf.pd_targets[e * nd + lc.dof0 + k]; }
-    qexp(q, L.qj);
-  }
-}
-
 // launch 1: pre_physics_step of every env (zeroed actions of reset envs, PD targets, residual root wrench, previous <- current
 // targets).  Warp per env, lane per body, 8 warps per CTA, no big shared-memory footprint -> full occupancy.
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
@@ -1048,12 +1018,8 @@ post_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gc
   const LaneConst lc = lane_const(M, lane);
   const int nd = M.nd;
   Lane<float> L;
-#pragma unroll
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0.f; L.qj[k] = 0.f; }
-  L.Q[3] = 1.f; L.qj[3] = 1.f;
+  lane_rest(L);
   float dq[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-  for (int k = 0; k < 3; k++) { L.p[k] = 0.f; L.w[k] = 0.f; L.v[k] = 0.f; L.wt[k] = 0.f; }
   if (lc.active) {
     const float* rb = bf.rigid_body_state + (e * bf.bodies_per_env + lane) * 13;
 #pragma unroll
@@ -1185,45 +1151,14 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #endif
 
     if (SPLIT) {
-      // all loads of the warp's EPW envs are issued before the first use (one memory latency instead of EPW)
-      float rq[EPW][3], rw[EPW][3], rp[EPW][3], r1[EPW];   // r1: lane j < 13 holds root_states[e][j], 13 <= j < 19 the residual wrench
-      const int nd = M.nd;
-#pragma unroll
-      for (int k = 0; k < EPW; k++) {
-        const int64_t ek = eb + k < end ? eb + k : end - 1;   // ragged tail: re-read the last env, never stored
-        const int64_t e = row(ek);
-        if (lc.dyn && lane > 0) {
-          const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
-#pragma unroll
-          for (int j = 0; j < 3; j++) { rq[k][j] = ds[2 * j]; rw[k][j] = ds[2 * j + 1]; rp[k][j] = bf.pd_targets[e * nd + lc.dof0 + j]; }
-        }
-        r1[k] = lane < 13 ? bf.root_states[e * bf.actors_per_env * 13 + lane] : (lane < 19 ? ext_wrench[e * 6 + lane - 13] : 0.f);
-      }
+      StateRows<EPW> rows;
+      gather_state_rows<EPW>(bf, M, lc, lane, eb, end, row, ext_wrench, rows);
 #pragma unroll
       for (int k = 0; k < EPW; k++) {
         if (eb + k >= end) break;
         Lane<float> L;
-        float pdtar[3] = {0.f, 0.f, 0.f}, extF[3] = {0.f, 0.f, 0.f}, extT[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < 4; j++) { L.Q[j] = 0.f; L.qj[j] = 0.f; }
-        L.Q[3] = 1.f; L.qj[3] = 1.f;
-#pragma unroll
-        for (int j = 0; j < 3; j++) { L.p[j] = 0.f; L.w[j] = 0.f; L.v[j] = 0.f; L.wt[j] = 0.f; }
-        float rr[19];
-#pragma unroll
-        for (int j = 0; j < 19; j++) rr[j] = __shfl_sync(FULL, r1[k], j);
-        if (lane == 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.p[j] = rr[j]; L.v[j] = rr[7 + j]; L.w[j] = rr[10 + j]; extF[j] = rr[13 + j]; extT[j] = rr[16 + j]; }
-#pragma unroll
-          for (int j = 0; j < 4; j++) L.Q[j] = rr[3 + j];
-          qnormalize(L.Q);
-        }
-        if (lc.dyn && lane > 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.wt[j] = rw[k][j]; pdtar[j] = rp[k][j]; }
-          qexp(rq[k], L.qj);
-        }
+        float pdtar[3], extF[3], extT[3];
+        unpack_state_row<EPW>(rows, k, lc, lane, L, pdtar, extF, extT);
         pk_store_state<float>(wrec + k * ENV_STRIDE, lc, lane, L, pdtar, extF, extT);
       }
     } else {
@@ -1318,45 +1253,14 @@ step_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b
     const int64_t eb = e0 + (int64_t)warp * EPW;
     if (!full_batch && eb >= num_envs) continue;
     {
-      // all loads of the warp's EPW envs are issued before the first use (one memory latency instead of EPW)
-      float rq[EPW][3], rw[EPW][3], rp[EPW][3], r1[EPW];   // r1: lane j < 13 holds root_states[e][j], 13 <= j < 19 the residual wrench
-      const int nd = M.nd;
-#pragma unroll
-      for (int k = 0; k < EPW; k++) {
-        const int64_t ek = eb + k < num_envs ? eb + k : (int64_t)num_envs - 1;   // ragged tail: re-read the last env, never stored
-        const int64_t e = row(ek);
-        if (lc.dyn && lane > 0) {
-          const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
-#pragma unroll
-          for (int j = 0; j < 3; j++) { rq[k][j] = ds[2 * j]; rw[k][j] = ds[2 * j + 1]; rp[k][j] = bf.pd_targets[e * nd + lc.dof0 + j]; }
-        }
-        r1[k] = lane < 13 ? bf.root_states[e * bf.actors_per_env * 13 + lane] : (lane < 19 ? ext_wrench[e * 6 + lane - 13] : 0.f);
-      }
+      StateRows<EPW> rows;
+      gather_state_rows<EPW>(bf, M, lc, lane, eb, num_envs, row, ext_wrench, rows);
 #pragma unroll
       for (int k = 0; k < EPW; k++) {
         if (eb + k >= num_envs) break;
         Lane<float> L;
-        float pdtar[3] = {0.f, 0.f, 0.f}, extF[3] = {0.f, 0.f, 0.f}, extT[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < 4; j++) { L.Q[j] = 0.f; L.qj[j] = 0.f; }
-        L.Q[3] = 1.f; L.qj[3] = 1.f;
-#pragma unroll
-        for (int j = 0; j < 3; j++) { L.p[j] = 0.f; L.w[j] = 0.f; L.v[j] = 0.f; L.wt[j] = 0.f; }
-        float rr[19];
-#pragma unroll
-        for (int j = 0; j < 19; j++) rr[j] = __shfl_sync(FULL, r1[k], j);
-        if (lane == 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.p[j] = rr[j]; L.v[j] = rr[7 + j]; L.w[j] = rr[10 + j]; extF[j] = rr[13 + j]; extT[j] = rr[16 + j]; }
-#pragma unroll
-          for (int j = 0; j < 4; j++) L.Q[j] = rr[3 + j];
-          qnormalize(L.Q);
-        }
-        if (lc.dyn && lane > 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.wt[j] = rw[k][j]; pdtar[j] = rp[k][j]; }
-          qexp(rq[k], L.qj);
-        }
+        float pdtar[3], extF[3], extT[3];
+        unpack_state_row<EPW>(rows, k, lc, lane, L, pdtar, extF, extT);
         pt_stage_in<float>(wrec + k * PT_ENV_STRIDE, lc, lane, L, pdtar, extF, extT);
       }
     }
@@ -1389,8 +1293,7 @@ step_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b
 template <int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, int n, int n_steps,
-                    float* root, float* dof_pos, float* dof_vel, const float* pd_tar, const float* ext, float* rb_out, float* contact_out,
-                    float* ballio, int32_t* hits) {
+                    EnvArrays<float> io) {
   typedef float T;
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
@@ -1408,29 +1311,15 @@ physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
     if (lc.active) lc.rix = B.t.rix[lane];
     const int nb = M.nb, nd = M.nd;
     PhysCfg<T> pc = make_phys_cfg<T>(*gcfg);
-    const bool with_ball = pc.has_ball && ballio != nullptr;
+    const bool with_ball = pc.has_ball && io.ball != nullptr;
     pc.has_ball = with_ball;
     const int g = lane >> 3, s = lane & 7;
     for (int k = 0; k < EPW; k++) {
       const int64_t e = eb + k;
       if (e >= n) break;
       Lane<T> L;
-      for (int j = 0; j < 4; j++) { L.Q[j] = 0; L.qj[j] = 0; }
-      L.Q[3] = 1; L.qj[3] = 1;
-      for (int j = 0; j < 3; j++) { L.p[j] = 0; L.w[j] = 0; L.v[j] = 0; L.wt[j] = 0; }
-      T pdt[3] = {0, 0, 0}, eF[3] = {0, 0, 0}, eT[3] = {0, 0, 0};
-      if (lane == 0) {
-        const T* rs = root + e * 13;
-        for (int j = 0; j < 3; j++) { L.p[j] = rs[j]; L.v[j] = rs[7 + j]; L.w[j] = rs[10 + j]; }
-        for (int j = 0; j < 4; j++) L.Q[j] = rs[3 + j];
-        qnormalize(L.Q);
-        if (ext) for (int j = 0; j < 3; j++) { eF[j] = ext[e * 6 + j]; eT[j] = ext[e * 6 + 3 + j]; }
-      }
-      if (lc.dyn && lane > 0) {
-        T q[3];
-        for (int j = 0; j < 3; j++) { q[j] = dof_pos[e * nd + lc.dof0 + j]; L.wt[j] = dof_vel[e * nd + lc.dof0 + j]; pdt[j] = pd_tar[e * nd + lc.dof0 + j]; }
-        qexp(q, L.qj);
-      }
+      T pdt[3], eF[3], eT[3];
+      env_arrays_load<T>(io, nd, lc, lane, e, L, pdt, eF, eT);
       pt_stage_in<T>(wrec + k * PT_ENV_STRIDE, lc, lane, L, pdt, eF, eT);
     }
     __syncwarp();
@@ -1438,11 +1327,8 @@ physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
     pt_adopt<T>(B, wrec, lane, valid, ps);
     Ball<T> ball;
     ball_clear(ball);
-    if (with_ball && valid && s == BALL_SLOT) {
-      const int64_t e = eb + g;
-      for (int j = 0; j < 3; j++) { ball.p[j] = ballio[e * 13 + j]; ball.v[j] = ballio[e * 13 + 7 + j]; ball.w[j] = ballio[e * 13 + 10 + j]; }
-    }
-    T* cf_env = (valid && contact_out) ? contact_out + (eb + g) * nb * 3 : nullptr;
+    if (with_ball && valid && s == BALL_SLOT) env_arrays_load_ball<T>(io, eb + g, ball);
+    T* cf_env = (valid && io.contact_out) ? io.contact_out + (eb + g) * nb * 3 : nullptr;
     for (int st_ = 0; st_ < n_steps; st_++) {
       control_step_t<T>(B, verts, pc, wrec, lane, valid, ball, ps, cf_env, false);
       if (st_ + 1 < n_steps) pt_requantize<T>(B, lane, valid, ps);   // the state crosses control steps as exp-map coordinates
@@ -1454,28 +1340,9 @@ physics_kernel_tmem(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
       if (e >= n) break;
       Lane<T> L;
       pt_load_state<T>(wrec + k * PT_ENV_STRIDE, lc, lane, L);
-      if (lane == 0) {
-        T* rs = root + e * 13;
-        for (int j = 0; j < 3; j++) { rs[j] = L.p[j]; rs[7 + j] = L.v[j]; rs[10 + j] = L.w[j]; }
-        for (int j = 0; j < 4; j++) rs[3 + j] = L.Q[j];
-      }
-      if (lc.dyn && lane > 0) {
-        T q[3];
-        qlog(L.qj, q);
-        for (int j = 0; j < 3; j++) { dof_pos[e * nd + lc.dof0 + j] = q[j]; dof_vel[e * nd + lc.dof0 + j] = L.wt[j]; }
-      }
-      if (lc.active) {
-        T* rb = rb_out + (e * nb + lane) * 13;
-        for (int j = 0; j < 3; j++) { rb[j] = L.p[j]; rb[7 + j] = L.v[j]; rb[10 + j] = L.w[j]; }
-        for (int j = 0; j < 4; j++) rb[3 + j] = L.Q[j];
-        if (contact_out && !lc.dyn) for (int j = 0; j < 3; j++) contact_out[(e * nb + lane) * 3 + j] = T(0);
-      }
+      env_arrays_store<T>(io, nb, nd, lc, lane, e, L, nullptr);   // control_step_t wrote the contact rows of the jointed bodies
     }
-    if (with_ball && valid && s == BALL_SLOT) {
-      const int64_t e = eb + g;
-      for (int j = 0; j < 3; j++) { ballio[e * 13 + j] = ball.p[j]; ballio[e * 13 + 7 + j] = ball.v[j]; ballio[e * 13 + 10 + j] = ball.w[j]; }
-      if (hits) hits[e] = ball.hits;
-    }
+    if (with_ball && valid && s == BALL_SLOT) env_arrays_store_ball<T>(io, eb + g, ball);
   }
 }
 
@@ -1564,45 +1431,15 @@ step_kernel_packed3(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
     const int64_t eb = e0 + (int64_t)warp * EPW3;
     if (eb >= num_envs) continue;
     {
-      // all loads of the warp's envs are issued before the first use
-      float rq[EPW3][3], rw[EPW3][3], rp[EPW3][3], r1[EPW3];
-      const int nd = M.nd;
-#pragma unroll
-      for (int k = 0; k < EPW3; k++) {
-        const int64_t ek = eb + k < num_envs ? eb + k : (int64_t)num_envs - 1;
-        const int64_t e = env_first + (int64_t)env_stride * ek;
-        if (lc.dyn && lane > 0) {
-          const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
-#pragma unroll
-          for (int j = 0; j < 3; j++) { rq[k][j] = ds[2 * j]; rw[k][j] = ds[2 * j + 1]; rp[k][j] = bf.pd_targets[e * nd + lc.dof0 + j]; }
-        }
-        r1[k] = lane < 13 ? bf.root_states[e * bf.actors_per_env * 13 + lane] : (lane < 19 ? ext_wrench[e * 6 + lane - 13] : 0.f);
-      }
+      StateRows<EPW3> rows;
+      gather_state_rows<EPW3>(bf, M, lc, lane, eb, num_envs, [&](int64_t i) -> int64_t { return env_first + (int64_t)env_stride * i; },
+                              ext_wrench, rows);
 #pragma unroll
       for (int k = 0; k < EPW3; k++) {
         if (eb + k >= num_envs) break;
         Lane<float> L;
-        float pdtar[3] = {0.f, 0.f, 0.f}, extF[3] = {0.f, 0.f, 0.f}, extT[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-        for (int j = 0; j < 4; j++) { L.Q[j] = 0.f; L.qj[j] = 0.f; }
-        L.Q[3] = 1.f; L.qj[3] = 1.f;
-#pragma unroll
-        for (int j = 0; j < 3; j++) { L.p[j] = 0.f; L.w[j] = 0.f; L.v[j] = 0.f; L.wt[j] = 0.f; }
-        float rr[19];
-#pragma unroll
-        for (int j = 0; j < 19; j++) rr[j] = __shfl_sync(FULL, r1[k], j);
-        if (lane == 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.p[j] = rr[j]; L.v[j] = rr[7 + j]; L.w[j] = rr[10 + j]; extF[j] = rr[13 + j]; extT[j] = rr[16 + j]; }
-#pragma unroll
-          for (int j = 0; j < 4; j++) L.Q[j] = rr[3 + j];
-          qnormalize(L.Q);
-        }
-        if (lc.dyn && lane > 0) {
-#pragma unroll
-          for (int j = 0; j < 3; j++) { L.wt[j] = rw[k][j]; pdtar[j] = rp[k][j]; }
-          qexp(rq[k], L.qj);
-        }
+        float pdtar[3], extF[3], extT[3];
+        unpack_state_row<EPW3>(rows, k, lc, lane, L, pdtar, extF, extT);
         pk_store_state<float>(wrec + k * ENV_STRIDE, lc, lane, L, pdtar, extF, extT);
       }
     }
@@ -1631,7 +1468,7 @@ step_kernel_packed3(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
 template <typename T, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, int n, int n_steps,
-                      T* root, T* dof_pos, T* dof_vel, const T* pd_tar, const T* ext, T* rb_out, T* contact_out, T* ballio, int32_t* hits) {
+                      EnvArrays<T> io) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
   load_blob(smem, gblob, blob_bytes, &mbar);
@@ -1646,57 +1483,25 @@ physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, co
   if (lc.active) lc.rix = B.t.rix[lane];
   const int nb = M.nb, nd = M.nd;
   PhysCfg<T> pc = make_phys_cfg<T>(*gcfg);
-  const bool with_ball = pc.has_ball && ballio != nullptr;
+  const bool with_ball = pc.has_ball && io.ball != nullptr;
   pc.has_ball = with_ball;
   const int g = lane >> 3, s = lane & 7;
   for (int k = 0; k < EPW; k++) {
     const int64_t e = eb + k;
     if (e >= n) break;
     Lane<T> L;
-    for (int j = 0; j < 4; j++) { L.Q[j] = 0; L.qj[j] = 0; }
-    L.Q[3] = 1; L.qj[3] = 1;
-    for (int j = 0; j < 3; j++) { L.p[j] = 0; L.w[j] = 0; L.v[j] = 0; L.wt[j] = 0; }
-    T pdt[3] = {0, 0, 0}, eF[3] = {0, 0, 0}, eT[3] = {0, 0, 0};
-    if (lane == 0) {
-      const T* rs = root + e * 13;
-      for (int j = 0; j < 3; j++) { L.p[j] = rs[j]; L.v[j] = rs[7 + j]; L.w[j] = rs[10 + j]; }
-      for (int j = 0; j < 4; j++) L.Q[j] = rs[3 + j];
-      qnormalize(L.Q);
-      if (ext) for (int j = 0; j < 3; j++) { eF[j] = ext[e * 6 + j]; eT[j] = ext[e * 6 + 3 + j]; }
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      for (int j = 0; j < 3; j++) { q[j] = dof_pos[e * nd + lc.dof0 + j]; L.wt[j] = dof_vel[e * nd + lc.dof0 + j]; pdt[j] = pd_tar[e * nd + lc.dof0 + j]; }
-      qexp(q, L.qj);
-    }
+    T pdt[3], eF[3], eT[3];
+    env_arrays_load<T>(io, nd, lc, lane, e, L, pdt, eF, eT);
     pk_store_state<T>(wrec + k * ENV_STRIDE, lc, lane, L, pdt, eF, eT);
   }
   __syncwarp();
   const bool valid = eb + g < n;
   Ball<T> ball;
   ball_clear(ball);
-  if (with_ball && valid && s == BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { ball.p[j] = ballio[e * 13 + j]; ball.v[j] = ballio[e * 13 + 7 + j]; ball.w[j] = ballio[e * 13 + 10 + j]; }
-  }
+  if (with_ball && valid && s == BALL_SLOT) env_arrays_load_ball<T>(io, eb + g, ball);
   for (int st_ = 0; st_ < n_steps; st_++) {
     control_step_packed<T>(B, verts, pc, wrec, lane, valid, ball, false);
-    if (st_ + 1 < n_steps) {  // the state crosses control steps as exp-map coordinates
-      for (int k = 0; k < EPW; k++) {
-        if (eb + k >= n) break;
-        if (lc.dyn && lane > 0) {
-          T* rec = wrec + k * ENV_STRIDE + lc.rix * REC;
-          T qj[4], q[3];
-          ldr<R_QJ, 4>(rec, qj);
-          qlog(qj, q);
-          qexp(q, qj);
-          str<R_QJ, 4>(rec, qj);
-        }
-        if (lane == 0) {  // the racket reaction does not carry over a control step in the lane kernel either (ball.rF is per substep)
-        }
-      }
-      __syncwarp();
-    }
+    if (st_ + 1 < n_steps) pk_requantize<T>(wrec, lc, lane, eb, n);
   }
   for (int k = 0; k < EPW; k++) {
     const int64_t e = eb + k;
@@ -1704,28 +1509,9 @@ physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, co
     Lane<T> L;
     T cf[3];
     pk_load_state<T>(wrec + k * ENV_STRIDE, lc, lane, L, cf);
-    if (lane == 0) {
-      T* rs = root + e * 13;
-      for (int j = 0; j < 3; j++) { rs[j] = L.p[j]; rs[7 + j] = L.v[j]; rs[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rs[3 + j] = L.Q[j];
-    }
-    if (lc.dyn && lane > 0) {
-      T q[3];
-      qlog(L.qj, q);
-      for (int j = 0; j < 3; j++) { dof_pos[e * nd + lc.dof0 + j] = q[j]; dof_vel[e * nd + lc.dof0 + j] = L.wt[j]; }
-    }
-    if (lc.active) {
-      T* rb = rb_out + (e * nb + lane) * 13;
-      for (int j = 0; j < 3; j++) { rb[j] = L.p[j]; rb[7 + j] = L.v[j]; rb[10 + j] = L.w[j]; }
-      for (int j = 0; j < 4; j++) rb[3 + j] = L.Q[j];
-      if (contact_out) for (int j = 0; j < 3; j++) contact_out[(e * nb + lane) * 3 + j] = cf[j];
-    }
+    env_arrays_store<T>(io, nb, nd, lc, lane, e, L, cf);
   }
-  if (with_ball && valid && s == BALL_SLOT) {
-    const int64_t e = eb + g;
-    for (int j = 0; j < 3; j++) { ballio[e * 13 + j] = ball.p[j]; ballio[e * 13 + 7 + j] = ball.v[j]; ballio[e * 13 + 10 + j] = ball.w[j]; }
-    if (hits) hits[e] = ball.hits;
-  }
+  if (with_ball && valid && s == BALL_SLOT) env_arrays_store_ball<T>(io, eb + g, ball);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2092,7 +1878,7 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
 template <typename T>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
 physics_kernel(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, int n, int n_steps,
-               T* root, T* dof_pos, T* dof_vel, const T* pd_tar, const T* ext, T* rb_out, T* contact_out, T* ballio, int32_t* hits) {
+               EnvArrays<T> io) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ __align__(8) uint64_t mbar;
   load_blob(smem, gblob, blob_bytes, &mbar);
@@ -2106,30 +1892,14 @@ physics_kernel(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b20
   const int nb = M.nb, nd = M.nd;
   const PhysCfg<T> pc = make_phys_cfg<T>(*gcfg);
   Lane<T> L;
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0; L.qj[k] = 0; }
-  L.Q[3] = 1; L.qj[3] = 1;
-  for (int k = 0; k < 3; k++) { L.p[k] = 0; L.w[k] = 0; L.v[k] = 0; L.wt[k] = 0; }
-  T pdt[3] = {0, 0, 0}, eF[3] = {0, 0, 0}, eT[3] = {0, 0, 0}, cf[3] = {0, 0, 0};
-  if (lane == 0) {
-    const T* rs = root + e * 13;
-    for (int k = 0; k < 3; k++) { L.p[k] = rs[k]; L.v[k] = rs[7 + k]; L.w[k] = rs[10 + k]; }
-    for (int k = 0; k < 4; k++) L.Q[k] = rs[3 + k];
-    qnormalize(L.Q);
-    if (ext) for (int k = 0; k < 3; k++) { eF[k] = ext[e * 6 + k]; eT[k] = ext[e * 6 + 3 + k]; }
-  }
-  if (lc.dyn && lane > 0) {
-    T q[3];
-    for (int k = 0; k < 3; k++) { q[k] = dof_pos[e * nd + lc.dof0 + k]; L.wt[k] = dof_vel[e * nd + lc.dof0 + k]; pdt[k] = pd_tar[e * nd + lc.dof0 + k]; }
-    qexp(q, L.qj);
-  }
+  T pdt[3], eF[3], eT[3], cf[3] = {0, 0, 0};
+  env_arrays_load<T>(io, nd, lc, lane, e, L, pdt, eF, eT);
   Ball<T> ball;
   ball_clear(ball);
-  const bool with_ball = pc.has_ball && ballio != nullptr;
+  const bool with_ball = pc.has_ball && io.ball != nullptr;
   PhysCfg<T> pcb = pc;
   pcb.has_ball = with_ball;
-  if (with_ball && lane == BALL_LANE) {
-    for (int k = 0; k < 3; k++) { ball.p[k] = ballio[e * 13 + k]; ball.v[k] = ballio[e * 13 + 7 + k]; ball.w[k] = ballio[e * 13 + 10 + k]; }
-  }
+  if (with_ball && lane == BALL_LANE) env_arrays_load_ball<T>(io, e, ball);
   for (int s = 0; s < n_steps; s++) {
     control_step<T>(B, verts, pcb, lc, lane, L, pdt, eF, eT, cf, ball);
     if (s + 1 < n_steps && lc.dyn && lane > 0) {  // the state crosses control steps as exp-map coordinates
@@ -2138,26 +1908,22 @@ physics_kernel(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b20
       qexp(q, L.qj);
     }
   }
-  if (lane == 0) {
-    T* rs = root + e * 13;
-    for (int k = 0; k < 3; k++) { rs[k] = L.p[k]; rs[7 + k] = L.v[k]; rs[10 + k] = L.w[k]; }
-    for (int k = 0; k < 4; k++) rs[3 + k] = L.Q[k];
-  }
-  if (lc.dyn && lane > 0) {
-    T q[3];
-    qlog(L.qj, q);
-    for (int k = 0; k < 3; k++) { dof_pos[e * nd + lc.dof0 + k] = q[k]; dof_vel[e * nd + lc.dof0 + k] = L.wt[k]; }
-  }
-  if (lc.active) {
-    T* rb = rb_out + (e * nb + lane) * 13;
-    for (int k = 0; k < 3; k++) { rb[k] = L.p[k]; rb[7 + k] = L.v[k]; rb[10 + k] = L.w[k]; }
-    for (int k = 0; k < 4; k++) rb[3 + k] = L.Q[k];
-    if (contact_out) for (int k = 0; k < 3; k++) contact_out[(e * nb + lane) * 3 + k] = cf[k];
-  }
-  if (with_ball && lane == BALL_LANE) {
-    for (int k = 0; k < 3; k++) { ballio[e * 13 + k] = ball.p[k]; ballio[e * 13 + 7 + k] = ball.v[k]; ballio[e * 13 + 10 + k] = ball.w[k]; }
-    if (hits) hits[e] = ball.hits;
-  }
+  env_arrays_store<T>(io, nb, nd, lc, lane, e, L, cf);
+  if (with_ball && lane == BALL_LANE) env_arrays_store_ball<T>(io, e, ball);
+}
+
+// one launch of a physics-only kernel over n envs: warps per CTA, envs per CTA, and the bytes of records each CTA keeps in shared memory
+// behind the header
+template <typename T>
+static int launch_physics_only(b200env* h, void (*kernel)(const DevBlob*, uint32_t, const b200_cfg_t*, int, int, EnvArrays<T>), int warps,
+                               int envs_per_cta, size_t rec_bytes, int n, int n_steps, const EnvArrays<T>& io, void* stream) {
+  const size_t sm = ((h->blob_bytes + 15) & ~(size_t)15) + rec_bytes;
+  CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  kernel<<<(n + envs_per_cta - 1) / envs_per_cta, warps * 32, sm, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes,
+                                                                                         h->d_cfg, n, n_steps, io);
+  CUDA_OK(cudaGetLastError());
+  h->launches++;
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2819,55 +2585,20 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
   if (!h || !root || !dof_pos || !dof_vel || !pd_tar || !rb_out) return fail(-1, "b200env_physics_only: null argument%s");
   if (n <= 0 || n_steps <= 0) return fail(-2, "b200env_physics_only: n and n_steps must be positive%s");
   if (h->num_assets) return fail(-2, "b200env_physics_only: not supported on a handle of several assets (b200env_create_assets)%s");
+  if (prec != 0 && prec != 1) return fail(-2, "b200env_physics_only: prec must be 0 (float) or 1 (double)%s");
   cudaSetDevice(h->device);
-  if (h->packed) {
-    const size_t bsm = (h->blob_bytes + 15) & ~(size_t)15;
-    if (prec == 0 && h->tmem) {
-      constexpr int W = 6;   // more than 4 warps: several CTA batches of the test kernel in small tests
-      const size_t sm = bsm + (size_t)W * EPW * PT_ENV_STRIDE * sizeof(float);
-      CUDA_OK(cudaFuncSetAttribute(physics_kernel_tmem<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      physics_kernel_tmem<W><<<(n + W * EPW - 1) / (W * EPW), W * 32, sm, (cudaStream_t)stream>>>(
-          (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, n, n_steps, (float*)root, (float*)dof_pos, (float*)dof_vel,
-          (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out, (float*)contact_out, (float*)ball, ball_hits);
-    } else if (prec == 0) {
-      constexpr int W = 4;
-      const size_t sm = bsm + (size_t)W * EPW * ENV_STRIDE * sizeof(float);
-      CUDA_OK(cudaFuncSetAttribute(physics_kernel_packed<float, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      physics_kernel_packed<float, W><<<(n + W * EPW - 1) / (W * EPW), W * 32, sm, (cudaStream_t)stream>>>(
-          (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, n, n_steps, (float*)root, (float*)dof_pos, (float*)dof_vel,
-          (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out, (float*)contact_out, (float*)ball, ball_hits);
-    } else if (prec == 1) {
-      constexpr int W = 2;
-      const size_t sm = bsm + (size_t)W * EPW * ENV_STRIDE * sizeof(double);
-      CUDA_OK(cudaFuncSetAttribute(physics_kernel_packed<double, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      physics_kernel_packed<double, W><<<(n + W * EPW - 1) / (W * EPW), W * 32, sm, (cudaStream_t)stream>>>(
-          (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, n, n_steps, (double*)root, (double*)dof_pos, (double*)dof_vel,
-          (const double*)pd_tar, (const double*)ext_wrench, (double*)rb_out, (double*)contact_out, (double*)ball, ball_hits);
-    } else {
-      return fail(-2, "b200env_physics_only: prec must be 0 (float) or 1 (double)%s");
-    }
-    CUDA_OK(cudaGetLastError());
-    h->launches++;
-    return 0;
-  }
-  const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-  const size_t smem = (h->blob_bytes + 15) & ~(size_t)15;
   if (prec == 0) {
-    CUDA_OK(cudaFuncSetAttribute(physics_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    physics_kernel<float><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(
-        (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, n, n_steps, (float*)root, (float*)dof_pos, (float*)dof_vel,
-        (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out, (float*)contact_out, (float*)ball, ball_hits);
-  } else if (prec == 1) {
-    CUDA_OK(cudaFuncSetAttribute(physics_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    physics_kernel<double><<<grid, WARPS_PER_CTA * 32, smem, (cudaStream_t)stream>>>(
-        (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, n, n_steps, (double*)root, (double*)dof_pos, (double*)dof_vel,
-        (const double*)pd_tar, (const double*)ext_wrench, (double*)rb_out, (double*)contact_out, (double*)ball, ball_hits);
-  } else {
-    return fail(-2, "b200env_physics_only: prec must be 0 (float) or 1 (double)%s");
+    const EnvArrays<float> io{(float*)root, (float*)dof_pos, (float*)dof_vel, (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out,
+                              (float*)contact_out, (float*)ball, ball_hits};
+    // the one-wave form at 6 warps (more than 4: several CTA batches of the test kernel in small tests)
+    if (h->packed && h->tmem) return launch_physics_only(h, physics_kernel_tmem<6>, 6, 6 * EPW, 6 * EPW * PT_ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
+    if (h->packed) return launch_physics_only(h, physics_kernel_packed<float, 4>, 4, 4 * EPW, 4 * EPW * ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
+    return launch_physics_only(h, physics_kernel<float>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
   }
-  CUDA_OK(cudaGetLastError());
-  h->launches++;
-  return 0;
+  const EnvArrays<double> io{(double*)root, (double*)dof_pos, (double*)dof_vel, (const double*)pd_tar, (const double*)ext_wrench, (double*)rb_out,
+                             (double*)contact_out, (double*)ball, ball_hits};
+  if (h->packed) return launch_physics_only(h, physics_kernel_packed<double, 2>, 2, 2 * EPW, 2 * EPW * ENV_STRIDE * sizeof(double), n, n_steps, io, stream);
+  return launch_physics_only(h, physics_kernel<double>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
 }
 
 #if PT_PROF

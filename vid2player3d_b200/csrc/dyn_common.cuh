@@ -319,6 +319,14 @@ template <typename T> struct Lane {
   T Q[4], p[3], w[3], v[3];  // world pose and velocity of the body origin
   T qj[4], wt[3];            // joint rotation (child in parent) and joint velocity (child frame)
 };
+// the body at rest: zero vectors, identity rotations (what a lane without a body, or without a joint, holds)
+template <typename T> __device__ __forceinline__ void lane_rest(Lane<T>& L) {
+#pragma unroll
+  for (int k = 0; k < 4; k++) { L.Q[k] = 0; L.qj[k] = 0; }
+  L.Q[3] = 1; L.qj[3] = 1;
+#pragma unroll
+  for (int k = 0; k < 3; k++) { L.p[k] = 0; L.w[k] = 0; L.v[k] = 0; L.wt[k] = 0; }
+}
 struct LaneConst {
   int par, depth, dof0;
   int rix;           // packed kernels: the body's record index (DevTree::rix); set by the kernel after lane_const()
@@ -834,5 +842,125 @@ __device__ __forceinline__ LaneConst lane_const(const b200_model_t& M, int lane)
   lc.dyn = lc.active && !M.fixed[lane];
   lc.rix = lane;
   return lc;
+}
+
+// ------------------------------------------------------------------------------------------
+// state I/O of one env (lane = body)
+
+// Middle launch of the split step: the state rows the pre_kernel left behind for the NE envs of the hand-out positions eb .. eb + NE - 1
+// (row(i) = the env row of position i): root row, joint state, PD targets and residual wrench (ext_wrench [N][6]).  Every load of the
+// NE envs is issued before the first use (one memory latency instead of NE); positions from end on (a ragged tail) re-read the last env
+// and are not unpacked.  gather_state_rows loads, unpack_state_row gives env eb + k as the physics wants it.  The caller keeps the
+// loop over k: with the loop and the record store inside one helper the step kernels' SASS is scheduled differently.
+template <int NE> struct StateRows {
+  float rq[NE][3], rw[NE][3], rp[NE][3];   // joint exp-map coordinates, joint velocity, PD target
+  float r1[NE];                            // lane j < 13: root_states[e][j], 13 <= j < 19: the residual wrench
+};
+template <int NE, typename Row>
+__device__ __forceinline__ void gather_state_rows(const b200_buffers_t& bf, const b200_model_t& M, const LaneConst& lc, int lane, int64_t eb,
+                                                  int64_t end, const Row& row, const float* __restrict__ ext_wrench, StateRows<NE>& r) {
+  const int nd = M.nd;
+#pragma unroll
+  for (int k = 0; k < NE; k++) {
+    const int64_t ek = eb + k < end ? eb + k : end - 1;
+    const int64_t e = row(ek);
+    if (lc.dyn && lane > 0) {
+      const float* ds = bf.dof_state + (e * nd + lc.dof0) * 2;
+#pragma unroll
+      for (int j = 0; j < 3; j++) { r.rq[k][j] = ds[2 * j]; r.rw[k][j] = ds[2 * j + 1]; r.rp[k][j] = bf.pd_targets[e * nd + lc.dof0 + j]; }
+    }
+    r.r1[k] = lane < 13 ? bf.root_states[e * bf.actors_per_env * 13 + lane] : (lane < 19 ? ext_wrench[e * 6 + lane - 13] : 0.f);
+  }
+}
+template <int NE>
+__device__ __forceinline__ void unpack_state_row(const StateRows<NE>& r, int k, const LaneConst& lc, int lane, Lane<float>& L, float* pdtar,
+                                                 float* extF, float* extT) {
+  lane_rest(L);
+#pragma unroll
+  for (int j = 0; j < 3; j++) { pdtar[j] = 0.f; extF[j] = 0.f; extT[j] = 0.f; }
+  float rr[19];
+#pragma unroll
+  for (int j = 0; j < 19; j++) rr[j] = __shfl_sync(FULL, r.r1[k], j);
+  if (lane == 0) {
+#pragma unroll
+    for (int j = 0; j < 3; j++) { L.p[j] = rr[j]; L.v[j] = rr[7 + j]; L.w[j] = rr[10 + j]; extF[j] = rr[13 + j]; extT[j] = rr[16 + j]; }
+#pragma unroll
+    for (int j = 0; j < 4; j++) L.Q[j] = rr[3 + j];
+    qnormalize(L.Q);
+  }
+  if (lc.dyn && lane > 0) {
+#pragma unroll
+    for (int j = 0; j < 3; j++) { L.wt[j] = r.rw[k][j]; pdtar[j] = r.rp[k][j]; }
+    qexp(r.rq[k], L.qj);
+  }
+}
+
+// The arrays of the physics-only entry (b200env_physics_only; the CPU lane emulator has the same signature): root [n][13],
+// dof_pos / dof_vel / pd_tar [n][nd], ext [n][6], rb_out [n][nb][13], contact_out [n][nb][3], ball [n][13] (p, -, v, w as a root row),
+// hits [n].  ext, contact_out, ball and hits may be null.
+template <typename T> struct EnvArrays {
+  T *root, *dof_pos, *dof_vel;
+  const T *pd_tar, *ext;
+  T *rb_out, *contact_out, *ball;
+  int32_t* hits;
+};
+template <typename T>
+__device__ __forceinline__ void env_arrays_load(const EnvArrays<T>& io, int nd, const LaneConst& lc, int lane, int64_t e, Lane<T>& L, T* pdt,
+                                                T* eF, T* eT) {
+  lane_rest(L);
+#pragma unroll
+  for (int j = 0; j < 3; j++) { pdt[j] = 0; eF[j] = 0; eT[j] = 0; }
+  if (lane == 0) {
+    const T* rs = io.root + e * 13;
+#pragma unroll
+    for (int j = 0; j < 3; j++) { L.p[j] = rs[j]; L.v[j] = rs[7 + j]; L.w[j] = rs[10 + j]; }
+#pragma unroll
+    for (int j = 0; j < 4; j++) L.Q[j] = rs[3 + j];
+    qnormalize(L.Q);
+    if (io.ext) for (int j = 0; j < 3; j++) { eF[j] = io.ext[e * 6 + j]; eT[j] = io.ext[e * 6 + 3 + j]; }
+  }
+  if (lc.dyn && lane > 0) {
+    T q[3];
+#pragma unroll
+    for (int j = 0; j < 3; j++) { q[j] = io.dof_pos[e * nd + lc.dof0 + j]; L.wt[j] = io.dof_vel[e * nd + lc.dof0 + j]; pdt[j] = io.pd_tar[e * nd + lc.dof0 + j]; }
+    qexp(q, L.qj);
+  }
+}
+// cf: the contact force of the lane's body, written for every body.  cf = null: the step wrote the rows of the jointed bodies itself
+// (control_step_t), a welded body's row is 0.
+template <typename T>
+__device__ __forceinline__ void env_arrays_store(const EnvArrays<T>& io, int nb, int nd, const LaneConst& lc, int lane, int64_t e, const Lane<T>& L,
+                                                 const T* cf) {
+  if (lane == 0) {
+    T* rs = io.root + e * 13;
+#pragma unroll
+    for (int j = 0; j < 3; j++) { rs[j] = L.p[j]; rs[7 + j] = L.v[j]; rs[10 + j] = L.w[j]; }
+#pragma unroll
+    for (int j = 0; j < 4; j++) rs[3 + j] = L.Q[j];
+  }
+  if (lc.dyn && lane > 0) {
+    T q[3];
+    qlog(L.qj, q);
+#pragma unroll
+    for (int j = 0; j < 3; j++) { io.dof_pos[e * nd + lc.dof0 + j] = q[j]; io.dof_vel[e * nd + lc.dof0 + j] = L.wt[j]; }
+  }
+  if (lc.active) {
+    T* rb = io.rb_out + (e * nb + lane) * 13;
+#pragma unroll
+    for (int j = 0; j < 3; j++) { rb[j] = L.p[j]; rb[7 + j] = L.v[j]; rb[10 + j] = L.w[j]; }
+#pragma unroll
+    for (int j = 0; j < 4; j++) rb[3 + j] = L.Q[j];
+    if (io.contact_out && (cf || !lc.dyn))
+      for (int j = 0; j < 3; j++) io.contact_out[(e * nb + lane) * 3 + j] = cf ? cf[j] : T(0);
+  }
+}
+template <typename T> __device__ __forceinline__ void env_arrays_load_ball(const EnvArrays<T>& io, int64_t e, Ball<T>& ball) {
+#pragma unroll
+  for (int j = 0; j < 3; j++) { ball.p[j] = io.ball[e * 13 + j]; ball.v[j] = io.ball[e * 13 + 7 + j]; ball.w[j] = io.ball[e * 13 + 10 + j]; }
+}
+template <typename T> __device__ __forceinline__ void env_arrays_store_ball(const EnvArrays<T>& io, int64_t e, const Ball<T>& ball) {
+#pragma unroll
+  for (int j = 0; j < 3; j++) { io.ball[e * 13 + j] = ball.p[j]; io.ball[e * 13 + 7 + j] = ball.v[j]; io.ball[e * 13 + 10 + j] = ball.w[j]; }
+  if (io.hits) io.hits[e] = ball.hits;
 }
 

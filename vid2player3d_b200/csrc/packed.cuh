@@ -906,11 +906,9 @@ template <typename T> __device__ __forceinline__ void pk_store_state(T* env, con
   }
 }
 template <typename T> __device__ __forceinline__ void pk_load_state(const T* env, const LaneConst& lc, int lane, Lane<T>& L, T* cf) {
+  lane_rest(L);
 #pragma unroll
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0; L.qj[k] = 0; }
-  L.Q[3] = 1; L.qj[3] = 1;
-#pragma unroll
-  for (int k = 0; k < 3; k++) { L.p[k] = 0; L.w[k] = 0; L.v[k] = 0; L.wt[k] = 0; cf[k] = 0; }
+  for (int k = 0; k < 3; k++) cf[k] = 0;
   if (lc.active) {
     const T* rec = env + lc.rix * REC;
     T o[16];
@@ -929,4 +927,20 @@ template <typename T> __device__ __forceinline__ void pk_load_state(const T* env
       }
     }
   }
+}
+// between two control steps of the test kernels the joint rotation crosses as exp-map coordinates (like the state rows do); the
+// records of the warp's NE envs eb, eb + 1, .. below n.  Twin of pt_requantize.
+template <typename T, int NE = EPW> __device__ __forceinline__ void pk_requantize(T* wrec, const LaneConst& lc, int lane, int64_t eb, int64_t n) {
+  for (int k = 0; k < NE; k++) {
+    if (eb + k >= n) break;
+    if (lc.dyn && lane > 0) {
+      T* rec = wrec + k * ENV_STRIDE + lc.rix * REC;
+      T qj[4], q[3];
+      ldr<R_QJ, 4>(rec, qj);
+      qlog(qj, q);
+      qexp(q, qj);
+      str<R_QJ, 4>(rec, qj);
+    }
+  }
+  __syncwarp();
 }

@@ -768,11 +768,7 @@ __device__ __forceinline__ void pt_requantize(const DevBlob& B, int lane, bool v
   }
 }
 template <typename T> __device__ __forceinline__ void pt_load_state(const T* env, const LaneConst& lc, int lane, Lane<T>& L) {
-#pragma unroll
-  for (int k = 0; k < 4; k++) { L.Q[k] = 0; L.qj[k] = 0; }
-  L.Q[3] = 1; L.qj[3] = 1;
-#pragma unroll
-  for (int k = 0; k < 3; k++) { L.p[k] = 0; L.w[k] = 0; L.v[k] = 0; L.wt[k] = 0; }
+  lane_rest(L);
   if (lc.active) {
     const T* rec = env + lc.rix * PT_REC;
     T o[13];
