@@ -76,7 +76,7 @@ typedef struct b200_cfg {
   float k_dof, k_vel, k_pos, k_rot, w_dof, w_vel, w_pos, w_rot; /* reward_specs :682 */
   int32_t num_key;
   int32_t key_body[B200_MAX_KEY];                         /* keyBodies */
-  int32_t shape_dim;                                      /* motion_bodies width (11) */
+  int32_t shape_dim;                                      /* motion_bodies width (11); create refuses it outside [0, 32] */
   float ground_tolerance;
   /* --- vid2player physics player env (vid2player/env/tasks/humanoid_smpl_im_mvae.py) --- */
   int32_t task_mode;   /* 0: HumanoidSMPLIM (MoCap target + obs + reward + reset fused in the step)
@@ -201,7 +201,8 @@ int b200env_motion_state(b200env_handle h, const int64_t* motion_ids, const floa
 
 /* replaces compute_humanoid_observations_imitation (humanoid_smpl_im.py:773-850 ==
  * models/im_network_builder.py:262-338): obs [n,1+..=734 for 24 bodies].  Bit 1 of `local_root_obs` selects the
- * 'joint_pos' variant compute_humanoid_observations_imitation_jpos (:853-915, 513 wide). */
+ * 'joint_pos' variant compute_humanoid_observations_imitation_jpos (:853-915, 513 wide).  Returns -2 before any launch when the
+ * row is wider than 768 columns or the humanoid has more than 32 bodies (one lane per body). */
 int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, const float* body_rot,
                           const float* target_pos, const float* target_rot, const float* dof_pos, const float* dof_vel,
                           const float* target_dof_pos, const float* body_vel, const float* body_ang_vel,
@@ -213,7 +214,10 @@ int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, co
  * instead of six contiguous gathers of them (what the reference's slicing + cat amounts to, humanoid_smpl_im_mvae.py:862-895).
  * obs_bf16 (may be NULL): additionally writes the policy's first-layer operand row, bf16(clamp((obs - mean) * rstd, -clamp, clamp)),
  * [n, ld_bf16] (RunningMeanStd + the +-5 clamp of ImitatorPlayer.run_one_step, vid2player/players/im_player.py:187-190; mean /
- * rstd NULL = no normalisation), so that the network forward (include/b200nn.h) starts without a cast launch. */
+ * rstd NULL = no normalisation), so that the network forward (include/b200nn.h) starts without a cast launch.  Bit 1 of
+ * `local_root_obs` selects the 'joint_pos' variant, as above.  Returns -2 before any launch on the refusals of
+ * b200env_obs_imitation, and when obs_bf16 is given with ld_bf16 smaller than the row width, an odd ld_bf16 or an address that is not
+ * 4-byte aligned (the row is stored as bf16 pairs). */
 int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_body_state, int32_t bodies_per_env, const float* dof_state,
                                const float* target_pos, const float* target_rot, const float* target_dof_pos, const float* motion_bodies,
                                int32_t local_root_obs, int32_t root_height_obs, float* obs, void* obs_bf16, int32_t ld_bf16, const float* mean,

@@ -1730,6 +1730,11 @@ reset_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __rest
 // element strides of the state arrays of obs_imitation_kernel: contiguous [n, nb, 3] / [n, nb, 4] / [n, nd] copies (legacy entry) or the
 // Isaac-layout rows themselves (rigid_body_state [n, bodies_per_env, 13], dof_state [n, nd, 2]) - no gather copies
 #define OBS_ROW_MAX 768   // widest observation row: 734 (24 bodies, 69 dof, shape 11)
+// row width of obs_imitation_kernel; jpos = compute_humanoid_observations_imitation_jpos (:853-915): no rotation / heading / dof targets
+__host__ __device__ inline int obs_row_width(int nb, int nd, int shape_dim, bool jpos) {
+  return jpos ? 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 2 + nb * 3 + shape_dim
+              : 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 6 + 2 + 2 + nd + nb * 3 + nb * 6 + shape_dim;
+}
 struct ObsStrides { int p_row, p_elem, q_row, q_elem, d_row, d_elem; };
 struct ObsBf16 { __nv_bfloat16* out; int ld; const float* mean; const float* rstd; float clamp; };
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
@@ -1741,15 +1746,13 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t e = (int64_t)blockIdx.x * WARPS_PER_CTA + warp;
   if (e >= n) return;
-  // jpos = compute_humanoid_observations_imitation_jpos (:853-915): no rotation / heading / dof targets
-  const int W = jpos ? 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 2 + nb * 3 + shape_dim
-                     : 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 6 + 2 + 2 + nd + nb * 3 + nb * 6 + shape_dim;
+  const int W = obs_row_width(nb, nd, shape_dim, jpos);
   // every value goes through put() into the warp's row in shared memory; the row leaves at the end as coalesced 8-byte stores
   // (the per-lane pieces - 3 / 6 values per body - are 12 / 24 bytes apart: written straight to global memory they made the launch
   // ~30 us for 36 MB) - the float row the reference returns and, when asked for, the bf16 operand row of the policy's first layer =
   // clamp((x - mean) * rstd, -clamp, clamp) (RunningMeanStd + the +-5 clamp of im_player.py:187-190) from the same values
   __shared__ __align__(16) float s_obs[WARPS_PER_CTA][OBS_ROW_MAX];
-  if (W > OBS_ROW_MAX) return;            // cannot happen with the 24-body SMPL humanoid (W = 734 / 513); the host entry points check nb
+  if (W > OBS_ROW_MAX) return;            // unreachable: both host entry points refuse W > OBS_ROW_MAX (and nb or shape_dim > 32)
   float* srow = s_obs[warp];
   auto put = [&](int idx, float val) { srow[idx] = val; };
   const bool act = lane < nb;
@@ -1868,7 +1871,7 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
       // torch.clamp semantics: a NaN feature stays NaN in the operand (fminf / fmaxf would hide a blown-up env behind -clamp)
       asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x0) : "f"(ob.clamp), "f"(-ob.clamp));
       asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x1) : "f"(ob.clamp), "f"(-ob.clamp));
-      if (k + 1 < W) *reinterpret_cast<__nv_bfloat162*>(brow + k) = __floats2bfloat162_rn(x0, x1);   // ld is a multiple of 64: 4-byte aligned
+      if (k + 1 < W) *reinterpret_cast<__nv_bfloat162*>(brow + k) = __floats2bfloat162_rn(x0, x1);   // the host checks: ld even, out 4-byte aligned
       else brow[k] = __float2bfloat16_rn(x0);
     }
   }
@@ -1944,6 +1947,7 @@ int b200env_create(const b200_model_t* model, const float* verts, const b200_cfg
     if (model->nverts[b] < 0 || model->nverts[b] > 64 || model->nverts[b] > model->vmax)
       return fail(-2, "b200env_create: at most 64 hull vertices per body (contact_hull keeps a 64-bit penetration mask)%s");
   if (num_envs < 1) return fail(-2, "b200env_create: num_envs must be positive%s");
+  if (cfg->shape_dim < 0 || cfg->shape_dim > 32) return fail(-2, "b200env_create: shape_dim must be in [0, 32] (one lane per column)%s");
   if (cfg->has_ball && model->nb > BALL_LANE) return fail(-2, "b200env_create: has_ball needs nb <= 31 (lane 31 integrates the ball)%s");
   if (cfg->has_ball && cfg->racket_body >= model->nb) return fail(-2, "b200env_create: racket_body out of range%s");
   int ndev = 0;
@@ -2105,6 +2109,8 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   if (!models || !verts || !env_asset || !cfg || !out) return fail(-1, "b200env_create_assets: null argument%s");
   if (num_assets < 1) return fail(-2, "b200env_create_assets: num_assets must be at least 1%s");
   if (num_envs < 1) return fail(-2, "b200env_create_assets: num_envs must be positive%s");
+  if (cfg->shape_dim < 0 || cfg->shape_dim > 32)
+    return fail(-2, "b200env_create_assets: shape_dim must be in [0, 32] (one lane per column)%s");
   const b200_model_t& m0 = models[0];
   for (int a = 0; a < num_assets; a++) {
     const b200_model_t& m = models[a];
@@ -2533,6 +2539,15 @@ int b200env_motion_context(b200env_handle h, const int64_t* env_ids, const int64
   return 0;
 }
 
+// obs_imitation_kernel gives a body and a motion-body column to each lane of a warp and builds the row in a shared-memory slot of
+// OBS_ROW_MAX floats: refuse what it cannot write instead of leaving the caller's rows stale
+static int obs_row_check(const char* who, int nbl, int shape_dim, int W) {
+  if (nbl > 32) return fail(-2, "%s: more than 32 humanoid bodies (one lane per body)", who);
+  if (shape_dim > 32) return fail(-2, "%s: shape_dim above 32 (one lane per motion-body column)", who);
+  if (W > OBS_ROW_MAX) return fail(-2, "%s: observation row wider than OBS_ROW_MAX (768) columns", who);
+  return 0;
+}
+
 int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, const float* body_rot, const float* target_pos,
                           const float* target_rot, const float* dof_pos, const float* dof_vel, const float* target_dof_pos,
                           const float* body_vel, const float* body_ang_vel, const float* motion_bodies, int32_t local_root_obs,
@@ -2542,8 +2557,10 @@ int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, co
   if (!body_pos || !body_rot || !target_pos || !target_rot || !dof_pos || !dof_vel || !target_dof_pos || !body_vel || !body_ang_vel ||
       !motion_bodies || !obs || n < 0)
     return fail(-1, "b200env_obs_imitation: bad arguments%s");
-  cudaSetDevice(h->device);
   const int nbl = h->has_ml ? h->ml.num_lib_bodies : (h->model.fixed[h->model.nb - 1] ? h->model.nb - 1 : h->model.nb);
+  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, (local_root_obs >> 1) & 1);
+  if (int rc = obs_row_check("b200env_obs_imitation", nbl, h->cfg.shape_dim, W)) return rc;
+  cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
   obs_imitation_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(n, nbl, h->model.nd, h->cfg.shape_dim, body_pos, body_rot,
                                                                               target_pos, target_rot, dof_pos, dof_vel, target_dof_pos,
@@ -2566,6 +2583,13 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
   if (bodies_per_env < nbl) return fail(-2, "b200env_obs_imitation_rows: bodies_per_env smaller than the humanoid%s");
   if ((mean == nullptr) != (rstd == nullptr)) return fail(-2, "b200env_obs_imitation_rows: mean and rstd go together%s");
   if (obs_bf16 && !(clamp > 0.f)) return fail(-2, "b200env_obs_imitation_rows: the bf16 row needs a positive clamp%s");
+  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, (local_root_obs >> 1) & 1);
+  if (int rc = obs_row_check("b200env_obs_imitation_rows", nbl, h->cfg.shape_dim, W)) return rc;
+  if (obs_bf16) {   // the row goes out as bfloat162 pairs from column 0 of every row
+    if (ld_bf16 < W) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 is smaller than the observation row%s");
+    if (ld_bf16 & 1) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 must be even%s");
+    if (reinterpret_cast<uintptr_t>(obs_bf16) & 3) return fail(-2, "b200env_obs_imitation_rows: obs_bf16 must be 4-byte aligned%s");
+  }
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
   const int nd = h->model.nd;

@@ -144,6 +144,13 @@ class Env:
         v.total_frames = t["gts"].shape[0]
         self._keep.append(t)
         _check(lib().b200env_set_motion_lib(self._h, C.byref(v)))
+        self._num_lib_bodies = int(num_lib_bodies)
+
+    @property
+    def lib_bodies(self):
+        """humanoid bodies of the observation: the motion library's body count, else the model's bodies without a welded last one"""
+        nb = int(self.model.nb)
+        return getattr(self, "_num_lib_bodies", nb - 1 if self.model.fixed[nb - 1] else nb)
 
     def set_hull_faces(self, planes, tris, ntris, tmax):
         """hull faces for the exact ball / convex-hull contact (abi.pack_faces); host numpy arrays, copied by the library"""
@@ -198,9 +205,17 @@ class Env:
                                             C.c_int32(int(num_frames)), C.c_int32(int(first_frame)), C.c_float(float(dt)), _ptr(feat),
                                             _ptr(mask), _stream()))
 
+    def obs_row_width(self, jpos=False):
+        """columns of the row the observation launches write: 734 (513 with jpos) for the 24-body humanoid, 69 dofs, shape_dim 11"""
+        nbl = self.lib_bodies
+        nd, sd = int(self.model.nd), int(self.cfg.shape_dim)
+        w = 1 + (nbl - 1) * 3 + nbl * 6 + nbl * 6 + nd + sd
+        return w + ((3 + nbl * 3) if jpos else (11 + nd + nbl * 9))
+
     def obs_imitation(self, body_pos, body_rot, target_pos, target_rot, dof_pos, dof_vel, target_dof_pos, body_vel,
                       body_ang_vel, motion_bodies, local_root_obs, root_height_obs, obs, jpos=False):
         n = int(body_pos.shape[0])
+        assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == self.obs_row_width(jpos), (tuple(obs.shape), self.obs_row_width(jpos))
         _check(lib().b200env_obs_imitation(self._h, C.c_int32(n), _ptr(body_pos), _ptr(body_rot), _ptr(target_pos),
                                            _ptr(target_rot), _ptr(dof_pos), _ptr(dof_vel), _ptr(target_dof_pos),
                                            _ptr(body_vel), _ptr(body_ang_vel), _ptr(motion_bodies),
@@ -208,12 +223,16 @@ class Env:
                                            _stream()))
 
     def obs_imitation_rows(self, n, rigid_body_state, bodies_per_env, dof_state, target_pos, target_rot, target_dof_pos, motion_bodies,
-                           local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0):
-        """the 734-d observation straight from the state rows (no gathers); obs_bf16: padded bf16 operand buffer of the policy's
-        first layer, written in the same launch (normalised by mean / rstd when given, clamped to +-clamp)"""
+                           local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0, jpos=False):
+        """the 734-d observation (513-d with jpos) straight from the state rows (no gathers); obs_bf16: padded bf16 operand buffer of
+        the policy's first layer, written in the same launch (normalised by mean / rstd when given, clamped to +-clamp)"""
+        W = self.obs_row_width(jpos)
+        assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == W, (tuple(obs.shape), W)
+        assert obs_bf16 is None or (obs_bf16.dim() == 2 and obs_bf16.shape[0] >= n), tuple(obs_bf16.shape)
         _check(lib().b200env_obs_imitation_rows(self._h, C.c_int32(int(n)), _ptr(rigid_body_state), C.c_int32(int(bodies_per_env)), _ptr(dof_state),
                                                 _ptr(target_pos), _ptr(target_rot), _ptr(target_dof_pos), _ptr(motion_bodies),
-                                                C.c_int32(int(bool(local_root_obs))), C.c_int32(int(root_height_obs)), _ptr(obs), _ptr(obs_bf16),
+                                                C.c_int32(int(bool(local_root_obs)) | (2 if jpos else 0)), C.c_int32(int(root_height_obs)),
+                                                _ptr(obs), _ptr(obs_bf16),
                                                 C.c_int32(int(obs_bf16.shape[1]) if obs_bf16 is not None else 0), _ptr(mean), _ptr(rstd),
                                                 C.c_float(float(clamp)), _stream()))
 

@@ -329,6 +329,7 @@ class PhysicsMVAEController:
         phys = env.get("physics", {})
         pcfg = {"env": dict(numEnvs=self.num_envs, episodeLength=self._max_episode_length, controlFrequencyInv=env.get("controlFrequencyInv", 2),
                             residual_force_scale=phys.get("residual_force_scale", 31.85), is_train=self._is_train,
+                            localRootObs=phys.get("localRootObs", True), rootHeightObs=phys.get("rootHeightObs", True),   # tennis_im.yaml:17
                             asset=dict(assetFileName=phys.get("assetFileName", "smpl_mesh_humanoid_federer.xml")),
                             plane=dict(staticFriction=1.0, dynamicFriction=1.0, restitution=phys.get("plane_restitution", 0.0)),
                             vid2player=dict(self.cfg_v2p),
