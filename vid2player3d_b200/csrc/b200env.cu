@@ -23,6 +23,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <climits>
 #include <vector>
 
 #include "../../include/b200env.h"
@@ -51,6 +52,11 @@
 #endif
 
 
+// The physics launch of b200env_step, chosen once per handle by choose_form (Grouped, Mixed: b200env_create_assets).  Lane and Fused
+// run the whole step in one launch; the others are the middle launch of pre_kernel -> physics -> post_kernel.  The kernel of each
+// form: physics_launch_config.
+enum class PhysForm { Lane, Fused, Split, Sorted, Tmem, Packed3, Grouped, Mixed };
+
 struct b200env {
   int device;
   int num_envs;
@@ -68,22 +74,17 @@ struct b200env {
   unsigned long long ticket_base;
   float* d_ext;                        // [num_envs rows of the bound tensors, 6] residual root wrench between pre_kernel and the physics launch
   int ext_rows;
-  int sort;                            // 1: envs handed out by contact load (B200ENV_SORT=1; split form, 4-envs-per-warp kernel)
-  int32_t *d_bin, *d_perm;             // [num_envs]
+  PhysForm form;                       // the physics launch of b200env_step, fixed at create
+  int32_t *d_bin, *d_perm;             // PhysForm::Sorted: [num_envs]
   uint32_t *d_pos, *d_cnt;             // [num_envs], [SORT_BINS]
-  int packed3;                         // 1: the physics launch is step_kernel_packed3 (B200ENV_KERNEL=packed3)
-  int tmem;                            // 1: the physics launch is step_kernel_tmem (56 envs per SM, private fields in thread-local memory; B200ENV_KERNEL=tmem)
-  int split;                           // 1: three launches (pre / physics / post), 0: one fused launch.  env B200ENV_SPLIT=0|1
   int env_first = 0, env_stride = 1;   // b200env_set_env_slice: local env i = row env_first + env_stride * i of the bound tensors
   int step_slots;                      // resident CTA slots of the persistent physics launch (0 = not computed yet)
   int step_grid;                       // CTAs of the physics launch: min(step_slots, batches of num_envs)
-  int packed;        // 1: 4-envs-per-warp kernels (packed.cuh); 0: lane-per-body kernels.  env B200ENV_KERNEL=lane|packed
-  int packed_ok;     // tree fits the packed layout (<= 8 bodies per depth, <= 25 bodies)
   int64_t launches;
   int timing;                          // b200env_set_kernel_timing: event pairs around the physics launch
   std::vector<cudaEvent_t>* tev;       // recorded (start, stop) pairs
   // b200env_create_assets: several assets of one topology (0 = a b200env_create handle).  d_blob holds asset 0 (what every launch but
-  // the physics launch reads: topology only); the physics launch step_kernel_packed<true, true> hands out the batches of the plan.
+  // the physics launch reads: topology only); the physics launch of PhysForm::Grouped hands out the batches of the plan.
   int num_assets;
   void* d_assets;                      // every asset's DevBlob header + SoA vertices, back to back
   const DevBlob** d_asset_ptr;         // [num_assets] into d_assets
@@ -91,9 +92,8 @@ struct b200env {
   int4* d_batches;                     // [num_batches] {asset, first position in d_rows, count, 0}
   int num_batches;
   std::vector<int32_t>* plan;          // host copy: rows [num_envs] | asset, first, count [num_batches] each
-  // the mixed plan (b200env_plan_assets_mixed, chosen by asset_plan_choice): batches of consecutive envs whatever their assets, run
-  // by step_kernel_packed<true, false, true>; d_env_blob[e] = env e's asset header in d_assets (d_rows / d_batches stay unset)
-  int mixed;
+  // the mixed plan (b200env_plan_assets_mixed, PhysForm::Mixed): batches of consecutive envs whatever their assets;
+  // d_env_blob[e] = env e's asset header in d_assets (d_rows / d_batches stay unset)
   const DevBlob** d_env_blob;
 };
 
@@ -107,6 +107,8 @@ static int fail(int code, const char* fmt, const char* detail = "") {
     cudaError_t _e = (x);                                            \
     if (_e != cudaSuccess) return fail(-10, "CUDA error: %s", cudaGetErrorString(_e)); \
   } while (0)
+// the same in the create functions: a failed call frees the handle h under construction and the device memory it holds
+#define CUDA_OK_H(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200env_destroy(h); return fail(-10, "CUDA error: %s", cudaGetErrorString(_e)); } } while (0)
 
 template <typename T>
 __device__ __forceinline__ void substep(const DevBlob& B, const float* __restrict__ verts, const PhysCfg<T>& c,
@@ -981,7 +983,7 @@ step_kernel(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_c
 
 
 // ------------------------------------------------------------------------------------------
-// three-launch form of the env step (b200env_step with h->split): pre_kernel -> step_kernel_packed<true> -> post_kernel.
+// three-launch form of the env step (b200env_step in every PhysForm but Lane and Fused): pre_kernel -> step_kernel_packed<true> -> post_kernel.
 // launch 1: pre_physics_step of every env (zeroed actions of reset envs, PD targets, residual root wrench, previous <- current
 // targets).  Warp per env, lane per body, 8 warps per CTA, no big shared-memory footprint -> full occupancy.
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
@@ -1929,6 +1931,98 @@ static int launch_physics_only(b200env* h, void (*kernel)(const DevBlob*, uint32
   return 0;
 }
 
+static bool env_is(const char* name, const char* value) {
+  const char* v = getenv(name);
+  return v && strcmp(v, value) == 0;
+}
+
+// The physics launch of a b200env_create handle, from the tree and the environment variables B200ENV_KERNEL, B200ENV_SPLIT and
+// B200ENV_SORT; an unknown value selects what leaving the variable unset does.  fits_packed: the tree fits the packed layout
+// (<= 8 bodies per depth, <= 25 bodies).
+static PhysForm choose_form(const DevBlob& hb, bool fits_packed) {
+  if (!fits_packed || env_is("B200ENV_KERNEL", "lane")) return PhysForm::Lane;
+  if (env_is("B200ENV_SPLIT", "0")) return PhysForm::Fused;
+#if B200ENV_WITH_PACKED3
+  // packed3 (2 envs per warp, 3 lanes per body in the backward pass; tools/variants/packed3.cuh): at most 5 bodies per tree depth
+  bool wide = false;
+  for (int d = 0; d < MAX_LEVELS; d++) if (hb.t.lvl_all[d][SLOTS3] >= 0) wide = true;
+  if (!wide && env_is("B200ENV_KERNEL", "packed3")) return PhysForm::Packed3;
+#endif
+  if (env_is("B200ENV_SORT", "1")) return PhysForm::Sorted;   // Split with the envs handed out by contact load
+  // one-wave form (csrc/packed_t.cuh): needs a tree that fits 3 column blocks x 8 owner slots.  Not the default: on an H100 SXM
+  // (700 W power limit) the primary workload at 8192 envs measured 1.69 ms per step with it against 1.25 ms with step_kernel_packed
+  // (physics launch 1.24 vs 0.80 ms) - the private store spills out of L1, which the shared-memory records of step_kernel_packed
+  // leave room for.
+  if (env_is("B200ENV_KERNEL", "tmem") && hb.t.pt_ok && hb.t.pt_nmbox <= PT_MBOX_MAX) return PhysForm::Tmem;
+  return PhysForm::Split;
+}
+
+// Runs one of the batch planners of b200env_create_assets (b200env_plan_assets or b200env_plan_assets_mixed) at the envs per batch
+// of step_kernel_packed<true, ...> into plan, compacted to rows [num_envs] | asset, first, count [*num_batches] each.
+static int make_asset_plan(decltype(&b200env_plan_assets) planner, const int32_t* env_asset, int32_t num_envs, int32_t num_assets,
+                           std::vector<int32_t>& plan, int32_t* num_batches) {
+  const size_t n = num_envs;
+  plan.assign(n * 4, 0);   // the planner's outputs, with room for one batch per env
+  int32_t* P = plan.data();
+  const int rc = planner(env_asset, num_envs, num_assets, pk_warps(true) * EPW, P, P + n, P + 2 * n, P + 3 * n, num_batches);
+  if (rc) return rc;
+  const size_t nb = *num_batches;
+  std::copy(P + 2 * n, P + 2 * n + nb, P + n + nb);
+  std::copy(P + 3 * n, P + 3 * n + nb, P + n + 2 * nb);
+  plan.resize(n + 3 * nb);
+  return 0;
+}
+
+// Shape of the physics launch of b200env_step: kernel, threads and dynamic shared memory per CTA, envs per CTA batch, and the most
+// resident CTAs per SM (below what the occupancy query allows)
+struct PhysLaunch { const void* kernel; int threads; size_t smem; int batch; int max_per_sm; };
+
+// The physics launch of h's form and its persistent grid.  The grid's resident CTA slots (per SM x SMs) are computed on the first
+// call and kept; a launch of num_envs envs runs min(slots, ceil(num_envs / batch)) CTAs (h->step_grid).
+static int physics_launch_config(b200env* h, PhysLaunch* out) {
+  // step_kernel_packed stages the DevBlob header only (its vertices stay in global memory); the other forms stage the whole blob
+  const size_t staged = (h->blob_bytes + 15) & ~(size_t)15;
+  const size_t pk_smem = sizeof(DevBlob) + (size_t)pk_warps(true) * EPW * ENV_STRIDE * sizeof(float);
+  const int pk_threads = pk_launch_warps(true) * 32, pk_batch = pk_warps(true) * EPW;
+  PhysLaunch L{};   // stays empty for Packed3 in a build without it, which choose_form never picks: the attribute call fails
+  switch (h->form) {
+    case PhysForm::Lane:
+      L = {(const void*)step_kernel, WARPS_PER_CTA * 32, staged + WARPS_PER_CTA * SCRATCH_FLOATS * sizeof(float), WARPS_PER_CTA, INT_MAX};
+      break;
+    case PhysForm::Fused:
+      L = {(const void*)step_kernel_packed<false>, pk_launch_warps(false) * 32,
+           sizeof(DevBlob) + PK_WARPS_FUSED * PK_SCRATCH * sizeof(float) + (size_t)pk_warps(false) * EPW * ENV_STRIDE * sizeof(float),
+           pk_warps(false) * EPW, INT_MAX};
+      break;
+    case PhysForm::Split:
+    case PhysForm::Sorted: L = {(const void*)step_kernel_packed<true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
+    case PhysForm::Grouped: L = {(const void*)step_kernel_packed<true, true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
+    case PhysForm::Mixed: L = {(const void*)step_kernel_packed<true, false, true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
+    case PhysForm::Tmem:   // one CTA per SM: its 56 envs take nearly all of the shared memory
+      L = {(const void*)step_kernel_tmem, PT_WARPS * 32, staged + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float), PT_WARPS * EPW, 1};
+      break;
+#if B200ENV_WITH_PACKED3
+    case PhysForm::Packed3:
+      L = {(const void*)step_kernel_packed3, PK3_WARPS * 32, staged + (size_t)PK3_WARPS * EPW3 * ENV_STRIDE * sizeof(float), PK3_WARPS * EPW3, INT_MAX};
+      break;
+#endif
+  }
+  if (h->step_slots == 0) {
+    int per_sm = 0, sms = 0;
+    CUDA_OK(cudaFuncSetAttribute(L.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.smem));
+    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, L.kernel, L.threads, L.smem));
+    per_sm = std::min(per_sm, L.max_per_sm);
+    CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    if (per_sm * sms < 1) return fail(-5, h->form != PhysForm::Lane ? "b200env_step: step_kernel_packed does not fit on this device%s"
+                                                                    : "b200env_step: step_kernel does not fit on this device%s");
+    h->step_slots = per_sm * sms;
+    const int need = h->num_assets ? h->num_batches : (h->num_envs + L.batch - 1) / L.batch;
+    h->step_grid = h->step_slots < need ? h->step_slots : need;
+  }
+  *out = L;
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // C ABI
 extern "C" {
@@ -1967,53 +2061,33 @@ int b200env_create(const b200_model_t* model, const float* verts, const b200_cfg
   const int trc = build_dev_blob(model, hb, &slots_ok);
   if (trc == -1) { delete h; return fail(-2, "b200env_create: bodies must be in topological order%s"); }
   if (trc == -2) { delete h; return fail(-2, "b200env_create: too many children per body%s"); }
-  h->packed_ok = model->nb <= B200_MAX_BODIES_PK && slots_ok;
   hull_vertex_radius(model, verts, hb.t.vrho);
   hull_bounding_spheres(model, verts, hb.t.bs);
-  const char* kv = getenv("B200ENV_KERNEL");
-  h->packed = h->packed_ok && !(kv && strcmp(kv, "lane") == 0);
-  const char* sv = getenv("B200ENV_SPLIT");
-  h->split = h->packed && !(sv && strcmp(sv, "0") == 0);
-  // packed3 (2 envs per warp, 3 lanes per body in the backward pass; csrc/packed3.cuh): needs the split form and at most 5 bodies
-  // per tree depth.  B200ENV_KERNEL=packed3 selects it (A/B against the 4-envs-per-warp kernel).
-#if B200ENV_WITH_PACKED3
-  int wide = 0;
-  for (int d = 0; d < MAX_LEVELS; d++) if (hb.t.lvl_all[d][SLOTS3] >= 0) wide = 1;
-  h->packed3 = h->split && !wide && kv && strcmp(kv, "packed3") == 0;
-#else
-  h->packed3 = 0;
-#endif
-  const char* so = getenv("B200ENV_SORT");
-  h->sort = h->split && !h->packed3 && so && strcmp(so, "1") == 0;
-  // one-wave form (csrc/packed_t.cuh): needs the split form and a tree that fits 3 column blocks x 8 owner slots
-  // B200ENV_KERNEL=tmem selects it.  Not the default: on an H100 SXM (700 W power limit) the primary workload at 8192 envs measured
-  // 1.69 ms per step with it against 1.25 ms with step_kernel_packed (physics launch 1.24 vs 0.80 ms) - the private store spills out
-  // of L1, which the shared-memory records of step_kernel_packed leave room for.
-  h->tmem = h->split && !h->packed3 && !h->sort && hb.t.pt_ok && hb.t.pt_nmbox <= PT_MBOX_MAX && kv && strcmp(kv, "tmem") == 0;
-  if (cfg->has_ball && cfg->ball_body_contact && !h->packed) {
+  h->form = choose_form(hb, model->nb <= B200_MAX_BODIES_PK && slots_ok);
+  if (cfg->has_ball && cfg->ball_body_contact && h->form == PhysForm::Lane) {
     delete h;
     return fail(-2, "b200env_create: ball_body_contact needs the packed kernels (the lane-per-body kernel does not have it)%s");
   }
   const size_t vbytes = (size_t)model->nb * model->vmax * 3 * sizeof(float);
   h->blob_bytes = sizeof(DevBlob) + ((vbytes + 15) & ~(size_t)15);
-  CUDA_OK(cudaMalloc(&h->d_blob, h->blob_bytes));
-  CUDA_OK(cudaMemset(h->d_blob, 0, h->blob_bytes));
-  CUDA_OK(cudaMemcpy(h->d_blob, &hb, sizeof(hb), cudaMemcpyHostToDevice));
+  CUDA_OK_H(cudaMalloc(&h->d_blob, h->blob_bytes));
+  CUDA_OK_H(cudaMemset(h->d_blob, 0, h->blob_bytes));
+  CUDA_OK_H(cudaMemcpy(h->d_blob, &hb, sizeof(hb), cudaMemcpyHostToDevice));
   {  // AoS [nb][vmax][3] (ABI) -> SoA [nb][3][vmax] (what contact_hull reads with 128-bit loads)
     std::vector<float> soa((size_t)model->nb * model->vmax * 3, 0.0f);
     verts_to_soa(model, verts, soa.data());
-    CUDA_OK(cudaMemcpy((char*)h->d_blob + sizeof(DevBlob), soa.data(), vbytes, cudaMemcpyHostToDevice));
+    CUDA_OK_H(cudaMemcpy((char*)h->d_blob + sizeof(DevBlob), soa.data(), vbytes, cudaMemcpyHostToDevice));
   }
-  CUDA_OK(cudaMalloc(&h->d_cfg, sizeof(b200_cfg_t)));
-  CUDA_OK(cudaMemcpy(h->d_cfg, cfg, sizeof(b200_cfg_t), cudaMemcpyHostToDevice));
-  if (h->sort) {
-    CUDA_OK(cudaMalloc(&h->d_bin, sizeof(int32_t) * num_envs));
-    CUDA_OK(cudaMalloc(&h->d_perm, sizeof(int32_t) * num_envs));
-    CUDA_OK(cudaMalloc(&h->d_pos, sizeof(uint32_t) * num_envs));
-    CUDA_OK(cudaMalloc(&h->d_cnt, sizeof(uint32_t) * SORT_BINS));
+  CUDA_OK_H(cudaMalloc(&h->d_cfg, sizeof(b200_cfg_t)));
+  CUDA_OK_H(cudaMemcpy(h->d_cfg, cfg, sizeof(b200_cfg_t), cudaMemcpyHostToDevice));
+  if (h->form == PhysForm::Sorted) {
+    CUDA_OK_H(cudaMalloc(&h->d_bin, sizeof(int32_t) * num_envs));
+    CUDA_OK_H(cudaMalloc(&h->d_perm, sizeof(int32_t) * num_envs));
+    CUDA_OK_H(cudaMalloc(&h->d_pos, sizeof(uint32_t) * num_envs));
+    CUDA_OK_H(cudaMalloc(&h->d_cnt, sizeof(uint32_t) * SORT_BINS));
   }
-  CUDA_OK(cudaMalloc(&h->d_ticket, sizeof(unsigned long long)));
-  CUDA_OK(cudaMemset(h->d_ticket, 0, sizeof(unsigned long long)));
+  CUDA_OK_H(cudaMalloc(&h->d_ticket, sizeof(unsigned long long)));
+  CUDA_OK_H(cudaMemset(h->d_ticket, 0, sizeof(unsigned long long)));
   *out = h;
   return 0;
 }
@@ -2102,8 +2176,6 @@ int b200env_choose_asset_plan(const int32_t* env_asset, int32_t num_envs, int32_
   return 0;
 }
 
-static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out);
-
 int b200env_create_assets(const b200_model_t* models, const float* const* verts, int32_t num_assets, const int32_t* env_asset,
                           const b200_cfg_t* cfg, int32_t num_envs, int32_t device, b200env_handle* out) {
   if (!models || !verts || !env_asset || !cfg || !out) return fail(-1, "b200env_create_assets: null argument%s");
@@ -2137,20 +2209,10 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   const char* pv = getenv("B200ENV_ASSET_PLAN");   // A/B and tests: run this plan instead of the one the rule chooses
   if (pv && strcmp(pv, "grouped") != 0 && strcmp(pv, "mixed") != 0)
     return fail(-2, "b200env_create_assets: B200ENV_ASSET_PLAN must be grouped or mixed%s");
-  // the planner and its outputs: rows | asset | first | count (at most one batch per env)
-  std::vector<int32_t>* plan = new std::vector<int32_t>((size_t)num_envs * 4);
+  std::vector<int32_t>* plan = new std::vector<int32_t>();
   int32_t nbat = 0;
-  int32_t* P = plan->data();
-  const int batch = pk_warps(true) * EPW;
-  int rc = b200env_plan_assets(env_asset, num_envs, num_assets, batch, P, P + num_envs, P + 2 * (size_t)num_envs, P + 3 * (size_t)num_envs, &nbat);
+  int rc = make_asset_plan(b200env_plan_assets, env_asset, num_envs, num_assets, *plan, &nbat);
   if (rc) { delete plan; return rc; }
-  std::vector<int4> bt(nbat);
-  for (int i = 0; i < nbat; i++) bt[i] = make_int4(P[num_envs + i], P[2 * num_envs + i], P[3 * num_envs + i], 0);
-  // compact to rows | asset [nbat] | first [nbat] | count [nbat]
-  std::copy(P + 2 * (size_t)num_envs, P + 2 * (size_t)num_envs + nbat, P + num_envs + nbat);
-  std::copy(P + 3 * (size_t)num_envs, P + 3 * (size_t)num_envs + nbat, P + num_envs + 2 * nbat);
-  plan->resize((size_t)num_envs + 3 * nbat);
-  P = plan->data();
   // asset 0 through the one-asset path: validation, kernel form, d_blob / d_cfg / ticket
   b200env_handle h = nullptr;
   rc = b200env_create(&models[0], verts[0], cfg, num_envs, device, &h);
@@ -2158,10 +2220,11 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   h->plan = plan;
   h->num_assets = num_assets;
   h->num_batches = nbat;
-  if (!h->packed || !h->split || h->sort || h->tmem || h->packed3) {
+  if (h->form != PhysForm::Split) {
     b200env_destroy(h);
     return fail(-2, "b200env_create_assets: several assets need the packed split form of the physics launch%s");
   }
+  h->form = PhysForm::Grouped;
   std::vector<size_t> off(num_assets + 1, 0);
   for (int a = 0; a < num_assets; a++)
     off[a + 1] = off[a] + sizeof(DevBlob) + (((size_t)models[a].nb * models[a].vmax * 3 * sizeof(float) + 15) & ~(size_t)15);
@@ -2175,7 +2238,6 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
     memcpy(host.data() + off[a], &hb, sizeof(hb));
     verts_to_soa(&models[a], verts[a], reinterpret_cast<float*>(host.data() + off[a] + sizeof(DevBlob)));
   }
-#define CUDA_OK_H(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { b200env_destroy(h); return fail(-10, "CUDA error: %s", cudaGetErrorString(_e)); } } while (0)
   CUDA_OK_H(cudaMalloc(&h->d_assets, host.size()));
   CUDA_OK_H(cudaMemcpy(h->d_assets, host.data(), host.size(), cudaMemcpyHostToDevice));
   std::vector<const DevBlob*> ptr(num_assets);
@@ -2185,24 +2247,18 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
   // the plan: the mixed one exactly when it takes fewer rounds of the persistent grid than the grouped one
   int32_t mixed = pv ? strcmp(pv, "mixed") == 0 : 0;
   if (!pv) {
-    size_t psmem;
-    int bsz;
+    PhysLaunch pl;
     CUDA_OK_H(cudaSetDevice(h->device));
-    rc = physics_launch_config(h, &psmem, &bsz);   // the grid (resident CTA slots); computed again below for the chosen plan
+    rc = physics_launch_config(h, &pl);   // the grid (resident CTA slots) of the grouped plan; computed again at the first step
     if (!rc) rc = b200env_choose_asset_plan(env_asset, num_envs, num_assets, h->step_slots, &mixed);
     if (rc) { b200env_destroy(h); return rc; }
     h->step_slots = 0;
   }
   if (mixed) {
-    plan->assign((size_t)num_envs * 4, 0);
-    P = plan->data();
-    rc = b200env_plan_assets_mixed(env_asset, num_envs, num_assets, batch, P, P + num_envs, P + 2 * (size_t)num_envs, P + 3 * (size_t)num_envs, &nbat);
+    rc = make_asset_plan(b200env_plan_assets_mixed, env_asset, num_envs, num_assets, *plan, &nbat);
     if (rc) { b200env_destroy(h); return rc; }
-    std::copy(P + 2 * (size_t)num_envs, P + 2 * (size_t)num_envs + nbat, P + num_envs + nbat);
-    std::copy(P + 3 * (size_t)num_envs, P + 3 * (size_t)num_envs + nbat, P + num_envs + 2 * nbat);
-    plan->resize((size_t)num_envs + 3 * nbat);
     h->num_batches = nbat;
-    h->mixed = 1;
+    h->form = PhysForm::Mixed;
     std::vector<const DevBlob*> eb(num_envs);
     for (int e = 0; e < num_envs; e++) eb[e] = ptr[env_asset[e]];
     CUDA_OK_H(cudaMalloc(&h->d_env_blob, sizeof(const DevBlob*) * num_envs));
@@ -2210,11 +2266,13 @@ int b200env_create_assets(const b200_model_t* models, const float* const* verts,
     *out = h;
     return 0;
   }
+  const int32_t* P = plan->data();
+  std::vector<int4> bt(nbat);
+  for (int i = 0; i < nbat; i++) bt[i] = make_int4(P[num_envs + i], P[num_envs + nbat + i], P[num_envs + 2 * nbat + i], 0);
   CUDA_OK_H(cudaMalloc(&h->d_rows, sizeof(int32_t) * num_envs));
   CUDA_OK_H(cudaMemcpy(h->d_rows, P, sizeof(int32_t) * num_envs, cudaMemcpyHostToDevice));
   CUDA_OK_H(cudaMalloc(&h->d_batches, sizeof(int4) * nbat));
   CUDA_OK_H(cudaMemcpy(h->d_batches, bt.data(), sizeof(int4) * nbat, cudaMemcpyHostToDevice));
-#undef CUDA_OK_H
   *out = h;
   return 0;
 }
@@ -2223,7 +2281,7 @@ int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batch
                        int32_t* batch_count, int32_t* mixed) {
   if (!h || !num_assets || !num_batches) return fail(-1, "b200env_asset_plan: null argument%s");
   if (!h->num_assets) return fail(-2, "b200env_asset_plan: not a handle of b200env_create_assets%s");
-  if (mixed) *mixed = h->mixed;
+  if (mixed) *mixed = h->form == PhysForm::Mixed;
   *num_assets = h->num_assets;
   *num_batches = h->num_batches;
   const int32_t* P = h->plan->data();
@@ -2304,79 +2362,14 @@ int b200env_set_motion_lib(b200env_handle h, const b200_motion_lib_t* ml) {
 }
 
 static int need_ctas(const b200env* h) { return (h->num_envs + WARPS_PER_CTA - 1) / WARPS_PER_CTA; }
-static size_t step_smem(const b200env* h) { return ((h->blob_bytes + 15) & ~(size_t)15) + WARPS_PER_CTA * SCRATCH_FLOATS * sizeof(float); }
-
-// Shape of the physics launch of b200env_step: dynamic shared memory, envs per CTA batch and the persistent grid.  The grid's
-// resident CTA slots (per SM x SMs) are computed on the first call and kept; a launch of num_envs envs runs
-// min(slots, ceil(num_envs / batch)) CTAs (h->step_grid).
-static int physics_launch_config(b200env* h, size_t* psmem_out, int* batch_out) {
-  size_t psmem;
-  int batch;
-  if (h->packed) {
-    // step_kernel_packed stages the DevBlob header only (its vertices stay in global memory); the other forms stage the whole blob
-    psmem = h->tmem ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float)
-#if B200ENV_WITH_PACKED3
-            : h->packed3 ? ((h->blob_bytes + 15) & ~(size_t)15) + (size_t)PK3_WARPS * EPW3 * ENV_STRIDE * sizeof(float)
-#endif
-                    : sizeof(DevBlob) + (h->split ? 0 : PK_WARPS_FUSED * PK_SCRATCH * sizeof(float)) +
-                          (size_t)pk_warps(h->split) * EPW * ENV_STRIDE * sizeof(float);
-    batch = h->tmem ? PT_WARPS * EPW :
-#if B200ENV_WITH_PACKED3
-            h->packed3 ? PK3_WARPS * EPW3 :
-#endif
-            pk_warps(h->split) * EPW;
-  } else {
-    psmem = step_smem(h);
-    batch = WARPS_PER_CTA;
-  }
-  if (h->step_slots == 0) {
-    int per_sm = 0, sms = 0;
-    if (!h->packed) {
-      CUDA_OK(cudaFuncSetAttribute(step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel, WARPS_PER_CTA * 32, psmem));
-    } else if (h->tmem) {
-      CUDA_OK(cudaFuncSetAttribute(step_kernel_tmem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-      CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_tmem, PT_WARPS * 32, psmem));
-      if (per_sm > 1) per_sm = 1;   // one CTA per SM: its 56 envs take nearly all of the shared memory
-    } else {
-      CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-      CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-#if B200ENV_WITH_PACKED3
-      if (h->packed3) {
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed3, PK3_WARPS * 32, psmem));
-      } else
-#endif
-      if (h->mixed) {
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true, false, true>, pk_launch_warps(true) * 32, psmem));
-      } else if (h->num_assets) {
-        CUDA_OK(cudaFuncSetAttribute(step_kernel_packed<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-        CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true, true>, pk_launch_warps(true) * 32, psmem));
-      } else
-      if (h->split) { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<true>, pk_launch_warps(true) * 32, psmem)); }
-      else { CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, step_kernel_packed<false>, pk_launch_warps(false) * 32, psmem)); }
-    }
-    CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-    if (per_sm * sms < 1) return fail(-5, h->packed ? "b200env_step: step_kernel_packed does not fit on this device%s"
-                                                     : "b200env_step: step_kernel does not fit on this device%s");
-    h->step_slots = per_sm * sms;
-    const int need = h->num_assets ? h->num_batches : (h->num_envs + batch - 1) / batch;
-    h->step_grid = h->step_slots < need ? h->step_slots : need;
-  }
-  *psmem_out = psmem;
-  *batch_out = batch;
-  return 0;
-}
 
 int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int32_t* grid) {
   if (!h || !envs_per_batch || !grid) return fail(-1, "b200env_physics_launch_shape: null argument%s");
   CUDA_OK(cudaSetDevice(h->device));
-  size_t psmem;
-  int batch;
-  const int rc = physics_launch_config(h, &psmem, &batch);
+  PhysLaunch pl;
+  const int rc = physics_launch_config(h, &pl);
   if (rc) return rc;
-  *envs_per_batch = batch;
+  *envs_per_batch = pl.batch;
   *grid = h->step_slots;
   return 0;
 }
@@ -2385,80 +2378,76 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
   if (!h || !actions) return fail(-1, "b200env_step: null argument%s");
   if (!h->bound || (!h->has_ml && h->cfg.task_mode == 0)) return fail(-4, "b200env_step: bind buffers and a motion lib first%s");
   cudaSetDevice(h->device);
-  size_t psmem;
-  int batch;
-  const int rc = physics_launch_config(h, &psmem, &batch);
+  PhysLaunch pl;
+  const int rc = physics_launch_config(h, &pl);
   if (rc) return rc;
-  if (h->packed) {
+  const cudaStream_t st = (cudaStream_t)stream;
+  const DevBlob* blob = (const DevBlob*)h->d_blob;
+  const uint32_t blob_bytes = (uint32_t)h->blob_bytes;
+  if (h->form == PhysForm::Lane || h->form == PhysForm::Fused) {   // the whole step in one launch
     // the ticket counter is re-zeroed on the stream before every launch: nothing in the launch depends on host-side
-    // history, so a step can be captured into a CUDA graph and replayed
-    if (!h->split) CUDA_OK(cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned long long), (cudaStream_t)stream));   // split form: pre_kernel zeroes it
-    if (h->split) {
-      const int rows = h->env_first + h->env_stride * (h->num_envs - 1) + 1;
-      if (rows > h->ext_rows) {  // first step (or a wider env slice): never inside a graph capture - the bound task warms up first
-        cudaFree(h->d_ext);
-        h->d_ext = nullptr;
-        CUDA_OK(cudaMalloc(&h->d_ext, (size_t)rows * 6 * sizeof(float)));
-        h->ext_rows = rows;
-      }
-      const int io_grid = need_ctas(h);
-      if (h->sort) {
-        CUDA_OK(cudaMemsetAsync(h->d_cnt, 0, sizeof(uint32_t) * SORT_BINS, (cudaStream_t)stream));
-        sort_count_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->bufs, h->num_envs, h->env_first,
-                                                                                    h->env_stride, h->d_bin, h->d_pos, h->d_cnt);
-        sort_perm_kernel<<<(h->num_envs + 255) / 256, 256, 0, (cudaStream_t)stream>>>(h->num_envs, h->d_bin, h->d_pos, h->d_cnt, h->d_perm);
-        h->launches += 2;
-      }
-      pre_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->bufs, h->ml, actions,
-                                                                           h->num_envs, h->env_first, h->env_stride, h->d_ext, h->d_ticket);
-      cudaEvent_t tv0 = nullptr, tv1 = nullptr;
-      if (h->timing && h->tev && h->tev->size() < 8192) {
-        if (cudaEventCreate(&tv0) == cudaSuccess && cudaEventCreate(&tv1) == cudaSuccess) cudaEventRecord(tv0, (cudaStream_t)stream);
-        else tv0 = tv1 = nullptr;
-      }
-      if (h->tmem)
-        step_kernel_tmem<<<h->step_grid, PT_WARPS * 32, psmem, (cudaStream_t)stream>>>(
-            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
-      else
-#if B200ENV_WITH_PACKED3
-      if (h->packed3)
-        step_kernel_packed3<<<h->step_grid, PK3_WARPS * 32, psmem, (cudaStream_t)stream>>>(
-            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
-      else
-#endif
-      if (h->mixed)
-        step_kernel_packed<true, false, true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
-            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext,
-            nullptr, h->d_env_blob);
-      else if (h->num_assets)
-        step_kernel_packed<true, true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
-            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext,
-            h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);
-      else
-        step_kernel_packed<true><<<h->step_grid, pk_launch_warps(true) * 32, psmem, (cudaStream_t)stream>>>(
-            (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first,
-            h->env_stride, h->d_ext, h->sort ? h->d_perm : nullptr);
-      if (tv0) { cudaEventRecord(tv1, (cudaStream_t)stream); h->tev->push_back(tv0); h->tev->push_back(tv1); }
-      if (h->cfg.task_mode == 0)
-        post_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->bufs, h->ml, h->num_envs,
-                                                                              h->env_first, h->env_stride);
-      CUDA_OK(cudaGetLastError());
-      h->launches += h->cfg.task_mode == 0 ? 3 : 2;
-      return 0;
-    }
-    step_kernel_packed<false><<<h->step_grid, pk_launch_warps(false) * 32, psmem, (cudaStream_t)stream>>>(
-        (const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first,
-        h->env_stride, nullptr, nullptr);
+    // history, so a step can be captured into a CUDA graph and replayed (in the other forms pre_kernel zeroes it)
+    CUDA_OK(cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned long long), st));
+    if (h->form == PhysForm::Lane)
+      step_kernel<<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first, h->env_stride);
+    else
+      step_kernel_packed<false><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first, h->env_stride, nullptr, nullptr);
     CUDA_OK(cudaGetLastError());
     h->launches++;
     return 0;
   }
-  CUDA_OK(cudaMemsetAsync(h->d_ticket, 0, sizeof(unsigned long long), (cudaStream_t)stream));
-  step_kernel<<<h->step_grid, WARPS_PER_CTA * 32, psmem, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, (uint32_t)h->blob_bytes,
-                                                                                 h->d_cfg, h->bufs, h->ml, actions, h->num_envs,
-                                                                                 h->d_ticket, h->env_first, h->env_stride);
+  const int rows = h->env_first + h->env_stride * (h->num_envs - 1) + 1;
+  if (rows > h->ext_rows) {  // first step (or a wider env slice): never inside a graph capture - the bound task warms up first
+    cudaFree(h->d_ext);
+    h->d_ext = nullptr;
+    CUDA_OK(cudaMalloc(&h->d_ext, (size_t)rows * 6 * sizeof(float)));
+    h->ext_rows = rows;
+  }
+  const int io_grid = need_ctas(h);
+  if (h->form == PhysForm::Sorted) {
+    CUDA_OK(cudaMemsetAsync(h->d_cnt, 0, sizeof(uint32_t) * SORT_BINS, st));
+    sort_count_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, st>>>(blob, h->bufs, h->num_envs, h->env_first, h->env_stride, h->d_bin, h->d_pos, h->d_cnt);
+    sort_perm_kernel<<<(h->num_envs + 255) / 256, 256, 0, st>>>(h->num_envs, h->d_bin, h->d_pos, h->d_cnt, h->d_perm);
+    h->launches += 2;
+  }
+  pre_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, st>>>(blob, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->env_first, h->env_stride, h->d_ext,
+                                                     h->d_ticket);
+  cudaEvent_t tv0 = nullptr, tv1 = nullptr;
+  if (h->timing && h->tev && h->tev->size() < 8192) {
+    if (cudaEventCreate(&tv0) == cudaSuccess && cudaEventCreate(&tv1) == cudaSuccess) cudaEventRecord(tv0, st);
+    else tv0 = tv1 = nullptr;
+  }
+  switch (h->form) {
+    case PhysForm::Tmem:
+      step_kernel_tmem<<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
+      break;
+#if B200ENV_WITH_PACKED3
+    case PhysForm::Packed3:
+      step_kernel_packed3<<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
+      break;
+#endif
+    case PhysForm::Grouped:
+      step_kernel_packed<true, true><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);
+      break;
+    case PhysForm::Mixed:
+      step_kernel_packed<true, false, true><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, nullptr, h->d_env_blob);
+      break;
+    default:   // Split, Sorted
+      step_kernel_packed<true><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext,
+          h->form == PhysForm::Sorted ? h->d_perm : nullptr);
+  }
+  if (tv0) { cudaEventRecord(tv1, st); h->tev->push_back(tv0); h->tev->push_back(tv1); }
+  if (h->cfg.task_mode == 0)
+    post_kernel<<<io_grid, WARPS_PER_CTA * 32, 0, st>>>(blob, h->d_cfg, h->bufs, h->ml, h->num_envs, h->env_first, h->env_stride);
   CUDA_OK(cudaGetLastError());
-  h->launches++;
+  h->launches += h->cfg.task_mode == 0 ? 3 : 2;
   return 0;
 }
 
@@ -2614,15 +2603,17 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
   if (prec == 0) {
     const EnvArrays<float> io{(float*)root, (float*)dof_pos, (float*)dof_vel, (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out,
                               (float*)contact_out, (float*)ball, ball_hits};
-    // the one-wave form at 6 warps (more than 4: several CTA batches of the test kernel in small tests)
-    if (h->packed && h->tmem) return launch_physics_only(h, physics_kernel_tmem<6>, 6, 6 * EPW, 6 * EPW * PT_ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
-    if (h->packed) return launch_physics_only(h, physics_kernel_packed<float, 4>, 4, 4 * EPW, 4 * EPW * ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
-    return launch_physics_only(h, physics_kernel<float>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
+    switch (h->form) {
+      case PhysForm::Lane: return launch_physics_only(h, physics_kernel<float>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
+      // the one-wave form at 6 warps (more than 4: several CTA batches of the test kernel in small tests)
+      case PhysForm::Tmem: return launch_physics_only(h, physics_kernel_tmem<6>, 6, 6 * EPW, 6 * EPW * PT_ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
+      default: return launch_physics_only(h, physics_kernel_packed<float, 4>, 4, 4 * EPW, 4 * EPW * ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
+    }
   }
   const EnvArrays<double> io{(double*)root, (double*)dof_pos, (double*)dof_vel, (const double*)pd_tar, (const double*)ext_wrench, (double*)rb_out,
                              (double*)contact_out, (double*)ball, ball_hits};
-  if (h->packed) return launch_physics_only(h, physics_kernel_packed<double, 2>, 2, 2 * EPW, 2 * EPW * ENV_STRIDE * sizeof(double), n, n_steps, io, stream);
-  return launch_physics_only(h, physics_kernel<double>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
+  if (h->form == PhysForm::Lane) return launch_physics_only(h, physics_kernel<double>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
+  return launch_physics_only(h, physics_kernel_packed<double, 2>, 2, 2 * EPW, 2 * EPW * ENV_STRIDE * sizeof(double), n, n_steps, io, stream);
 }
 
 #if PT_PROF
@@ -2632,7 +2623,10 @@ extern "C" int b200env_debug_prof(unsigned long long* out, int n) {
 }
 #endif
 int64_t b200env_launch_count(b200env_handle h) { return h ? h->launches : 0; }
-int32_t b200env_kernel_form(b200env_handle h) { return !h ? -1 : (h->tmem ? 3 : (h->packed3 ? 2 : (h->packed ? 1 : 0))); }
+int32_t b200env_kernel_form(b200env_handle h) {   // 1: every form of step_kernel_packed
+  if (!h) return -1;
+  return h->form == PhysForm::Lane ? 0 : h->form == PhysForm::Packed3 ? 2 : h->form == PhysForm::Tmem ? 3 : 1;
+}
 
 int b200env_set_kernel_timing(b200env_handle h, int32_t on) {
   if (!h) return fail(-1, "b200env_set_kernel_timing: null handle%s");
