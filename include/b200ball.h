@@ -21,7 +21,7 @@ typedef struct b200ball_sim {
   int32_t num_frames;       /* samples per trajectory (30 Hz frames for `simulate`) */
   int32_t control_freq_inv; /* sim steps per frame (2) */
   int32_t substeps;         /* substeps per sim step; > 2 also selects the 6R (else 4R) bounce-flag threshold (:185-188) */
-  int32_t first_comp;       /* first position component written to traj (0: xyz, 1: yz like the in-table) */
+  int32_t first_comp;       /* first position component written to traj (0: xyz, 1: yz like the in-table, 2: z) */
   float sim_dt;             /* 1/60 */
   float spin_scale;
   float gravity_z;
@@ -38,8 +38,11 @@ int b200ball_simulate(const b200ball_sim_t* cfg, int64_t n, int32_t prec, const 
 /* replaces simulate_without_bounce() (tennis_ball_out_estimator.py:21-121) for n rows launched straight out
  * (vel = (0, vel_h, vel_v)) over a world without ground; heights are relative to the launch height.
  * grid_x [ngx] / col_x [ngx]: the values of torch.arange(*TRAJ_X_RANGE) and the column each one is written to (int(x*2));
- * grid_y / col_y likewise (int(y*10)).  out_x [n, nx] and out_y [n, ny, 2] must be zero-initialised by the caller
- * (columns no grid value maps to stay 0, like the reference's torch.zeros).
+ * grid_y / col_y likewise (int(y*10)).  The grids may be unsorted and may map several values to one column: the columns are
+ * written in grid order, so the last of them wins.  A column outside [0, nx) (resp. [0, ny)) is skipped, never stored: the
+ * caller wraps the reference's negative Python indices first.  ngx, ngy in [0, 4096].
+ * out_x [n, nx] and out_y [n, ny, 2] must be zero-initialised by the caller (columns no grid value maps to stay 0, like the
+ * reference's torch.zeros); any base address works, 16-byte aligned ones take the vector stores.
  * cfg->num_frames = 60 -> (num_frames + 1) * control_freq_inv samples at 60 Hz (:55-57). */
 int b200ball_out_rows(const b200ball_sim_t* cfg, int64_t n, int32_t prec, const void* vel_h, const void* vel_v, const void* vspin,
                       const float* grid_x, const int32_t* col_x, int32_t ngx, int32_t nx, const float* grid_y, const int32_t* col_y,

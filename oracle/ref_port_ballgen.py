@@ -50,24 +50,25 @@ class BallWorld:
             p += h * v
             if not self.ground:
                 continue
-            hit = (p[:, 2] < R) & (v[:, 2] < 0)
-            for i in np.nonzero(hit)[0]:
-                # contact point -R z; u = v + w x (-R z)
-                u = v[i] + np.cross(w[i], np.array([0.0, 0.0, -R]))
-                un = u[2]
-                if un < 0:
-                    jn = ((1.0 + self.e) if -un > self.vth else 1.0) * (-un) * m
-                    ut = np.array([u[0], u[1], 0.0])
-                    utn = np.linalg.norm(ut)
-                    jt = 0.0
-                    if utn > 1e-9:
-                        stick = m * utn / (1.0 + m * R * R / I)
-                        jt = min(self.mu * jn, stick)
-                        ut = ut / utn
-                    J = np.array([0.0, 0.0, jn]) - jt * ut
-                    v[i] += J / m
-                    w[i] += np.cross(np.array([0.0, 0.0, -R]), J) / I
-                p[i, 2] = R
+            hit = np.nonzero((p[:, 2] < R) & (v[:, 2] < 0))[0]
+            if len(hit) == 0:
+                continue
+            # contact point -R z; u = v + w x (-R z); the balls in contact at once, row by row the same arithmetic
+            r = np.array([0.0, 0.0, -R])
+            u = v[hit] + np.cross(w[hit], r)
+            i = hit[u[:, 2] < 0]
+            u = u[u[:, 2] < 0]
+            un = u[:, 2]
+            jn = np.where(-un > self.vth, 1.0 + self.e, 1.0) * (-un) * m
+            ut = np.stack([u[:, 0], u[:, 1], np.zeros(len(u))], 1)
+            utn = np.sqrt(u[:, 0] * u[:, 0] + u[:, 1] * u[:, 1])
+            slide = utn > 1e-9
+            jt = np.where(slide, np.minimum(self.mu * jn, m * utn / (1.0 + m * R * R / I)), 0.0)
+            ut[slide] /= utn[slide, None]
+            J = np.stack([np.zeros(len(u)), np.zeros(len(u)), jn], 1) - jt[:, None] * ut
+            v[i] += J / m
+            w[i] += np.cross(r, J) / I
+            p[hit, 2] = R
 
 
 def _aero(vel, angvel, launch_vspin, spin_scale, dt):
@@ -109,7 +110,7 @@ def simulate(launch_pos, launch_vel, launch_vspin, control_freq_inv=2, num_frame
     st = launch_state(np.asarray(launch_pos), np.asarray(launch_vel), np.asarray(launch_vspin), dt)
     lvspin = np.array(launch_vspin, dt)
     traj = np.zeros((n, num_frames, 3), dt)
-    bounce_pos = np.zeros((n, 3), np.float32)
+    bounce_pos = np.zeros((n, 3), dt)
     bounce_idx = np.zeros(n, np.int64) + num_frames - 1
     has_bounce, has_pass_net, pass_ok = np.zeros(n, bool), np.zeros(n, bool), np.zeros(n, bool)
     thr = world.R * 6 if substeps > 2 else world.R * 4
@@ -138,10 +139,23 @@ def torch_arange(lo, hi, step):
     return (lo + np.arange(n, dtype=np.float64) * step).astype(np.float32)
 
 
+def grid(rng, scale):
+    """values of torch.arange(*rng), the column int(v * scale) the reference writes each one to (:98, :110; negative = counted
+    from the end of the row) and the row width"""
+    v = torch_arange(*rng)
+    return v, np.array([int(x * np.float32(scale)) for x in v], np.int64), int((rng[1] - rng[0]) / rng[2])
+
+
 def simulate_without_bounce(launch_pos, launch_vel, launch_vspin, traj_x_range=(0, 30, 0.5), traj_y_range=(0, 3, 0.1),
-                            control_freq_inv=2, num_frames=60, substeps=6, spin_scale=5, state32=True, world_kw=None):
+                            control_freq_inv=2, num_frames=60, substeps=6, spin_scale=5, state32=True, world_kw=None, grid_x=None,
+                            grid_y=None, table_dtype=np.float32, walk=None):
     """tennis_ball_out_estimator.py:21-121 -> traj_x[n, NX] (height over launch at horizontal distance x),
-    traj_y[n, NY, 2] (distance, time at which the ball has dropped y below the launch height)"""
+    traj_y[n, NY, 2] (distance, time at which the ball has dropped y below the launch height)
+
+    grid_x / grid_y: explicit (values, columns, row width) instead of grid(traj_x_range, 2) / grid(traj_y_range, 10).  The columns
+    are written in grid order with Python's index semantics (negative counts from the end, outside [-NX, NX) raises IndexError).
+    table_dtype: the tables' storage type (the reference's float32 by default).  walk: a dict that receives the (y, z) samples
+    [n, T, 2] and the sample index each grid value stopped at, t_x [n, ngx] / t_y [n, ngy] (the value interpolates samples t-1, t)."""
     dt = np.float32 if state32 else np.float64
     n = len(launch_pos)
     world = BallWorld(n, substeps=substeps, ground=False, **(world_kw or {}))
@@ -159,36 +173,41 @@ def simulate_without_bounce(launch_pos, launch_vel, launch_vspin, traj_x_range=(
     traj[:, :, 1] -= traj[0, 0, 1].copy()                # :83 height relative to the launch height (value taken ONCE: the reference's
                                                          # in-place op aliases its operand, see tests/golden/make_golden_ballgen.py)
     T = traj.shape[1]
-    nx = int((traj_x_range[1] - traj_x_range[0]) / traj_x_range[2])
-    ny = int((traj_y_range[1] - traj_y_range[0]) / traj_y_range[2])
-    traj_x = np.zeros((n, nx), np.float32)
-    traj_y = np.zeros((n, ny, 2), np.float32)
+    gx, cx, nx = grid(traj_x_range, 2) if grid_x is None else grid_x
+    gy, cy, ny = grid(traj_y_range, 10) if grid_y is None else grid_y
+    traj_x = np.zeros((n, nx), table_dtype)
+    traj_y = np.zeros((n, ny, 2), table_dtype)
     ids = np.arange(n)
+    t_x, t_y = np.zeros((n, len(gx)), np.int64), np.zeros((n, len(gy)), np.int64)
     t = np.zeros(n, np.int64)
-    for x in torch_arange(*traj_x_range):                # :90-98
-        while True:
-            adv = (t < T - 1) & (traj[ids, t, 0] < x)
-            if adv.sum() > 0:
-                t[adv] += 1
-            else:
-                break
-        x1, x2 = traj[ids, t - 1, 0], traj[ids, t, 0]    # t - 1 == -1 wraps to the last sample, like torch
-        w = (x - x1) / (x2 - x1)
-        traj_x[:, int(np.float32(x) * np.float32(2))] = traj[ids, t - 1, 1] * (1 - w) + traj[ids, t, 1] * w
-    t = np.zeros(n, np.int64)
-    for y in torch_arange(*traj_y_range):                # :101-110
-        while True:
-            adv = (t < T - 1) & (-traj[ids, t, 1] < y)
-            if adv.sum() > 0:
-                t[adv] += 1
-            else:
-                break
-        y1, y2 = traj[ids, t - 1, 1], traj[ids, t, 1]
-        w = (-y - y1) / (y2 - y1)
-        j = int(np.float32(y) * np.float32(10))
-        traj_y[:, j, 0] = traj[ids, t - 1, 0] * (1 - w) + traj[ids, t, 0] * w
-        tt = (t - 1).astype(dt) * (1 - w) + t.astype(dt) * w     # torch: int64 * float32 -> float32
-        traj_y[:, j, 1] = tt / (control_freq_inv * 30)
+    with np.errstate(divide="ignore", invalid="ignore"):    # two equal samples: inf / nan entries, like the reference
+        for j, (x, c) in enumerate(zip(np.asarray(gx, np.float32), cx)):   # :90-98
+            while True:
+                adv = (t < T - 1) & (traj[ids, t, 0] < x)
+                if adv.sum() > 0:
+                    t[adv] += 1
+                else:
+                    break
+            t_x[:, j] = t
+            x1, x2 = traj[ids, t - 1, 0], traj[ids, t, 0]    # t - 1 == -1 wraps to the last sample, like torch
+            w = (x - x1) / (x2 - x1)
+            traj_x[:, int(c)] = traj[ids, t - 1, 1] * (1 - w) + traj[ids, t, 1] * w
+        t = np.zeros(n, np.int64)
+        for j, (y, c) in enumerate(zip(np.asarray(gy, np.float32), cy)):   # :101-110
+            while True:
+                adv = (t < T - 1) & (-traj[ids, t, 1] < y)
+                if adv.sum() > 0:
+                    t[adv] += 1
+                else:
+                    break
+            t_y[:, j] = t
+            y1, y2 = traj[ids, t - 1, 1], traj[ids, t, 1]
+            w = (-y - y1) / (y2 - y1)
+            traj_y[:, int(c), 0] = traj[ids, t - 1, 0] * (1 - w) + traj[ids, t, 0] * w
+            tt = (t - 1).astype(dt) * (1 - w) + t.astype(dt) * w     # torch: int64 * float32 -> float32
+            traj_y[:, int(c), 1] = tt / (control_freq_inv * 30)
+    if walk is not None:
+        walk.update(samples=traj, t_x=t_x, t_y=t_y)
     return traj_x, traj_y
 
 

@@ -144,9 +144,18 @@ def test_full_size_tables_properties():
     del tx, ty
     tab = ball_gen.generate_incoming_table()
     assert tab.shape == (1125000, 50, 2) and bool(torch.isfinite(tab).all())
-    hh = P.launch_grid_in()[0]
+    hh, ivx, ivz, isp = P.launch_grid_in()
     assert np.abs(tab[:, 0, 1].cpu().numpy() - hh).max() < 1e-6 and bool((tab[:, 0, 0] == 0).all())   # frame 0 = the launch point
     assert bool((tab[:, :, 1] >= 0.032 - 1e-4).all())                                                 # never below the ground
+    pick = np.arange(0, len(hh), 37501)
+    m = len(pick)
+    lp = np.stack([np.zeros(m), np.zeros(m), hh[pick]], 1).astype(np.float32)
+    lv = np.stack([np.zeros(m), ivx[pick], ivz[pick]], 1).astype(np.float32)
+    again, _, _, _ = ball_gen.simulate(lp, lv, isp[pick], num_frames=50, first_comp=1)
+    assert torch.equal(again, tab[pick])                                                              # rows do not depend on the batch
+    ref = P.simulate(lp.astype(np.float64), lv.astype(np.float64), isp[pick].astype(np.float64), num_frames=50, state32=False,
+                     world_kw=P.f32_physics())[0]
+    assert np.abs(tab[pick].cpu().numpy() - ref[:, :, 1:]).max() < 2e-3
 
 
 @gpu

@@ -86,10 +86,17 @@ def simulate(launch_pos, launch_vel, launch_vspin, control_freq_inv=2, num_frame
 
 
 def _grid(rng, scale):
-    """values of torch.arange(*rng) and the column `int(v * scale)` the reference writes each one to (:98, :110)"""
+    """values of torch.arange(*rng), the column `int(v * scale)` the reference writes each one to (:98, :110) with Python's
+    index semantics (a negative column counts from the end of the row, one outside [-n, n) raises IndexError), and the row width n"""
     v = torch.arange(*rng)
-    col = torch.tensor([int(x * scale) for x in v], dtype=torch.int32)
-    return v.to(torch.float32), col, int((rng[1] - rng[0]) / rng[2])
+    n = int((rng[1] - rng[0]) / rng[2])
+    col = []
+    for x in v:
+        c = int(x * scale)
+        if not -n <= c < n:
+            raise IndexError(f"grid value {float(x)} maps to column {c} of a row of {n}")
+        col.append(c % n)
+    return v.to(torch.float32), torch.tensor(col, dtype=torch.int32), n
 
 
 def simulate_without_bounce(launch_vel_h, launch_vel_v, launch_vspin, params=traj_out_params, control_freq_inv=2, num_frames=60,
@@ -151,6 +158,16 @@ def torch_sample_range(size, lo, hi, generator=None):   # tennis_ball.py:41-42
     return torch.rand(size, generator=generator) * (hi - lo) + lo
 
 
+def pool_valid(traj, bounce_pos, bounce_idx, pass_net, bmin, bmax):
+    """the pool's validity rule (tennis_ball.py:319-327): passes the net, first bounce inside the far box, rebound higher than 1 m.
+    `bounce_pos.sum() != 0` is over the whole tensor, as in the reference."""
+    valid = pass_net & (bounce_pos.sum() != 0) & (bounce_pos[:, 0] > bmin[0]) & (bounce_pos[:, 0] < bmax[0]) & \
+        (bounce_pos[:, 1] > bmin[1]) & (bounce_pos[:, 1] < bmax[1])
+    frame = torch.arange(traj.shape[1], device=traj.device)[None, :]
+    after = torch.where(frame >= bounce_idx[:, None], traj[:, :, 2], torch.full_like(traj[:, :, 2], -math.inf))
+    return valid & (after.max(dim=1).values > 1.0)      # `traj[i, bounce_idx[i]:, 2].max() > 1.0` without the Python loop over envs
+
+
 class TennisBallGeneratorB200:
     """TennisBallGeneratorIsaac (tennis_ball.py:221-356) without Isaac Gym: `num_env` launches per reset() drawn from the same
     ranges, simulated by one kernel launch, filtered by the same validity rules."""
@@ -186,13 +203,7 @@ class TennisBallGeneratorB200:
         launch_pos, launch_vel, launch_vspin = origin.to(self.device), vel.contiguous().to(self.device), vspin.to(self.device)
         traj, bounce_pos, bounce_idx, pass_net = simulate(launch_pos, launch_vel, launch_vspin, num_frames=self.traj_length,
                                                           substeps=self.substeps, spin_scale=self.spin_scale, device=self.device)
-        # good trajectory: passes the net, first bounce inside the far box, rebound higher than 1 m (:299-311)
-        bmin, bmax = self.bounce_min.to(self.device), self.bounce_max.to(self.device)
-        valid = pass_net & (bounce_pos.sum() != 0) & (bounce_pos[:, 0] > bmin[0]) & (bounce_pos[:, 0] < bmax[0]) & \
-            (bounce_pos[:, 1] > bmin[1]) & (bounce_pos[:, 1] < bmax[1])
-        frame = torch.arange(traj.shape[1], device=self.device)[None, :]
-        after = torch.where(frame >= bounce_idx[:, None], traj[:, :, 2], torch.full_like(traj[:, :, 2], -math.inf))
-        valid &= after.max(dim=1).values > 1.0      # `traj[i, bounce_idx[i]:, 2].max() > 1.0` without the Python loop over envs
+        valid = pool_valid(traj, bounce_pos, bounce_idx, pass_net, self.bounce_min.to(self.device), self.bounce_max.to(self.device))
         assert valid.sum() > 0
         self.traj_pool = traj[valid].cpu()
         self.launch_pos, self.launch_vel, self.launch_vspin = launch_pos[valid].cpu(), launch_vel[valid].cpu(), launch_vspin[valid].cpu()

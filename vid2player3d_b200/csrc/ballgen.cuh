@@ -153,11 +153,13 @@ ball_out_rows_kernel(b200ball_sim_t c, int64_t n, const T* __restrict__ vel_h, c
   // Both walks emit their columns in ascending order, a few samples apart.  Written one float at a time, every store of a warp
   // hits 32 different sectors and every sector is written 8 times (ncu r1h: 8.8 GB of DRAM traffic for 4.06 GB of tables).  So a
   // thread collects the current group of 8 floats (8 columns of out_x, 4 (distance, time) pairs of out_y) in shared memory and
-  // writes it with two 128-bit stores = one full sector; incomplete or out-of-order groups fall back to scalar stores.
+  // writes it with two 128-bit stores = one full sector; incomplete or out-of-order groups, and tables whose base address is not
+  // 16-byte aligned, fall back to scalar stores.
   T* bxs = reinterpret_cast<T*>(bg_smem + (((size_t)(ngx + ngy) * 8 + 15) & ~(size_t)15));   // [8][threads] x group, then y group
   T* bys = bxs + 8 * BALLGEN_THREADS;
   const int tid = threadIdx.x;
-  const bool vec_ok = sizeof(T) == 4 && (nx & 3) == 0 && ((ny * 2) & 3) == 0;
+  const bool vec_ok = sizeof(T) == 4 && (nx & 3) == 0 && ((ny * 2) & 3) == 0 &&
+                      ((reinterpret_cast<uintptr_t>(out_x) | reinterpret_cast<uintptr_t>(out_y)) & 15) == 0;
   int gxb = -1, gyb = -1;
   unsigned mx = 0u, my = 0u;
   auto flush = [&](T* dst, const T* buf, int g, unsigned& m) {       // group g of a row: 8 floats at dst + 8 g
@@ -175,6 +177,7 @@ ball_out_rows_kernel(b200ball_sim_t c, int64_t n, const T* __restrict__ vel_h, c
     m = 0u;
   };
   auto put_x = [&](int col, T val) {
+    if ((unsigned)col >= (unsigned)nx) return;   // a column outside the row is never stored
     const int g = col >> 3;
     if (g != gxb) { if (mx) flush(ox, bxs, gxb, mx); gxb = g; }
     bxs[(col & 7) * BALLGEN_THREADS + tid] = val;
@@ -182,6 +185,7 @@ ball_out_rows_kernel(b200ball_sim_t c, int64_t n, const T* __restrict__ vel_h, c
     if (mx == 0xFFu) flush(ox, bxs, gxb, mx);
   };
   auto put_y = [&](int col, T d, T tm) {
+    if ((unsigned)col >= (unsigned)ny) return;
     const int g = col >> 2, k = (col & 3) * 2;
     if (g != gyb) { if (my) flush(oy, bys, gyb, my); gyb = g; }
     bys[k * BALLGEN_THREADS + tid] = d;
@@ -246,12 +250,19 @@ ball_out_rows_kernel(b200ball_sim_t c, int64_t n, const T* __restrict__ vel_h, c
   if (my) flush(oy, bys, gyb, my);
   // Grid values reached at sample 0 pair sample 0 with sample "-1" = the last one.  For the value 0 (the only one the shipped
   // grids have there) the interpolation weight is (0 - a)/(0 - a) = 1 and the result 0 - already written - unless the last
-  // sample is degenerate; anything else is recomputed the reference's way and stored over the placeholder.
+  // sample is degenerate; anything else is recomputed the reference's way and stored over the placeholder.  The reference writes
+  // the columns in grid order, so an entry whose column a later grid value also maps to is left to that later value.
   const bool plain = y1 != T(0) && z1 != T(0) && fabs(y1) < T(1e30) && fabs(z1) < T(1e30);
+  auto kept = [](const int32_t* col, int j, int ng, int ncol) {
+    if ((unsigned)col[j] >= (unsigned)ncol) return false;
+    for (int k = j + 1; k < ng; k++)
+      if (col[k] == col[j]) return false;
+    return true;
+  };
   for (int j = 0; j < n0x; j++)
-    if (!(plain && sgx[j] == 0.f)) ox[scx[j]] = val_x(j, y1, z1, T(0), T(0));
+    if (!(plain && sgx[j] == 0.f) && kept(scx, j, ngx, nx)) ox[scx[j]] = val_x(j, y1, z1, T(0), T(0));
   for (int j = 0; j < n0y; j++)
-    if (!(plain && sgy[j] == 0.f)) {
+    if (!(plain && sgy[j] == 0.f) && kept(scy, j, ngy, ny)) {
       T d, tm;
       val_y(j, y1, z1, T(0), T(0), 0, d, tm);
       oy[scy[j] * 2] = d; oy[scy[j] * 2 + 1] = tm;
@@ -298,6 +309,9 @@ int b200ball_out_rows(const b200ball_sim_t* cfg, int64_t n, int32_t prec, const 
   const unsigned grid = (unsigned)((n + BALLGEN_THREADS - 1) / BALLGEN_THREADS);
   const size_t smem = (((size_t)(ngx + ngy) * (sizeof(float) + sizeof(int32_t)) + 15) & ~(size_t)15) +
                       (size_t)16 * BALLGEN_THREADS * (prec == 0 ? sizeof(float) : sizeof(double));   // grids + the two 8-float groups per thread
+  if (smem > 48 * 1024)   // grids of thousands of values: opt in to more than the default 48 KB of dynamic shared memory (at most 80 KB)
+    CUDA_OK(prec == 0 ? cudaFuncSetAttribute(ball_out_rows_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+                      : cudaFuncSetAttribute(ball_out_rows_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   if (prec == 0)
     ball_out_rows_kernel<float><<<grid, BALLGEN_THREADS, smem, (cudaStream_t)stream>>>(*cfg, n, (const float*)vel_h, (const float*)vel_v,
                                                                                       (const float*)vspin, grid_x, col_x, ngx, nx, grid_y, col_y, ngy,
