@@ -12,44 +12,115 @@ import torch
 from conftest import golden
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+ENV_HEADERS = ("b200env.h", "b200env_v2p.h", "b200ball.h")     # the C ABI of libb200env.so
+
+# the ctypes type a binding gives each C type of a prototype (a pointer of any kind is c_void_p, handled by the reader)
+C_TYPES = {"int": C.c_int, "int32_t": C.c_int32, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "float": C.c_float, "double": C.c_double,
+           "const char*": C.c_char_p, "b200env_handle": C.c_void_p, "b200nn_linear_handle": C.c_void_p}
+
+# (module of vid2player3d_b200, ctypes mirror, C type of the headers)
+STRUCT_MIRRORS = [("abi", "Model", "b200_model_t"), ("abi", "Cfg", "b200_cfg_t"), ("abi", "MotionLibView", "b200_motion_lib_t"),
+                  ("abi", "Buffers", "b200_buffers_t"), ("abi", "V2PState", "b200v2p_state_t"), ("abi", "V2PCtrl", "b200v2p_ctrl_t"),
+                  ("abi", "V2PPreStep", "b200v2p_prestep_t"), ("abi", "V2PStream", "b200v2p_stream_t"),
+                  ("abi", "V2PTaskReset", "b200v2p_treset_t"), ("abi", "V2PActorReset", "b200v2p_areset_t"),
+                  ("ball_gen", "BallSim", "b200ball_sim_t"), ("nn", "LinearDesc", "b200nn_linear_desc_t")]
 
 
-def test_library_exports_every_declared_symbol():
-    from vid2player3d_b200 import build, native
+def header_prototypes(*headers):
+    """name -> (restype, [argtypes]) of every b200* function the headers declare, in the ctypes types of C_TYPES"""
+    protos = {}
+    for h in headers:
+        text = open(os.path.join(ROOT, "include", h)).read()
+        text = re.sub(r"/\*.*?\*/|//[^\n]*|^[ \t]*#[^\n]*", " ", text, flags=re.S | re.M)
+        for ret, name, params in re.findall(r"([A-Za-z_][\w\s*]*?)\s*\b(b200\w+)\s*\(([^()]*)\)\s*;", text):
+            args = []
+            for p in (" ".join(p.split()) for p in params.split(",")):
+                if p != "void":
+                    args.append(C.c_void_p if "*" in p else C_TYPES[p.rsplit(" ", 1)[0]])
+            protos[name] = (C_TYPES[re.sub(r"\s*\*", "*", " ".join(ret.split()))], args)
+    return protos
+
+
+def signature_mismatches(table, headers):
+    """how a binding table (name -> (restype, [argtypes])) departs from the headers' prototypes"""
+    want = header_prototypes(*headers)
+    bad = [f"{n}: not declared" for n in table if n not in want] + [f"{n}: not bound" for n in want if n not in table]
+    for name in sorted(set(table) & set(want)):
+        (res, args), (wres, wargs) = table[name], want[name]
+        if res is not wres:
+            bad.append(f"{name}: returns {res.__name__}, header {wres.__name__}")
+        if len(args) != len(wargs):
+            bad.append(f"{name}: {len(args)} parameters, header {len(wargs)}")
+        bad += [f"{name}: parameter {i} is {a.__name__}, header {w.__name__}" for i, (a, w) in enumerate(zip(args, wargs)) if a is not w]
+    return bad
+
+
+def layout_mismatches(tmp_path):
+    """sizeof of every mirrored struct and the offset and size of every field its ctypes mirror names, from gcc on the headers,
+    against ctypes"""
+    import importlib
+    lines, want = [], []
+    for mod, cls, ctype in STRUCT_MIRRORS:
+        S = getattr(importlib.import_module("vid2player3d_b200." + mod), cls)
+        lines.append(f'printf("{ctype} %zu\\n", sizeof({ctype}));')
+        want.append(f"{ctype} {C.sizeof(S)}")
+        for f, _ in S._fields_:
+            lines.append(f'printf("{ctype}.{f} %zu %zu\\n", offsetof({ctype}, {f}), sizeof((({ctype}*)0)->{f}));')
+            want.append(f"{ctype}.{f} {getattr(S, f).offset} {getattr(S, f).size}")
+    src, exe = tmp_path / "layout.c", tmp_path / "layout"
+    src.write_text("#include <stdio.h>\n#include <stddef.h>\n" + "".join(f'#include "{h}"\n' for h in ENV_HEADERS + ("b200nn.h",)) +
+                   "int main(void) {\n" + "\n".join(lines) + "\nreturn 0;\n}\n")
+    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    got = subprocess.check_output([str(exe)], text=True).splitlines()
+    assert len(got) == len(want)
+    return [f"ctypes {w!r}, header {g!r}" for w, g in zip(want, got) if w != g]
+
+
+def test_env_bindings_match_header_prototypes():
+    """abi.SIGNATURES is the prototypes of include/b200env.h, b200env_v2p.h and b200ball.h (name, return type, every parameter's
+    type); every entry resolves in the built libb200env.so and native.lib() gives it those types"""
+    from vid2player3d_b200 import abi, build, native
     lib = build.build()
-    from vid2player3d_b200 import native_v2p
-    from vid2player3d_b200 import ball_gen
-    hdr = "".join(open(os.path.join(ROOT, "include", h)).read() for h in ("b200env.h", "b200env_v2p.h", "b200ball.h"))
-    declared = sorted(set(re.findall(r"\b(b200(?:env|v2p|ball)_[a-z_0-9]+)\s*\(", hdr)))
-    assert declared == sorted(native.SYMBOLS + native_v2p.SYMBOLS + ball_gen.SYMBOLS)
+    assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == []
     L = C.CDLL(lib)  # loads without a GPU; no compute call is made here
-    for name in declared:
+    for name in abi.SIGNATURES:
         assert hasattr(L, name), name
-    from vid2player3d_b200 import abi
+    for name, (res, args) in abi.SIGNATURES.items():
+        fn = getattr(native.lib(), name)
+        assert fn.restype is res and list(fn.argtypes) == args, name
     assert L.b200env_abi_version() == abi.ABI_VERSION
 
 
-def test_struct_layouts_match_header(tmp_path):
+def test_signature_check_rejects_a_dropped_or_widened_parameter(monkeypatch):
+    """negative controls of the prototype check: a table with one parameter dropped, or one int32_t bound as int64"""
     from vid2player3d_b200 import abi
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "%s/include/b200env.h"\n'
-                   'int main(){printf("%%zu %%zu %%zu %%zu %%zu %%zu\\n",sizeof(b200_model_t),sizeof(b200_cfg_t),'
-                   'sizeof(b200_motion_lib_t),sizeof(b200_buffers_t),offsetof(b200_model_t,kp),offsetof(b200_cfg_t,key_body));}' % ROOT)
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    want = [C.sizeof(abi.Model), C.sizeof(abi.Cfg), C.sizeof(abi.MotionLibView), C.sizeof(abi.Buffers), abi.Model.kp.offset,
-            abi.Cfg.key_body.offset]
-    assert got == want
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "%s/include/b200env_v2p.h"\n'
-                   'int main(){printf("%%zu %%zu %%zu %%zu %%zu %%zu %%zu %%zu\\n",sizeof(b200v2p_state_t),sizeof(b200v2p_ctrl_t),'
-                   'offsetof(b200v2p_state_t,root_pos),offsetof(b200v2p_ctrl_t,est_x),sizeof(b200v2p_treset_t),sizeof(b200v2p_areset_t),'
-                   'offsetof(b200v2p_treset_t,swing_type_cycle),offsetof(b200v2p_areset_t,terminate_buf));}' % ROOT)
-    subprocess.check_call(["gcc", str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    assert got == [C.sizeof(abi.V2PState), C.sizeof(abi.V2PCtrl), abi.V2PState.root_pos.offset, abi.V2PCtrl.est_x.offset,
-                   C.sizeof(abi.V2PTaskReset), C.sizeof(abi.V2PActorReset), abi.V2PTaskReset.swing_type_cycle.offset,
-                   abi.V2PActorReset.terminate_buf.offset]
+    table = dict(abi.SIGNATURES)
+    res, args = table["b200env_reset_masked"]
+    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200env_reset_masked=(res, args[:-1])))
+    assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == ["b200env_reset_masked: 17 parameters, header 18"]
+    res, args = table["b200v2p_ball_in_estimate"]
+    assert args[3] is C.c_int32                                   # the ball row stride; table_rows next to it is the int64_t
+    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200v2p_ball_in_estimate=(res, args[:3] + [C.c_int64] + args[4:])))
+    assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == [
+        f"b200v2p_ball_in_estimate: parameter 3 is {C.c_int64.__name__}, header {C.c_int32.__name__}"]
+
+
+def test_struct_layouts_match_header(tmp_path):
+    """every struct the bindings mirror has the headers' size, and each field its mirror names the headers' offset and size"""
+    assert layout_mismatches(tmp_path) == []
+
+
+def test_layout_check_rejects_swapped_fields(tmp_path, monkeypatch):
+    """negative control of the layout check: a mirror of b200ball_sim_t with two neighbouring float fields swapped (same size, so
+    only the offsets give it away)"""
+    from vid2player3d_b200 import ball_gen
+    f = list(ball_gen.BallSim._fields_)
+    i = [n for n, _ in f].index("e_ground")
+    assert f[i + 1][0] == "mu_ground"
+    f[i], f[i + 1] = f[i + 1], f[i]
+    monkeypatch.setattr(ball_gen, "BallSim", type("BallSim", (C.Structure,), {"_fields_": f}))
+    bad = layout_mismatches(tmp_path)
+    assert len(bad) == 2 and "b200ball_sim_t.mu_ground" in bad[0] and "b200ball_sim_t.e_ground" in bad[1], bad
 
 
 def test_no_gpu_means_loud_failure():
@@ -267,25 +338,17 @@ def test_quaternion_to_angle_axis_matches_scipy():
     assert np.all(got[0] == 0)
 
 
-def test_nn_library_exports_and_layout(tmp_path):
-    """libb200nn.so (include/b200nn.h): loads without a GPU, exports every declared symbol, descriptor layout == ctypes mirror,
-    and refuses to build a layer without a CUDA device (no fallback)."""
+def test_nn_bindings_match_header_prototypes():
+    """libb200nn.so (include/b200nn.h): loads without a GPU, nn.SIGNATURES is the header's prototypes and every entry resolves with
+    those types (the descriptor layout is among test_struct_layouts_match_header's), and it refuses to build a layer without a CUDA
+    device (no fallback)."""
     from vid2player3d_b200 import build, nn
     build.build()
-    hdr = open(os.path.join(ROOT, "include", "b200nn.h")).read()
-    declared = sorted(set(re.findall(r"\b(b200nn_[a-z_0-9]+)\s*\(", hdr)))
-    assert declared == sorted(nn.SYMBOLS)
+    assert signature_mismatches(nn.SIGNATURES, ("b200nn.h",)) == []
     L = nn.lib()
-    for name in declared:
-        assert hasattr(L, name), name
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "%s/include/b200nn.h"\n'
-                   'int main(){printf("%%zu %%zu %%zu\\n",sizeof(b200nn_linear_desc_t),offsetof(b200nn_linear_desc_t,out),'
-                   'offsetof(b200nn_linear_desc_t,k_padded));}' % ROOT)
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    assert got == [C.sizeof(nn.LinearDesc), nn.LinearDesc.out.offset, nn.LinearDesc.k_padded.offset]
+    for name, (res, args) in nn.SIGNATURES.items():
+        fn = getattr(L, name)
+        assert fn.restype is res and list(fn.argtypes) == args, name
     if not torch.cuda.is_available():
         with pytest.raises(RuntimeError, match="CUDA device only"):
             nn.Linear(torch.zeros(128, 64, dtype=torch.bfloat16), torch.zeros(8, 64), torch.zeros(8), torch.zeros(128, 64, dtype=torch.bfloat16), 4)
@@ -347,19 +410,6 @@ def test_nn_linear_create_rejects_bad_descriptors():
                dict(out_col0=32, ldo=136, n=100, out_min=-1.0, out_max=1.0)):
         rc, err = create(desc(**kw))
         assert rc == want, (kw, rc, err)
-
-
-def test_v2p_glue_struct_layouts(tmp_path):
-    from vid2player3d_b200 import abi
-    src = tmp_path / "sz.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "%s/include/b200env_v2p.h"\n'
-                   'int main(){printf("%%zu %%zu %%zu %%zu %%zu %%zu %%zu\\n",sizeof(b200v2p_prestep_t),offsetof(b200v2p_prestep_t,actions),'
-                   'sizeof(b200v2p_stream_t),offsetof(b200v2p_stream_t,ring_phase),offsetof(b200v2p_ctrl_t,advance),offsetof(b200v2p_ctrl_t,touch_mask),offsetof(b200v2p_state_t,only_mask));}' % ROOT)
-    exe = tmp_path / "sz"
-    subprocess.check_call(["gcc", str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    assert got == [C.sizeof(abi.V2PPreStep), abi.V2PPreStep.actions.offset, C.sizeof(abi.V2PStream), abi.V2PStream.ring_phase.offset,
-                   abi.V2PCtrl.advance.offset, abi.V2PCtrl.touch_mask.offset, abi.V2PState.only_mask.offset]
 
 
 def test_motion_lib_formats_directory_and_merge(tmp_path):

@@ -1,5 +1,5 @@
-"""ctypes mirror of include/b200env.h (structs + packing helpers).  Product code: the native
-binding (native.py) and the tests' oracle wrapper both build their arguments from these."""
+"""ctypes mirror of include/b200env.h, include/b200env_v2p.h and include/b200ball.h (structs, entry-point signatures, packing
+helpers).  Product code: the native binding (native.py) and the tests' oracle wrapper both build their arguments from these."""
 import ctypes as C
 
 import numpy as np
@@ -330,3 +330,57 @@ class V2PActorReset(C.Structure):
         ("pd_target_dof_pos", C.c_void_p), ("target_root_pos", C.c_void_p),
         ("progress_buf", C.c_void_p), ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p), ("mask", C.c_void_p),
     ]
+
+
+# ---------------------------------------------------------------- entry points of libb200env.so
+# name -> (restype, argtypes) of every function include/b200env.h, include/b200env_v2p.h and include/b200ball.h declare; native.lib()
+# applies all of them when it loads the library, so an argument too many or too few, or one that does not convert to its C type,
+# raises ctypes.ArgumentError at the call instead of reaching the library as an undefined register.  Pointers and opaque handles
+# are c_void_p.  tests/test_host.py holds the table to the headers.
+_i32, _i64, _u64, _f32, _p = C.c_int32, C.c_int64, C.c_uint64, C.c_float, C.c_void_p
+SIGNATURES = {
+    # include/b200env.h
+    "b200env_abi_version": (C.c_int, []),
+    "b200env_last_error": (C.c_char_p, []),
+    "b200env_create": (C.c_int, [_p, _p, _p, _i32, _i32, _p]),
+    "b200env_destroy": (C.c_int, [_p]),
+    "b200env_bind": (C.c_int, [_p, _p]),
+    "b200env_set_motion_lib": (C.c_int, [_p, _p]),
+    "b200env_step": (C.c_int, [_p, _p, _p]),
+    "b200env_reset": (C.c_int, [_p, _p, _p, _i32, _p]),
+    "b200env_reset_masked": (C.c_int, [_p, _p, _i32, _f32, _f32, _u64, _p, _p, _p, _p, _p, _i32, _i32, _f32, _p, _p, _p, _p]),
+    "b200env_motion_state": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200env_obs_imitation": (C.c_int, [_p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _p]),
+    "b200env_obs_imitation_rows": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _f32, _p]),
+    "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200env_motion_context": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _i32, _f32, _p, _p, _p]),
+    "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
+    "b200env_set_hull_faces": (C.c_int, [_p, _p, _p, _p, _i32]),
+    "b200env_kernel_form": (_i32, [_p]),
+    "b200env_physics_launch_shape": (C.c_int, [_p, _p, _p]),
+    "b200env_create_assets": (C.c_int, [_p, _p, _i32, _p, _p, _i32, _i32, _p]),
+    "b200env_plan_assets": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
+    "b200env_plan_assets_mixed": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
+    "b200env_choose_asset_plan": (C.c_int, [_p, _i32, _i32, _i32, _p]),
+    "b200env_asset_plan": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200env_launch_count": (_i64, [_p]),
+    "b200env_set_kernel_timing": (C.c_int, [_p, _i32]),
+    "b200env_kernel_ms": (C.c_int, [_p, _p, _p]),
+    # include/b200env_v2p.h
+    "b200v2p_last_error": (C.c_char_p, []),
+    "b200v2p_smpl_to_sim": (C.c_int, [_i32, _p, _p, _p, _i32, _p, _p, _f32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200v2p_fix_head": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p]),
+    "b200v2p_ball_aero": (C.c_int, [_i32, _p, _i32, _p, _p, _p, _p, _i32, _f32, _p]),
+    "b200v2p_ball_reset": (C.c_int, [_i32, _p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "b200v2p_update_state": (C.c_int, [_p, _p]),
+    "b200v2p_controller_post": (C.c_int, [_p, _p]),
+    "b200v2p_pre_step": (C.c_int, [_p, _p]),
+    "b200v2p_ctrl_reset": (C.c_int, [_i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200v2p_stream_gather": (C.c_int, [_p, _p]),
+    "b200v2p_ball_in_estimate": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _p, _p, _p, _p]),
+    "b200v2p_task_reset": (C.c_int, [_p, _p]),
+    "b200v2p_actor_reset": (C.c_int, [_p, _p]),
+    # include/b200ball.h
+    "b200ball_simulate": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200ball_out_rows": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _i32, _p, _p, _p]),
+}

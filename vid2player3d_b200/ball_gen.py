@@ -23,8 +23,6 @@ import torch
 
 from . import native
 
-SYMBOLS = ["b200ball_simulate", "b200ball_out_rows"]
-
 
 class BallSim(C.Structure):
     """b200ball_sim_t"""
@@ -79,7 +77,7 @@ def simulate(launch_pos, launch_vel, launch_vspin, control_freq_inv=2, num_frame
     pnet = torch.empty(n, dtype=torch.uint8, device=lp.device)
     cfg = _cfg(num_frames, control_freq_inv, substeps, spin_scale, first_comp, **physics)
     with torch.cuda.device(lp.device):
-        native._check(native.lib().b200ball_simulate(C.byref(cfg), C.c_int64(n), C.c_int32(0 if dtype == torch.float32 else 1), native._ptr(lp),
+        native._check(native.lib().b200ball_simulate(C.byref(cfg), n, 0 if dtype == torch.float32 else 1, native._ptr(lp),
                                                      native._ptr(lv), native._ptr(ls), native._ptr(traj), native._ptr(bpos), native._ptr(bidx),
                                                      native._ptr(pnet), native._stream()))
     return traj, bpos, bidx, pnet.bool()
@@ -116,9 +114,9 @@ def simulate_without_bounce(launch_vel_h, launch_vel_v, launch_vspin, params=tra
     out_y = alloc(n, ny, 2, dtype=dtype, device=vh.device)
     cfg = _cfg(num_frames, control_freq_inv, substeps, spin_scale, 0, **physics)
     with torch.cuda.device(vh.device):
-        native._check(native.lib().b200ball_out_rows(C.byref(cfg), C.c_int64(n), C.c_int32(0 if dtype == torch.float32 else 1), native._ptr(vh),
-                                                     native._ptr(vv), native._ptr(vs), native._ptr(gx), native._ptr(cx), C.c_int32(len(gx)),
-                                                     C.c_int32(nx), native._ptr(gy), native._ptr(cy), C.c_int32(len(gy)), C.c_int32(ny),
+        native._check(native.lib().b200ball_out_rows(C.byref(cfg), n, 0 if dtype == torch.float32 else 1, native._ptr(vh),
+                                                     native._ptr(vv), native._ptr(vs), native._ptr(gx), native._ptr(cx), len(gx),
+                                                     nx, native._ptr(gy), native._ptr(cy), len(gy), ny,
                                                      native._ptr(out_x), native._ptr(out_y), native._stream()))
     return out_x, out_y
 

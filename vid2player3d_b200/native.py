@@ -11,13 +11,6 @@ from .build import LIB
 
 _lib = None
 
-SYMBOLS = ["b200env_abi_version", "b200env_last_error", "b200env_create", "b200env_destroy", "b200env_bind",
-           "b200env_set_motion_lib", "b200env_step", "b200env_reset", "b200env_motion_state", "b200env_obs_imitation",
-           "b200env_physics_only", "b200env_launch_count", "b200env_set_env_slice", "b200env_motion_context", "b200env_set_kernel_timing",
-           "b200env_kernel_ms", "b200env_obs_imitation_rows", "b200env_set_hull_faces", "b200env_kernel_form",
-           "b200env_physics_launch_shape", "b200env_create_assets", "b200env_plan_assets", "b200env_asset_plan", "b200env_reset_masked",
-           "b200env_plan_assets_mixed", "b200env_choose_asset_plan"]
-
 ENVS_PER_BATCH = 32   # envs per CTA batch of the default physics launch (step_kernel_packed<true>): the batch size of the asset plan
 
 
@@ -28,11 +21,9 @@ def lib():
             raise RuntimeError(f"{LIB} not built - run `python -c 'import __graft_entry__ as g; g.build()'` "
                                "(the environment has no CPU fallback)")
         L = C.CDLL(LIB)
-        L.b200env_last_error.restype = C.c_char_p
-        L.b200env_launch_count.restype = C.c_int64
-        L.b200env_launch_count.argtypes = [C.c_void_p]
-        for name in SYMBOLS:
-            getattr(L, name)
+        for name, (restype, argtypes) in abi.SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         if L.b200env_abi_version() != abi.ABI_VERSION:
             raise RuntimeError("libb200env.so ABI version mismatch - rebuild")
         _lib = L
@@ -45,12 +36,12 @@ def _check(rc):
 
 
 def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+    return t.data_ptr() if t is not None else None
 
 
 def _stream():
     import torch
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):
@@ -64,7 +55,7 @@ def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=Fals
     nb = C.c_int32(0)
     p = lambda a: a.ctypes.data_as(C.c_void_p)  # noqa: E731
     fn = lib().b200env_plan_assets_mixed if mixed else lib().b200env_plan_assets
-    _check(fn(p(ea), C.c_int32(n), C.c_int32(int(num_assets)), C.c_int32(int(envs_per_batch)), p(rows), p(ba), p(bf), p(bc), C.byref(nb)))
+    _check(fn(p(ea), n, num_assets, envs_per_batch, p(rows), p(ba), p(bf), p(bc), C.byref(nb)))
     k = nb.value
     return rows[:n], np.stack([ba[:k], bf[:k], bc[:k]], 1)
 
@@ -75,8 +66,7 @@ def choose_asset_plan(env_asset, num_assets, grid):
     import numpy as np
     ea = np.ascontiguousarray(env_asset, np.int32)
     m = C.c_int32(0)
-    _check(lib().b200env_choose_asset_plan(ea.ctypes.data_as(C.c_void_p), C.c_int32(len(ea)), C.c_int32(int(num_assets)), C.c_int32(int(grid)),
-                                           C.byref(m)))
+    _check(lib().b200env_choose_asset_plan(ea.ctypes.data_as(C.c_void_p), len(ea), num_assets, grid, C.byref(m)))
     return bool(m.value)
 
 
@@ -92,8 +82,8 @@ class Env:
         import numpy as np
         if env_asset is None:
             verts = np.ascontiguousarray(verts, np.float32)
-            _check(lib().b200env_create(C.byref(model_struct), verts.ctypes.data_as(C.c_void_p), C.byref(cfg_struct),
-                                        C.c_int32(num_envs), C.c_int32(device_index), C.byref(self._h)))
+            _check(lib().b200env_create(C.byref(model_struct), verts.ctypes.data_as(C.c_void_p), C.byref(cfg_struct), num_envs, device_index,
+                                        C.byref(self._h)))
         else:
             models, vs = list(model_struct), [np.ascontiguousarray(v, np.float32) for v in verts]
             ea = np.ascontiguousarray(env_asset, np.int32)
@@ -101,8 +91,8 @@ class Env:
                 raise ValueError(f"{len(models)} models, {len(vs)} vertex arrays and {len(ea)} env_asset entries for {num_envs} envs")
             marr = (abi.Model * len(models))(*models)
             varr = (C.c_void_p * len(vs))(*[v.ctypes.data for v in vs])
-            _check(lib().b200env_create_assets(marr, varr, C.c_int32(len(models)), ea.ctypes.data_as(C.c_void_p), C.byref(cfg_struct),
-                                               C.c_int32(num_envs), C.c_int32(device_index), C.byref(self._h)))
+            _check(lib().b200env_create_assets(marr, varr, len(models), ea.ctypes.data_as(C.c_void_p), C.byref(cfg_struct), num_envs,
+                                               device_index, C.byref(self._h)))
             model_struct = models[0]
         self.model, self.cfg, self.num_envs = model_struct, cfg_struct, num_envs
 
@@ -159,11 +149,11 @@ class Env:
         tris = np.ascontiguousarray(tris, np.uint8)
         ntris = np.ascontiguousarray(ntris, np.int32)
         _check(lib().b200env_set_hull_faces(self._h, planes.ctypes.data_as(C.c_void_p), tris.ctypes.data_as(C.c_void_p),
-                                            ntris.ctypes.data_as(C.c_void_p), C.c_int32(int(tmax))))
+                                            ntris.ctypes.data_as(C.c_void_p), tmax))
 
     def set_env_slice(self, first, stride):
         """this handle steps rows first, first+stride, ... of the bound tensors (one handle per asset in dual mode)"""
-        _check(lib().b200env_set_env_slice(self._h, C.c_int32(int(first)), C.c_int32(int(stride))))
+        _check(lib().b200env_set_env_slice(self._h, first, stride))
 
     def step(self, actions):
         if not (actions.is_cuda and actions.is_contiguous() and actions.dtype.is_floating_point):
@@ -175,7 +165,7 @@ class Env:
     def reset(self, env_ids, motion_times):
         n = int(env_ids.shape[0])
         if n:
-            _check(lib().b200env_reset(self._h, _ptr(env_ids), _ptr(motion_times), C.c_int32(n), _stream()))
+            _check(lib().b200env_reset(self._h, _ptr(env_ids), _ptr(motion_times), n, _stream()))
 
     def reset_masked(self, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos, init_dof_vel, reset_times,
                      num_frames, first_frame, dt, feat, feat_mask, work):
@@ -185,25 +175,21 @@ class Env:
         assert mask.shape[0] == self.num_envs and work.shape[0] >= self.num_envs + 2
         for t in (mask, counter, init_root, init_dof_pos, init_dof_vel, reset_times, feat, feat_mask, work):
             assert t is None or (t.is_cuda and t.is_contiguous())
-        _check(lib().b200env_reset_masked(self._h, _ptr(mask), C.c_int32(int(bool(sample_time))), C.c_float(float(truncate)),
-                                          C.c_float(float(ref_prob)), C.c_uint64(int(seed) & 0xFFFFFFFFFFFFFFFF), _ptr(counter),
-                                          _ptr(init_root), _ptr(init_dof_pos), _ptr(init_dof_vel), _ptr(reset_times),
-                                          C.c_int32(int(num_frames)), C.c_int32(int(first_frame)), C.c_float(float(dt)), _ptr(feat),
-                                          _ptr(feat_mask), _ptr(work), _stream()))
+        _check(lib().b200env_reset_masked(self._h, _ptr(mask), int(bool(sample_time)), truncate, ref_prob, int(seed), _ptr(counter),
+                                          _ptr(init_root), _ptr(init_dof_pos), _ptr(init_dof_vel), _ptr(reset_times), num_frames, first_frame,
+                                          dt, _ptr(feat), _ptr(feat_mask), _ptr(work), _stream()))
 
     def motion_state(self, ids, times, out):
         """out: dict name -> tensor or None for root_pos, root_rot, dof_pos, root_vel, root_ang_vel, dof_vel, key_pos,
         rb_pos, rb_rot."""
         names = ("root_pos", "root_rot", "dof_pos", "root_vel", "root_ang_vel", "dof_vel", "key_pos", "rb_pos", "rb_rot")
-        _check(lib().b200env_motion_state(self._h, _ptr(ids), _ptr(times), C.c_int32(int(ids.shape[0])),
-                                          *[_ptr(out.get(k)) for k in names], _stream()))
+        _check(lib().b200env_motion_state(self._h, _ptr(ids), _ptr(times), ids.shape[0], *[_ptr(out.get(k)) for k in names], _stream()))
 
     def motion_context(self, env_ids, motion_ids, motion_times, num_frames, first_frame, dt, feat, mask):
         """feat [N, num_frames, W] float32, mask [N, num_frames] bool; rows env_ids (None: rows 0..n-1)"""
         assert feat.is_cuda and feat.is_contiguous() and mask.is_contiguous() and motion_ids.is_contiguous() and motion_times.is_contiguous()
-        _check(lib().b200env_motion_context(self._h, _ptr(env_ids), _ptr(motion_ids), _ptr(motion_times), C.c_int32(int(motion_ids.shape[0])),
-                                            C.c_int32(int(num_frames)), C.c_int32(int(first_frame)), C.c_float(float(dt)), _ptr(feat),
-                                            _ptr(mask), _stream()))
+        _check(lib().b200env_motion_context(self._h, _ptr(env_ids), _ptr(motion_ids), _ptr(motion_times), motion_ids.shape[0], num_frames,
+                                            first_frame, dt, _ptr(feat), _ptr(mask), _stream()))
 
     def obs_row_width(self, jpos=False):
         """columns of the row the observation launches write: 734 (513 with jpos) for the 24-body humanoid, 69 dofs, shape_dim 11"""
@@ -216,11 +202,10 @@ class Env:
                       body_ang_vel, motion_bodies, local_root_obs, root_height_obs, obs, jpos=False):
         n = int(body_pos.shape[0])
         assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == self.obs_row_width(jpos), (tuple(obs.shape), self.obs_row_width(jpos))
-        _check(lib().b200env_obs_imitation(self._h, C.c_int32(n), _ptr(body_pos), _ptr(body_rot), _ptr(target_pos),
+        _check(lib().b200env_obs_imitation(self._h, n, _ptr(body_pos), _ptr(body_rot), _ptr(target_pos),
                                            _ptr(target_rot), _ptr(dof_pos), _ptr(dof_vel), _ptr(target_dof_pos),
                                            _ptr(body_vel), _ptr(body_ang_vel), _ptr(motion_bodies),
-                                           C.c_int32(int(bool(local_root_obs)) | (2 if jpos else 0)), C.c_int32(int(root_height_obs)), _ptr(obs),
-                                           _stream()))
+                                           int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _stream()))
 
     def obs_imitation_rows(self, n, rigid_body_state, bodies_per_env, dof_state, target_pos, target_rot, target_dof_pos, motion_bodies,
                            local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0, jpos=False):
@@ -229,26 +214,23 @@ class Env:
         W = self.obs_row_width(jpos)
         assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == W, (tuple(obs.shape), W)
         assert obs_bf16 is None or (obs_bf16.dim() == 2 and obs_bf16.shape[0] >= n), tuple(obs_bf16.shape)
-        _check(lib().b200env_obs_imitation_rows(self._h, C.c_int32(int(n)), _ptr(rigid_body_state), C.c_int32(int(bodies_per_env)), _ptr(dof_state),
+        _check(lib().b200env_obs_imitation_rows(self._h, n, _ptr(rigid_body_state), bodies_per_env, _ptr(dof_state),
                                                 _ptr(target_pos), _ptr(target_rot), _ptr(target_dof_pos), _ptr(motion_bodies),
-                                                C.c_int32(int(bool(local_root_obs)) | (2 if jpos else 0)), C.c_int32(int(root_height_obs)),
-                                                _ptr(obs), _ptr(obs_bf16),
-                                                C.c_int32(int(obs_bf16.shape[1]) if obs_bf16 is not None else 0), _ptr(mean), _ptr(rstd),
-                                                C.c_float(float(clamp)), _stream()))
+                                                int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _ptr(obs_bf16),
+                                                obs_bf16.shape[1] if obs_bf16 is not None else 0, _ptr(mean), _ptr(rstd), clamp, _stream()))
 
     def physics_only(self, root, dof_pos, dof_vel, pd_tar, ext_wrench, rb_out, contact_out, n_steps=1, ball=None, ball_hits=None):
         import torch
         prec = {torch.float32: 0, torch.float64: 1}[root.dtype]
         for t in (dof_pos, dof_vel, pd_tar, rb_out):
             assert t.dtype == root.dtype and t.is_cuda and t.is_contiguous()
-        _check(lib().b200env_physics_only(self._h, C.c_int32(prec), C.c_int32(int(root.shape[0])), C.c_int32(n_steps),
-                                          _ptr(root), _ptr(dof_pos), _ptr(dof_vel), _ptr(pd_tar), _ptr(ext_wrench),
-                                          _ptr(rb_out), _ptr(contact_out), _ptr(ball), _ptr(ball_hits), _stream()))
+        _check(lib().b200env_physics_only(self._h, prec, root.shape[0], n_steps, _ptr(root), _ptr(dof_pos), _ptr(dof_vel), _ptr(pd_tar),
+                                          _ptr(ext_wrench), _ptr(rb_out), _ptr(contact_out), _ptr(ball), _ptr(ball_hits), _stream()))
 
     @property
     def kernel_form(self):
         """'lane' | 'packed' | 'packed3' | 'tmem' (include/b200env.h: b200env_kernel_form)"""
-        return ("lane", "packed", "packed3", "tmem")[int(lib().b200env_kernel_form(self._h))]
+        return ("lane", "packed", "packed3", "tmem")[lib().b200env_kernel_form(self._h)]
 
     @property
     def physics_launch_shape(self):
@@ -281,11 +263,11 @@ class Env:
 
     @property
     def launch_count(self):
-        return int(lib().b200env_launch_count(self._h))
+        return lib().b200env_launch_count(self._h)
 
     def set_kernel_timing(self, on=True):
         """event pairs around the physics launch of every step (measurement aid, include/b200env.h)"""
-        _check(lib().b200env_set_kernel_timing(self._h, C.c_int32(1 if on else 0)))
+        _check(lib().b200env_set_kernel_timing(self._h, 1 if on else 0))
 
     def kernel_ms(self):
         """(mean ms, count) of the physics launches since the last call"""

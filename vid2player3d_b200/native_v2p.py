@@ -4,17 +4,13 @@ import ctypes as C
 from . import abi
 from .native import _ptr, _stream, lib
 
-SYMBOLS = ["b200v2p_last_error", "b200v2p_smpl_to_sim", "b200v2p_ball_aero", "b200v2p_ball_reset", "b200v2p_ball_in_estimate", "b200v2p_update_state",
-           "b200v2p_controller_post", "b200v2p_task_reset", "b200v2p_actor_reset", "b200v2p_fix_head", "b200v2p_pre_step", "b200v2p_stream_gather", "b200v2p_ctrl_reset"]
 GRIP_NORMAL = {'eastern': (0.0, 1.0, 0.0), 'semi_western': (0.0, 2.0 ** -0.5, 2.0 ** -0.5)}
 REWARD_TYPES = {'reach': 0, 'return': 1, 'return_w_estimate': 2}
 
 
 def _check(rc):
     if rc != 0:
-        L = lib()
-        L.b200v2p_last_error.restype = C.c_char_p
-        raise RuntimeError(f"b200v2p error {rc}: {L.b200v2p_last_error().decode()}")
+        raise RuntimeError(f"b200v2p error {rc}: {lib().b200v2p_last_error().decode()}")
 
 
 def _c(t):
@@ -29,27 +25,25 @@ def smpl_to_sim(root_pos, joint_rotmat, rest, parents, smpl_2_mujoco, dt, out, p
     n = int(root_pos.shape[0])
     num_rest = 1 if rest.dim() == 2 else int(rest.shape[0])      # rest [24,3] or [S,24,3]: env e uses shape e % S
     assert rest.is_contiguous() and rest.shape[-2:] == (24, 3)
-    _check(lib().b200v2p_smpl_to_sim(C.c_int32(n), _c(root_pos), _c(joint_rotmat), _c(rest), C.c_int32(num_rest), _c(parents), _c(smpl_2_mujoco), C.c_float(dt),
+    _check(lib().b200v2p_smpl_to_sim(n, _c(root_pos), _c(joint_rotmat), _c(rest), num_rest, _c(parents), _c(smpl_2_mujoco), dt,
                                      _c(prev_root_pos), _c(prev_rb_rot), _c(out["root_rot"]), _c(out["dof_pos"]), _c(out["root_vel"]),
                                      _c(out["root_ang_vel"]), _c(out["dof_vel"]), _c(out["rb_pos"]), _c(out["rb_rot"]), _c(prev_root_pos_update),
                                      _c(target_root_pos_out), _c(only_mask), _stream()))
 
 
 def fix_head(rb_pos, rb_rot, ball_pos, root_pos, joint_rotmat, head_body=13):
-    _check(lib().b200v2p_fix_head(C.c_int32(int(rb_pos.shape[0])), _c(rb_pos), _c(rb_rot), C.c_int32(head_body), _c(ball_pos), _c(root_pos),
-                                  _c(joint_rotmat), _stream()))
+    _check(lib().b200v2p_fix_head(rb_pos.shape[0], _c(rb_pos), _c(rb_rot), head_body, _c(ball_pos), _c(root_pos), _c(joint_rotmat), _stream()))
 
 
 def ball_aero(ball_states, has_bounce, has_bounce_now, bounce_pos, force, substeps, spin_scale, stride=None):
-    n = int(has_bounce.shape[0])
-    _check(lib().b200v2p_ball_aero(C.c_int32(n), _c(ball_states), C.c_int32(stride or ball_states.stride(0)), _c(has_bounce), _c(has_bounce_now),
-                                   _c(bounce_pos), _c(force), C.c_int32(substeps), C.c_float(spin_scale), _stream()))
+    _check(lib().b200v2p_ball_aero(has_bounce.shape[0], _c(ball_states), stride or ball_states.stride(0), _c(has_bounce), _c(has_bounce_now),
+                                   _c(bounce_pos), _c(force), substeps, spin_scale, _stream()))
 
 
 def ball_reset(env_ids, pool_index, pool, ball_states, ball_pos, ball_vel, has_bounce, bounce_pos, has_contact, traj, stride=None):
     """ball_states: first ball row; `stride` floats between consecutive envs' ball rows (26 when the ball is actor 1 of 2)"""
-    _check(lib().b200v2p_ball_reset(C.c_int32(int(env_ids.shape[0])), _c(env_ids), _c(pool_index), _c(pool), _c(ball_states),
-                                    C.c_int32(stride or ball_states.stride(0)), _c(ball_pos), _c(ball_vel), _c(has_bounce), _c(bounce_pos),
+    _check(lib().b200v2p_ball_reset(env_ids.shape[0], _c(env_ids), _c(pool_index), _c(pool), _c(ball_states),
+                                    stride or ball_states.stride(0), _c(ball_pos), _c(ball_vel), _c(has_bounce), _c(bounce_pos),
                                     _c(has_contact), _c(traj), _stream()))
 
 
@@ -83,8 +77,8 @@ def ball_in_estimate(contact_ids, ball_states, stride, table, params, traj, stat
     for x in (contact_ids, table, traj, states_in, states_out):
         assert x.is_cuda and x.is_contiguous()
     assert table.shape[1:] == (50, 2) and traj.shape == (n, 50, 3) and states_in.shape == (n, 13) and states_out.shape == (n, 13)
-    _check(lib().b200v2p_ball_in_estimate(C.c_int32(n), _ptr(contact_ids), _ptr(ball_states), C.c_int32(stride), _ptr(table),
-                                          C.c_int64(int(table.shape[0])), p.ctypes.data_as(C.c_void_p), _ptr(traj), _ptr(states_in),
+    _check(lib().b200v2p_ball_in_estimate(n, _ptr(contact_ids), _ptr(ball_states), stride, _ptr(table),
+                                          table.shape[0], p.ctypes.data_as(C.c_void_p), _ptr(traj), _ptr(states_in),
                                           _ptr(states_out), _stream()))
 
 
@@ -196,5 +190,5 @@ def stream_gather(n, frames, advance, t, reseed_mask=None, seed=0):
 def ctrl_reset(mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):
     for x in (mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):
         assert x.is_cuda and x.is_contiguous()
-    _check(lib().b200v2p_ctrl_reset(C.c_int32(int(mask.shape[0])), _ptr(mask), _ptr(progress_buf), _ptr(reset_buf), _ptr(terminate_buf),
+    _check(lib().b200v2p_ctrl_reset(mask.shape[0], _ptr(mask), _ptr(progress_buf), _ptr(reset_buf), _ptr(terminate_buf),
                                     _ptr(num_reset_reaction), _ptr(distance), _ptr(num_reset), _stream()))

@@ -21,8 +21,6 @@ from .build import LIB_NN
 ACT = {None: 0, "none": 0, "relu": 1, "elu": 2}
 _lib = None
 
-SYMBOLS = ["b200nn_abi_version", "b200nn_last_error", "b200nn_linear_create", "b200nn_linear_destroy", "b200nn_linear_run",
-           "b200nn_cast_rows", "b200nn_cast_rows3", "b200nn_cast_rows_masked", "b200nn_gate_softmax"]
 ABI_VERSION = 1
 
 
@@ -33,15 +31,32 @@ class LinearDesc(C.Structure):
                 ("out_min", C.c_float), ("out_max", C.c_float)]
 
 
+# name -> (restype, argtypes) of every function include/b200nn.h declares; lib() applies all of them when it loads the library, so an
+# argument too many or too few, or one that does not convert to its C type, raises ctypes.ArgumentError at the call.  Pointers and
+# opaque handles are c_void_p.  tests/test_host.py holds the table to the header.
+_i32, _f32, _p = C.c_int32, C.c_float, C.c_void_p
+SIGNATURES = {
+    "b200nn_abi_version": (C.c_int, []),
+    "b200nn_last_error": (C.c_char_p, []),
+    "b200nn_linear_create": (C.c_int, [_p, _i32, _p]),
+    "b200nn_linear_destroy": (C.c_int, [_p]),
+    "b200nn_linear_run": (C.c_int, [_p, _p]),
+    "b200nn_cast_rows": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _p, _p, _f32, _f32, _p]),
+    "b200nn_cast_rows_masked": (C.c_int, [_p, _i32, _p, _i32, _i32, _i32, _p, _f32, _f32, _p]),
+    "b200nn_cast_rows3": (C.c_int, [_p, _i32, _p, _p, _p, _i32, _i32, _i32, _p]),
+    "b200nn_gate_softmax": (C.c_int, [_p, _i32, _i32, _p, _p, _i32, _p, _i32, _p]),
+}
+
+
 def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_NN):
             raise RuntimeError(f"{LIB_NN} not built - run `python -c 'import __graft_entry__ as g; g.build()'` (no fallback)")
         L = C.CDLL(LIB_NN)
-        L.b200nn_last_error.restype = C.c_char_p
-        for name in SYMBOLS:
-            getattr(L, name)
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         if L.b200nn_abi_version() != ABI_VERSION:
             raise RuntimeError("libb200nn.so ABI version mismatch - rebuild")
         _lib = L
@@ -54,7 +69,7 @@ def _check(rc):
 
 
 def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return torch.cuda.current_stream().cuda_stream
 
 
 def _up(x, m):
@@ -101,7 +116,7 @@ class Linear:
                        rows=rows, n=N, n_padded=self.n_padded, k_padded=self.k_padded, num_experts=E, act=ACT[act], out_bf16=int(out_bf16),
                        out_min=out_clamp[0] if out_clamp else 0.0, out_max=out_clamp[1] if out_clamp else 0.0)
         self._h = C.c_void_p()
-        _check(lib().b200nn_linear_create(C.byref(d), C.c_int32(dev.index or 0), C.byref(self._h)))
+        _check(lib().b200nn_linear_create(C.byref(d), dev.index or 0, C.byref(self._h)))
         self.flops = 2.0 * rows * N * K * E
 
     def run(self):
@@ -119,9 +134,9 @@ class Linear:
 def cast_rows(src, dst, cols, mean=None, rstd=None, lo=-3.0e38, hi=3.0e38):
     """dst[:, :cols] = bf16(clamp((src - mean) * rstd, lo, hi)); src float [rows, >= cols], dst bf16 buffer"""
     assert src.dtype == torch.float32 and src.stride(-1) == 1 and dst.dtype == torch.bfloat16
-    _check(lib().b200nn_cast_rows(C.c_void_p(src.data_ptr()), C.c_int32(src.stride(0)), C.c_void_p(dst.data_ptr()), C.c_int32(dst.shape[1]),
-                                  C.c_int32(src.shape[0]), C.c_int32(cols), C.c_void_p(mean.data_ptr()) if mean is not None else None,
-                                  C.c_void_p(rstd.data_ptr()) if rstd is not None else None, C.c_float(lo), C.c_float(hi), _stream()))
+    _check(lib().b200nn_cast_rows(src.data_ptr(), src.stride(0), dst.data_ptr(), dst.shape[1], src.shape[0], cols,
+                                  mean.data_ptr() if mean is not None else None, rstd.data_ptr() if rstd is not None else None, lo, hi,
+                                  _stream()))
 
 
 class PolicyMLP:
@@ -221,15 +236,14 @@ class MixedDecoder:
         """z float [rows, latent], c float [rows, >= cond] -> float [rows, out_dim] (static buffer).  c = None: the condition block
         already sits in the first layer's operand buffer (`set_condition`, or the autoregressive `feed_back`)."""
         assert z.dtype == torch.float32 and z.stride(-1) == 1
-        _check(lib().b200nn_cast_rows3(C.c_void_p(z.data_ptr()), C.c_int32(z.stride(0)), C.c_void_p(self.x0.data_ptr()), C.c_void_p(self.x1.data_ptr()),
-                                       C.c_void_p(self.x2.data_ptr()), C.c_int32(self.x0.shape[1]), C.c_int32(self.rows), C.c_int32(self.L), _stream()))
+        _check(lib().b200nn_cast_rows3(z.data_ptr(), z.stride(0), self.x0.data_ptr(), self.x1.data_ptr(), self.x2.data_ptr(), self.x0.shape[1],
+                                       self.rows, self.L, _stream()))
         if c is not None:
             self.set_condition(c, c_clamp)
         self.gate1.run()
         self.gate2.run()
-        _check(lib().b200nn_gate_softmax(C.c_void_p(self.g2.data_ptr()), C.c_int32(self.g2.shape[1]), C.c_int32(self.gw.shape[1]),
-                                         C.c_void_p(self.gw.data_ptr()), C.c_void_p(self.gb.data_ptr()), C.c_int32(self.E),
-                                         C.c_void_p(self.coef.data_ptr()), C.c_int32(self.rows), _stream()))
+        _check(lib().b200nn_gate_softmax(self.g2.data_ptr(), self.g2.shape[1], self.gw.shape[1], self.gw.data_ptr(), self.gb.data_ptr(), self.E,
+                                         self.coef.data_ptr(), self.rows, _stream()))
         self.l1.run()
         self.l2.run()
         self.l3.run()
@@ -272,9 +286,7 @@ def _cast_cols(src, dst, col0, cols, lo=-3.0e38, hi=3.0e38, row_mask=None):
     view_ptr = dst.data_ptr() + col0 * 2
     if row_mask is not None:
         assert row_mask.dtype == torch.bool and row_mask.is_contiguous() and row_mask.shape[0] == src.shape[0]
-        _check(lib().b200nn_cast_rows_masked(C.c_void_p(src.data_ptr()), C.c_int32(src.stride(0)), C.c_void_p(view_ptr), C.c_int32(dst.shape[1]),
-                                             C.c_int32(src.shape[0]), C.c_int32(cols), C.c_void_p(row_mask.data_ptr()), C.c_float(lo), C.c_float(hi),
-                                             _stream()))
+        _check(lib().b200nn_cast_rows_masked(src.data_ptr(), src.stride(0), view_ptr, dst.shape[1], src.shape[0], cols, row_mask.data_ptr(),
+                                             lo, hi, _stream()))
         return
-    _check(lib().b200nn_cast_rows(C.c_void_p(src.data_ptr()), C.c_int32(src.stride(0)), C.c_void_p(view_ptr), C.c_int32(dst.shape[1]),
-                                  C.c_int32(src.shape[0]), C.c_int32(cols), None, None, C.c_float(lo), C.c_float(hi), _stream()))
+    _check(lib().b200nn_cast_rows(src.data_ptr(), src.stride(0), view_ptr, dst.shape[1], src.shape[0], cols, None, None, lo, hi, _stream()))
