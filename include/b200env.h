@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 7
+#define B200_ABI_VERSION 8
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:
@@ -149,6 +149,14 @@ typedef struct b200_buffers {
   uint8_t* has_bounce_now;   /* [N] _has_bounce_now (cleared at the start of every step, :688) */
   float* bounce_pos;         /* [N,3] _bounce_pos */
   uint8_t* racket_hit_now;   /* [N] exact racket-ball impact during this step (contact-force sensor path, :771-779) */
+  /* DOF force sensors (enable_actor_dof_force_sensors + acquire_dof_force_tensor, embodied_pose/env/tasks/humanoid_smpl_im.py:369,
+   * humanoid_smpl.py:77-78), NULL = none.  [N, nd]: dof_force[e, 3j + k] = the generalized force joint j's PD drive and its limit
+   * spring-damper applied during the LAST substep of the step, in the joint's child frame (the frame of the dof velocities), taken at
+   * the end-of-substep velocity qd+ = qd + h qdd of the implicit drive: kp (pd - q - h qd+) - kd qd+ [+ limk (lim - q - h qd+) - limc qd+
+   * while a limit is active].  Armature (inertia), contact and joint-reaction forces are not part of it.  Written by the physics
+   * launch of b200env_step (rows of the handle's env slice only); b200env_bind refuses it for the A/B kernel forms
+   * (B200ENV_KERNEL=lane|tmem|packed3, B200ENV_SPLIT=0). */
+  float* dof_force;
 } b200_buffers_t;
 
 typedef struct b200env* b200env_handle;
@@ -230,10 +238,12 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
  * float64 CPU restatement (oracle/physics_ref.c).  root [n,13], dof_pos/dof_vel/pd_tar [n,nd],
  * ext_wrench [n,6] (force, torque on body 0, world frame, first sim step only),
  * rb_out [n,nb,13], contact_out [n,nb,3].  n_steps control steps are run back to back.
- * ball: in/out [n,13] (pos, quat unused, lin vel, ang vel) or NULL; ball_hits [n] counts racket impacts (or NULL). */
+ * ball: in/out [n,13] (pos, quat unused, lin vel, ang vel) or NULL; ball_hits [n] counts racket impacts (or NULL).
+ * dof_force_out: [n,nd] in the precision of prec, the DOF force sensor of the last control step (b200_buffers_t::dof_force), or NULL;
+ * refused like the sensor at b200env_bind on a handle of an A/B kernel form. */
 int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_steps, void* root, void* dof_pos,
                          void* dof_vel, const void* pd_tar, const void* ext_wrench, void* rb_out, void* contact_out,
-                         void* ball, int32_t* ball_hits, void* stream);
+                         void* ball, int32_t* ball_hits, void* stream, void* dof_force_out);
 
 /* replaces HumanoidSMPLIM._init_context (embodied_pose/env/tasks/humanoid_smpl_im.py:530-563): for listed env i and frame
  * j in [0, num_frames): t = motion_times[i] + dt + (first_frame + j) * dt; writes

@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class Model(C.Structure):
@@ -69,6 +69,7 @@ class Buffers(C.Structure):
         ("p_dof_pos", C.c_void_p), ("p_dof_vel", C.c_void_p), ("p_rb_pos", C.c_void_p), ("p_rb_rot", C.c_void_p),
         ("pd_targets", C.c_void_p), ("actions_used", C.c_void_p), ("num_actions", C.c_int32),
         ("has_bounce", C.c_void_p), ("has_bounce_now", C.c_void_p), ("bounce_pos", C.c_void_p), ("racket_hit_now", C.c_void_p),
+        ("dof_force", C.c_void_p),
     ]
 
 
@@ -352,7 +353,7 @@ SIGNATURES = {
     "b200env_motion_state": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200env_obs_imitation": (C.c_int, [_p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _p]),
     "b200env_obs_imitation_rows": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _f32, _p]),
-    "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200env_motion_context": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _i32, _f32, _p, _p, _p]),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
     "b200env_set_hull_faces": (C.c_int, [_p, _p, _p, _p, _i32]),

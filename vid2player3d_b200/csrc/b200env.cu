@@ -75,6 +75,7 @@ struct b200env {
   float* d_ext;                        // [num_envs rows of the bound tensors, 6] residual root wrench between pre_kernel and the physics launch
   int ext_rows;
   PhysForm form;                       // the physics launch of b200env_step, fixed at create
+  bool dof_force;                      // the physics launch is the DOF force sensor instantiation (bufs.dof_force bound; fixed at bind)
   int32_t *d_bin, *d_perm;             // PhysForm::Sorted: [num_envs]
   uint32_t *d_pos, *d_cnt;             // [num_envs], [SORT_BINS]
   int env_first = 0, env_stride = 1;   // b200env_set_env_slice: local env i = row env_first + env_stride * i of the bound tensors
@@ -1069,7 +1070,9 @@ __host__ __device__ constexpr int pk_launch_warps(bool split) { return pk_warps(
 // memory is asset 0's and only its topology is used; each lane reads the numeric constants and the hull vertices of its own env's
 // asset from that asset's header in global memory, assets[e] for env e, through L1.  The per-env rows stay out of shared memory because
 // they would not fit next to 32 envs of records (DESIGN.md 5).
-template <bool SPLIT, bool MULTI = false, bool MIXED = false>
+// DOF_FORCE = true (split form only): the DOF force sensor (packed.cuh::pk_dof_force) into the bound bf.dof_force rows; nothing else
+// of the launch changes.
+template <bool SPLIT, bool MULTI = false, bool MIXED = false, bool DOF_FORCE = false>
 __global__ void __launch_bounds__(PK_BOUND(SPLIT) * 32, 1)
 step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, b200_buffers_t bf,
                    b200_motion_lib_t ml, const float* __restrict__ actions, int num_envs, unsigned long long* __restrict__ ticket,
@@ -1109,6 +1112,7 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
 #endif
   static_assert(!MULTI || (SPLIT && PK_GROUPS == 1 && !PK_WARP_TICKETS), "several assets: split form, one group of warps per CTA");
   static_assert(!MIXED || (SPLIT && !MULTI && !PK_SHADOW), "mixed batches: split form, one plan");
+  static_assert(!DOF_FORCE || (SPLIT && !PK_SHADOW), "DOF force sensor: split form");
   constexpr int G0 = PK_GROUPS == 1 ? PK_WARPS_K : (PK_WARPS_K + 1) / 2;   // warps in group 0
   const int grp = warp < G0 ? 0 : 1;
   const int gw0 = grp == 0 ? 0 : G0, gwn = grp == 0 ? G0 : PK_WARPS_K - G0;   // first warp / number of warps of my group
@@ -1180,11 +1184,13 @@ step_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const
     ball_clear(ball);
     const int64_t erow_g = SPLIT ? row(valid ? eb + g : eb) : env_first + (int64_t)env_stride * (eb + g);
     if (cfg.has_ball && valid && s == BALL_SLOT) ball_load(bf, erow_g, ball);
+    float* const dof_force = DOF_FORCE && valid ? bf.dof_force + erow_g * M.nd : nullptr;   // my env's sensor row
     if constexpr (MIXED) {
       const DevBlob* an = assets[valid ? eb + g : eb];   // my env's asset (a lane without an env: the warp's first env's, never stored)
-      if (ABL != 1) control_step_packed<float>(B, an->m, reinterpret_cast<const float*>(an + 1), pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
+      if (ABL != 1) control_step_packed<float, DOF_FORCE>(B, an->m, reinterpret_cast<const float*>(an + 1), pc, wrec, lane, valid, ball,
+                                                          STEP_SYNC && full_batch, dof_force);
     } else {
-      if (ABL != 1) control_step_packed<float>(B, verts, pc, wrec, lane, valid, ball, STEP_SYNC && full_batch);
+      if (ABL != 1) control_step_packed<float, DOF_FORCE>(B, M, verts, pc, wrec, lane, valid, ball, STEP_SYNC && full_batch, dof_force);
     }
 #if POST_SYNC
     // fused form only: re-aligns the warps before the long straight-line epilogue (I-cache).  The split form's epilogue is a
@@ -1467,7 +1473,8 @@ step_kernel_packed3(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, cons
 #endif  // B200ENV_WITH_PACKED3
 
 
-template <typename T, int WARPS>
+// DOF_FORCE: the DOF force sensor of every control step into io.dof_force (the last one stays)
+template <typename T, int WARPS, bool DOF_FORCE = false>
 __global__ void __launch_bounds__(WARPS * 32, 1)
 physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, const b200_cfg_t* __restrict__ gcfg, int n, int n_steps,
                       EnvArrays<T> io) {
@@ -1501,8 +1508,9 @@ physics_kernel_packed(const DevBlob* __restrict__ gblob, uint32_t blob_bytes, co
   Ball<T> ball;
   ball_clear(ball);
   if (with_ball && valid && s == BALL_SLOT) env_arrays_load_ball<T>(io, eb + g, ball);
+  T* const dof_force = DOF_FORCE && valid ? io.dof_force + (eb + g) * nd : nullptr;
   for (int st_ = 0; st_ < n_steps; st_++) {
-    control_step_packed<T>(B, verts, pc, wrec, lane, valid, ball, false);
+    control_step_packed<T, DOF_FORCE>(B, M, verts, pc, wrec, lane, valid, ball, false, dof_force);
     if (st_ + 1 < n_steps) pk_requantize<T>(wrec, lc, lane, eb, n);
   }
   for (int k = 0; k < EPW; k++) {
@@ -1973,6 +1981,12 @@ static int make_asset_plan(decltype(&b200env_plan_assets) planner, const int32_t
   return 0;
 }
 
+// The forms whose physics launch has the DOF force sensor: step_kernel_packed<true, ...> (split, sorted, grouped and mixed), and
+// physics_kernel_packed behind b200env_physics_only.  The A/B forms refuse it.
+static bool sensor_form(const b200env* h) {
+  return h->form == PhysForm::Split || h->form == PhysForm::Sorted || h->form == PhysForm::Grouped || h->form == PhysForm::Mixed;
+}
+
 // Shape of the physics launch of b200env_step: kernel, threads and dynamic shared memory per CTA, envs per CTA batch, and the most
 // resident CTAs per SM (below what the occupancy query allows)
 struct PhysLaunch { const void* kernel; int threads; size_t smem; int batch; int max_per_sm; };
@@ -1995,9 +2009,18 @@ static int physics_launch_config(b200env* h, PhysLaunch* out) {
            pk_warps(false) * EPW, INT_MAX};
       break;
     case PhysForm::Split:
-    case PhysForm::Sorted: L = {(const void*)step_kernel_packed<true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
-    case PhysForm::Grouped: L = {(const void*)step_kernel_packed<true, true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
-    case PhysForm::Mixed: L = {(const void*)step_kernel_packed<true, false, true>, pk_threads, pk_smem, pk_batch, INT_MAX}; break;
+    case PhysForm::Sorted:
+      L = {h->dof_force ? (const void*)step_kernel_packed<true, false, false, true> : (const void*)step_kernel_packed<true>, pk_threads, pk_smem,
+           pk_batch, INT_MAX};
+      break;
+    case PhysForm::Grouped:
+      L = {h->dof_force ? (const void*)step_kernel_packed<true, true, false, true> : (const void*)step_kernel_packed<true, true>, pk_threads,
+           pk_smem, pk_batch, INT_MAX};
+      break;
+    case PhysForm::Mixed:
+      L = {h->dof_force ? (const void*)step_kernel_packed<true, false, true, true> : (const void*)step_kernel_packed<true, false, true>,
+           pk_threads, pk_smem, pk_batch, INT_MAX};
+      break;
     case PhysForm::Tmem:   // one CTA per SM: its 56 envs take nearly all of the shared memory
       L = {(const void*)step_kernel_tmem, PT_WARPS * 32, staged + (size_t)PT_WARPS * EPW * PT_ENV_STRIDE * sizeof(float), PT_WARPS * EPW, 1};
       break;
@@ -2021,6 +2044,28 @@ static int physics_launch_config(b200env* h, PhysLaunch* out) {
   }
   *out = L;
   return 0;
+}
+
+// The physics launch of b200env_step in the forms of step_kernel_packed<true, ...> (Split, Sorted, Grouped, Mixed); DOF_FORCE: the
+// sensor instantiation, which the handle runs when b200env_bind was given dof_force
+template <bool DOF_FORCE>
+static void launch_split_physics(b200env* h, const PhysLaunch& pl, const float* actions, cudaStream_t st) {
+  const DevBlob* blob = (const DevBlob*)h->d_blob;
+  const uint32_t blob_bytes = (uint32_t)h->blob_bytes;
+  switch (h->form) {
+    case PhysForm::Grouped:
+      step_kernel_packed<true, true, false, DOF_FORCE><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);
+      break;
+    case PhysForm::Mixed:
+      step_kernel_packed<true, false, true, DOF_FORCE><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, nullptr, h->d_env_blob);
+      break;
+    default:   // Split, Sorted
+      step_kernel_packed<true, false, false, DOF_FORCE><<<h->step_grid, pl.threads, pl.smem, st>>>(
+          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext,
+          h->form == PhysForm::Sorted ? h->d_perm : nullptr);
+  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2344,6 +2389,11 @@ int b200env_bind(b200env_handle h, const b200_buffers_t* bufs) {
     return fail(-2, "b200env_bind: num_actions must be nd (no residual wrench) or nd + 6%s");
   if (h->cfg.res_force_scale > 0.f && bufs->num_actions != h->model.nd + 6)
     return fail(-2, "b200env_bind: res_force_scale > 0 needs num_actions = nd + 6 (force + torque columns)%s");
+  const bool dof_force = bufs->dof_force != nullptr;
+  if (dof_force && !sensor_form(h))
+    return fail(-2, "b200env_bind: the DOF force sensor (dof_force) runs in the default kernel form only (unset B200ENV_KERNEL and B200ENV_SPLIT)%s");
+  if (dof_force != h->dof_force) h->step_slots = 0;   // another kernel: its shared-memory attribute is set at the next launch config
+  h->dof_force = dof_force;
   h->bufs = *bufs;
   h->bound = true;
   return 0;
@@ -2430,18 +2480,9 @@ int b200env_step(b200env_handle h, const float* actions, void* stream) {
           blob, blob_bytes, h->d_cfg, h->bufs, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext);
       break;
 #endif
-    case PhysForm::Grouped:
-      step_kernel_packed<true, true><<<h->step_grid, pl.threads, pl.smem, st>>>(
-          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, h->d_rows, h->d_asset_ptr, h->d_batches, h->num_batches);
-      break;
-    case PhysForm::Mixed:
-      step_kernel_packed<true, false, true><<<h->step_grid, pl.threads, pl.smem, st>>>(
-          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, 0, 1, h->d_ext, nullptr, h->d_env_blob);
-      break;
-    default:   // Split, Sorted
-      step_kernel_packed<true><<<h->step_grid, pl.threads, pl.smem, st>>>(
-          blob, blob_bytes, h->d_cfg, h->bufs, h->ml, actions, h->num_envs, h->d_ticket, h->env_first, h->env_stride, h->d_ext,
-          h->form == PhysForm::Sorted ? h->d_perm : nullptr);
+    default:   // Split, Sorted, Grouped, Mixed
+      if (h->dof_force) launch_split_physics<true>(h, pl, actions, st);
+      else launch_split_physics<false>(h, pl, actions, st);
   }
   if (tv0) { cudaEventRecord(tv1, st); h->tev->push_back(tv0); h->tev->push_back(tv1); }
   if (h->cfg.task_mode == 0)
@@ -2594,15 +2635,19 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
 
 int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_steps, void* root, void* dof_pos, void* dof_vel,
                          const void* pd_tar, const void* ext_wrench, void* rb_out, void* contact_out, void* ball, int32_t* ball_hits,
-                         void* stream) {
+                         void* stream, void* dof_force_out) {
   if (!h || !root || !dof_pos || !dof_vel || !pd_tar || !rb_out) return fail(-1, "b200env_physics_only: null argument%s");
   if (n <= 0 || n_steps <= 0) return fail(-2, "b200env_physics_only: n and n_steps must be positive%s");
   if (h->num_assets) return fail(-2, "b200env_physics_only: not supported on a handle of several assets (b200env_create_assets)%s");
   if (prec != 0 && prec != 1) return fail(-2, "b200env_physics_only: prec must be 0 (float) or 1 (double)%s");
+  if (dof_force_out && !sensor_form(h))
+    return fail(-2, "b200env_physics_only: the DOF force sensor (dof_force_out) runs in the default kernel form only (unset B200ENV_KERNEL and B200ENV_SPLIT)%s");
   cudaSetDevice(h->device);
   if (prec == 0) {
     const EnvArrays<float> io{(float*)root, (float*)dof_pos, (float*)dof_vel, (const float*)pd_tar, (const float*)ext_wrench, (float*)rb_out,
-                              (float*)contact_out, (float*)ball, ball_hits};
+                              (float*)contact_out, (float*)ball, ball_hits, (float*)dof_force_out};
+    if (dof_force_out)
+      return launch_physics_only(h, physics_kernel_packed<float, 4, true>, 4, 4 * EPW, 4 * EPW * ENV_STRIDE * sizeof(float), n, n_steps, io, stream);
     switch (h->form) {
       case PhysForm::Lane: return launch_physics_only(h, physics_kernel<float>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
       // the one-wave form at 6 warps (more than 4: several CTA batches of the test kernel in small tests)
@@ -2611,7 +2656,9 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
     }
   }
   const EnvArrays<double> io{(double*)root, (double*)dof_pos, (double*)dof_vel, (const double*)pd_tar, (const double*)ext_wrench, (double*)rb_out,
-                             (double*)contact_out, (double*)ball, ball_hits};
+                             (double*)contact_out, (double*)ball, ball_hits, (double*)dof_force_out};
+  if (dof_force_out)
+    return launch_physics_only(h, physics_kernel_packed<double, 2, true>, 2, 2 * EPW, 2 * EPW * ENV_STRIDE * sizeof(double), n, n_steps, io, stream);
   if (h->form == PhysForm::Lane) return launch_physics_only(h, physics_kernel<double>, WARPS_PER_CTA, WARPS_PER_CTA, 0, n, n_steps, io, stream);
   return launch_physics_only(h, physics_kernel_packed<double, 2>, 2, 2 * EPW, 2 * EPW * ENV_STRIDE * sizeof(double), n, n_steps, io, stream);
 }

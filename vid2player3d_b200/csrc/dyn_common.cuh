@@ -897,12 +897,14 @@ __device__ __forceinline__ void unpack_state_row(const StateRows<NE>& r, int k, 
 
 // The arrays of the physics-only entry (b200env_physics_only; the CPU lane emulator has the same signature): root [n][13],
 // dof_pos / dof_vel / pd_tar [n][nd], ext [n][6], rb_out [n][nb][13], contact_out [n][nb][3], ball [n][13] (p, -, v, w as a root row),
-// hits [n].  ext, contact_out, ball and hits may be null.
+// hits [n], dof_force [n][nd] (the DOF force sensor of the last control step, packed.cuh::pk_dof_force; read by the sensor instantiation
+// of physics_kernel_packed only).  ext, contact_out, ball, hits and dof_force may be null.
 template <typename T> struct EnvArrays {
   T *root, *dof_pos, *dof_vel;
   const T *pd_tar, *ext;
   T *rb_out, *contact_out, *ball;
   int32_t* hits;
+  T* dof_force;
 };
 template <typename T>
 __device__ __forceinline__ void env_arrays_load(const EnvArrays<T>& io, int nd, const LaneConst& lc, int lane, int64_t e, Lane<T>& L, T* pdt,

@@ -432,9 +432,12 @@ template <typename T> __device__ __forceinline__ void pk_root(const PhysCfg<T>& 
 }
 
 // forward step of one dynamic non-root body: accelerations, integrate the joint state; the new joint rotation / velocity are also
-// returned in registers for the kinematics that follow at once (pk_fk<.., JOINT_IN_REGS>)
-template <typename T>
-__device__ __forceinline__ void pk_forward(const DevBlob& B, const PhysCfg<T>& c, T* env, int b, T* qn, T* wt) {
+// returned in registers for the kinematics that follow at once (pk_fk<.., JOINT_IN_REGS>).
+// SENSOR && stash (last substep of a control step with the DOF force sensor): the joint's exp-map coordinates q at the start of the
+// substep and the implicit drive's velocity qd + h qdd (before damping and the clamp) go into the body's E slot, dead once D^-1 has
+// been read here, for pk_dof_force.
+template <typename T, bool SENSOR = false>
+__device__ __forceinline__ void pk_forward(const DevBlob& B, const PhysCfg<T>& c, T* env, int b, T* qn, T* wt, bool stash = false) {
   const b200_model_t& M = B.m;
   T* rec = env + RIX(B, b) * REC;
   const T* par = env + RIX(B, M.parent[b]) * REC;
@@ -458,6 +461,13 @@ __device__ __forceinline__ void pk_forward(const DevBlob& B, const PhysCfg<T>& c
   str<R_ACC, 6>(rec, acc);
   T cq[4] = {-Q[0], -Q[1], -Q[2], Q[3]};
   qrot(cq, gam, wd);  // R^T gam
+  if (SENSOR && stash) {
+    T st[6];
+    qlog(qj, st);
+#pragma unroll
+    for (int k = 0; k < 3; k++) st[3 + k] = wt[k] + c.h * wd[k];
+    str<R_E, 6>(rec, st);
+  }
 #pragma unroll
   for (int k = 0; k < 3; k++) wt[k] = (wt[k] + c.h * wd[k]) * c.damp;
   T n2 = wt[0] * wt[0] + wt[1] * wt[1] + wt[2] * wt[2];
@@ -769,14 +779,46 @@ __device__ __forceinline__ void pk_ball_contacts_group(const DevBlob& B, const f
   }
 }
 
+// DOF force sensor (b200_buffers_t::dof_force).  out[3j + k] = the generalized force that joint j's drive and its limit spring-damper
+// applied in the last substep of the control step, in the joint's child frame (the frame of dof_vel, so out . dof_vel is the drive's
+// power).  The drive is implicit, so the force is taken at the end-of-substep velocity qd+ = qd + h qdd, not the start-of-substep one:
+//   tau = kp (pd - q - h qd+) - kd qd+  [+ limk (lim - q - h qd+) - limc qd+ while the limit is active]
+// i.e. the explicit torque of pk_body minus (h kd + h^2 kp [+ h limc + h^2 limk]) qdd.  Armature is inertia, not a force; contact and
+// joint-reaction forces are not part of it.  Run after the last substep by the lane that owns the body's PD target (pk_pd_take), from
+// q and qd+ that pk_forward left in the body's E slot; the three values go straight to global memory.
+template <typename T, int LPE = SLOTS>
+__device__ __forceinline__ void pk_dof_force(const DevBlob& B, const b200_model_t& MN, const PhysCfg<T>& c, const T* env, int s, bool valid,
+                                             const T (&pd)[PK_PD_SLOTS][3], T* __restrict__ out) {
+  const b200_model_t& M = B.m;
+  for (int rr = 0; rr * LPE < M.nb; rr++) {
+    const int b = rr * LPE + s;
+    if (!valid || b == 0 || b >= M.nb || M.fixed[b]) continue;
+    T st[6], p[3];   // q[3] qd+[3]
+    ldr<R_E, 6>(env + RIX(B, b) * REC, st);
+    pk_pd_pick<T>(pd, rr, p);
+    const int d0 = M.dof_of_body[b];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+      const T q = st[k], qd = st[3 + k];
+      const T kp = T(MN.kp[d0 + k]), kd = T(MN.kd[d0 + k]);
+      T tau = kp * (p[k] - q - c.h * qd) - kd * qd;
+      const T lo = T(MN.lim_lo[d0 + k]), hi = T(MN.lim_hi[d0 + k]);
+      if (q < lo) tau += c.limk * (lo - q - c.h * qd) - c.limc * qd;
+      else if (q > hi) tau += c.limk * (hi - q - c.h * qd) - c.limc * qd;
+      out[d0 + k] = tau;
+    }
+  }
+}
+
 // One control step for the warp's EPW envs.  wrec: the warp's records; valid: this lane's env exists.
 // The ball of env g is carried by lane (g, BALL_SLOT) in registers.
 // B: the tree tables and topology every env of the warp shares; MN / verts: the numeric constants and hull vertices of this lane's
 // env (B.m and its vertices when the warp's envs are of one asset).  The ball paths read B only: a handle whose envs have different
 // assets has no ball (b200env_create_assets).
-template <typename T>
+// DOF_FORCE: the DOF force sensor (pk_dof_force) into dof_force = the [nd] row of this lane's env (null on a lane without an env).
+template <typename T, bool DOF_FORCE = false>
 __device__ __forceinline__ void control_step_packed(const DevBlob& B, const b200_model_t& MN, const float* verts, const PhysCfg<T>& c, T* wrec,
-                                                    int lane, bool valid, Ball<T>& ball, bool cta_sync) {
+                                                    int lane, bool valid, Ball<T>& ball, bool cta_sync, T* dof_force = nullptr) {
   const b200_model_t& M = B.m;
   const int g = lane >> 3, s = lane & 7;
   T* env = wrec + g * ENV_STRIDE;
@@ -863,7 +905,7 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const b200
         if (b >= 0) {
           if (!M.fixed[b]) {
             T qn[4], wt[3];
-            pk_forward<T>(B, c, env, b, qn, wt);
+            pk_forward<T, DOF_FORCE>(B, c, env, b, qn, wt, DOF_FORCE && sim == c.cfi - 1 && sub == c.substeps - 1);
             pk_fk<T, true, true>(B, MN, env, b, qn, wt);
           } else {
             pk_fk<T, true>(B, MN, env, b);
@@ -873,6 +915,7 @@ __device__ __forceinline__ void control_step_packed(const DevBlob& B, const b200
       }
     }
   }
+  if (DOF_FORCE) pk_dof_force<T>(B, MN, c, env, s, valid && dof_force != nullptr, pd, dof_force);
   pk_pd_park<T>(B, env, s, valid, pd);
 }
 template <typename T>

@@ -108,14 +108,22 @@ class Env:
             pass
 
     def bind(self, tensors, actors_per_env, bodies_per_env, num_obs):
+        """tensors: name -> CUDA tensor of every b200_buffers_t pointer; the ball flag buffers only for the vid2player player env, and
+        "dof_force" ([rows, nd] float32) only with DOF force sensors"""
+        import torch
         b = abi.Buffers()
         for name, _ in abi.Buffers._fields_:
             if name in ("actors_per_env", "bodies_per_env", "num_obs", "num_actions"):
                 continue
             if name in ("has_bounce", "has_bounce_now", "bounce_pos", "racket_hit_now") and name not in tensors:
                 continue  # ball flag buffers: only for the vid2player player env
+            if name == "dof_force" and tensors.get(name) is None:
+                continue  # DOF force sensors off: the physics launch writes no sensor rows
             t = tensors[name]
             assert t.is_cuda and t.is_contiguous(), name
+            if name == "dof_force":
+                assert t.dtype == torch.float32 and tuple(t.shape) == (int(tensors["actions_used"].shape[0]), int(self.model.nd)), \
+                    f"dof_force must be float32 [{int(tensors['actions_used'].shape[0])}, {int(self.model.nd)}], got {t.dtype} {tuple(t.shape)}"
             setattr(b, name, t.data_ptr())
         b.actors_per_env, b.bodies_per_env, b.num_obs = actors_per_env, bodies_per_env, num_obs
         b.num_actions = self.num_actions = int(tensors["actions_used"].shape[-1])   # row width of `actions` in step()
@@ -219,13 +227,16 @@ class Env:
                                                 int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _ptr(obs_bf16),
                                                 obs_bf16.shape[1] if obs_bf16 is not None else 0, _ptr(mean), _ptr(rstd), clamp, _stream()))
 
-    def physics_only(self, root, dof_pos, dof_vel, pd_tar, ext_wrench, rb_out, contact_out, n_steps=1, ball=None, ball_hits=None):
+    def physics_only(self, root, dof_pos, dof_vel, pd_tar, ext_wrench, rb_out, contact_out, n_steps=1, ball=None, ball_hits=None,
+                     dof_force=None):
+        """dof_force: [n, nd] of root's dtype, receives the DOF force sensor of the last control step (include/b200env.h)"""
         import torch
         prec = {torch.float32: 0, torch.float64: 1}[root.dtype]
-        for t in (dof_pos, dof_vel, pd_tar, rb_out):
+        for t in (dof_pos, dof_vel, pd_tar, rb_out) + ((dof_force,) if dof_force is not None else ()):
             assert t.dtype == root.dtype and t.is_cuda and t.is_contiguous()
         _check(lib().b200env_physics_only(self._h, prec, root.shape[0], n_steps, _ptr(root), _ptr(dof_pos), _ptr(dof_vel), _ptr(pd_tar),
-                                          _ptr(ext_wrench), _ptr(rb_out), _ptr(contact_out), _ptr(ball), _ptr(ball_hits), _stream()))
+                                          _ptr(ext_wrench), _ptr(rb_out), _ptr(contact_out), _ptr(ball), _ptr(ball_hits), _stream(),
+                                          _ptr(dof_force)))
 
     @property
     def kernel_form(self):

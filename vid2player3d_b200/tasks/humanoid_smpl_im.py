@@ -227,6 +227,9 @@ class HumanoidSMPLIM(BaseTask):
         self._rigid_body_vel, self._rigid_body_ang_vel = rbs[..., 7:10], rbs[..., 10:13]
         self._contact_force_tensor = f(N * B, 3)
         self._contact_forces = self._contact_force_tensor.view(N, B, 3)
+        # DOF force sensors (enable_actor_dof_force_sensors, :369; include/b200env.h b200_buffers_t::dof_force): with
+        # cfg.env.dof_force_sensors the physics launch of every step writes the joints' drive + limit torques of its last substep here
+        # (same storage for the task's lifetime); without it the tensor stays zero
         self.dof_force_tensor = f(N, D)
         K, S = self._cfg_struct.num_key, self._cfg_struct.shape_dim
         if "motion_assets" not in self.cfg["env"]:   # with motion_assets create_sim sampled them
@@ -258,6 +261,8 @@ class HumanoidSMPLIM(BaseTask):
                  t_rb_rot=self._target_rb_rot, p_dof_pos=self._prev_target_dof_pos, p_dof_vel=self._prev_target_dof_vel,
                  p_rb_pos=self._prev_target_rb_pos, p_rb_rot=self._prev_target_rb_rot,
                  pd_targets=self._pd_target_dof_pos, actions_used=self.actions)
+        if self.cfg["env"].get("dof_force_sensors", False):
+            t["dof_force"] = self.dof_force_tensor
         self._env.bind(t, actors_per_env=1, bodies_per_env=B, num_obs=self.num_obs)
         self._env.set_motion_lib(self._ml_t, nbl)
         self.extras["terminate"] = self._terminate_buf

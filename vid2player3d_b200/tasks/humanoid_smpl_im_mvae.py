@@ -172,6 +172,9 @@ class HumanoidSMPLIMMVAE(BaseTask):
         self._prev_target_rb_pos, self._prev_target_rb_rot = f(N, 24, 3), f(N, 24, 4)
         self._prev_target_rb_rot[..., 3] = 1.0
         self._pd_target_dof_pos = f(N, D)
+        # DOF force sensors (:381, refreshed after every step :588; include/b200env.h b200_buffers_t::dof_force): written by the physics
+        # launch of every step with cfg.env.dof_force_sensors (each handle of dual mode its own rows), else zeros
+        self.dof_force_tensor = f(N, D)
         self.actions = f(N, self._num_actions)
         self._reset_ref_motion_bodies = f(N, 11)
         self._reset_ref_motion_bodies[:, 0] = 1          # gender male (:254-260)
@@ -195,6 +198,8 @@ class HumanoidSMPLIMMVAE(BaseTask):
                  p_dof_vel=self._prev_target_dof_vel, p_rb_pos=self._prev_target_rb_pos, p_rb_rot=self._prev_target_rb_rot,
                  pd_targets=self._pd_target_dof_pos, actions_used=self.actions, has_bounce=self._has_bounce,
                  has_bounce_now=self._has_bounce_now, bounce_pos=self._bounce_pos, racket_hit_now=self._racket_hit_now)
+        if self.cfg["env"].get("dof_force_sensors", False):
+            t["dof_force"] = self.dof_force_tensor
         for h in self._envs:
             h.bind(t, actors_per_env=2, bodies_per_env=26, num_obs=self.num_obs)
         # SMPL kinematic constants for the FK targets (rest joints of the shipped skeletons, SMPL joint order), one per asset
