@@ -93,6 +93,18 @@ typedef struct b200v2p_ctrl {
   const uint8_t* touch_mask; /* NULL, or bool [n] with obs_only: the humanoids just reset.  Rows of envs that are neither in it nor flagged
                                 reset_reaction / reset_recovery are still current and skipped; the task flags of the envs in it are cleared
                                 at the end (tail of _reset_envs, :176-177) */
+  /* test-time reset rule of MVAEControllerVis._compute_reset / _compute_stats (env/tasks/mvae_controller_vis.py:64-93), used when
+   * eval = 1 (not with dual; ignored with obs_only) instead of the training FSM: terminate = reset = progress > eval_episode_length;
+   * in_time = tar_time >= tar_time_total; reaction = (contact & tar_action == 0 & has_bounce & in_time) | (!contact & in_time);
+   * recovery = tar_action == 1 & (contact | ball_y < root_y - 1 | |ball_vel_y| < 2); a reset sets reaction and clears recovery.  No
+   * NaN / court / early termination, distance not advanced.  The envs in recovery then update the four AverageMeterUnSync meters
+   * (utils/common.py:40-63) in place, meter m of env e at [m * n + e]: 0 hit_rate (contact), 1 fh_ratio (swing_type_cycle == 1),
+   * 2 bounce_in_rate (est_bounce_in), 3 bounce_in_pos_error (|est_bounce_pos - target_bounce_pos|, envs with est_bounce_in only):
+   * sum += v, count += 1, avg = sum / count, max = v > max ? v : max. */
+  int32_t eval, eval_episode_length;
+  const float* ball_vel;           /* [n,3]; eval only */
+  float *meter_sum, *meter_avg, *meter_max; /* [4,n]; eval only */
+  int64_t* meter_count;            /* [4,n]; eval only */
 } b200v2p_ctrl_t;
 int b200v2p_controller_post(const b200v2p_ctrl_t* c, void* stream);
 
@@ -189,6 +201,45 @@ typedef struct b200v2p_areset {
                                0..N-1, n = N; no id list has to be built on the host, the launch can live in a CUDA graph) */
 } b200v2p_areset_t;
 int b200v2p_actor_reset(const b200v2p_areset_t* r, void* stream);
+
+/* Rally recorder of the test-time tasks: the frame MVAEControllerVis.render_vis (env/tasks/mvae_controller_vis.py:140-146) and
+ * MVAEControllerVisDual.render_vis (mvae_controller_vis_dual.py:156-162) append on every call, written for all n envs into
+ * device-resident buffers [n, cap, ...] at row r: r = *row_counter (single; the launch advances the counter by one) or
+ * r = progress_buf[e] (dual, row_counter NULL).  Rows at or past cap are not written (the reference's 1800-row buffer would raise).
+ * rec_target_pos (single) and rec_tar_action (dual) may be NULL. */
+typedef struct b200v2p_rec {
+  int32_t n, cap;
+  int64_t* row_counter;        /* [1] or NULL */
+  uint32_t* done_counter;      /* [1] scratch, zero between launches (with row_counter) */
+  const int64_t* progress_buf; /* [n] (dual) */
+  const float *joint_rot, *root_pos, *ball_pos, *target_pos, *phase; /* [n,24,3], [n,3] x3, [n] */
+  const int64_t *swing_type, *tar_action;                            /* [n] */
+  float *rec_joint_rot, *rec_root_pos, *rec_ball_pos, *rec_target_pos, *rec_phase;
+  int64_t *rec_swing_type, *rec_tar_action;
+} b200v2p_rec_t;
+int b200v2p_eval_record(const b200v2p_rec_t* r, void* stream);
+
+/* Best-episode list of MVAEControllerVisDual.render_vis (mvae_controller_vis_dual.py:164-195), on the device.  Does nothing when
+ * no reset_buf is set.  Otherwise the flagged pairs (2k, 2k+1; the dual reset FSM flags both players) are reduced to the first
+ * argmax of distance[2k] + distance[2k+1]; it enters the list when the list is empty or it beats the list's last distance, in
+ * front of the first entry it beats; the list keeps num_eg entries.  The list is order[i] = slot of the i-th best, with
+ * best_distance / best_env (the pair's even env) / best_nframes (min(progress_buf, cap)) by slot, so an insertion moves slot
+ * indices.  A second launch copies rows [0, nframes) of both envs of the chosen pair from the recording (b200v2p_eval_record's
+ * rec_* buffers [n, cap, ...]) into best_* [num_eg, 2, cap, ...] at the chosen slot; copy_slot [1] holds that slot, or -1. */
+typedef struct b200v2p_best {
+  int32_t n, cap, num_eg, pad_;
+  const int64_t *reset_buf, *progress_buf;
+  const float* distance;
+  int64_t* list_len;     /* [1] */
+  int64_t* order;        /* [num_eg] */
+  float* best_distance;  /* [num_eg] */
+  int64_t *best_env, *best_nframes, *copy_slot;
+  const float *rec_joint_rot, *rec_root_pos, *rec_ball_pos, *rec_phase;
+  const int64_t *rec_swing_type, *rec_tar_action;
+  float *best_joint_rot, *best_root_pos, *best_ball_pos, *best_phase;
+  int64_t *best_swing_type, *best_tar_action;
+} b200v2p_best_t;
+int b200v2p_eval_best(const b200v2p_best_t* b, void* stream);
 
 #ifdef __cplusplus
 }

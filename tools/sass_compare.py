@@ -39,6 +39,8 @@ def demangle(names):
 def normalise_name(name, drops):
     for d in drops:
         name = name.replace(", " + d + ">", ">")
+        if "<" + d + ">(" in name:     # the only template argument: f<false>(...) of a kernel that was not a template before
+            name = re.sub(r"^void ", "", name.replace("<" + d + ">(", "("))
     return name
 
 

@@ -281,6 +281,8 @@ class V2PCtrl(C.Structure):
         ("est_bounce_pos", C.c_void_p), ("est_bounce_time", C.c_void_p), ("est_max_height", C.c_void_p), ("distance", C.c_void_p),
         ("obs_buf", C.c_void_p), ("rew_buf", C.c_void_p), ("sub_rewards", C.c_void_p),
         ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p), ("ball_obs", C.c_void_p), ("touch_mask", C.c_void_p),
+        ("eval", C.c_int32), ("eval_episode_length", C.c_int32), ("ball_vel", C.c_void_p),
+        ("meter_sum", C.c_void_p), ("meter_avg", C.c_void_p), ("meter_max", C.c_void_p), ("meter_count", C.c_void_p),
     ]
 
 
@@ -333,6 +335,29 @@ class V2PActorReset(C.Structure):
     ]
 
 
+class V2PRec(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("cap", C.c_int32), ("row_counter", C.c_void_p), ("done_counter", C.c_void_p), ("progress_buf", C.c_void_p),
+        ("joint_rot", C.c_void_p), ("root_pos", C.c_void_p), ("ball_pos", C.c_void_p), ("target_pos", C.c_void_p), ("phase", C.c_void_p),
+        ("swing_type", C.c_void_p), ("tar_action", C.c_void_p),
+        ("rec_joint_rot", C.c_void_p), ("rec_root_pos", C.c_void_p), ("rec_ball_pos", C.c_void_p), ("rec_target_pos", C.c_void_p),
+        ("rec_phase", C.c_void_p), ("rec_swing_type", C.c_void_p), ("rec_tar_action", C.c_void_p),
+    ]
+
+
+class V2PBest(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("cap", C.c_int32), ("num_eg", C.c_int32), ("pad_", C.c_int32),
+        ("reset_buf", C.c_void_p), ("progress_buf", C.c_void_p), ("distance", C.c_void_p),
+        ("list_len", C.c_void_p), ("order", C.c_void_p), ("best_distance", C.c_void_p), ("best_env", C.c_void_p),
+        ("best_nframes", C.c_void_p), ("copy_slot", C.c_void_p),
+        ("rec_joint_rot", C.c_void_p), ("rec_root_pos", C.c_void_p), ("rec_ball_pos", C.c_void_p), ("rec_phase", C.c_void_p),
+        ("rec_swing_type", C.c_void_p), ("rec_tar_action", C.c_void_p),
+        ("best_joint_rot", C.c_void_p), ("best_root_pos", C.c_void_p), ("best_ball_pos", C.c_void_p), ("best_phase", C.c_void_p),
+        ("best_swing_type", C.c_void_p), ("best_tar_action", C.c_void_p),
+    ]
+
+
 # ---------------------------------------------------------------- entry points of libb200env.so
 # name -> (restype, argtypes) of every function include/b200env.h, include/b200env_v2p.h and include/b200ball.h declare; native.lib()
 # applies all of them when it loads the library, so an argument too many or too few, or one that does not convert to its C type,
@@ -381,6 +406,8 @@ SIGNATURES = {
     "b200v2p_ball_in_estimate": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _p, _p, _p, _p]),
     "b200v2p_task_reset": (C.c_int, [_p, _p]),
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
+    "b200v2p_eval_record": (C.c_int, [_p, _p]),
+    "b200v2p_eval_best": (C.c_int, [_p, _p]),
     # include/b200ball.h
     "b200ball_simulate": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200ball_out_rows": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _i32, _p, _p, _p]),

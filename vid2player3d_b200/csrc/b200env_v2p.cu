@@ -348,6 +348,42 @@ __device__ __forceinline__ float est_index(float v, const float* r) {  // clamp 
   v = fminf(fmaxf(v, r[0]), r[1] - r[2]);
   return rintf((v - r[0]) / r[2]);
 }
+// AverageMeterUnSync.update (utils/common.py:52-63) of meter m for env e; envs are independent, so no atomics
+__device__ __forceinline__ void meter_update(const b200v2p_ctrl_t& c, int m, int64_t e, float v) {
+  const int64_t i = (int64_t)m * c.n + e;
+  const float s = __fadd_rn(c.meter_sum[i], v);
+  const int64_t k = c.meter_count[i] + 1;
+  c.meter_sum[i] = s;
+  c.meter_count[i] = k;
+  c.meter_avg[i] = __fdiv_rn(s, __ll2float_rn(k));   // float32 / int64 promotes to float32
+  if (v > c.meter_max[i]) c.meter_max[i] = v;
+}
+// MVAEControllerVis._compute_reset + _compute_stats (env/tasks/mvae_controller_vis.py:64-93): flags, reset masking, then stats
+__device__ __forceinline__ void eval_reset(const b200v2p_ctrl_t& c, int64_t e, const float* rp, const float* bp, bool has_contact) {
+  const int64_t ta = c.tar_action[e];
+  const bool terminate = c.progress_buf[e] > (int64_t)c.eval_episode_length;
+  const bool in_time = c.tar_time[e] >= c.tar_time_total[e];
+  bool reaction = (has_contact && ta == 0 && c.has_bounce[e] && in_time) || (!has_contact && in_time);
+  bool recovery = ta == 1 && (has_contact || bp[1] < rp[1] - 1.0f || fabsf(c.ball_vel[e * 3 + 1]) < 2.0f);
+  if (terminate) { reaction = true; recovery = false; }
+  c.terminate_buf[e] = terminate ? 1 : 0;
+  c.reset_buf[e] = terminate ? 1 : 0;
+  c.reset_reaction[e] = reaction ? 1 : 0;
+  c.reset_recovery[e] = recovery ? 1 : 0;
+  if (!recovery) return;
+  meter_update(c, 0, e, has_contact ? 1.0f : 0.0f);
+  meter_update(c, 1, e, c.swing_type_cycle[e] == 1 ? 1.0f : 0.0f);
+  const bool bin = c.est_bounce_in[e] != 0;
+  meter_update(c, 2, e, bin ? 1.0f : 0.0f);
+  if (bin) {
+    float d[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) d[k] = __fsub_rn(c.est_bounce_pos[e * 3 + k], c.target_bounce_pos[e * 3 + k]);
+    meter_update(c, 3, e, sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2]))));
+  }
+}
+// EVAL: the reset rule of the test-time task replaces the training FSM; the training / dual instantiation is the kernel as it was
+template <bool EVAL>
 __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p_ctrl_t c) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t e = (int64_t)blockIdx.x * V2P_WARPS + warp;
@@ -487,6 +523,10 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
   if (c.use_target && lane < 2) { float v = c.target_bounce_pos[e * 3 + lane] - rp[lane]; o[225 + c.obs_traj_len * 3 + lane] = v; nan |= isnan(v); }
   const bool has_nan = __any_sync(FULL, nan);
   // ---- dual reset FSM (physics_mvae_controller_dual.py:92-120): the opponent's flags are recomputed from its inputs (no exchange)
+  if (EVAL) {
+    if (lane == 0 && !c.obs_only) eval_reset(c, e, rp, bp, has_contact);
+    return;
+  }
   if (lane == 0 && !c.obs_only && c.dual) {
     const int64_t p = e ^ 1;
     bool rec[2], term[2];
@@ -527,6 +567,90 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
     c.reset_recovery[e] = recovery ? 1 : 0;
   }
   if (lane == 0 && c.obs_only && touched) { c.reset_reaction[e] = 0; c.reset_recovery[e] = 0; }   // tail of _reset_envs (:176-177) for the reset humanoids
+}
+
+// ------------------------------------------------------------------------------------------ test-time rally recorder
+__device__ __forceinline__ void last_block_advance(int64_t* counter, unsigned int* done, int64_t inc);
+// render_vis's per-frame append (mvae_controller_vis.py:140-146, mvae_controller_vis_dual.py:156-162): one warp per env writes the
+// env's frame at row *row_counter (single; the last block advances the counter) or progress_buf[e] (dual); rows >= cap are dropped
+__global__ void __launch_bounds__(V2P_WARPS * 32) eval_record_kernel(b200v2p_rec_t r) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int64_t e = (int64_t)blockIdx.x * V2P_WARPS + warp;
+  if (e < r.n) {
+    const int64_t row = r.row_counter ? r.row_counter[0] : r.progress_buf[e];
+    if (row >= 0 && row < r.cap) {
+      const int64_t o = e * r.cap + row;
+      for (int k = lane; k < 72; k += 32) r.rec_joint_rot[o * 72 + k] = r.joint_rot[e * 72 + k];
+      if (lane < 3) {
+        r.rec_root_pos[o * 3 + lane] = r.root_pos[e * 3 + lane];
+        r.rec_ball_pos[o * 3 + lane] = r.ball_pos[e * 3 + lane];
+        if (r.rec_target_pos) r.rec_target_pos[o * 3 + lane] = r.target_pos[e * 3 + lane];
+      }
+      if (lane == 3) r.rec_phase[o] = r.phase[e];
+      if (lane == 4) r.rec_swing_type[o] = r.swing_type[e];
+      if (lane == 5 && r.rec_tar_action) r.rec_tar_action[o] = r.tar_action[e];
+    }
+  }
+  if (r.row_counter) last_block_advance(r.row_counter, r.done_counter, 1);
+}
+
+// ------------------------------------------------------------------------------------------ dual best-episode list
+// mvae_controller_vis_dual.py:164-195 on one CTA: first argmax over the flagged pairs, then the insertion rule on the slot order
+__global__ void __launch_bounds__(1024) eval_best_select_kernel(b200v2p_best_t b) {
+  __shared__ float sd[32];
+  __shared__ int64_t sk[32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  float d = 0.0f;
+  int64_t k = -1;   // a thread walks its pairs in increasing order, so a strict > keeps the first of equal distances
+  for (int64_t p = threadIdx.x; p < b.n / 2; p += blockDim.x) {
+    if (b.reset_buf[2 * p] == 0) continue;
+    const float v = __fadd_rn(b.distance[2 * p], b.distance[2 * p + 1]);
+    if (k < 0 || v > d) { d = v; k = p; }
+  }
+  // (d, k) beats (od, ok) when it is valid and either the other is not, or its distance is larger, or equal with a lower pair
+  const auto take = [](float od, int64_t ok, float d, int64_t k) { return ok >= 0 && (k < 0 || od > d || (od == d && ok < k)); };
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    const float od = __shfl_down_sync(FULL, d, s);
+    const int64_t ok = __shfl_down_sync(FULL, k, s);
+    if (take(od, ok, d, k)) { d = od; k = ok; }
+  }
+  if (lane == 0) { sd[warp] = d; sk[warp] = k; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < (int)(blockDim.x >> 5); w++)
+    if (take(sd[w], sk[w], d, k)) { d = sd[w]; k = sk[w]; }
+  b.copy_slot[0] = -1;
+  if (k < 0) return;
+  const int64_t L = b.list_len[0];
+  if (L > 0 && !(d > b.best_distance[b.order[L - 1]])) return;   // the list grows only past its last entry, even while short
+  int64_t ins = 0;
+  while (ins < L && !(d > b.best_distance[b.order[ins]])) ins++;
+  const int64_t slot = L < b.num_eg ? L : b.order[b.num_eg - 1];   // a free slot, or the one of the entry that falls off the end
+  const int64_t nl = L < b.num_eg ? L + 1 : L;
+  for (int64_t i = nl - 1; i > ins; i--) b.order[i] = b.order[i - 1];
+  b.order[ins] = slot;
+  b.list_len[0] = nl;
+  b.best_distance[slot] = d;
+  b.best_env[slot] = 2 * k;
+  const int64_t nf = b.progress_buf[2 * k];
+  b.best_nframes[slot] = nf < b.cap ? nf : b.cap;
+  b.copy_slot[0] = slot;
+}
+// rows [0, best_nframes) of both envs of the chosen pair -> best_*[slot]: block (row, player), thread = one value of the row
+__global__ void __launch_bounds__(96) eval_best_copy_kernel(b200v2p_best_t b) {
+  const int64_t slot = b.copy_slot[0];
+  if (slot < 0) return;
+  const int64_t row = blockIdx.x;
+  if (row >= b.best_nframes[slot]) return;
+  const int t = threadIdx.x;
+  const int64_t s = (b.best_env[slot] + blockIdx.y) * b.cap + row, o = (slot * 2 + blockIdx.y) * b.cap + row;
+  if (t < 72) b.best_joint_rot[o * 72 + t] = b.rec_joint_rot[s * 72 + t];
+  else if (t < 75) b.best_root_pos[o * 3 + t - 72] = b.rec_root_pos[s * 3 + t - 72];
+  else if (t < 78) b.best_ball_pos[o * 3 + t - 75] = b.rec_ball_pos[s * 3 + t - 75];
+  else if (t == 78) b.best_phase[o] = b.rec_phase[s];
+  else if (t == 79) b.best_swing_type[o] = b.rec_swing_type[s];
+  else if (t == 80) b.best_tar_action[o] = b.rec_tar_action[s];
 }
 
 // ------------------------------------------------------------------------------------------ dual mode: incoming-ball table
@@ -937,7 +1061,44 @@ int b200v2p_controller_post(const b200v2p_ctrl_t* c, void* stream) {
   if (c->dual && (c->n & 1)) return vfail(-2, "b200v2p_controller_post: dual mode needs an even number of envs (pairs 2k, 2k+1)");
   if (c->reward_type < 0 || c->reward_type > 2) return vfail(-2, "b200v2p_controller_post: reward_type must be 0 (reach), 1 (return) or 2 (return_w_estimate)");
   if (c->use_history && !c->ball_obs) return vfail(-2, "b200v2p_controller_post: use_history needs the ball_obs buffer");
-  controller_post_kernel<<<(c->n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*c);
+  const unsigned grid = (c->n + V2P_WARPS - 1) / V2P_WARPS;
+  if (c->eval && !c->obs_only) {
+    if (c->dual) return vfail(-2, "b200v2p_controller_post: the test-time reset rule is single-player (dual keeps its FSM)");
+    if (!c->ball_vel || !c->meter_sum || !c->meter_count || !c->meter_avg || !c->meter_max)
+      return vfail(-1, "b200v2p_controller_post: eval needs ball_vel and the four meters' arrays");
+    controller_post_kernel<true><<<grid, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*c);
+  } else {
+    controller_post_kernel<false><<<grid, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*c);
+  }
+  V_CUDA_OK();
+  return 0;
+}
+
+int b200v2p_eval_record(const b200v2p_rec_t* r, void* stream) {
+  if (!r) return vfail(-1, "b200v2p_eval_record: null");
+  if (r->n == 0) return 0;
+  if (r->n < 0 || r->cap < 1 || !r->joint_rot || !r->root_pos || !r->ball_pos || !r->phase || !r->swing_type || !r->rec_joint_rot ||
+      !r->rec_root_pos || !r->rec_ball_pos || !r->rec_phase || !r->rec_swing_type || (r->rec_target_pos && !r->target_pos) ||
+      (r->rec_tar_action && !r->tar_action))
+    return vfail(-1, "b200v2p_eval_record: bad arguments");
+  if (r->row_counter ? !r->done_counter : !r->progress_buf)
+    return vfail(-2, "b200v2p_eval_record: a row counter (with its done counter) or progress_buf is needed");
+  eval_record_kernel<<<(r->n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*r);
+  V_CUDA_OK();
+  return 0;
+}
+
+int b200v2p_eval_best(const b200v2p_best_t* b, void* stream) {
+  if (!b) return vfail(-1, "b200v2p_eval_best: null");
+  if (b->n == 0) return 0;
+  if (b->n < 0 || (b->n & 1)) return vfail(-2, "b200v2p_eval_best: needs an even number of envs (pairs 2k, 2k+1)");
+  if (b->cap < 1 || b->num_eg < 1 || !b->reset_buf || !b->progress_buf || !b->distance || !b->list_len || !b->order || !b->best_distance ||
+      !b->best_env || !b->best_nframes || !b->copy_slot || !b->rec_joint_rot || !b->rec_root_pos || !b->rec_ball_pos || !b->rec_phase ||
+      !b->rec_swing_type || !b->rec_tar_action || !b->best_joint_rot || !b->best_root_pos || !b->best_ball_pos || !b->best_phase ||
+      !b->best_swing_type || !b->best_tar_action)
+    return vfail(-1, "b200v2p_eval_best: bad arguments");
+  eval_best_select_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(*b);
+  eval_best_copy_kernel<<<dim3(b->cap, 2), 96, 0, (cudaStream_t)stream>>>(*b);
   V_CUDA_OK();
   return 0;
 }

@@ -93,16 +93,18 @@ def controller_post(cfg, t):
     c.dual = int(cfg.get("dual", 0))
     c.use_history = int(cfg.get("use_history", 0))
     c.advance = int(cfg.get("advance", 0))
+    c.eval = int(cfg.get("eval", 0))
+    c.eval_episode_length = int(cfg.get("eval_episode_length", 0))
     for k in ("court_min", "court_max", "est_params"):
         for i, v in enumerate(cfg[k]):
             getattr(c, k)[i] = float(v)
-    scalars = {f for f, _ in abi.V2PCtrl._fields_ if f in cfg} | {"obs_only", "dual", "use_history", "advance"}
+    scalars = {f for f, _ in abi.V2PCtrl._fields_ if f in cfg} | {"obs_only", "dual", "use_history", "advance", "eval", "eval_episode_length"}
     for name, _ in abi.V2PCtrl._fields_:
         if name in scalars:
             continue
         x = t.get(name)
         if x is None:
-            assert name in ("est_x", "est_y", "ball_obs", "touch_mask"), name
+            assert name in ("est_x", "est_y", "ball_obs", "touch_mask", "ball_vel", "meter_sum", "meter_avg", "meter_max", "meter_count"), name
             setattr(c, name, None)
         else:
             assert x.is_cuda and x.is_contiguous(), name
@@ -185,6 +187,35 @@ def stream_gather(n, frames, advance, t, reseed_mask=None, seed=0):
         assert x.is_cuda and x.is_contiguous(), name
         setattr(s, name, x.data_ptr())
     _check(lib().b200v2p_stream_gather(C.byref(s), _stream()))
+
+
+def _fill_ptrs(s, t, optional=()):
+    for name, _ in s._fields_:
+        if name in t:
+            x = t[name]
+            if x is None:
+                assert name in optional, name
+                setattr(s, name, None)
+            else:
+                assert x.is_cuda and x.is_contiguous(), name
+                setattr(s, name, x.data_ptr())
+
+
+def eval_record(n, cap, t):
+    """t: the source fields (joint_rot, root_pos, ball_pos, target_pos, phase, swing_type, tar_action), the rec_* buffers [n, cap, ...]
+    and the row source: row_counter + done_counter (single) or progress_buf (dual); see include/b200env_v2p.h b200v2p_rec_t"""
+    r = abi.V2PRec()
+    r.n, r.cap = int(n), int(cap)
+    _fill_ptrs(r, t, optional=("row_counter", "done_counter", "progress_buf", "target_pos", "tar_action", "rec_target_pos", "rec_tar_action"))
+    _check(lib().b200v2p_eval_record(C.byref(r), _stream()))
+
+
+def eval_best(n, cap, num_eg, t):
+    """t: tensors keyed like the pointer fields of b200v2p_best_t (include/b200env_v2p.h)"""
+    b = abi.V2PBest()
+    b.n, b.cap, b.num_eg = int(n), int(cap), int(num_eg)
+    _fill_ptrs(b, t)
+    _check(lib().b200v2p_eval_best(C.byref(b), _stream()))
 
 
 def ctrl_reset(mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):

@@ -155,6 +155,9 @@ class HumanoidSMPLIMMVAE(BaseTask):
         self._rigid_body_pos, self._rigid_body_rot = rbs[:, :25, 0:3], rbs[:, :25, 3:7]
         if not self._is_train:   # :113-116 test-time export of the simulated pose (SMPL joint order)
             self._joint_rot = torch.zeros((self.num_envs, 24, 3), device=self.device, dtype=torch.float32)
+            # device index tensors: a Python-list index is a host-to-device copy, which a CUDA graph capture of the step refuses
+            self._xyzw_to_wxyz_t = torch.tensor([3, 0, 1, 2], device=self.device)
+            self._mujoco_2_smpl_t = torch.tensor(self._mujoco_2_smpl, device=self.device)
         self._rigid_body_vel, self._rigid_body_ang_vel = rbs[:, :25, 7:10], rbs[:, :25, 10:13]
         self._contact_force_tensor = f(N * 26, 3)
         self._contact_forces = self._contact_force_tensor.view(N, 26, 3)
@@ -295,9 +298,9 @@ class HumanoidSMPLIMMVAE(BaseTask):
                                     grip=self._grip(), wrist_body=self._racket_wrist_body_id, only_mask=only_mask)
         if not self._is_train:
             # :814-820 test-time export of the simulated pose as SMPL joint rotations (root angle-axis | dof_pos, SMPL joint order)
-            root_rot = quaternion_wxyz_to_angle_axis(self._rigid_body_rot[:, 0][..., [3, 0, 1, 2]])
+            root_rot = quaternion_wxyz_to_angle_axis(self._rigid_body_rot[:, 0][..., self._xyzw_to_wxyz_t])
             self._joint_rot[:] = torch.cat((root_rot.reshape(self.num_envs, 1, 3), self._dof_pos.reshape(self.num_envs, -1, 3)),
-                                           dim=1)[:, self._mujoco_2_smpl]
+                                           dim=1)[:, self._mujoco_2_smpl_t]
 
     def _grip(self):
         g = self.cfg_v2p.get('grip', 'eastern')            # a pair in dual_mode 'different' (:839-842)

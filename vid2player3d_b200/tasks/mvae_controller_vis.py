@@ -1,0 +1,200 @@
+"""Test-time tasks of the tennis controller (vid2player/env/tasks/mvae_controller_vis.py, mvae_controller_vis_dual.py): what
+`run.py --test` builds from a controller cfg's `test_name`.  The rollout step is the training task's; what differs:
+
+  MVAEControllerVis      the evaluation reset rule and the four per-env statistics (:64-93), inside the post launch
+  both                   render_vis: every call records all envs' frame into device buffers (one launch, no host sync); after
+                         num_rec_frames calls the chosen episodes are written as .npz files and SystemExit is raised like the
+                         reference's exit()
+  MVAEControllerVisDual  the best-episode list of finished rallies (:164-195), kept on the device (two launches per call)
+
+The renderer (SMPL meshes, video, HTML) is not part of this package: the .npz files hold exactly the arrays the reference's
+render_one_result is given, so they can be rendered with its visualizer.  Deliberate departures from the reference:
+  - a rally longer than the recording capacity keeps its first `capacity` rows (the reference raises IndexError);
+  - fewer candidates (single) or list entries (dual) than num_eg: the ones that exist are written (`self.exported` lists them);
+  - select_best orders candidates of equal distance by env id (stable sort);
+  - fix_two_hand_backhand_post (an offline IK fix applied before rendering) is not applied to the written arrays.
+Reference quirks kept: the meters' avg of an env that never recovered stays 1; the dual recording row 0 of an env is written by the
+init call only, and an exported rally is rows [0, progress) - it starts with that row and leaves out the last frame; the dual list
+grows only when a candidate beats its current last entry, even while it holds fewer than num_eg.
+"""
+import os
+import warnings
+
+import numpy as np
+import torch
+
+from .. import native_v2p
+from .physics_mvae_controller import PhysicsMVAEController, PhysicsMVAEControllerDual
+
+METERS = ("hit_rate", "fh_ratio", "bounce_in_rate", "bounce_in_pos_error")   # rows of the meter arrays the post launch updates
+DUAL_CAPACITY = 1800                                                            # mvae_controller_vis_dual.py:51 "hardcode maximum length"
+
+
+class AverageMeterUnSync:
+    """utils/common.py:40-63 with its tensors on the device: views of row `m` of the [4, N] meter arrays that the post launch
+    updates in place for the envs in recovery"""
+
+    def __init__(self, sums, counts, avgs, maxs, m):
+        self.sum, self.count, self.avg, self.max = sums[m], counts[m], avgs[m], maxs[m]
+
+    def reset(self):
+        self.sum.zero_()
+        self.count.zero_()
+        self.avg.fill_(1.0)
+        self.max.zero_()
+
+
+def _check_eval_cfg(cfg, headless):
+    """refuse what the test-time tasks cannot do, before anything is allocated"""
+    env = cfg["env"]
+    if int(env.get("num_eg", 1)) < 1:
+        raise ValueError("num_eg must be at least 1")
+    if int(env.get("num_rec_frames", 300)) < 1:
+        raise ValueError("num_rec_frames must be at least 1")
+    if not headless and not (env.get("record") or env.get("record_scenepic")):
+        raise ValueError("there is no online viewer: run headless, with record to write the episodes")
+    env["is_train"] = False          # utils/config.py:159 (--test); also makes the physics task export _joint_rot
+
+
+class _EvalRecorder:
+    """host side shared by both tasks: frame counting, episode paths and the .npz export"""
+
+    def _init_eval(self, cfg):
+        env = cfg["env"]
+        self.frame_index = 0
+        self._record = bool(env.get("record") or env.get("record_scenepic"))
+        self._num_rec_frames = int(env.get("num_rec_frames", 300))
+        self._num_eg = int(env.get("num_eg", 1))
+        self._start_eg_id = int(env.get("start_eg_id", 1))
+        self._rec_fname = env.get("rec_fname")
+        self._cfg_name = getattr(cfg.get("args"), "cfg", None) or cfg.get("name", "eval")
+        self.exported = []
+        if self.cfg_v2p.get("fix_two_hand_backhand_post"):
+            warnings.warn("fix_two_hand_backhand_post: the episodes are written without the two-hand backhand fix", stacklevel=3)
+
+    def _episode_path(self, eg_id):
+        return self._rec_fname or os.path.join("out", "episodes", f"{self._cfg_name}_{eg_id:03d}.npz")
+
+    def _write(self, eg_id, arrays):
+        path = self._episode_path(eg_id)
+        os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
+        with open(path, "wb") as f:
+            np.savez(f, **{k: v.cpu().numpy() if torch.is_tensor(v) else np.asarray(v) for k, v in arrays.items()})
+        self.exported.append(path)
+
+    def _rec_buffers(self, n, cap, fields):
+        dev = self.device
+        shapes = dict(joint_rot=((24, 3), torch.float), root_pos=((3,), torch.float), ball_pos=((3,), torch.float),
+                      target_pos=((3,), torch.float), phase=((), torch.float), swing_type=((), torch.long), tar_action=((), torch.long))
+        return {k: torch.zeros((*n, cap, *shapes[k][0]), device=dev, dtype=shapes[k][1]) for k in fields}
+
+
+class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
+    def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
+        _check_eval_cfg(cfg, headless)
+        super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
+                         headless=headless)
+        self._init_eval(cfg)
+        N, dev = self.num_envs, self.device
+        self._meter_sum = torch.zeros(4, N, device=dev)
+        self._meter_count = torch.zeros(4, N, device=dev, dtype=torch.long)
+        self._meter_avg = torch.ones(4, N, device=dev)
+        self._meter_max = torch.zeros(4, N, device=dev)
+        for m, name in enumerate(METERS):
+            setattr(self, name, AverageMeterUnSync(self._meter_sum, self._meter_count, self._meter_avg, self._meter_max, m))
+        # :64-79 compares progress with cfg.env.episodeLength (default 600) itself, strictly
+        self._post_cfg.update(eval=1, eval_episode_length=int(cfg["env"].get("episodeLength", 600)))
+        if self._record:
+            self._rec = self._rec_buffers((N,), self._num_rec_frames,
+                                          ("joint_rot", "root_pos", "ball_pos", "target_pos", "phase", "swing_type"))
+            self._rec_row = torch.zeros(1, device=dev, dtype=torch.long)
+            self._rec_done = torch.zeros(1, device=dev, dtype=torch.int32)
+
+    def _tensors(self):
+        t = super()._tensors()
+        t.update(ball_vel=self._physics_player.task._ball_vel, meter_sum=self._meter_sum, meter_count=self._meter_count,
+                 meter_avg=self._meter_avg, meter_max=self._meter_max)
+        return t
+
+    def render_vis(self, init=False):
+        """:95-170 without the renderer: record the frame of every env; after num_rec_frames calls write the chosen episodes"""
+        self.frame_index += 1
+        if not self._record:
+            return
+        t, p = self._physics_player.task, self._mvae_player
+        native_v2p.eval_record(self.num_envs, self._num_rec_frames, dict(
+            row_counter=self._rec_row, done_counter=self._rec_done, joint_rot=t._joint_rot, root_pos=t._root_pos, ball_pos=t._ball_pos,
+            target_pos=self._target_bounce_pos, phase=p._phase_pred, swing_type=p._swing_type_cycle,
+            **{"rec_" + k: v for k, v in self._rec.items()}))
+        if self.frame_index >= self._num_rec_frames:
+            self.export_episodes()
+            raise SystemExit(0)
+
+    def select_candidates(self):
+        """:152-159: with select_best the envs with bounce_in_rate.avg > 0.95 and fh_ratio.avg < 0.6, by distance travelled over the
+        recording, longest first; otherwise every env in order"""
+        if not self.cfg["env"].get("select_best"):
+            return torch.arange(self.num_envs, device=self.device)
+        rp = self._rec["root_pos"]
+        dist = (rp[:, 1:] - rp[:, :-1]).norm(dim=-1).sum(dim=-1)
+        cand = (self.bounce_in_rate.avg > 0.95) & (self.fh_ratio.avg < 0.6)
+        ids = cand.nonzero(as_tuple=False).flatten()
+        return ids[torch.argsort(dist[cand], descending=True, stable=True)]
+
+    def export_episodes(self):
+        ids = self.select_candidates()[:self._num_eg].tolist()
+        if len(ids) < self._num_eg:
+            warnings.warn(f"{len(ids)} of the {self._num_eg} requested episodes qualify; writing those", stacklevel=2)
+        for i, e in enumerate(ids):
+            self._write(self._start_eg_id + i, dict(env_id=e, **{k: v[e] for k, v in self._rec.items()}))
+        return self.exported
+
+
+class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
+    def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless, capacity=DUAL_CAPACITY):
+        _check_eval_cfg(cfg, headless)
+        super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
+                         headless=headless)
+        self._init_eval(cfg)
+        self._cap = int(capacity)
+        if self._record:
+            N, E, dev = self.num_envs, self._num_eg, self.device
+            fields = ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action")
+            self._rec = self._rec_buffers((N,), self._cap, fields)
+            self._best = self._rec_buffers((E, 2), self._cap, fields)
+            i64 = lambda *s: torch.zeros(*s, device=dev, dtype=torch.long)  # noqa: E731
+            self._list = dict(list_len=i64(1), order=i64(E), best_distance=torch.zeros(E, device=dev), best_env=i64(E),
+                              best_nframes=i64(E), copy_slot=i64(1))
+
+    def render_vis(self, init=False):
+        """:87-202 without the renderer: record the frame of every env at row progress_buf, update the best-episode list with the
+        rallies that ended on this step; after num_rec_frames calls write the list's episodes"""
+        self.frame_index += 1
+        if not self._record:
+            return
+        t, p = self._physics_player.task, self._mvae_player
+        rec = {"rec_" + k: v for k, v in self._rec.items()}
+        native_v2p.eval_record(self.num_envs, self._cap, dict(
+            progress_buf=self.progress_buf, joint_rot=t._joint_rot, root_pos=t._root_pos, ball_pos=t._ball_pos, phase=p._phase_pred,
+            swing_type=p._swing_type_cycle, tar_action=self._tar_action, **rec))
+        native_v2p.eval_best(self.num_envs, self._cap, self._num_eg, dict(
+            reset_buf=self.reset_buf, progress_buf=self.progress_buf, distance=self._distance, **self._list, **rec,
+            **{"best_" + k: v for k, v in self._best.items()}))
+        if self.frame_index >= self._num_rec_frames:
+            self.export_episodes()
+            raise SystemExit(0)
+
+    def best_list(self):
+        """the list in rank order: (slot, even env of the pair, distance, frames) per entry"""
+        L = int(self._list["list_len"].item())
+        slots = self._list["order"][:L].tolist()
+        return [(s, int(self._list["best_env"][s]), float(self._list["best_distance"][s]), int(self._list["best_nframes"][s])) for s in slots]
+
+    def export_episodes(self):
+        entries = self.best_list()
+        if len(entries) < self._num_eg:
+            warnings.warn(f"{len(entries)} of the {self._num_eg} requested episodes were kept; writing those", stacklevel=2)
+        for i, (s, e, d, nf) in enumerate(entries):
+            self._write(self._start_eg_id + i, dict(env_ids=np.array([e, e + 1]), distance=np.float32(d),
+                                                    **{k: v[s, :, :nf] for k, v in self._best.items()}))
+        return self.exported
