@@ -756,7 +756,11 @@ __device__ __forceinline__ void step_prologue(const b200_buffers_t& bf, const b2
       // _action_to_pd_targets: clamp(action, q -+ lim) (humanoid_smpl_im.py:391-396) or, for the vid2player player env,
       // clamp(target_dof + action, q -+ lim) (humanoid_smpl_im_mvae.py:693-709, no_scale_action / pd_target_base target_pos)
       if (cfg.pd_mode == 1) a += bf.t_dof_pos[e * nd + lc.dof0 + k];
-      pdtar[k] = fmaxf(fminf(a, q[k] + cfg.pd_tar_lim), q[k] - cfg.pd_tar_lim);
+      // torch.maximum / torch.minimum propagate NaN, fmaxf / fminf drop it: a NaN action or joint angle must give a NaN target (the
+      // reference's NaN checks then see it), not the plausible target q + lim
+      float t = a;
+      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(t) : "f"(q[k] + cfg.pd_tar_lim), "f"(q[k] - cfg.pd_tar_lim));
+      pdtar[k] = t;
       bf.pd_targets[e * nd + lc.dof0 + k] = pdtar[k];
     }
     qexp(q, L.qj);
