@@ -241,6 +241,44 @@ typedef struct b200v2p_best {
 } b200v2p_best_t;
 int b200v2p_eval_best(const b200v2p_best_t* b, void* stream);
 
+/* Two-hand backhand fix of an exported episode (cfg vid2player.fix_two_hand_backhand_post): HumanoidSMPLIMMVAE.optimize_two_hand_backhand
+ * with single=True (env/tasks/humanoid_smpl_im_mvae.py:948-1031) and the frame selection and write-back of its callers
+ * (mvae_controller_vis.py:181-191, mvae_controller_vis_dual.py:213-231), one CTA per problem, all problems in one launch.
+ * A problem is one player of one episode: the frames with swing_type == 2 and 2 < phase < 5 are taken in frame order as one batch
+ * (neighbouring batch rows are coupled by the smoothness term even across segments); the free arm's Wrist, Elbow, Shoulder and
+ * Collar angle-axis get a delta that `iters` Adam steps (lr 0.005) fit so that the free hand reaches 2 hand - wrist of the racket
+ * arm (L1 target + 0.2 L1 delta + 0.5 L1 smoothness).  out: the selected rows are all 24 joints round-tripped through
+ * angle_axis_to_rotation_matrix / rotation_matrix_to_angle_axis with the fitted arm; every other row is joint_rot's, bit for bit.
+ * The FK uses the problem's own rest joints for every frame (the reference reads envs 0..M-1's) and rb_pos is the 7th output of
+ * _smpl_to_sim (the reference unpacks nine of eight values).  Float arrays are float or double as `precision` says. */
+typedef struct b200v2p_bhprob {
+  const void* joint_rot;       /* [T,24,3] axis-angle rows (SMPL joint order) */
+  const void* phase;           /* [T] */
+  const int64_t* swing_type;   /* [swing_type_len], swing_type_len >= T */
+  const void* rest;            /* [24,3] rest joints of the player, SMPL order */
+  void* out;                   /* [T,24,3]; may be joint_rot itself */
+  int64_t T, swing_type_len;   /* the arrays may be NULL when T is 0 */
+  int32_t righthand, pad_;     /* 1: the racket is in the right hand, the left arm is fitted */
+} b200v2p_bhprob_t;
+
+/* the scratch a launch needs: the problem table, then one int32 frame index and B200V2P_BHFIX_FRAME_WORDS scalars of the precision per
+ * frame, each part 256-byte aligned; F = the sum over the problems of T rounded up to a multiple of 32 */
+#define B200V2P_BHFIX_FRAME_WORDS 75
+#define B200V2P_BHFIX_ALIGN(x) ((((int64_t)(x)) + 255) / 256 * 256)
+#define B200V2P_BHFIX_SCRATCH_BYTES(P, F, S) (B200V2P_BHFIX_ALIGN((int64_t)(P) * (int64_t)sizeof(b200v2p_bhprob_t)) + B200V2P_BHFIX_ALIGN((int64_t)(F) * 4) + (int64_t)(F) * B200V2P_BHFIX_FRAME_WORDS * (S))
+
+typedef struct b200v2p_bhfix {
+  int32_t num_problems;
+  int32_t iters;                      /* Adam steps: 500 in the reference */
+  const b200v2p_bhprob_t* problems;   /* host array [num_problems], copied into the scratch on the stream (the one entry point here
+                                         that copies from the host: from pageable memory the copy first waits for the stream) */
+  void* scratch;                      /* device, 16-byte aligned, scratch_bytes >= B200V2P_BHFIX_SCRATCH_BYTES(num_problems, F, 4 or 8) */
+  int64_t scratch_bytes;
+  void* losses;                       /* optional [num_problems,3]: target, reg, smooth terms of the last evaluated step (NaN: none) */
+  int32_t precision, pad_;            /* 0 float32, 1 float64 */
+} b200v2p_bhfix_t;
+int b200v2p_backhand_fix(const b200v2p_bhfix_t* f, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

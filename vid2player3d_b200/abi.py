@@ -358,6 +358,30 @@ class V2PBest(C.Structure):
     ]
 
 
+class V2PBhProb(C.Structure):
+    _fields_ = [
+        ("joint_rot", C.c_void_p), ("phase", C.c_void_p), ("swing_type", C.c_void_p), ("rest", C.c_void_p), ("out", C.c_void_p),
+        ("T", C.c_int64), ("swing_type_len", C.c_int64), ("righthand", C.c_int32), ("pad_", C.c_int32),
+    ]
+
+
+class V2PBhFix(C.Structure):
+    _fields_ = [
+        ("num_problems", C.c_int32), ("iters", C.c_int32), ("problems", C.c_void_p), ("scratch", C.c_void_p), ("scratch_bytes", C.c_int64),
+        ("losses", C.c_void_p), ("precision", C.c_int32), ("pad_", C.c_int32),
+    ]
+
+
+BHFIX_FRAME_WORDS = 75    # B200V2P_BHFIX_FRAME_WORDS
+
+
+def bhfix_scratch_bytes(Ts, scalar_bytes):
+    """B200V2P_BHFIX_SCRATCH_BYTES for problems of T = Ts"""
+    al = lambda x: (x + 255) // 256 * 256  # noqa: E731
+    F = sum((int(t) + 31) // 32 * 32 for t in Ts)
+    return al(len(Ts) * C.sizeof(V2PBhProb)) + al(4 * F) + F * BHFIX_FRAME_WORDS * scalar_bytes
+
+
 # ---------------------------------------------------------------- entry points of libb200env.so
 # name -> (restype, argtypes) of every function include/b200env.h, include/b200env_v2p.h and include/b200ball.h declare; native.lib()
 # applies all of them when it loads the library, so an argument too many or too few, or one that does not convert to its C type,
@@ -408,6 +432,7 @@ SIGNATURES = {
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
     "b200v2p_eval_record": (C.c_int, [_p, _p]),
     "b200v2p_eval_best": (C.c_int, [_p, _p]),
+    "b200v2p_backhand_fix": (C.c_int, [_p, _p]),
     # include/b200ball.h
     "b200ball_simulate": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200ball_out_rows": (C.c_int, [_p, _i64, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _i32, _p, _p, _p]),

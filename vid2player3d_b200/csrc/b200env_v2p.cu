@@ -32,39 +32,45 @@ static int vfail(int code, const char* msg) {
   } while (0)
 
 // ------------------------------------------------------------------------------------------ konia conversions
-__device__ __forceinline__ float safe_div(float num, float den) {  // safe_zero_division, eps 1e-6
-  if (fabsf(den) < 1e-6f) den += 1e-6f;
+// templated on the scalar type: the float instantiation is what the float launches always ran (the float overloads of sqrt, fmax,
+// atan2, ... are sqrtf, fmaxf, atan2f), the double one serves the double instantiation of the backhand fix
+template <typename T>
+__device__ __forceinline__ T safe_div(T num, T den) {  // safe_zero_division, eps 1e-6
+  if (fabs(den) < T(1e-6)) den += T(1e-6);
   return num / den;
 }
 // rotation matrix (row-major) -> quaternion wxyz  (konia_transform.py:348-438)
-__device__ __forceinline__ void rotmat_to_quat_wxyz(const float* m, float* q) {
-  const float m00 = m[0], m01 = m[1], m02 = m[2], m10 = m[3], m11 = m[4], m12 = m[5], m20 = m[6], m21 = m[7], m22 = m[8];
-  const float trace = m00 + m11 + m22;
-  if (trace > 0.0f) {
-    float sq = sqrtf(fmaxf(trace + 1.0f, 1e-6f)) * 2.0f;
-    q[0] = 0.25f * sq; q[1] = safe_div(m21 - m12, sq); q[2] = safe_div(m02 - m20, sq); q[3] = safe_div(m10 - m01, sq);
+template <typename T>
+__device__ __forceinline__ void rotmat_to_quat_wxyz(const T* m, T* q) {
+  const T m00 = m[0], m01 = m[1], m02 = m[2], m10 = m[3], m11 = m[4], m12 = m[5], m20 = m[6], m21 = m[7], m22 = m[8];
+  const T trace = m00 + m11 + m22;
+  if (trace > T(0)) {
+    T sq = sqrt(fmax(trace + T(1), T(1e-6))) * T(2);
+    q[0] = T(0.25) * sq; q[1] = safe_div(m21 - m12, sq); q[2] = safe_div(m02 - m20, sq); q[3] = safe_div(m10 - m01, sq);
   } else if ((m00 > m11) && (m00 > m22)) {
-    float sq = sqrtf(fmaxf(1.0f + m00 - m11 - m22, 1e-6f)) * 2.0f;
-    q[0] = safe_div(m21 - m12, sq); q[1] = 0.25f * sq; q[2] = safe_div(m01 + m10, sq); q[3] = safe_div(m02 + m20, sq);
+    T sq = sqrt(fmax(T(1) + m00 - m11 - m22, T(1e-6))) * T(2);
+    q[0] = safe_div(m21 - m12, sq); q[1] = T(0.25) * sq; q[2] = safe_div(m01 + m10, sq); q[3] = safe_div(m02 + m20, sq);
   } else if (m11 > m22) {
-    float sq = sqrtf(fmaxf(1.0f + m11 - m00 - m22, 1e-6f)) * 2.0f;
-    q[0] = safe_div(m02 - m20, sq); q[1] = safe_div(m01 + m10, sq); q[2] = 0.25f * sq; q[3] = safe_div(m12 + m21, sq);
+    T sq = sqrt(fmax(T(1) + m11 - m00 - m22, T(1e-6))) * T(2);
+    q[0] = safe_div(m02 - m20, sq); q[1] = safe_div(m01 + m10, sq); q[2] = T(0.25) * sq; q[3] = safe_div(m12 + m21, sq);
   } else {
-    float sq = sqrtf(fmaxf(1.0f + m22 - m00 - m11, 1e-6f)) * 2.0f;
-    q[0] = safe_div(m10 - m01, sq); q[1] = safe_div(m02 + m20, sq); q[2] = safe_div(m12 + m21, sq); q[3] = 0.25f * sq;
+    T sq = sqrt(fmax(T(1) + m22 - m00 - m11, T(1e-6))) * T(2);
+    q[0] = safe_div(m10 - m01, sq); q[1] = safe_div(m02 + m20, sq); q[2] = safe_div(m12 + m21, sq); q[3] = T(0.25) * sq;
   }
 }
-__device__ __forceinline__ float safe_atan2(float y, float x) {  // torch_safe_atan2 (:41-49)
-  if (fabsf(y) < 1e-6f && fabsf(x) < 1e-6f) y += 1e-6f;
-  return atan2f(y, x);
+template <typename T>
+__device__ __forceinline__ T safe_atan2(T y, T x) {  // torch_safe_atan2 (:41-49)
+  if (fabs(y) < T(1e-6) && fabs(x) < T(1e-6)) y += T(1e-6);
+  return atan2(y, x);
 }
 // quaternion wxyz -> rotation vector (konia_transform.py:558-628)
-__device__ __forceinline__ void quat_wxyz_to_angle_axis(const float* q, float* aa) {
-  const float c = q[0], q1 = q[1], q2 = q[2], q3 = q[3];
-  const float s2 = q1 * q1 + q2 * q2 + q3 * q3;
-  const float s = sqrtf(fmaxf(s2, 1e-6f));
-  const float two_theta = 2.0f * (c < 0.0f ? safe_atan2(-s, -c) : safe_atan2(s, c));
-  const float k = s2 > 0.0f ? safe_div(two_theta, s) : 2.0f;
+template <typename T>
+__device__ __forceinline__ void quat_wxyz_to_angle_axis(const T* q, T* aa) {
+  const T c = q[0], q1 = q[1], q2 = q[2], q3 = q[3];
+  const T s2 = q1 * q1 + q2 * q2 + q3 * q3;
+  const T s = sqrt(fmax(s2, T(1e-6)));
+  const T two_theta = T(2) * (c < T(0) ? safe_atan2(-s, -c) : safe_atan2(s, c));
+  const T k = s2 > T(0) ? safe_div(two_theta, s) : T(2);
   aa[0] = q1 * k; aa[1] = q2 * k; aa[2] = q3 * k;
 }
 // quaternion (given in the converter's WXYZ slot order) -> rotation matrix (konia_transform.py:474-555)
@@ -87,6 +93,16 @@ __device__ __forceinline__ void qmul_xyzw(const float* a, const float* b, float*
 }
 
 // ------------------------------------------------------------------------------------------ a13: SMPL FK targets
+// one link of the SMPL chain (hybrik.py:597-652): G = G_parent R ; P = G_parent rel + P_parent
+template <typename T>
+__device__ __forceinline__ void chain_link(const T* pG, const T* pP, const T* R, const T* rel, T* G, T* P) {
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) G[r * 3 + c] = pG[r * 3] * R[c] + pG[r * 3 + 1] * R[3 + c] + pG[r * 3 + 2] * R[6 + c];
+    P[r] = pG[r * 3] * rel[0] + pG[r * 3 + 1] * rel[1] + pG[r * 3 + 2] * rel[2] + pP[r];
+  }
+}
 __global__ void __launch_bounds__(V2P_WARPS * 32)
 smpl_to_sim_kernel(int n, const float* __restrict__ root_pos, const float* __restrict__ rotmat, const float* __restrict__ rest_all,
                    int num_rest, const int32_t* __restrict__ parents, const int32_t* __restrict__ smpl_2_mujoco, float dt,
@@ -131,12 +147,7 @@ smpl_to_sim_kernel(int n, const float* __restrict__ root_pos, const float* __res
     for (int k = 0; k < 3; k++) pP[k] = __shfl_sync(FULL, P[k], par);
     const bool pdone = __shfl_sync(FULL, (int)done, par) != 0;
     if (act && !done && pdone) {
-#pragma unroll
-      for (int r = 0; r < 3; r++) {
-#pragma unroll
-        for (int c = 0; c < 3; c++) G[r * 3 + c] = pG[r * 3] * Rl[c] + pG[r * 3 + 1] * Rl[3 + c] + pG[r * 3 + 2] * Rl[6 + c];
-        P[r] = pG[r * 3] * rel[0] + pG[r * 3 + 1] * rel[1] + pG[r * 3 + 2] * rel[2] + pP[r];
-      }
+      chain_link(pG, pP, Rl, rel, G, P);
       done = true;
     }
   }
@@ -205,17 +216,18 @@ smpl_to_sim_kernel(int n, const float* __restrict__ root_pos, const float* __res
 
 // ------------------------------------------------------------------------------------------ a13b: head look-at correction
 // angle_axis_to_rotation_matrix (konia_transform.py:250-334)
-__device__ __forceinline__ void aa_to_rotmat(const float* aa, float* m) {
-  const float theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
-  if (theta2 > 1e-6f) {
-    const float theta = sqrtf(fmaxf(theta2, 1e-6f));
-    const float wx = aa[0] / (theta + 1e-6f), wy = aa[1] / (theta + 1e-6f), wz = aa[2] / (theta + 1e-6f);
-    const float c = cosf(theta), s = sinf(theta), k = 1.0f - c;
+template <typename T>
+__device__ __forceinline__ void aa_to_rotmat(const T* aa, T* m) {
+  const T theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
+  if (theta2 > T(1e-6)) {
+    const T theta = sqrt(fmax(theta2, T(1e-6)));
+    const T wx = aa[0] / (theta + T(1e-6)), wy = aa[1] / (theta + T(1e-6)), wz = aa[2] / (theta + T(1e-6));
+    const T c = cos(theta), s = sin(theta), k = T(1) - c;
     m[0] = c + wx * wx * k; m[1] = wx * wy * k - wz * s; m[2] = wy * s + wx * wz * k;
     m[3] = wz * s + wx * wy * k; m[4] = c + wy * wy * k; m[5] = -wx * s + wy * wz * k;
     m[6] = -wy * s + wx * wz * k; m[7] = wx * s + wy * wz * k; m[8] = c + wz * wz * k;
   } else {
-    m[0] = 1.0f; m[1] = -aa[2]; m[2] = aa[1]; m[3] = aa[2]; m[4] = 1.0f; m[5] = -aa[0]; m[6] = -aa[1]; m[7] = aa[0]; m[8] = 1.0f;
+    m[0] = T(1); m[1] = -aa[2]; m[2] = aa[1]; m[3] = aa[2]; m[4] = T(1); m[5] = -aa[0]; m[6] = -aa[1]; m[7] = aa[0]; m[8] = T(1);
   }
 }
 __global__ void fix_head_kernel(int n, const float* __restrict__ rb_pos, const float* __restrict__ rb_rot, int head_body,
@@ -651,6 +663,294 @@ __global__ void __launch_bounds__(96) eval_best_copy_kernel(b200v2p_best_t b) {
   else if (t == 78) b.best_phase[o] = b.rec_phase[s];
   else if (t == 79) b.best_swing_type[o] = b.rec_swing_type[s];
   else if (t == 80) b.best_tar_action[o] = b.rec_tar_action[s];
+}
+
+// ------------------------------------------------------------------------------------------ two-hand backhand fix
+// HumanoidSMPLIMMVAE.optimize_two_hand_backhand (env/tasks/humanoid_smpl_im_mvae.py:948-1031, single=True) with the selection and
+// write-back of its callers (mvae_controller_vis.py:181-191, mvae_controller_vis_dual.py:213-231).  One CTA per problem (one player of
+// one episode): it compacts its selected frames into a batch of M rows, computes each row's fixed Spine3 (joint 9) transform and
+// target once, then runs every Adam step in the kernel: FK of the free arm (collar, shoulder, elbow, wrist, hand), the L1 gradients,
+// reverse mode through the chain and the konia exp map, the Adam update.  The delta is double-buffered and one barrier per step
+// makes every row read its neighbour's delta of the same step.  Per-row state lives in the caller's scratch (M has no bound).
+#define BHFIX_THREADS 256
+enum { BH_BASE = 0, BH_G9 = 12, BH_P9 = 21, BH_TGT = 24, BH_M = 27, BH_V = 39, BH_D = 51 };   // BH_D: two 12-word delta buffers
+static_assert(BH_D + 24 == B200V2P_BHFIX_FRAME_WORDS, "scratch words per frame");
+
+template <typename T>
+__device__ __forceinline__ T l1_sign(T x) { return x > T(0) ? T(1) : (x < T(0) ? T(-1) : T(0)); }   // torch.sgn: 0 at 0 and at NaN
+
+// reverse mode of aa_to_rotmat: dL/daa from dL/dR for the formula as written.  Normal branch: theta = sqrt(theta2),
+// w = aa / (theta + 1e-6), R = c I + s [w]x + (1 - c) w w^T; where theta2 <= 1e-6 autograd sees the Taylor branch I + [aa]x alone
+template <typename T>
+__device__ __forceinline__ void aa_to_rotmat_vjp(const T* aa, const T* dR, T* g) {
+  const T v[3] = {dR[7] - dR[5], dR[2] - dR[6], dR[3] - dR[1]};   // <dR, d[w]x / dw>
+  const T theta2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
+  if (!(theta2 > T(1e-6))) {
+    g[0] = v[0]; g[1] = v[1]; g[2] = v[2];
+    return;
+  }
+  const T theta = sqrt(theta2), d = theta + T(1e-6);
+  const T w[3] = {aa[0] / d, aa[1] / d, aa[2] / d};
+  const T c = cos(theta), s = sin(theta), k = T(1) - c;
+  T Sw[3];   // (dR + dR^T) w
+#pragma unroll
+  for (int r = 0; r < 3; r++) Sw[r] = (dR[r * 3] + dR[r]) * w[0] + (dR[r * 3 + 1] + dR[3 + r]) * w[1] + (dR[r * 3 + 2] + dR[6 + r]) * w[2];
+  const T dk = T(0.5) * (w[0] * Sw[0] + w[1] * Sw[1] + w[2] * Sw[2]);
+  const T dc = dR[0] + dR[4] + dR[8] - dk;
+  const T ds = w[0] * v[0] + w[1] * v[1] + w[2] * v[2];
+  T dw[3];
+#pragma unroll
+  for (int r = 0; r < 3; r++) dw[r] = s * v[r] + k * Sw[r];
+  const T dd = -(dw[0] * w[0] + dw[1] * w[1] + dw[2] * w[2]) / d;
+  const T dtheta = -s * dc + c * ds + dd;
+#pragma unroll
+  for (int r = 0; r < 3; r++) g[r] = dw[r] / d + aa[r] * dtheta / theta;
+}
+
+template <typename T>
+__device__ __forceinline__ void rel_joint(const T* rest, int j, int par, T* rel) {
+#pragma unroll
+  for (int k = 0; k < 3; k++) rel[k] = rest[j * 3 + k] - rest[par * 3 + k];
+}
+
+template <typename T>
+__global__ void __launch_bounds__(BHFIX_THREADS) backhand_fix_kernel(const b200v2p_bhprob_t* __restrict__ probs, int32_t* __restrict__ idx_all,
+                                                                      T* __restrict__ state_all, int iters, T* __restrict__ losses) {
+  __shared__ T rest[72];
+  __shared__ int s_warp[BHFIX_THREADS / 32];
+  __shared__ int s_count;
+  __shared__ T s_red[3][BHFIX_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const b200v2p_bhprob_t pr = probs[blockIdx.x];
+  int64_t off = 0;   // frames of the problems before this one, each rounded up to a warp's 32
+  for (unsigned q = 0; q < blockIdx.x; q++) off += (probs[q].T + 31) / 32 * 32;
+  const int64_t Tn = pr.T;
+  const T* jr = (const T*)pr.joint_rot;
+  const T* ph = (const T*)pr.phase;
+  T* out = (T*)pr.out;
+  int32_t* idx = idx_all + off;
+  T* st = state_all + off * B200V2P_BHFIX_FRAME_WORDS;
+  // scratch word w of batch row i: rows grouped by 32, one word of a group's rows contiguous (a warp's access is coalesced and the
+  // word offsets are immediates)
+  const auto row_of = [&](int i) { return st + (int64_t)(i >> 5) * (B200V2P_BHFIX_FRAME_WORDS * 32) + (i & 31); };
+  if (Tn > 0)
+    for (int k = tid; k < 72; k += BHFIX_THREADS) rest[k] = ((const T*)pr.rest)[k];
+  if (tid == 0) s_count = 0;
+  __syncthreads();
+
+  // need_fix = (swing_type == 2) & (phase > 2) & (phase < 5), compacted in frame order; the other rows are copied through
+  for (int64_t c0 = 0; c0 < Tn; c0 += BHFIX_THREADS) {
+    const int64_t f = c0 + tid;
+    bool sel = false;
+    if (f < Tn) {
+      const T phf = ph[f];
+      sel = pr.swing_type[f] == 2 && phf > T(2) && phf < T(5);
+      if (!sel && out != jr)
+        for (int k = 0; k < 72; k++) out[f * 72 + k] = jr[f * 72 + k];
+    }
+    const unsigned b = __ballot_sync(FULL, sel);
+    if (lane == 0) s_warp[warp] = __popc(b);
+    __syncthreads();
+    int base = s_count;
+    for (int w = 0; w < warp; w++) base += s_warp[w];
+    if (sel) idx[base + __popc(b & ((1u << lane) - 1u))] = (int32_t)f;
+    __syncthreads();
+    if (tid == 0)
+      for (int w = 0; w < BHFIX_THREADS / 32; w++) s_count += s_warp[w];
+    __syncthreads();
+  }
+  const int M = s_count;
+  // free arm (fitted) and racket arm, from the collar to the hand; delta row k = 3 - chain position (Wrist, Elbow, Shoulder, Collar)
+  // SMPL left arm from the collar: 13, 16, 18, 20, 22 (L_Hand); the right arm's joints are one further each
+  const int L = pr.righthand ? 0 : 1;
+  const auto left_arm = [](int c) { return c ? 14 + 2 * c : 13; };
+  const auto fc = [&](int c) { return left_arm(c) + L; };
+  const auto rc = [&](int c) { return left_arm(c) + 1 - L; };
+  __shared__ T frel[5][3];
+  if (tid < 5) rel_joint(rest, fc(tid), tid ? fc(tid - 1) : 9, frel[tid]);
+  __syncthreads();
+
+  // per row: Spine3's global transform, the target 2 hand - wrist - root of the racket arm (root_pos = 0: rb = P - rest[0]),
+  // the base angle-axis of the fitted joints (rotation_matrix_to_angle_axis of angle_axis_to_rotation_matrix), Adam state
+  for (int i = tid; i < M; i += BHFIX_THREADS) {
+    const T* a = jr + (int64_t)idx[i] * 72;
+    T* row = row_of(i);
+    T R[9], G[9], P[3], Gn[9], Pn[3], rel[3];
+    aa_to_rotmat(a, G);
+#pragma unroll
+    for (int k = 0; k < 3; k++) P[k] = rest[k];
+    const int spine[3] = {3, 6, 9};
+#pragma unroll
+    for (int s = 0; s < 3; s++) {
+      aa_to_rotmat(a + spine[s] * 3, R);
+      rel_joint(rest, spine[s], s ? spine[s - 1] : 0, rel);
+      chain_link(G, P, R, rel, Gn, Pn);
+#pragma unroll
+      for (int k = 0; k < 9; k++) G[k] = Gn[k];
+#pragma unroll
+      for (int k = 0; k < 3; k++) P[k] = Pn[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 9; k++) row[(BH_G9 + k) * 32] = G[k];
+#pragma unroll
+    for (int k = 0; k < 3; k++) row[(BH_P9 + k) * 32] = P[k];
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      aa_to_rotmat(a + rc(c) * 3, R);
+      rel_joint(rest, rc(c), c ? rc(c - 1) : 9, rel);
+      chain_link(G, P, R, rel, Gn, Pn);
+#pragma unroll
+      for (int k = 0; k < 9; k++) G[k] = Gn[k];
+#pragma unroll
+      for (int k = 0; k < 3; k++) P[k] = Pn[k];
+    }
+    rel_joint(rest, rc(4), rc(3), rel);
+#pragma unroll
+    for (int r = 0; r < 3; r++) {
+      const T hand = G[r * 3] * rel[0] + G[r * 3 + 1] * rel[1] + G[r * 3 + 2] * rel[2] + P[r];
+      const T root = rest[r] - (rest[r] - T(0));
+      row[(BH_TGT + r) * 32] = T(2) * (hand - (rest[r] - T(0))) - (P[r] - (rest[r] - T(0))) - root;
+    }
+#pragma unroll
+    for (int c = 0; c < 4; c++) {
+      T q[4], aa[3];
+      aa_to_rotmat(a + fc(c) * 3, R);
+      rotmat_to_quat_wxyz(R, q);
+      quat_wxyz_to_angle_axis(q, aa);
+#pragma unroll
+      for (int k = 0; k < 3; k++) row[(BH_BASE + (3 - c) * 3 + k) * 32] = aa[k];
+    }
+#pragma unroll
+    for (int k = 0; k < 12; k++) { row[(BH_M + k) * 32] = T(0); row[(BH_V + k) * 32] = T(0); row[(BH_D + k) * 32] = T(0); }
+  }
+  __syncthreads();
+
+  // L1Loss(mean) * weight: d/dx = weight / numel * sgn(x)
+  const T w_tgt = T(1) / T(3 * (int64_t)M), w_reg = T(0.2) / T(12 * (int64_t)M), w_smooth = T(0.5) / T(12 * ((int64_t)M - 1));
+  T sum_tgt = T(0), sum_reg = T(0), sum_smooth = T(0);
+  for (int it = 0; it < iters; it++) {
+    // torch.optim.Adam(lr=0.005, betas=(0.9, 0.999), eps=1e-8): bias corrections in double like the Python scalars, then the tensor type
+    const double bc1 = 1.0 - pow(0.9, (double)(it + 1)), bc2 = 1.0 - pow(0.999, (double)(it + 1));
+    const T step_size = T(0.005 / bc1), bc2_sqrt = T(sqrt(bc2));
+    const int dc = BH_D + 12 * (it & 1), dn = BH_D + 12 * ((it + 1) & 1);   // delta words read / written by this step
+    const bool last = it == iters - 1;
+    for (int i = tid; i < M; i += BHFIX_THREADS) {
+      T* row = row_of(i);
+      const T* prev = row_of(i - 1);
+      // the fitted joint c's angle-axis is re-read where it is needed (scratch, cache-resident) rather than held in registers
+      const auto joint_aa = [&](int c, T* a) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) a[k] = row[(BH_BASE + (3 - c) * 3 + k) * 32] + row[(dc + (3 - c) * 3 + k) * 32];
+      };
+      T G[4][9], P[3], R[9], a[3];
+#pragma unroll
+      for (int k = 0; k < 9; k++) G[0][k] = row[(BH_G9 + k) * 32];
+#pragma unroll
+      for (int k = 0; k < 3; k++) P[k] = row[(BH_P9 + k) * 32];
+      // forward: G[c] is the parent transform of chain joint c (G[0] = Spine3); the wrist's transform ends in Gw
+      T Gw[9];
+#pragma unroll
+      for (int c = 0; c < 4; c++) {
+        T Pn[3];
+        joint_aa(c, a);
+        aa_to_rotmat(a, R);
+        chain_link(G[c], P, R, frel[c], c < 3 ? G[c + 1] : Gw, Pn);
+#pragma unroll
+        for (int k = 0; k < 3; k++) P[k] = Pn[k];
+      }
+      T gh[3], diff[3];
+#pragma unroll
+      for (int r = 0; r < 3; r++) {
+        const T hand = Gw[r * 3] * frel[4][0] + Gw[r * 3 + 1] * frel[4][1] + Gw[r * 3 + 2] * frel[4][2] + P[r];
+        diff[r] = (hand - (rest[r] - T(0))) - row[(BH_TGT + r) * 32];
+        gh[r] = w_tgt * l1_sign(diff[r]);
+      }
+      // reverse: dG = dL/d(transform of chain joint c); P_c = G[c] rel_c + P_{c-1} passes gh to every link.  Each joint's three
+      // components take their reg and smoothness terms and the Adam update as soon as their FK gradient is known.
+      T dG[9], s_reg = T(0), s_smooth = T(0);
+#pragma unroll
+      for (int r = 0; r < 3; r++)
+#pragma unroll
+        for (int k = 0; k < 3; k++) dG[r * 3 + k] = gh[r] * frel[4][k];
+#pragma unroll
+      for (int c = 3; c >= 0; c--) {
+        T dR[9], dGp[9], g[3];
+        joint_aa(c, a);
+        aa_to_rotmat(a, R);
+#pragma unroll
+        for (int r = 0; r < 3; r++)
+#pragma unroll
+          for (int k = 0; k < 3; k++) {
+            dR[r * 3 + k] = G[c][r] * dG[k] + G[c][3 + r] * dG[3 + k] + G[c][6 + r] * dG[6 + k];
+            dGp[r * 3 + k] = dG[r * 3] * R[k * 3] + dG[r * 3 + 1] * R[k * 3 + 1] + dG[r * 3 + 2] * R[k * 3 + 2] + gh[r] * frel[c][k];
+          }
+        aa_to_rotmat_vjp(a, dR, g);
+#pragma unroll
+        for (int k = 0; k < 9; k++) dG[k] = dGp[k];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+          const int64_t w = (3 - c) * 3 + k;
+          const T dl = row[(dc + w) * 32];
+          T gk = g[k] + w_reg * l1_sign(dl);
+          s_reg += fabs(dl);
+          if (i > 0) {
+            const T dd = dl - prev[(dc + w) * 32];
+            gk += w_smooth * l1_sign(dd);
+            s_smooth += fabs(dd);
+          }
+          T m = row[(BH_M + w) * 32], v = row[(BH_V + w) * 32];
+          m = m + T(1.0 - 0.9) * (gk - m);                       // lerp_(grad, 1 - beta1), weight < 0.5 form
+          v = v * T(0.999) + T(1.0 - 0.999) * gk * gk;          // mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
+          row[(BH_M + w) * 32] = m;
+          row[(BH_V + w) * 32] = v;
+          row[(dn + w) * 32] = dl - step_size * (m / (sqrt(v) / bc2_sqrt + T(1e-8)));
+        }
+      }
+      if (last) {
+        sum_tgt += fabs(diff[0]) + fabs(diff[1]) + fabs(diff[2]);
+        sum_reg += s_reg;
+        sum_smooth += s_smooth;
+      }
+    }
+    __syncthreads();
+  }
+
+  // write-back: all 24 joints of a selected row through rotation_matrix_to_angle_axis, the fitted four from base + delta
+  const int df = BH_D + 12 * (iters & 1);
+  for (int i = tid; i < M; i += BHFIX_THREADS) {
+    const int64_t f = idx[i];
+    const T* row = row_of(i);
+    for (int j = 0; j < 24; j++) {
+      T a[3], R[9], q[4], o[3];
+      const int c = j == fc(0) ? 0 : (j == fc(1) ? 1 : (j == fc(2) ? 2 : (j == fc(3) ? 3 : -1)));
+#pragma unroll
+      for (int k = 0; k < 3; k++)
+        a[k] = c < 0 ? jr[f * 72 + j * 3 + k] : row[(BH_BASE + (3 - c) * 3 + k) * 32] + row[(df + (3 - c) * 3 + k) * 32];
+      aa_to_rotmat(a, R);
+      rotmat_to_quat_wxyz(R, q);
+      quat_wxyz_to_angle_axis(q, o);
+#pragma unroll
+      for (int k = 0; k < 3; k++) out[f * 72 + j * 3 + k] = o[k];
+    }
+  }
+  if (!losses) return;
+  T part[3] = {sum_tgt, sum_reg, sum_smooth};
+#pragma unroll
+  for (int t = 0; t < 3; t++) {
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) part[t] += __shfl_down_sync(FULL, part[t], s);
+    if (lane == 0) s_red[t][warp] = part[t];
+  }
+  __syncthreads();
+  if (tid != 0) return;
+  T tot[3] = {T(0), T(0), T(0)};
+  for (int w = 0; w < BHFIX_THREADS / 32; w++)
+    for (int t = 0; t < 3; t++) tot[t] += s_red[t][w];
+  // the mean of an empty L1 is NaN: every term at M = 0, the smoothness term at M <= 1; all three when no step was evaluated
+  const T nan = T(NAN);
+  losses[blockIdx.x * 3] = iters ? tot[0] / T(3 * (int64_t)M) : nan;
+  losses[blockIdx.x * 3 + 1] = iters ? tot[1] / T(12 * (int64_t)M) * T(0.2) : nan;
+  losses[blockIdx.x * 3 + 2] = iters && M > 1 ? tot[2] / T(12 * ((int64_t)M - 1)) * T(0.5) : nan;
 }
 
 // ------------------------------------------------------------------------------------------ dual mode: incoming-ball table
@@ -1099,6 +1399,42 @@ int b200v2p_eval_best(const b200v2p_best_t* b, void* stream) {
     return vfail(-1, "b200v2p_eval_best: bad arguments");
   eval_best_select_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(*b);
   eval_best_copy_kernel<<<dim3(b->cap, 2), 96, 0, (cudaStream_t)stream>>>(*b);
+  V_CUDA_OK();
+  return 0;
+}
+
+int b200v2p_backhand_fix(const b200v2p_bhfix_t* f, void* stream) {
+  if (!f) return vfail(-1, "b200v2p_backhand_fix: null");
+  if (f->num_problems < 0 || f->iters < 0) return vfail(-1, "b200v2p_backhand_fix: negative problem count or iters");
+  if (f->num_problems == 0) return 0;
+  if (!f->problems || !f->scratch) return vfail(-1, "b200v2p_backhand_fix: null problem table or scratch");
+  if (f->precision != 0 && f->precision != 1) return vfail(-2, "b200v2p_backhand_fix: precision must be 0 (float32) or 1 (float64)");
+  if ((uintptr_t)f->scratch & 15) return vfail(-2, "b200v2p_backhand_fix: scratch must be 16-byte aligned");
+  int64_t frames = 0;
+  for (int p = 0; p < f->num_problems; p++) {
+    const b200v2p_bhprob_t& q = f->problems[p];
+    if (q.T < 0 || q.T > INT32_MAX) return vfail(-1, "b200v2p_backhand_fix: T must lie in [0, 2^31)");
+    if (q.T > 0 && (!q.joint_rot || !q.phase || !q.swing_type || !q.rest || !q.out))   // an empty episode may come with null arrays
+      return vfail(-1, "b200v2p_backhand_fix: null problem array");
+    if (q.swing_type_len < q.T) return vfail(-2, "b200v2p_backhand_fix: swing_type row shorter than T");
+    frames += (q.T + 31) / 32 * 32;
+  }
+  const int S = f->precision ? 8 : 4;
+  if (f->scratch_bytes < B200V2P_BHFIX_SCRATCH_BYTES(f->num_problems, frames, S)) return vfail(-2, "b200v2p_backhand_fix: scratch too small");
+  char* s = (char*)f->scratch;
+  const int64_t idx_at = B200V2P_BHFIX_ALIGN((int64_t)f->num_problems * (int64_t)sizeof(b200v2p_bhprob_t));
+  const int64_t state_at = idx_at + B200V2P_BHFIX_ALIGN(frames * 4);
+  // pageable source: the call returns once the table is staged, so the caller's array may go right away
+  if (cudaMemcpyAsync(s, f->problems, f->num_problems * sizeof(b200v2p_bhprob_t), cudaMemcpyHostToDevice, (cudaStream_t)stream) != cudaSuccess)
+    return vfail(-10, cudaGetErrorString(cudaGetLastError()));
+  const b200v2p_bhprob_t* probs = (const b200v2p_bhprob_t*)s;
+  int32_t* idx = (int32_t*)(s + idx_at);
+  if (f->precision)
+    backhand_fix_kernel<double><<<f->num_problems, BHFIX_THREADS, 0, (cudaStream_t)stream>>>(probs, idx, (double*)(s + state_at), f->iters,
+                                                                                              (double*)f->losses);
+  else
+    backhand_fix_kernel<float><<<f->num_problems, BHFIX_THREADS, 0, (cudaStream_t)stream>>>(probs, idx, (float*)(s + state_at), f->iters,
+                                                                                             (float*)f->losses);
   V_CUDA_OK();
   return 0;
 }

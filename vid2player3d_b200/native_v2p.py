@@ -1,6 +1,8 @@
 """ctypes binding of the vid2player entry points (include/b200env_v2p.h) - same library, no CPU fallback."""
 import ctypes as C
 
+import torch
+
 from . import abi
 from .native import _ptr, _stream, lib
 
@@ -216,6 +218,41 @@ def eval_best(n, cap, num_eg, t):
     b.n, b.cap, b.num_eg = int(n), int(cap), int(num_eg)
     _fill_ptrs(b, t)
     _check(lib().b200v2p_eval_best(C.byref(b), _stream()))
+
+
+BACKHAND_ITERS = 500    # optimize_two_hand_backhand(single=True): 500 Adam steps
+
+
+def backhand_fix(problems, iters=BACKHAND_ITERS):
+    """the two-hand backhand fix of include/b200env_v2p.h b200v2p_backhand_fix, every problem in one launch.  problems: dicts with
+    joint_rot [T,24,3], phase [T], swing_type [>= T] int64, rest [24,3], righthand (bool) and optionally out [T,24,3] (joint_rot itself
+    fixes in place); float tensors all float32 or all float64 on the device.  Returns (outs, losses): the fixed rows per problem and
+    the [P,3] target / reg / smooth loss terms of the last evaluated step (NaN where none was)."""
+    P = len(problems)
+    assert P > 0
+    dtype, dev = problems[0]["joint_rot"].dtype, problems[0]["joint_rot"].device
+    assert dtype in (torch.float32, torch.float64)
+    table, outs = (abi.V2PBhProb * P)(), []
+    for q, pr in zip(table, problems):
+        jr = pr["joint_rot"]
+        out = pr.get("out")
+        out = torch.empty_like(jr) if out is None else out
+        T = int(jr.shape[0])
+        for k, x in (("joint_rot", jr), ("phase", pr["phase"]), ("rest", pr["rest"]), ("out", out)):
+            assert x.dtype == dtype and x.device == dev, k
+        assert jr.shape[1:] == (24, 3) and out.shape == jr.shape and pr["rest"].shape == (24, 3) and pr["phase"].numel() >= T
+        assert pr["swing_type"].dtype == torch.int64 and pr["swing_type"].device == dev
+        q.joint_rot, q.phase, q.swing_type, q.rest, q.out = (_c(x) for x in (jr, pr["phase"], pr["swing_type"], pr["rest"], out))
+        q.T, q.swing_type_len, q.righthand = T, pr["swing_type"].numel(), int(bool(pr["righthand"]))
+        outs.append(out)
+    S = 8 if dtype == torch.float64 else 4
+    nbytes = abi.bhfix_scratch_bytes([q.T for q in table], S)
+    scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    losses = torch.empty(P, 3, dtype=dtype, device=dev)
+    f = abi.V2PBhFix(num_problems=P, iters=int(iters), problems=C.addressof(table), scratch=scratch.data_ptr(), scratch_bytes=nbytes,
+                     losses=losses.data_ptr(), precision=int(S == 8))
+    _check(lib().b200v2p_backhand_fix(C.byref(f), _stream()))
+    return outs, losses
 
 
 def ctrl_reset(mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):

@@ -11,12 +11,21 @@ The renderer (SMPL meshes, video, HTML) is not part of this package: the .npz fi
 render_one_result is given, so they can be rendered with its visualizer.  Deliberate departures from the reference:
   - a rally longer than the recording capacity keeps its first `capacity` rows (the reference raises IndexError);
   - fewer candidates (single) or list entries (dual) than num_eg: the ones that exist are written (`self.exported` lists them);
-  - select_best orders candidates of equal distance by env id (stable sort);
-  - fix_two_hand_backhand_post (an offline IK fix applied before rendering) is not applied to the written arrays.
+  - select_best orders candidates of equal distance by env id (stable sort).
+With fix_two_hand_backhand_post (cfgs djokovic, nadal, federer_djokovic, nadal_federer) the written episode also holds
+joint_rot_fixed ([T,24,3] single, [2,T,24,3] dual): the rows of the two-hand backhand fix the reference's render_one_result applies
+before rendering (optimize_two_hand_backhand, env/tasks/humanoid_smpl_im_mvae.py:948-1031), made for all exported episodes and players
+by one device launch (native_v2p.backhand_fix); joint_rot stays as recorded, since render_one_result applies the fix itself.  Dual
+mode fixes each player of the pair whose name does not start with 'federer'.  The released optimiser does not run as it stands; the
+launch keeps its evident intent: rb_pos is the 7th output of _smpl_to_sim (the reference unpacks nine of eight values), the FK uses
+the fixed player's own rest joints for every frame (the reference reads the rest joints of envs 0..M-1), and the device is the
+task's (the reference hard-codes cuda:0).  The loss terms the reference prints are kept in `backhand_losses` (episode id -> [3], or
+[2,3] in dual mode with NaN for a player left alone).
 Reference quirks kept: the meters' avg of an env that never recovered stays 1; the dual recording row 0 of an env is written by the
 init call only, and an exported rally is rows [0, progress) - it starts with that row and leaves out the last frame; the dual list
 grows only when a candidate beats its current last entry, even while it holds fewer than num_eg.
 """
+import math
 import os
 import warnings
 
@@ -69,8 +78,8 @@ class _EvalRecorder:
         self._rec_fname = env.get("rec_fname")
         self._cfg_name = getattr(cfg.get("args"), "cfg", None) or cfg.get("name", "eval")
         self.exported = []
-        if self.cfg_v2p.get("fix_two_hand_backhand_post"):
-            warnings.warn("fix_two_hand_backhand_post: the episodes are written without the two-hand backhand fix", stacklevel=3)
+        self._fix_backhand = bool(self.cfg_v2p.get("fix_two_hand_backhand_post"))
+        self.backhand_losses = {}
 
     def _episode_path(self, eg_id):
         return self._rec_fname or os.path.join("out", "episodes", f"{self._cfg_name}_{eg_id:03d}.npz")
@@ -81,6 +90,16 @@ class _EvalRecorder:
         with open(path, "wb") as f:
             np.savez(f, **{k: v.cpu().numpy() if torch.is_tensor(v) else np.asarray(v) for k, v in arrays.items()})
         self.exported.append(path)
+
+    def _players(self):
+        """(skip, righthand) of player j of a pair: mvae_controller_vis_dual.py:216-223"""
+        v = self.cfg_v2p
+        for j in range(2):
+            if v.get("dual_mode") == "different":
+                player, rh = v["player"][j], v["righthand"][j]
+            else:
+                player, rh = v.get("player"), v.get("righthand", True)
+            yield str(player).startswith("federer"), bool(rh)
 
     def _rec_buffers(self, n, cap, fields):
         dev = self.device
@@ -145,8 +164,17 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
         ids = self.select_candidates()[:self._num_eg].tolist()
         if len(ids) < self._num_eg:
             warnings.warn(f"{len(ids)} of the {self._num_eg} requested episodes qualify; writing those", stacklevel=2)
+        fixed = {}
+        if self._fix_backhand and ids:
+            rest, rh = self._physics_player.task._rest_t[0], bool(self.cfg_v2p.get("righthand", True))
+            outs, losses = native_v2p.backhand_fix([dict(joint_rot=self._rec["joint_rot"][e], phase=self._rec["phase"][e],
+                                                    swing_type=self._rec["swing_type"][e], rest=rest, righthand=rh) for e in ids],
+                                                   iters=native_v2p.BACKHAND_ITERS)
+            for i, e in enumerate(ids):
+                fixed[e] = dict(joint_rot_fixed=outs[i])
+                self.backhand_losses[self._start_eg_id + i] = losses[i].cpu().numpy()
         for i, e in enumerate(ids):
-            self._write(self._start_eg_id + i, dict(env_id=e, **{k: v[e] for k, v in self._rec.items()}))
+            self._write(self._start_eg_id + i, dict(env_id=e, **{k: v[e] for k, v in self._rec.items()}, **fixed.get(e, {})))
         return self.exported
 
 
@@ -194,7 +222,25 @@ class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
         entries = self.best_list()
         if len(entries) < self._num_eg:
             warnings.warn(f"{len(entries)} of the {self._num_eg} requested episodes were kept; writing those", stacklevel=2)
+        fixed = {}
+        if self._fix_backhand and entries:
+            rest_t = self._physics_player.task._rest_t          # [K,24,3]: player j of a pair has shape j % K
+            problems, slots = [], []
+            for i, (s, e, d, nf) in enumerate(entries):
+                fixed[i] = self._best["joint_rot"][s, :, :nf].clone()
+                for j, (skip, rh) in enumerate(self._players()):
+                    if not skip:
+                        problems.append(dict(joint_rot=self._best["joint_rot"][s, j, :nf], phase=self._best["phase"][s, j, :nf],
+                                             swing_type=self._best["swing_type"][s, j], rest=rest_t[j % rest_t.shape[0]], righthand=rh,
+                                             out=fixed[i][j]))
+                        slots.append((i, j))
+            losses = native_v2p.backhand_fix(problems, iters=native_v2p.BACKHAND_ITERS)[1].cpu().numpy() if problems else np.zeros((0, 3))
+            for i in range(len(entries)):
+                self.backhand_losses[self._start_eg_id + i] = np.full((2, 3), math.nan)
+            for (i, j), row in zip(slots, losses):
+                self.backhand_losses[self._start_eg_id + i][j] = row
         for i, (s, e, d, nf) in enumerate(entries):
+            extra = dict(joint_rot_fixed=fixed[i]) if i in fixed else {}
             self._write(self._start_eg_id + i, dict(env_ids=np.array([e, e + 1]), distance=np.float32(d),
-                                                    **{k: v[s, :, :nf] for k, v in self._best.items()}))
+                                                    **{k: v[s, :, :nf] for k, v in self._best.items()}, **extra))
         return self.exported
