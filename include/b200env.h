@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 8
+#define B200_ABI_VERSION 9
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:

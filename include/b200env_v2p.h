@@ -105,6 +105,18 @@ typedef struct b200v2p_ctrl {
   const float* ball_vel;           /* [n,3]; eval only */
   float *meter_sum, *meter_avg, *meter_max; /* [4,n]; eval only */
   int64_t* meter_count;            /* [4,n]; eval only */
+  /* the high-level policy's first-layer operand (V2PPlayer.get_action, players/v2p_player.py:113-131), written from the same values as
+   * every observation row this launch writes, obs_only included (rows it skips are left alone): column k < num_obs of env e's row is
+   * bf16(clamp((clamp(obs[e,k], -policy_clip_obs, policy_clip_obs) - mean[k]) * rstd[k], -clip, clip)), i.e. the wrapper's observation
+   * clamp, then the normaliser (rl_games RunningMeanStd or RunningNorm with rstd precomputed, the clamp c).  policy_x NULL: not written.
+   * policy_dual: env e's row is (e & 1) * n/2 + (e >> 1), so each player's rows are one block (n even), and player e & 1 uses row e & 1
+   * of mean / rstd ([2, num_obs]) and clip = policy_clip[e & 1]; otherwise row e, mean / rstd [num_obs], policy_clip[0].
+   * mean / rstd NULL: no normalisation (clamps still applied).  Columns [num_obs, policy_ld) are not written. */
+  void* policy_x;                  /* bf16 [rows, policy_ld] */
+  const float *policy_mean, *policy_rstd;
+  int32_t policy_ld, policy_dual;
+  float policy_clip_obs, policy_clip[2];
+  int32_t pad_;
 } b200v2p_ctrl_t;
 int b200v2p_controller_post(const b200v2p_ctrl_t* c, void* stream);
 

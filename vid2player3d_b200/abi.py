@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 
 class Model(C.Structure):
@@ -283,6 +283,8 @@ class V2PCtrl(C.Structure):
         ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p), ("ball_obs", C.c_void_p), ("touch_mask", C.c_void_p),
         ("eval", C.c_int32), ("eval_episode_length", C.c_int32), ("ball_vel", C.c_void_p),
         ("meter_sum", C.c_void_p), ("meter_avg", C.c_void_p), ("meter_max", C.c_void_p), ("meter_count", C.c_void_p),
+        ("policy_x", C.c_void_p), ("policy_mean", C.c_void_p), ("policy_rstd", C.c_void_p), ("policy_ld", C.c_int32),
+        ("policy_dual", C.c_int32), ("policy_clip_obs", C.c_float), ("policy_clip", C.c_float * 2), ("pad_", C.c_int32),
     ]
 
 

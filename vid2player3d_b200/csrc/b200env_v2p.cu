@@ -9,6 +9,7 @@
 //   _update_state_from_sim                    env/tasks/humanoid_smpl_im_mvae.py:799-860
 //   controller post_physics_step              env/tasks/physics_mvae_controller.py:271-314,333-360,368-436,481-602
 //   TennisBallOutEstimator.estimate           utils/tennis_ball_out_estimator.py:126-205
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -394,6 +395,30 @@ __device__ __forceinline__ void eval_reset(const b200v2p_ctrl_t& c, int64_t e, c
     meter_update(c, 3, e, sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2]))));
   }
 }
+// min / max that keep a NaN (torch.clamp semantics), as the cast of libb200nn.so does: an env whose observation blew up gets a NaN
+// operand, and so NaN actions, instead of plausible clamped ones
+__device__ __forceinline__ float clamp_nan(float x, float lo, float hi) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(lo));
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(r), "f"(hi));
+  return r;
+}
+// the high-level policy's bf16 operand row of env e from the observation row `o` the warp has just stored (see b200v2p_ctrl_t.policy_x)
+__device__ __forceinline__ void policy_row(const b200v2p_ctrl_t& c, int64_t e, const float* o, int lane) {
+  __syncwarp();   // the row's values were stored by the other lanes
+  const int p = c.policy_dual ? (int)(e & 1) : 0;
+  const int64_t r = c.policy_dual ? p * (int64_t)(c.n >> 1) + (e >> 1) : e;
+  __nv_bfloat16* x = reinterpret_cast<__nv_bfloat16*>(c.policy_x) + r * c.policy_ld;
+  const float* mean = c.policy_mean ? c.policy_mean + p * c.num_obs : nullptr;
+  const float* rstd = c.policy_rstd ? c.policy_rstd + p * c.num_obs : nullptr;
+  const float clip = c.policy_clip[p];
+  for (int k = lane; k < c.num_obs; k += 32) {
+    float v = clamp_nan(o[k], -c.policy_clip_obs, c.policy_clip_obs);
+    if (mean) v = (v - __ldg(mean + k)) * __ldg(rstd + k);
+    x[k] = __float2bfloat16_rn(clamp_nan(v, -clip, clip));
+  }
+}
+
 // EVAL: the reset rule of the test-time task replaces the training FSM; the training / dual instantiation is the kernel as it was
 template <bool EVAL>
 __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p_ctrl_t c) {
@@ -534,6 +559,7 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
   for (int k = lane; k < L3; k += 32) { float v = src[k] - rk[k % 3]; o[225 + k] = v; nan |= isnan(v); }
   if (c.use_target && lane < 2) { float v = c.target_bounce_pos[e * 3 + lane] - rp[lane]; o[225 + c.obs_traj_len * 3 + lane] = v; nan |= isnan(v); }
   const bool has_nan = __any_sync(FULL, nan);
+  if (c.policy_x) policy_row(c, e, o, lane);
   // ---- dual reset FSM (physics_mvae_controller_dual.py:92-120): the opponent's flags are recomputed from its inputs (no exchange)
   if (EVAL) {
     if (lane == 0 && !c.obs_only) eval_reset(c, e, rp, bp, has_contact);
@@ -1361,6 +1387,13 @@ int b200v2p_controller_post(const b200v2p_ctrl_t* c, void* stream) {
   if (c->dual && (c->n & 1)) return vfail(-2, "b200v2p_controller_post: dual mode needs an even number of envs (pairs 2k, 2k+1)");
   if (c->reward_type < 0 || c->reward_type > 2) return vfail(-2, "b200v2p_controller_post: reward_type must be 0 (reach), 1 (return) or 2 (return_w_estimate)");
   if (c->use_history && !c->ball_obs) return vfail(-2, "b200v2p_controller_post: use_history needs the ball_obs buffer");
+  if (c->policy_x) {
+    if (c->policy_ld < c->num_obs) return vfail(-2, "b200v2p_controller_post: policy_ld is smaller than the observation row");
+    if ((c->policy_mean == nullptr) != (c->policy_rstd == nullptr)) return vfail(-2, "b200v2p_controller_post: policy_mean and policy_rstd go together");
+    if (c->policy_dual && (c->n & 1)) return vfail(-2, "b200v2p_controller_post: policy_dual needs an even number of envs");
+    if (!(c->policy_clip_obs > 0.f) || !(c->policy_clip[0] > 0.f) || (c->policy_dual && !(c->policy_clip[1] > 0.f)))
+      return vfail(-2, "b200v2p_controller_post: the policy row's clamps must be positive (inf: none)");
+  }
   const unsigned grid = (c->n + V2P_WARPS - 1) / V2P_WARPS;
   if (c->eval && !c->obs_only) {
     if (c->dual) return vfail(-2, "b200v2p_controller_post: the test-time reset rule is single-player (dual keeps its FSM)");

@@ -85,7 +85,9 @@ def ball_in_estimate(contact_ids, ball_states, stride, table, params, traj, stat
 
 
 def controller_post(cfg, t):
-    """cfg: dict of scalars (see abi.V2PCtrl); t: dict of tensors keyed like the struct's pointer fields (est_x/est_y may be None)."""
+    """cfg: dict of scalars (see abi.V2PCtrl); t: dict of tensors keyed like the struct's pointer fields (est_x/est_y may be None).
+    The high-level policy's operand row is written when t holds `policy_x` (bf16 [rows, policy_ld]); its scalars policy_dual,
+    policy_clip_obs and policy_clip (one float, or one per player with policy_dual) come in cfg."""
     c = abi.V2PCtrl()
     for k in ("n", "bodies_per_env", "ball_stride", "racket_body", "num_obs", "obs_traj_len", "use_target", "reward_type",
               "early_termination", "max_episode_length", "est_nx", "est_ny", "scale_pos", "scale_phase", "scale_bounce_pos",
@@ -100,13 +102,24 @@ def controller_post(cfg, t):
     for k in ("court_min", "court_max", "est_params"):
         for i, v in enumerate(cfg[k]):
             getattr(c, k)[i] = float(v)
-    scalars = {f for f, _ in abi.V2PCtrl._fields_ if f in cfg} | {"obs_only", "dual", "use_history", "advance", "eval", "eval_episode_length"}
+    px = t.get("policy_x")
+    if px is not None:
+        assert px.dtype == torch.bfloat16 and px.dim() == 2, "policy_x: bf16 [rows, policy_ld]"
+        c.policy_ld, c.policy_dual = int(px.shape[1]), int(cfg.get("policy_dual", 0))
+        assert px.shape[0] >= c.n, "policy_x has fewer rows than there are envs"
+        c.policy_clip_obs = float(cfg.get("policy_clip_obs", float("inf")))
+        clip = cfg.get("policy_clip", float("inf"))
+        clip = list(clip) if isinstance(clip, (list, tuple)) else [clip, clip]
+        c.policy_clip[0], c.policy_clip[1] = float(clip[0]), float(clip[1])
+    scalars = {f for f, _ in abi.V2PCtrl._fields_ if f in cfg} | {"obs_only", "dual", "use_history", "advance", "eval", "eval_episode_length",
+                                                                  "policy_ld", "policy_dual", "policy_clip_obs", "policy_clip", "pad_"}
     for name, _ in abi.V2PCtrl._fields_:
         if name in scalars:
             continue
         x = t.get(name)
         if x is None:
-            assert name in ("est_x", "est_y", "ball_obs", "touch_mask", "ball_vel", "meter_sum", "meter_avg", "meter_max", "meter_count"), name
+            assert name in ("est_x", "est_y", "ball_obs", "touch_mask", "ball_vel", "meter_sum", "meter_avg", "meter_max", "meter_count",
+                            "policy_x", "policy_mean", "policy_rstd"), name
             setattr(c, name, None)
         else:
             assert x.is_cuda and x.is_contiguous(), name

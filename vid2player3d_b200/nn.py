@@ -199,6 +199,150 @@ class PolicyMLP:
         return cls(layers, num_envs, device, **kw)
 
 
+V2P_ACTOR_KEYS = ("actor_mlp.0", "actor_mlp.2", "actor_mlp.4", "mu")   # rl_games A2C actor: Linear / ReLU pairs, then the mu head
+
+
+def _load(cp):
+    return torch.load(cp, map_location="cpu", weights_only=False) if isinstance(cp, (str, os.PathLike)) else cp
+
+
+def _pad_first(w, obs_dim):
+    """the zero-padded first layer of V2PPlayer.restore / load_dual_cp when the network's obs dim is larger than the checkpoint's"""
+    if obs_dim is None or w.shape[1] == obs_dim:
+        return w
+    if w.shape[1] > obs_dim:
+        raise ValueError(f"the checkpoint's first layer takes {w.shape[1]} observations, the env has {obs_dim}")
+    return torch.cat([w, w.new_zeros(w.shape[0], obs_dim - w.shape[1])], 1)
+
+
+def _prefix(full, part):
+    full[:part.shape[0]] = part.float()
+    return full
+
+
+def v2p_networks_from_checkpoint(checkpoint, obs_dim=None, normalize_input=True, dual=False):
+    """What V2PPlayer.restore (vid2player/players/v2p_player.py:71-111; dual: load_dual_cp :21-69) reads from the controller
+    checkpoint(s), as one dict per network: `layers` [(weight, bias)] x 4 (actor_mlp.{0,2,4}, mu; the first zero-padded to obs_dim
+    columns), `mean` / `rstd` [obs_dim] (None: no normaliser) and `clip` (the normaliser's clamp, inf for none).
+      single (normalize_input): rl_games RunningMeanStd of `running_mean_std`, rstd = 1 / sqrt(var + 1e-5), clamp 5; with a padded
+              first layer only the checkpoint's prefix is loaded, the rest keeps the fresh statistics (mean 0, var 1).
+      dual:   each network's RunningNorm (running_obs_type 'ours'): `running_obs.{n,mean,std}` of the model, or else rl_games statistics
+              of the checkpoint's `running_mean_std` or of the model's `running_obs.{running_mean,running_var,count}` with std = sqrt(var);
+              a prefix leaves mean 0, std 0 behind it (rstd 1e8).  rstd = 1 / (std + 1e-8), clamp 5; identity while n == 0.
+    checkpoint: a path or a loaded dict (dual: a pair).  CPU tensors, float32."""
+    out = []
+    for cp in (checkpoint if dual else [checkpoint]):
+        ck = _load(cp)
+        model = {k[len("a2c_network."):]: v for k, v in ck["model"].items() if k.startswith("a2c_network.")}
+        layers = [(model[k + ".weight"].float(), model[k + ".bias"].float()) for k in V2P_ACTOR_KEYS]
+        D = obs_dim or layers[0][0].shape[1]
+        layers[0] = (_pad_first(layers[0][0], D), layers[0][1])
+        net = dict(layers=layers, mean=None, rstd=None, clip=float("inf"))
+        if not dual:
+            if normalize_input:
+                rms = ck["running_mean_std"]
+                net["mean"] = _prefix(torch.zeros(D), rms["running_mean"])
+                var = _prefix(torch.ones(D), rms["running_var"])
+                net["rstd"], net["clip"] = 1.0 / torch.sqrt(var + 1e-5), 5.0
+        else:
+            mean, std, n = torch.zeros(D), torch.zeros(D), 0
+            if "running_obs.n" in model:
+                n = int(model["running_obs.n"])
+                _prefix(mean, model["running_obs.mean"])
+                _prefix(std, model["running_obs.std"])
+            elif "running_mean_std" in ck or "running_obs.running_mean" in model:
+                rms = ck["running_mean_std"] if "running_mean_std" in ck else \
+                    {k: model["running_obs." + k] for k in ("running_mean", "running_var", "count")}
+                n = int(rms["count"])
+                _prefix(mean, rms["running_mean"])
+                _prefix(std, torch.sqrt(rms["running_var"].float()))
+            if n > 0:
+                net["mean"], net["rstd"], net["clip"] = mean, 1.0 / (std + 1e-8), 5.0
+        out.append(net)
+    return out
+
+
+class V2PPolicy:
+    """The tennis controller's trained high-level policy at test time (V2PPlayer.get_action with the deterministic `mu`,
+    players/v2p_player.py:113-131; V2PBuilder.Network.eval_actor, models/v2p_network_builder.py:52-81): per network
+    mu = W4 relu(W3 relu(W2 relu(W1 x + b1) + b2) + b3) + b4, x = clamp((clamp(obs, -clip_obs, clip_obs) - mean) * rstd, -c, c),
+    the wrapper's `clip_actions` folded into the last layer's clamp.  Single: one chain of four wgmma layers over all envs.  Dual
+    (V2PBuilderDual.Network.eval_actor, models/v2p_network_builder_dual.py:39-47): network p acts for envs p, p + 2, ...; its operand
+    rows are one contiguous block (env e at row (e & 1) * N/2 + (e >> 1)) and its last layer writes rows p, p + 2, ... of `out`
+    (ldo = 2 * actions, first column p * actions), so `out` is [N, actions] in env order.
+
+    The operand `x` is normally written by the controller's post launch (`operand()` gives it the fields of b200v2p_ctrl_t), and
+    `forward_prepared()` runs the layers only; `forward(obs)` fills it from a float observation first.  bf16 operands, fp32 accumulation."""
+
+    def __init__(self, networks, num_envs, device, clip_obs=float("inf"), clip_actions=None, activation="relu"):
+        self.dual = len(networks) == 2
+        if len(networks) not in (1, 2):
+            raise ValueError("one network (single) or two (dual)")
+        if self.dual and num_envs % 2:
+            raise ValueError("dual mode needs an even number of envs")
+        self.rows, self.device = num_envs, torch.device(device)
+        self.in_dim = networks[0]["layers"][0][0].shape[1]
+        self.out_dim = networks[0]["layers"][-1][0].shape[0]
+        self.clip_obs, self.clip_actions = float(clip_obs), clip_actions
+        P, dev = len(networks), self.device
+        if all(n["mean"] is None for n in networks):
+            self.mean = self.rstd = None
+        else:   # a network without a normaliser (RunningNorm with n == 0) is the identity: mean 0, rstd 1, no clamp
+            self.mean = torch.stack([n["mean"] if n["mean"] is not None else torch.zeros(self.in_dim) for n in networks]).to(dev, torch.float32)
+            self.rstd = torch.stack([n["rstd"] if n["rstd"] is not None else torch.ones(self.in_dim) for n in networks]).to(dev, torch.float32)
+        self.clip = [float(n["clip"]) for n in networks]
+        H = num_envs // P                                        # rows per chain
+        self.x = torch.zeros(H * (P - 1) + padded_rows(H), _up(self.in_dim, 64), device=dev, dtype=torch.bfloat16)
+        self.out = torch.zeros(num_envs, self.out_dim, device=dev)
+        out_view = self.out.view(H, P * self.out_dim)
+        self.layers = []
+        for p, net in enumerate(networks):
+            a = self.x[p * H:]
+            for i, (w, b) in enumerate(net["layers"]):
+                last = i == len(net["layers"]) - 1
+                o = out_view if last else padded_bf16(H, w.shape[0], dev)
+                self.layers.append(Linear(a, w, b, o, H, act=None if last else activation, out_col0=p * self.out_dim if last else 0,
+                                          out_clamp=(-clip_actions, clip_actions) if (last and clip_actions) else None))
+                a = o
+        self.flops = sum(l.flops for l in self.layers)
+
+    @classmethod
+    def from_checkpoint(cls, checkpoint, num_envs, device, obs_dim=None, normalize_input=True, clip_obs=float("inf"), clip_actions=None,
+                        deterministic=True):
+        """checkpoint: a path or loaded dict (single, V2PPlayer.restore), or a pair of them (dual, load_dual_cp); clip_obs / clip_actions:
+        the wrapper's clamps (VecTaskPython.clip_obs / clip_actions)"""
+        if not deterministic:
+            raise ValueError("V2PPolicy serves the deterministic action (mu) only: the sampled action of a stochastic player "
+                             "(mu + sigma * N(0, 1)) is not implemented")
+        dual = isinstance(checkpoint, (list, tuple))
+        nets = v2p_networks_from_checkpoint(checkpoint, obs_dim=obs_dim, normalize_input=normalize_input, dual=dual)
+        return cls(nets, num_envs, device, clip_obs=clip_obs, clip_actions=clip_actions)
+
+    def operand(self):
+        """(scalars, tensors) of b200v2p_ctrl_t's policy fields for native_v2p.controller_post"""
+        return (dict(policy_dual=int(self.dual), policy_clip_obs=self.clip_obs, policy_clip=self.clip * (1 if self.dual else 2)),
+                dict(policy_x=self.x, policy_mean=self.mean, policy_rstd=self.rstd))
+
+    def forward_prepared(self):
+        """the layers only, on the operand rows the post launch wrote; -> float [N, actions] (a static buffer)"""
+        for l in self.layers:
+            l.run()
+        return self.out
+
+    def forward(self, obs):
+        """obs float [N, >= in_dim] in env order -> the action (static buffer); the operand is cast from obs first"""
+        obs = torch.clamp(obs, -self.clip_obs, self.clip_obs) if self.clip_obs != float("inf") else obs
+        P, H = (2, self.rows // 2) if self.dual else (1, self.rows)
+        for p in range(P):
+            src = obs[p::P] if self.dual else obs
+            mean = self.mean[p] if self.mean is not None else None
+            rstd = self.rstd[p] if self.rstd is not None else None
+            cast_rows(src, self.x[p * H:], self.in_dim, mean, rstd, -self.clip[p], self.clip[p])
+        return self.forward_prepared()
+
+    __call__ = forward
+
+
 class MixedDecoder:
     """MixedDecoder.forward(z, c) (vid2player/motion_vae/model.py:237-252) with the reference's parameter layout:
     `weights[i]` [E, in_i, out_i], `biases[i]` [E, out_i] for the three decoder layers (input of every layer = cat(z, previous

@@ -101,6 +101,77 @@ class _EvalRecorder:
                 player, rh = v.get("player"), v.get("righthand", True)
             yield str(player).startswith("federer"), bool(rh)
 
+    def _tensors(self):
+        t = super()._tensors()
+        t.update(getattr(self, "_policy_t", {}))
+        return t
+
+    def render_vis(self, init=False):
+        """the reference's render_vis without the renderer: record the frame of every env (device launches); after num_rec_frames
+        calls write the chosen episodes and raise SystemExit"""
+        self._record_frame()
+        self._render_host()
+
+    def _render_host(self):
+        self.frame_index += 1
+        if self._record and self.frame_index >= self._num_rec_frames:
+            self.export_episodes()
+            raise SystemExit(0)
+
+    # ------------------------------------------------------------------ test loop of V2PPlayer.run (players/v2p_player.py:133-156)
+    def set_policy(self, policy):
+        """the high-level policy of the test loop (nn.V2PPolicy).  From now on every post launch, the reset's observation refresh
+        included, also writes the policy's operand rows, so the policy needs no launch of its own before its layers.  Set it before
+        reset(), which writes the first rows."""
+        if policy.rows != self.num_envs or policy.in_dim != self.num_obs or policy.dual != bool(self._post_cfg.get("dual")):
+            raise ValueError("the policy's env count, observation width or dual mode differs from the task's")
+        cfg, t = policy.operand()
+        self._post_cfg.update(cfg)
+        self._policy_t, self._policy = t, policy
+        self._test_mask = torch.zeros(self.num_envs, device=self.device, dtype=torch.bool)
+        self._test_graphs = None
+
+    def run_test(self, policy, max_steps, graph=True):
+        """V2PPlayer.run with the deterministic action: reset, render_vis(init=True), then `max_steps` test_step() calls.  Ends like
+        the reference, with SystemExit once num_rec_frames frames are recorded (with record)."""
+        self.set_policy(policy)
+        self.reset()
+        self.render_vis(init=True)
+        for _ in range(max_steps):
+            self.test_step(graph)
+
+    def test_step(self, graph=True):
+        """one iteration of V2PPlayer.run's loop: reset of the finished envs (mask-driven, from reset_buf), policy, env step,
+        render_vis.  graph=True: the first iteration runs eagerly (one-time set-up of the launches), then the reset and the rest are
+        captured as two CUDA graphs and every later iteration is two replays; the host only counts frames."""
+        if self._test_graphs is not None:
+            for g in self._test_graphs:
+                g.replay()
+        else:
+            self._test_reset()
+            self._test_launches()
+            if graph:
+                torch.cuda.synchronize()
+                rg, sg = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+                with torch.cuda.graph(rg):
+                    self._test_reset()
+                with torch.cuda.graph(sg, pool=rg.pool()):
+                    self._test_launches()
+                self._test_graphs = (rg, sg)
+        self._render_host()
+
+    def _test_reset(self):
+        torch.ne(self.reset_buf, 0, out=self._test_mask)
+        self._reset_envs_masked(self._test_mask)
+
+    def _test_launches(self):
+        with torch.no_grad():
+            actions = self._policy.forward_prepared()
+        self.pre_physics_step(actions)
+        self.physics_step()
+        self.post_physics_step()
+        self._record_frame()
+
     def _rec_buffers(self, n, cap, fields):
         dev = self.device
         shapes = dict(joint_rot=((24, 3), torch.float), root_pos=((3,), torch.float), ball_pos=((3,), torch.float),
@@ -135,9 +206,8 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
                  meter_avg=self._meter_avg, meter_max=self._meter_max)
         return t
 
-    def render_vis(self, init=False):
-        """:95-170 without the renderer: record the frame of every env; after num_rec_frames calls write the chosen episodes"""
-        self.frame_index += 1
+    def _record_frame(self):
+        """:95-170's per-call device work: every env's frame into the recording (one launch)"""
         if not self._record:
             return
         t, p = self._physics_player.task, self._mvae_player
@@ -145,9 +215,6 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
             row_counter=self._rec_row, done_counter=self._rec_done, joint_rot=t._joint_rot, root_pos=t._root_pos, ball_pos=t._ball_pos,
             target_pos=self._target_bounce_pos, phase=p._phase_pred, swing_type=p._swing_type_cycle,
             **{"rec_" + k: v for k, v in self._rec.items()}))
-        if self.frame_index >= self._num_rec_frames:
-            self.export_episodes()
-            raise SystemExit(0)
 
     def select_candidates(self):
         """:152-159: with select_best the envs with bounce_in_rate.avg > 0.95 and fh_ratio.avg < 0.6, by distance travelled over the
@@ -194,10 +261,9 @@ class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
             self._list = dict(list_len=i64(1), order=i64(E), best_distance=torch.zeros(E, device=dev), best_env=i64(E),
                               best_nframes=i64(E), copy_slot=i64(1))
 
-    def render_vis(self, init=False):
-        """:87-202 without the renderer: record the frame of every env at row progress_buf, update the best-episode list with the
-        rallies that ended on this step; after num_rec_frames calls write the list's episodes"""
-        self.frame_index += 1
+    def _record_frame(self):
+        """:87-202's per-call device work: record the frame of every env at row progress_buf, update the best-episode list with the
+        rallies that ended on this step (two launches; the list's decisions are made on the device)"""
         if not self._record:
             return
         t, p = self._physics_player.task, self._mvae_player
@@ -208,9 +274,6 @@ class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
         native_v2p.eval_best(self.num_envs, self._cap, self._num_eg, dict(
             reset_buf=self.reset_buf, progress_buf=self.progress_buf, distance=self._distance, **self._list, **rec,
             **{"best_" + k: v for k, v in self._best.items()}))
-        if self.frame_index >= self._num_rec_frames:
-            self.export_episodes()
-            raise SystemExit(0)
 
     def best_list(self):
         """the list in rank order: (slot, even env of the pair, distance, frames) per entry"""
