@@ -23,7 +23,8 @@ STRUCT_MIRRORS = [("abi", "Model", "b200_model_t"), ("abi", "Cfg", "b200_cfg_t")
                   ("abi", "Buffers", "b200_buffers_t"), ("abi", "V2PState", "b200v2p_state_t"), ("abi", "V2PCtrl", "b200v2p_ctrl_t"),
                   ("abi", "V2PPreStep", "b200v2p_prestep_t"), ("abi", "V2PStream", "b200v2p_stream_t"),
                   ("abi", "V2PTaskReset", "b200v2p_treset_t"), ("abi", "V2PActorReset", "b200v2p_areset_t"),
-                  ("ball_gen", "BallSim", "b200ball_sim_t"), ("nn", "LinearDesc", "b200nn_linear_desc_t")]
+                  ("abi", "V2PRec", "b200v2p_rec_t"), ("abi", "V2PBest", "b200v2p_best_t"), ("abi", "V2PBhProb", "b200v2p_bhprob_t"),
+                  ("abi", "V2PBhFix", "b200v2p_bhfix_t"), ("ball_gen", "BallSim", "b200ball_sim_t"), ("nn", "LinearDesc", "b200nn_linear_desc_t")]
 
 
 def header_prototypes(*headers):

@@ -8,6 +8,26 @@ MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
 ABI_VERSION = 9
 
 
+# Pointer fields of the descriptor structs below carry the element type the header points at; native.fill refuses a tensor of any
+# other dtype, tests/test_descriptor_fill.py holds the pointee types to the headers.  void* fields (and pointers to host structs)
+# stay c_void_p.  Each struct also names the pointers that may be NULL (_nullable_) and the scalars a caller may omit, which stay 0
+# (_defaults_).
+class F32P(C.c_void_p):
+    pointee = C.c_float
+
+
+class I64P(C.c_void_p):
+    pointee = C.c_int64
+
+
+class U8P(C.c_void_p):
+    pointee = C.c_uint8
+
+
+class U32P(C.c_void_p):
+    pointee = C.c_uint32
+
+
 class Model(C.Structure):
     _fields_ = [
         ("nb", C.c_int32), ("nd", C.c_int32), ("vmax", C.c_int32), ("max_depth", C.c_int32),
@@ -47,30 +67,33 @@ class Cfg(C.Structure):
 
 class MotionLibView(C.Structure):
     _fields_ = [
-        ("gts", C.c_void_p), ("grs", C.c_void_p), ("lrs", C.c_void_p), ("grvs", C.c_void_p), ("gravs", C.c_void_p),
-        ("dvs", C.c_void_p), ("motion_lengths", C.c_void_p), ("num_frames", C.c_void_p), ("motion_dt", C.c_void_p),
-        ("length_starts", C.c_void_p), ("min_verts_h", C.c_void_p),
+        ("gts", F32P), ("grs", F32P), ("lrs", F32P), ("grvs", F32P), ("gravs", F32P),
+        ("dvs", F32P), ("motion_lengths", F32P), ("num_frames", I64P), ("motion_dt", F32P),
+        ("length_starts", I64P), ("min_verts_h", F32P),
         ("num_motions", C.c_int32), ("num_lib_bodies", C.c_int32), ("total_frames", C.c_int64),
     ]
+    _nullable_, _defaults_ = (), ()
 
 
 class Buffers(C.Structure):
     _fields_ = [
-        ("root_states", C.c_void_p), ("actors_per_env", C.c_int32),
-        ("dof_state", C.c_void_p), ("rigid_body_state", C.c_void_p), ("contact_forces", C.c_void_p),
+        ("root_states", F32P), ("actors_per_env", C.c_int32),
+        ("dof_state", F32P), ("rigid_body_state", F32P), ("contact_forces", F32P),
         ("bodies_per_env", C.c_int32),
-        ("obs_buf", C.c_void_p), ("num_obs", C.c_int32),
-        ("rew_buf", C.c_void_p), ("sub_rewards", C.c_void_p), ("reset_buf", C.c_void_p), ("progress_buf", C.c_void_p),
-        ("terminate_buf", C.c_void_p), ("motion_ids", C.c_void_p), ("ref_motion_times", C.c_void_p),
-        ("motion_bodies", C.c_void_p),
-        ("t_root_pos", C.c_void_p), ("t_root_rot", C.c_void_p), ("t_dof_pos", C.c_void_p), ("t_root_vel", C.c_void_p),
-        ("t_root_ang_vel", C.c_void_p), ("t_dof_vel", C.c_void_p), ("t_key_pos", C.c_void_p), ("t_rb_pos", C.c_void_p),
-        ("t_rb_rot", C.c_void_p),
-        ("p_dof_pos", C.c_void_p), ("p_dof_vel", C.c_void_p), ("p_rb_pos", C.c_void_p), ("p_rb_rot", C.c_void_p),
-        ("pd_targets", C.c_void_p), ("actions_used", C.c_void_p), ("num_actions", C.c_int32),
-        ("has_bounce", C.c_void_p), ("has_bounce_now", C.c_void_p), ("bounce_pos", C.c_void_p), ("racket_hit_now", C.c_void_p),
-        ("dof_force", C.c_void_p),
+        ("obs_buf", F32P), ("num_obs", C.c_int32),
+        ("rew_buf", F32P), ("sub_rewards", F32P), ("reset_buf", I64P), ("progress_buf", I64P),
+        ("terminate_buf", I64P), ("motion_ids", I64P), ("ref_motion_times", F32P),
+        ("motion_bodies", F32P),
+        ("t_root_pos", F32P), ("t_root_rot", F32P), ("t_dof_pos", F32P), ("t_root_vel", F32P),
+        ("t_root_ang_vel", F32P), ("t_dof_vel", F32P), ("t_key_pos", F32P), ("t_rb_pos", F32P),
+        ("t_rb_rot", F32P),
+        ("p_dof_pos", F32P), ("p_dof_vel", F32P), ("p_rb_pos", F32P), ("p_rb_rot", F32P),
+        ("pd_targets", F32P), ("actions_used", F32P), ("num_actions", C.c_int32),
+        ("has_bounce", U8P), ("has_bounce_now", U8P), ("bounce_pos", F32P), ("racket_hit_now", U8P),
+        ("dof_force", F32P),
     ]
+    _nullable_ = ("has_bounce", "has_bounce_now", "bounce_pos", "racket_hit_now", "dof_force")
+    _defaults_ = ()
 
 
 def _fill(arr, values):
@@ -252,12 +275,13 @@ class V2PState(C.Structure):
         ("n", C.c_int32), ("bodies_per_env", C.c_int32), ("ball_stride", C.c_int32), ("root_stride", C.c_int32),
         ("racket_body", C.c_int32), ("wrist_body", C.c_int32), ("grip_normal", C.c_float * 3),
         ("dual", C.c_int32), ("racket_body2", C.c_int32), ("wrist_body2", C.c_int32), ("grip_normal2", C.c_float * 3),
-        ("rigid_body_state", C.c_void_p), ("root_states", C.c_void_p), ("ball_states", C.c_void_p),
-        ("has_contact", C.c_void_p), ("has_contact_now", C.c_void_p),
-        ("root_pos", C.c_void_p), ("root_vel", C.c_void_p), ("racket_pos", C.c_void_p), ("racket_vel", C.c_void_p),
-        ("racket_normal", C.c_void_p), ("ball_pos", C.c_void_p), ("ball_vel", C.c_void_p), ("ball_vspin", C.c_void_p),
-        ("only_mask", C.c_void_p),
+        ("rigid_body_state", F32P), ("root_states", F32P), ("ball_states", F32P),
+        ("has_contact", U8P), ("has_contact_now", U8P),
+        ("root_pos", F32P), ("root_vel", F32P), ("racket_pos", F32P), ("racket_vel", F32P),
+        ("racket_normal", F32P), ("ball_pos", F32P), ("ball_vel", F32P), ("ball_vspin", F32P),
+        ("only_mask", U8P),
     ]
+    _nullable_, _defaults_ = ("only_mask",), ()
 
 
 class V2PCtrl(C.Structure):
@@ -269,57 +293,64 @@ class V2PCtrl(C.Structure):
         ("scale_pos", C.c_float), ("scale_phase", C.c_float), ("scale_bounce_pos", C.c_float), ("scale_bounce_time", C.c_float),
         ("w_pos", C.c_float), ("w_ball_pos", C.c_float),
         ("court_min", C.c_float * 2), ("court_max", C.c_float * 2), ("est_params", C.c_float * 15),
-        ("rigid_body_state", C.c_void_p), ("ball_states", C.c_void_p),
-        ("root_pos", C.c_void_p), ("root_vel", C.c_void_p), ("racket_pos", C.c_void_p), ("racket_normal", C.c_void_p),
-        ("ball_pos", C.c_void_p),
-        ("has_contact", C.c_void_p), ("has_contact_now", C.c_void_p), ("has_bounce", C.c_void_p), ("has_bounce_now", C.c_void_p),
-        ("bounce_pos", C.c_void_p), ("ball_traj", C.c_void_p), ("target_bounce_pos", C.c_void_p), ("phase", C.c_void_p),
-        ("swing_type", C.c_void_p), ("swing_type_cycle", C.c_void_p), ("tar_action", C.c_void_p), ("tar_time", C.c_void_p),
-        ("tar_time_total", C.c_void_p), ("progress_buf", C.c_void_p),
-        ("est_x", C.c_void_p), ("est_y", C.c_void_p),
-        ("bounce_in", C.c_void_p), ("est_bounce_in", C.c_void_p), ("reset_reaction", C.c_void_p), ("reset_recovery", C.c_void_p),
-        ("est_bounce_pos", C.c_void_p), ("est_bounce_time", C.c_void_p), ("est_max_height", C.c_void_p), ("distance", C.c_void_p),
-        ("obs_buf", C.c_void_p), ("rew_buf", C.c_void_p), ("sub_rewards", C.c_void_p),
-        ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p), ("ball_obs", C.c_void_p), ("touch_mask", C.c_void_p),
-        ("eval", C.c_int32), ("eval_episode_length", C.c_int32), ("ball_vel", C.c_void_p),
-        ("meter_sum", C.c_void_p), ("meter_avg", C.c_void_p), ("meter_max", C.c_void_p), ("meter_count", C.c_void_p),
-        ("policy_x", C.c_void_p), ("policy_mean", C.c_void_p), ("policy_rstd", C.c_void_p), ("policy_ld", C.c_int32),
+        ("rigid_body_state", F32P), ("ball_states", F32P),
+        ("root_pos", F32P), ("root_vel", F32P), ("racket_pos", F32P), ("racket_normal", F32P),
+        ("ball_pos", F32P),
+        ("has_contact", U8P), ("has_contact_now", U8P), ("has_bounce", U8P), ("has_bounce_now", U8P),
+        ("bounce_pos", F32P), ("ball_traj", F32P), ("target_bounce_pos", F32P), ("phase", F32P),
+        ("swing_type", I64P), ("swing_type_cycle", I64P), ("tar_action", I64P), ("tar_time", I64P),
+        ("tar_time_total", I64P), ("progress_buf", I64P),
+        ("est_x", F32P), ("est_y", F32P),
+        ("bounce_in", U8P), ("est_bounce_in", U8P), ("reset_reaction", U8P), ("reset_recovery", U8P),
+        ("est_bounce_pos", F32P), ("est_bounce_time", F32P), ("est_max_height", F32P), ("distance", F32P),
+        ("obs_buf", F32P), ("rew_buf", F32P), ("sub_rewards", F32P),
+        ("reset_buf", I64P), ("terminate_buf", I64P), ("ball_obs", F32P), ("touch_mask", U8P),
+        ("eval", C.c_int32), ("eval_episode_length", C.c_int32), ("ball_vel", F32P),
+        ("meter_sum", F32P), ("meter_avg", F32P), ("meter_max", F32P), ("meter_count", I64P),
+        ("policy_x", C.c_void_p), ("policy_mean", F32P), ("policy_rstd", F32P), ("policy_ld", C.c_int32),
         ("policy_dual", C.c_int32), ("policy_clip_obs", C.c_float), ("policy_clip", C.c_float * 2), ("pad_", C.c_int32),
     ]
+    _nullable_ = ("est_x", "est_y", "ball_obs", "touch_mask", "ball_vel", "meter_sum", "meter_avg", "meter_max", "meter_count",
+                  "policy_x", "policy_mean", "policy_rstd")
+    _defaults_ = ("obs_only", "dual", "use_history", "advance", "eval", "eval_episode_length", "policy_ld", "policy_dual",
+                  "policy_clip_obs", "policy_clip", "pad_")
 
 
 class V2PPreStep(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("num_actions", C.c_int32), ("num_latent", C.c_int32), ("num_res_dof", C.c_int32),
         ("random_walk_in_recovery", C.c_int32), ("vae_action_scale", C.c_float), ("residual_dof_scale", C.c_float), ("seed", C.c_uint64),
-        ("actions", C.c_void_p), ("tar_action", C.c_void_p), ("step_counter", C.c_void_p), ("done_counter", C.c_void_p),
-        ("mvae_actions", C.c_void_p), ("res_dof_actions", C.c_void_p),
+        ("actions", F32P), ("tar_action", I64P), ("step_counter", I64P), ("done_counter", U32P),
+        ("mvae_actions", F32P), ("res_dof_actions", F32P),
     ]
+    _nullable_, _defaults_ = ("res_dof_actions",), ()
 
 
 class V2PStream(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("frames", C.c_int32), ("advance", C.c_int32), ("pad_", C.c_int32),
-        ("clock", C.c_void_p), ("done_counter", C.c_void_p), ("offset", C.c_void_p), ("reseed_mask", C.c_void_p), ("seed", C.c_uint64),
-        ("ring_rotmat", C.c_void_p), ("rotmat", C.c_void_p), ("ring_root_pos", C.c_void_p), ("root_pos", C.c_void_p),
-        ("ring_racket_pos", C.c_void_p), ("racket_pos", C.c_void_p), ("ring_phase", C.c_void_p), ("phase", C.c_void_p),
-        ("ring_swing_type", C.c_void_p), ("swing_type", C.c_void_p), ("ring_swing_type_cycle", C.c_void_p), ("swing_type_cycle", C.c_void_p),
+        ("clock", I64P), ("done_counter", U32P), ("offset", I64P), ("reseed_mask", U8P), ("seed", C.c_uint64),
+        ("ring_rotmat", F32P), ("rotmat", F32P), ("ring_root_pos", F32P), ("root_pos", F32P),
+        ("ring_racket_pos", F32P), ("racket_pos", F32P), ("ring_phase", F32P), ("phase", F32P),
+        ("ring_swing_type", I64P), ("swing_type", I64P), ("ring_swing_type_cycle", I64P), ("swing_type_cycle", I64P),
     ]
+    _nullable_, _defaults_ = ("reseed_mask",), ("pad_",)
 
 
 class V2PTaskReset(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("pool_size", C.c_int32), ("ball_stride", C.c_int32), ("bodies_per_env", C.c_int32),
         ("reaction_nframes", C.c_int32), ("target_mode", C.c_int32), ("target_min", C.c_float * 3), ("target_max", C.c_float * 3),
-        ("reset_reaction", C.c_void_p), ("reset_recovery", C.c_void_p),
-        ("pool_rand", C.c_void_p), ("side_rand", C.c_void_p), ("frame_rand", C.c_void_p), ("target_seed", C.c_void_p),
-        ("pool", C.c_void_p), ("ball_states", C.c_void_p), ("rigid_body_state", C.c_void_p),
-        ("ball_pos", C.c_void_p), ("ball_vel", C.c_void_p), ("bounce_pos", C.c_void_p), ("ball_traj", C.c_void_p),
-        ("est_bounce_pos", C.c_void_p), ("est_bounce_time", C.c_void_p), ("est_max_height", C.c_void_p), ("target_bounce_pos", C.c_void_p),
-        ("has_bounce", C.c_void_p), ("has_contact", C.c_void_p), ("bounce_in", C.c_void_p), ("est_bounce_in", C.c_void_p),
-        ("tar_time", C.c_void_p), ("tar_time_total", C.c_void_p), ("tar_action", C.c_void_p), ("num_reset_reaction", C.c_void_p),
-        ("swing_type_cycle", C.c_void_p), ("ball_obs", C.c_void_p), ("obs_traj_len", C.c_int32), ("pad_", C.c_int32),
+        ("reset_reaction", U8P), ("reset_recovery", U8P),
+        ("pool_rand", I64P), ("side_rand", I64P), ("frame_rand", I64P), ("target_seed", F32P),
+        ("pool", F32P), ("ball_states", F32P), ("rigid_body_state", F32P),
+        ("ball_pos", F32P), ("ball_vel", F32P), ("bounce_pos", F32P), ("ball_traj", F32P),
+        ("est_bounce_pos", F32P), ("est_bounce_time", F32P), ("est_max_height", F32P), ("target_bounce_pos", F32P),
+        ("has_bounce", U8P), ("has_contact", U8P), ("bounce_in", U8P), ("est_bounce_in", U8P),
+        ("tar_time", I64P), ("tar_time_total", I64P), ("tar_action", I64P), ("num_reset_reaction", I64P),
+        ("swing_type_cycle", I64P), ("ball_obs", F32P), ("obs_traj_len", C.c_int32), ("pad_", C.c_int32),
     ]
+    _nullable_, _defaults_ = ("ball_obs",), ("obs_traj_len", "pad_")
 
 
 class V2PActorReset(C.Structure):
@@ -327,42 +358,46 @@ class V2PActorReset(C.Structure):
         ("n", C.c_int32), ("num_dof", C.c_int32), ("bodies_per_env", C.c_int32), ("root_stride", C.c_int32),
         ("racket_body", C.c_int32), ("racket_parent", C.c_int32), ("racket_offset", C.c_float * 3),
         ("dual", C.c_int32), ("racket_offset2", C.c_float * 3), ("racket_parent2", C.c_int32), ("pad_", C.c_int32),
-        ("env_ids", C.c_void_p),
-        ("src_root_pos", C.c_void_p), ("src_root_rot", C.c_void_p), ("src_dof_pos", C.c_void_p), ("src_rb_pos", C.c_void_p),
-        ("src_rb_rot", C.c_void_p),
-        ("root_states", C.c_void_p), ("dof_state", C.c_void_p), ("rigid_body_state", C.c_void_p),
-        ("prev_target_root_pos", C.c_void_p), ("prev_target_rb_rot", C.c_void_p), ("root_pos", C.c_void_p), ("root_vel", C.c_void_p),
-        ("pd_target_dof_pos", C.c_void_p), ("target_root_pos", C.c_void_p),
-        ("progress_buf", C.c_void_p), ("reset_buf", C.c_void_p), ("terminate_buf", C.c_void_p), ("mask", C.c_void_p),
+        ("env_ids", I64P),
+        ("src_root_pos", F32P), ("src_root_rot", F32P), ("src_dof_pos", F32P), ("src_rb_pos", F32P),
+        ("src_rb_rot", F32P),
+        ("root_states", F32P), ("dof_state", F32P), ("rigid_body_state", F32P),
+        ("prev_target_root_pos", F32P), ("prev_target_rb_rot", F32P), ("root_pos", F32P), ("root_vel", F32P),
+        ("pd_target_dof_pos", F32P), ("target_root_pos", F32P),
+        ("progress_buf", I64P), ("reset_buf", I64P), ("terminate_buf", I64P), ("mask", U8P),
     ]
+    _nullable_, _defaults_ = ("mask",), ("dual", "racket_offset2", "racket_parent2", "pad_")
 
 
 class V2PRec(C.Structure):
     _fields_ = [
-        ("n", C.c_int32), ("cap", C.c_int32), ("row_counter", C.c_void_p), ("done_counter", C.c_void_p), ("progress_buf", C.c_void_p),
-        ("joint_rot", C.c_void_p), ("root_pos", C.c_void_p), ("ball_pos", C.c_void_p), ("target_pos", C.c_void_p), ("phase", C.c_void_p),
-        ("swing_type", C.c_void_p), ("tar_action", C.c_void_p),
-        ("rec_joint_rot", C.c_void_p), ("rec_root_pos", C.c_void_p), ("rec_ball_pos", C.c_void_p), ("rec_target_pos", C.c_void_p),
-        ("rec_phase", C.c_void_p), ("rec_swing_type", C.c_void_p), ("rec_tar_action", C.c_void_p),
+        ("n", C.c_int32), ("cap", C.c_int32), ("row_counter", I64P), ("done_counter", U32P), ("progress_buf", I64P),
+        ("joint_rot", F32P), ("root_pos", F32P), ("ball_pos", F32P), ("target_pos", F32P), ("phase", F32P),
+        ("swing_type", I64P), ("tar_action", I64P),
+        ("rec_joint_rot", F32P), ("rec_root_pos", F32P), ("rec_ball_pos", F32P), ("rec_target_pos", F32P),
+        ("rec_phase", F32P), ("rec_swing_type", I64P), ("rec_tar_action", I64P),
     ]
+    _nullable_ = ("row_counter", "done_counter", "progress_buf", "target_pos", "tar_action", "rec_target_pos", "rec_tar_action")
+    _defaults_ = ()
 
 
 class V2PBest(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("cap", C.c_int32), ("num_eg", C.c_int32), ("pad_", C.c_int32),
-        ("reset_buf", C.c_void_p), ("progress_buf", C.c_void_p), ("distance", C.c_void_p),
-        ("list_len", C.c_void_p), ("order", C.c_void_p), ("best_distance", C.c_void_p), ("best_env", C.c_void_p),
-        ("best_nframes", C.c_void_p), ("copy_slot", C.c_void_p),
-        ("rec_joint_rot", C.c_void_p), ("rec_root_pos", C.c_void_p), ("rec_ball_pos", C.c_void_p), ("rec_phase", C.c_void_p),
-        ("rec_swing_type", C.c_void_p), ("rec_tar_action", C.c_void_p),
-        ("best_joint_rot", C.c_void_p), ("best_root_pos", C.c_void_p), ("best_ball_pos", C.c_void_p), ("best_phase", C.c_void_p),
-        ("best_swing_type", C.c_void_p), ("best_tar_action", C.c_void_p),
+        ("reset_buf", I64P), ("progress_buf", I64P), ("distance", F32P),
+        ("list_len", I64P), ("order", I64P), ("best_distance", F32P), ("best_env", I64P),
+        ("best_nframes", I64P), ("copy_slot", I64P),
+        ("rec_joint_rot", F32P), ("rec_root_pos", F32P), ("rec_ball_pos", F32P), ("rec_phase", F32P),
+        ("rec_swing_type", I64P), ("rec_tar_action", I64P),
+        ("best_joint_rot", F32P), ("best_root_pos", F32P), ("best_ball_pos", F32P), ("best_phase", F32P),
+        ("best_swing_type", I64P), ("best_tar_action", I64P),
     ]
+    _nullable_, _defaults_ = (), ("pad_",)
 
 
 class V2PBhProb(C.Structure):
     _fields_ = [
-        ("joint_rot", C.c_void_p), ("phase", C.c_void_p), ("swing_type", C.c_void_p), ("rest", C.c_void_p), ("out", C.c_void_p),
+        ("joint_rot", C.c_void_p), ("phase", C.c_void_p), ("swing_type", I64P), ("rest", C.c_void_p), ("out", C.c_void_p),
         ("T", C.c_int64), ("swing_type_len", C.c_int64), ("righthand", C.c_int32), ("pad_", C.c_int32),
     ]
 

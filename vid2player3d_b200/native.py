@@ -39,6 +39,61 @@ def _ptr(t):
     return t.data_ptr() if t is not None else None
 
 
+_layouts = {}
+
+
+def _layout(S):
+    """(scalar fields as (name, array length or None), pointer fields as (name, accepted dtypes or None)) of S"""
+    lay = _layouts.get(S)
+    if lay is None:
+        import torch
+        dtypes = {abi.F32P: (torch.float32,), abi.I64P: (torch.int64,), abi.U8P: (torch.uint8, torch.bool),
+                  abi.U32P: (torch.int32, torch.uint32)}
+        scalars = [(name, ct._length_ if issubclass(ct, C.Array) else None) for name, ct in S._fields_ if not issubclass(ct, C.c_void_p)]
+        ptrs = [(name, dtypes.get(ct)) for name, ct in S._fields_ if issubclass(ct, C.c_void_p)]
+        lay = _layouts[S] = (scalars, ptrs)
+    return lay
+
+
+def fill(S, scalars, tensors):
+    """a launch descriptor S (a struct of abi.py) filled from `scalars` (field -> number, a sequence for an array field) and `tensors`
+    (field -> tensor or None).  Every scalar field must be given except those of S._defaults_, which stay 0 when left out or None; a
+    pointer may be None only in S._nullable_.  A tensor must have the dtype of its field's pointee (any for void*), be contiguous and
+    lie on the one CUDA device of all of them.  Keys that name no field are ignored.  Refusals raise ValueError naming the field."""
+    scalar_fields, ptr_fields = _layout(S)
+    s = S()
+    for name, length in scalar_fields:
+        v = scalars.get(name)
+        if v is None:
+            if name not in S._defaults_:
+                raise ValueError(f"{S.__name__}.{name}: missing")
+        elif length is None:
+            setattr(s, name, v)
+        elif len(v) != length:
+            raise ValueError(f"{S.__name__}.{name}: {len(v)} values for {length}")
+        else:
+            getattr(s, name)[:] = v
+    dev, off_device = None, None
+    for name, dtypes in ptr_fields:
+        x = tensors.get(name)
+        if x is None:
+            if name not in S._nullable_:
+                raise ValueError(f"{S.__name__}.{name}: None, but the header allows no NULL here")
+            continue
+        if dtypes is not None and x.dtype not in dtypes:
+            raise ValueError(f"{S.__name__}.{name}: {x.dtype}, the header's pointee needs {' or '.join(map(str, dtypes))}")
+        if not x.is_contiguous():
+            raise ValueError(f"{S.__name__}.{name}: not contiguous")
+        d = x.get_device()
+        dev = d if dev is None else dev
+        if off_device is None and (d < 0 or d != dev):
+            off_device = name
+        setattr(s, name, x.data_ptr())
+    if off_device is not None:
+        raise ValueError(f"{S.__name__}.{off_device}: not on the CUDA device of the other tensors")
+    return s
+
+
 def _stream():
     import torch
     return torch.cuda.current_stream().cuda_stream
@@ -110,36 +165,19 @@ class Env:
     def bind(self, tensors, actors_per_env, bodies_per_env, num_obs):
         """tensors: name -> CUDA tensor of every b200_buffers_t pointer; the ball flag buffers only for the vid2player player env, and
         "dof_force" ([rows, nd] float32) only with DOF force sensors"""
-        import torch
-        b = abi.Buffers()
-        for name, _ in abi.Buffers._fields_:
-            if name in ("actors_per_env", "bodies_per_env", "num_obs", "num_actions"):
-                continue
-            if name in ("has_bounce", "has_bounce_now", "bounce_pos", "racket_hit_now") and name not in tensors:
-                continue  # ball flag buffers: only for the vid2player player env
-            if name == "dof_force" and tensors.get(name) is None:
-                continue  # DOF force sensors off: the physics launch writes no sensor rows
-            t = tensors[name]
-            assert t.is_cuda and t.is_contiguous(), name
-            if name == "dof_force":
-                assert t.dtype == torch.float32 and tuple(t.shape) == (int(tensors["actions_used"].shape[0]), int(self.model.nd)), \
-                    f"dof_force must be float32 [{int(tensors['actions_used'].shape[0])}, {int(self.model.nd)}], got {t.dtype} {tuple(t.shape)}"
-            setattr(b, name, t.data_ptr())
-        b.actors_per_env, b.bodies_per_env, b.num_obs = actors_per_env, bodies_per_env, num_obs
-        b.num_actions = self.num_actions = int(tensors["actions_used"].shape[-1])   # row width of `actions` in step()
-        self.num_envs_bound = int(tensors["actions_used"].shape[0])   # rows of the bound tensors (>= num_envs with an env slice)
+        self.num_actions = int(tensors["actions_used"].shape[-1])      # row width of `actions` in step()
+        self.num_envs_bound = int(tensors["actions_used"].shape[0])    # rows of the bound tensors (>= num_envs with an env slice)
+        f = tensors.get("dof_force")
+        assert f is None or tuple(f.shape) == (self.num_envs_bound, int(self.model.nd)), \
+            f"dof_force must be [{self.num_envs_bound}, {int(self.model.nd)}], got {tuple(f.shape)}"
+        b = fill(abi.Buffers, dict(actors_per_env=actors_per_env, bodies_per_env=bodies_per_env, num_obs=num_obs,
+                                   num_actions=self.num_actions), tensors)
         self._keep.append(tensors)
         _check(lib().b200env_bind(self._h, C.byref(b)))
 
     def set_motion_lib(self, t, num_lib_bodies):
-        v = abi.MotionLibView()
-        for k in ("gts", "grs", "lrs", "grvs", "gravs", "dvs", "motion_lengths", "num_frames", "motion_dt", "length_starts",
-                  "min_verts_h"):
-            assert t[k].is_cuda and t[k].is_contiguous(), k
-            setattr(v, k, t[k].data_ptr())
-        v.num_motions = t["motion_lengths"].shape[0]
-        v.num_lib_bodies = num_lib_bodies
-        v.total_frames = t["gts"].shape[0]
+        v = fill(abi.MotionLibView, dict(num_motions=t["motion_lengths"].shape[0], num_lib_bodies=num_lib_bodies,
+                                         total_frames=t["gts"].shape[0]), t)
         self._keep.append(t)
         _check(lib().b200env_set_motion_lib(self._h, C.byref(v)))
         self._num_lib_bodies = int(num_lib_bodies)

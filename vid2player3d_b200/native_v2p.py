@@ -4,7 +4,7 @@ import ctypes as C
 import torch
 
 from . import abi
-from .native import _ptr, _stream, lib
+from .native import _ptr, _stream, fill, lib
 
 GRIP_NORMAL = {'eastern': (0.0, 1.0, 0.0), 'semi_western': (0.0, 2.0 ** -0.5, 2.0 ** -0.5)}
 REWARD_TYPES = {'reach': 0, 'return': 1, 'return_w_estimate': 2}
@@ -52,22 +52,14 @@ def ball_reset(env_ids, pool_index, pool, ball_states, ball_pos, ball_vel, has_b
 def update_state(n, bodies_per_env, rigid_body_state, root_states, root_stride, ball_states, ball_stride, t, grip='eastern',
                  racket_body=24, wrist_body=22, only_mask=None):
     """grip / racket_body / wrist_body may be 2-sequences (dual_mode 'different': even envs, odd envs)"""
-    s = abi.V2PState()
     pair = lambda v: (v[0], v[1], 1) if isinstance(v, (list, tuple)) else (v, v, 0)  # noqa: E731
     g0, g1, d0 = pair(grip)
     r0, r1, d1 = pair(racket_body)
     w0, w1, d2 = pair(wrist_body)
-    s.n, s.bodies_per_env, s.ball_stride, s.root_stride, s.racket_body, s.wrist_body = n, bodies_per_env, ball_stride, root_stride, r0, w0
-    s.dual, s.racket_body2, s.wrist_body2 = int(bool(d0 or d1 or d2)), r1, w1
-    for i in range(3):
-        s.grip_normal[i] = GRIP_NORMAL[g0][i]
-        s.grip_normal2[i] = GRIP_NORMAL[g1][i]
-    s.rigid_body_state, s.root_states, s.ball_states = rigid_body_state.data_ptr(), root_states.data_ptr(), ball_states.data_ptr()
-    for k in ("has_contact", "has_contact_now", "root_pos", "root_vel", "racket_pos", "racket_vel", "racket_normal", "ball_pos", "ball_vel",
-              "ball_vspin"):
-        assert t[k].is_cuda and t[k].is_contiguous(), k
-        setattr(s, k, t[k].data_ptr())
-    s.only_mask = only_mask.data_ptr() if only_mask is not None else None
+    s = fill(abi.V2PState, dict(n=n, bodies_per_env=bodies_per_env, ball_stride=ball_stride, root_stride=root_stride, racket_body=r0,
+                                wrist_body=w0, grip_normal=GRIP_NORMAL[g0], dual=int(bool(d0 or d1 or d2)), racket_body2=r1, wrist_body2=w1,
+                                grip_normal2=GRIP_NORMAL[g1]),
+             dict(t, rigid_body_state=rigid_body_state, root_states=root_states, ball_states=ball_states, only_mask=only_mask))
     _check(lib().b200v2p_update_state(C.byref(s), _stream()))
 
 
@@ -88,149 +80,51 @@ def controller_post(cfg, t):
     """cfg: dict of scalars (see abi.V2PCtrl); t: dict of tensors keyed like the struct's pointer fields (est_x/est_y may be None).
     The high-level policy's operand row is written when t holds `policy_x` (bf16 [rows, policy_ld]); its scalars policy_dual,
     policy_clip_obs and policy_clip (one float, or one per player with policy_dual) come in cfg."""
-    c = abi.V2PCtrl()
-    for k in ("n", "bodies_per_env", "ball_stride", "racket_body", "num_obs", "obs_traj_len", "use_target", "reward_type",
-              "early_termination", "max_episode_length", "est_nx", "est_ny", "scale_pos", "scale_phase", "scale_bounce_pos",
-              "scale_bounce_time", "w_pos", "w_ball_pos"):
-        setattr(c, k, cfg[k])
-    c.obs_only = int(cfg.get("obs_only", 0))
-    c.dual = int(cfg.get("dual", 0))
-    c.use_history = int(cfg.get("use_history", 0))
-    c.advance = int(cfg.get("advance", 0))
-    c.eval = int(cfg.get("eval", 0))
-    c.eval_episode_length = int(cfg.get("eval_episode_length", 0))
-    for k in ("court_min", "court_max", "est_params"):
-        for i, v in enumerate(cfg[k]):
-            getattr(c, k)[i] = float(v)
     px = t.get("policy_x")
     if px is not None:
         assert px.dtype == torch.bfloat16 and px.dim() == 2, "policy_x: bf16 [rows, policy_ld]"
-        c.policy_ld, c.policy_dual = int(px.shape[1]), int(cfg.get("policy_dual", 0))
-        assert px.shape[0] >= c.n, "policy_x has fewer rows than there are envs"
-        c.policy_clip_obs = float(cfg.get("policy_clip_obs", float("inf")))
+        assert px.shape[0] >= cfg["n"], "policy_x has fewer rows than there are envs"
         clip = cfg.get("policy_clip", float("inf"))
-        clip = list(clip) if isinstance(clip, (list, tuple)) else [clip, clip]
-        c.policy_clip[0], c.policy_clip[1] = float(clip[0]), float(clip[1])
-    scalars = {f for f, _ in abi.V2PCtrl._fields_ if f in cfg} | {"obs_only", "dual", "use_history", "advance", "eval", "eval_episode_length",
-                                                                  "policy_ld", "policy_dual", "policy_clip_obs", "policy_clip", "pad_"}
-    for name, _ in abi.V2PCtrl._fields_:
-        if name in scalars:
-            continue
-        x = t.get(name)
-        if x is None:
-            assert name in ("est_x", "est_y", "ball_obs", "touch_mask", "ball_vel", "meter_sum", "meter_avg", "meter_max", "meter_count",
-                            "policy_x", "policy_mean", "policy_rstd"), name
-            setattr(c, name, None)
-        else:
-            assert x.is_cuda and x.is_contiguous(), name
-            setattr(c, name, x.data_ptr())
-    _check(lib().b200v2p_controller_post(C.byref(c), _stream()))
+        cfg = dict(cfg, policy_ld=int(px.shape[1]), policy_clip_obs=cfg.get("policy_clip_obs", float("inf")),
+                   policy_clip=clip if isinstance(clip, (list, tuple)) else (clip, clip))
+    _check(lib().b200v2p_controller_post(C.byref(fill(abi.V2PCtrl, cfg, t)), _stream()))
 
 
 def task_reset(cfg, t):
     """cfg: scalars of abi.V2PTaskReset (n, pool_size, ball_stride, bodies_per_env, reaction_nframes, target_mode, target_min/max);
     t: tensors keyed like the struct's pointer fields"""
-    r = abi.V2PTaskReset()
-    for k in ("n", "pool_size", "ball_stride", "bodies_per_env", "reaction_nframes", "target_mode"):
-        setattr(r, k, int(cfg[k]))
-    for k in ("target_min", "target_max"):
-        for i, v in enumerate(cfg[k]):
-            getattr(r, k)[i] = float(v)
-    r.obs_traj_len = int(cfg.get("obs_traj_len", 0))
-    for name, _ in abi.V2PTaskReset._fields_:
-        if name in cfg or name in ("obs_traj_len", "pad_"):
-            continue
-        x = t.get(name)
-        if x is None:
-            assert name == "ball_obs", name
-            setattr(r, name, None)
-            continue
-        assert x.is_cuda and x.is_contiguous(), name
-        setattr(r, name, x.data_ptr())
-    _check(lib().b200v2p_task_reset(C.byref(r), _stream()))
+    _check(lib().b200v2p_task_reset(C.byref(fill(abi.V2PTaskReset, cfg, t)), _stream()))
 
 
 def actor_reset(cfg, t):
-    r = abi.V2PActorReset()
-    for k in ("n", "num_dof", "bodies_per_env", "root_stride", "racket_body", "racket_parent"):
-        setattr(r, k, int(cfg[k]))
-    for i, v in enumerate(cfg["racket_offset"]):
-        r.racket_offset[i] = float(v)
-    if cfg.get("racket_offset2") is not None:
-        r.dual = 1
-        r.racket_parent2 = int(cfg.get("racket_parent2", cfg["racket_parent"]))
-        for i, v in enumerate(cfg["racket_offset2"]):
-            r.racket_offset2[i] = float(v)
-    for name, _ in abi.V2PActorReset._fields_:
-        if name in cfg or name in ("dual", "racket_offset2", "racket_parent2", "pad_"):
-            continue
-        x = t.get(name)
-        if x is None:
-            assert name == "mask", name
-            setattr(r, name, None)
-            continue
-        assert x.is_cuda and x.is_contiguous(), name
-        setattr(r, name, x.data_ptr())
-    _check(lib().b200v2p_actor_reset(C.byref(r), _stream()))
+    """cfg: scalars of abi.V2PActorReset; racket_offset2 (with racket_parent2, default racket_parent) sets dual"""
+    two = cfg.get("racket_offset2") is not None
+    cfg = dict(cfg, dual=int(two), racket_parent2=cfg.get("racket_parent2", cfg["racket_parent"]) if two else None)
+    _check(lib().b200v2p_actor_reset(C.byref(fill(abi.V2PActorReset, cfg, t)), _stream()))
 
 
 def pre_step(cfg, t):
     """cfg: n, num_actions, num_latent, num_res_dof, random_walk_in_recovery, vae_action_scale, residual_dof_scale, seed;
     t: actions, tar_action, step_counter (int64 [1]), done_counter (int32 [1]), mvae_actions, res_dof_actions (or None)"""
-    p = abi.V2PPreStep()
-    for k in ("n", "num_actions", "num_latent", "num_res_dof", "random_walk_in_recovery", "seed"):
-        setattr(p, k, int(cfg[k]))
-    p.vae_action_scale, p.residual_dof_scale = float(cfg["vae_action_scale"]), float(cfg["residual_dof_scale"])
-    for k in ("actions", "tar_action", "step_counter", "done_counter", "mvae_actions", "res_dof_actions"):
-        x = t.get(k)
-        assert x is None or (x.is_cuda and x.is_contiguous()), k
-        setattr(p, k, x.data_ptr() if x is not None else None)
-    _check(lib().b200v2p_pre_step(C.byref(p), _stream()))
+    _check(lib().b200v2p_pre_step(C.byref(fill(abi.V2PPreStep, cfg, t)), _stream()))
 
 
 def stream_gather(n, frames, advance, t, reseed_mask=None, seed=0):
     """t: clock (int64 [1]), done_counter (int32 [1]), offset [n] int64, ring_* / live buffers of include/b200env_v2p.h b200v2p_stream_t;
     reseed_mask (bool [n]): the masked envs draw a new offset and re-read their frame, the others are left alone"""
-    s = abi.V2PStream()
-    s.n, s.frames, s.advance = int(n), int(frames), int(advance)
-    s.seed = int(seed)
-    s.reseed_mask = reseed_mask.data_ptr() if reseed_mask is not None else None
-    for name, _ in abi.V2PStream._fields_[4:]:
-        if name in ("reseed_mask", "seed"):
-            continue
-        x = t[name]
-        assert x.is_cuda and x.is_contiguous(), name
-        setattr(s, name, x.data_ptr())
+    s = fill(abi.V2PStream, dict(n=n, frames=frames, advance=advance, seed=seed), dict(t, reseed_mask=reseed_mask))
     _check(lib().b200v2p_stream_gather(C.byref(s), _stream()))
-
-
-def _fill_ptrs(s, t, optional=()):
-    for name, _ in s._fields_:
-        if name in t:
-            x = t[name]
-            if x is None:
-                assert name in optional, name
-                setattr(s, name, None)
-            else:
-                assert x.is_cuda and x.is_contiguous(), name
-                setattr(s, name, x.data_ptr())
 
 
 def eval_record(n, cap, t):
     """t: the source fields (joint_rot, root_pos, ball_pos, target_pos, phase, swing_type, tar_action), the rec_* buffers [n, cap, ...]
     and the row source: row_counter + done_counter (single) or progress_buf (dual); see include/b200env_v2p.h b200v2p_rec_t"""
-    r = abi.V2PRec()
-    r.n, r.cap = int(n), int(cap)
-    _fill_ptrs(r, t, optional=("row_counter", "done_counter", "progress_buf", "target_pos", "tar_action", "rec_target_pos", "rec_tar_action"))
-    _check(lib().b200v2p_eval_record(C.byref(r), _stream()))
+    _check(lib().b200v2p_eval_record(C.byref(fill(abi.V2PRec, dict(n=n, cap=cap), t)), _stream()))
 
 
 def eval_best(n, cap, num_eg, t):
     """t: tensors keyed like the pointer fields of b200v2p_best_t (include/b200env_v2p.h)"""
-    b = abi.V2PBest()
-    b.n, b.cap, b.num_eg = int(n), int(cap), int(num_eg)
-    _fill_ptrs(b, t)
-    _check(lib().b200v2p_eval_best(C.byref(b), _stream()))
+    _check(lib().b200v2p_eval_best(C.byref(fill(abi.V2PBest, dict(n=n, cap=cap, num_eg=num_eg), t)), _stream()))
 
 
 BACKHAND_ITERS = 500    # optimize_two_hand_backhand(single=True): 500 Adam steps
