@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 9
+#define B200_ABI_VERSION 10
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:
@@ -230,6 +230,67 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
                                const float* target_pos, const float* target_rot, const float* target_dof_pos, const float* motion_bodies,
                                int32_t local_root_obs, int32_t root_height_obs, float* obs, void* obs_bf16, int32_t ld_bf16, const float* mean,
                                const float* rstd, float clamp, void* stream);
+
+/* The imitation policy's first-layer operand at test time (ImitatorBuilder.Network.preprocess_input, non-training branch, + running_obs,
+ * embodied_pose/models/im_network_builder.py:117-189): the 734-wide observation of compute_humanoid_observations_imitation with
+ * local_root_obs = root_height_obs = 1, built from
+ *   - obs_buf [n, num_obs], the raw observation the step writes, split as obs_names / obs_dims (body_pos | body_rot | dof_pos | dof_vel |
+ *     body_vel | body_ang_vel | motion_bodies, humanoid_smpl_im.py:198-211); every value is clamped to +-clip_obs as it is loaded (the
+ *     wrapper's torch.clamp(obs_buf, -clip_obs, clip_obs); inf = no clamp);
+ *   - the target body_pos | body_rot | dof_pos of frame context_padding + (step[0] % context_length) of context_feat [n, num_frames,
+ *     feat_width] (the window b200env_motion_context writes; forward_context(flatten=False) + obtain_cur_context(t) :117-145).
+ * Writes x [n, ld] bf16 = clamp((obs - mean) * rstd, -clip, clip) (RunningNorm / RunningMeanStd; mean / rstd NULL: the row as it is, no
+ * clamp) and resid [n, nd] = the slot's target dof_pos (the residual action of eval_actor :226-228, added by the last GEMM layer's
+ * epilogue, include/b200nn.h).  `step` is a device counter (b200env_play_stats advances it), so one capture replays every step. */
+typedef struct b200_im_policy {
+  int32_t n;               /* envs: rows 0 .. n-1 of every array */
+  int32_t num_obs;         /* row stride of obs_buf (>= the 7 named blocks) */
+  int32_t num_frames;      /* frames of a context window (context_length + 2 context_padding) */
+  int32_t feat_width;      /* floats of a context frame (>= 7 bodies + dofs: body_pos | body_rot | dof_pos | ...) */
+  int32_t context_padding;
+  int32_t context_length;
+  int32_t ld;              /* bf16 elements per row of x: even, >= the observation width */
+  float clip_obs;          /* clamp of the raw observation; inf = none */
+  float clip;              /* the normaliser's clamp (with mean / rstd only) */
+  int32_t pad_;
+  const float* obs_buf;
+  const float* context_feat;
+  const int64_t* step;     /* [1] */
+  const float* mean;       /* [734] or NULL */
+  const float* rstd;       /* [734] or NULL */
+  void* x;                 /* bf16, 4-byte aligned */
+  float* resid;            /* [n, nd] */
+} b200_im_policy_t;
+
+/* One launch (the observation launch's per-env warp code, obs_imitation_kernel).  Returns -2 before any launch on the refusals of
+ * b200env_obs_imitation, an ld smaller than the row, odd or an x that is not 4-byte aligned, an obs_buf row narrower than the named
+ * blocks, a context frame narrower than its three target blocks, a slot outside the window (context_padding < 0, context_length < 1 or
+ * context_padding + context_length > num_frames), mean without rstd or a normaliser clamp that is not positive.  A handle of several
+ * assets is served: the launch reads only the topology they share. */
+int b200env_im_policy_rows(b200env_handle h, const b200_im_policy_t* d, void* stream);
+
+/* ImitatorPlayer.run's bookkeeping of one step (embodied_pose/players/im_player.py:226-304, num_agents = 1), one CTA in a fixed
+ * summation order (replays give the same sums).  Per env: done = reset_buf != 0, cr += rew, steps += 1, step_done = done (1 - prev_done).
+ * When any step_done is set: totals += (sum cr, sum steps) over them (double), games[0] += their count, cr *= 1 - done,
+ * steps *= 1 - done, and (count, sum cr, sum steps) is appended to log [max_log, 3] at row games[2] (games[2] += 1; a full log keeps
+ * counting but writes nothing).  The float sums are summed in float32, like the reference's cr[done].sum().  Then prev_done = done,
+ * games[1] (stop) = games[0] >= n_games or done of env 0, and step[0] += 1.  While games[1] is set the call changes nothing. */
+typedef struct b200_play_stats {
+  int32_t n;
+  int32_t max_log;
+  int64_t n_games;         /* games_num * n_game_life */
+  const float* rew;        /* [n] */
+  const int64_t* reset_buf;/* [n] */
+  float* cr;               /* [n] */
+  float* steps;            /* [n] */
+  float* prev_dones;       /* [n] */
+  double* totals;          /* [2]: sum_rewards, sum_steps */
+  double* log;             /* [max_log, 3] */
+  int64_t* games;          /* [3]: games_played, stop, log rows */
+  int64_t* step;           /* [1] */
+} b200_play_stats_t;
+
+int b200env_play_stats(const b200_play_stats_t* d, void* stream);
 
 /* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1): a separate test launch
  * (physics_kernel_packed; physics_kernel_tmem / physics_kernel for the other forms) that shares the control step

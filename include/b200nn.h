@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define B200NN_ABI_VERSION 1
+#define B200NN_ABI_VERSION 2
 
 enum { B200NN_ACT_NONE = 0, B200NN_ACT_RELU = 1, B200NN_ACT_ELU = 2 };
 
@@ -51,6 +51,12 @@ typedef struct b200nn_linear_desc {
   int32_t act;        /* B200NN_ACT_* */
   int32_t out_bf16;   /* 1: bf16 output (feeds the next layer), 0: float output */
   float out_min, out_max; /* clamp applied after the activation (im_player.py:198 clamps the action to +-1); out_min >= out_max: none */
+  /* residual (single-expert layer, float output): out = clamp(act(acc + bias + resid[row * ld_resid + col])) for col < resid_cols, i.e.
+   * eval_actor's `mu[:, :69] += target_dof_pos` (embodied_pose/models/im_network_builder.py:226-228) before the wrapper's action
+   * clamp.  resid NULL and the two counts 0: no residual (the meaning of a descriptor without these fields). */
+  const float* resid; /* [rows, ld_resid] float, 4-byte aligned */
+  int32_t ld_resid;   /* >= resid_cols */
+  int32_t resid_cols; /* 1..n */
 } b200nn_linear_desc_t;
 
 int b200nn_abi_version(void);
@@ -59,7 +65,8 @@ const char* b200nn_last_error(void);
 /* builds the TMA tensor maps of the operands (host side, once); the device buffers must stay where they are.  Returns -2 (before any
  * driver call) for a descriptor the kernel cannot run: num_experts outside 1..6, K / lda / ldw not padded to 64, n_padded not a
  * multiple of the tile or n outside 1..n_padded, rows < 1, bf16 ldo / out_col0 not multiples of 8, operands not 16-byte aligned,
- * out_col0 < 0, ldo < out_col0 + n, an unknown act. */
+ * out_col0 < 0, ldo < out_col0 + n, an unknown act; and a residual on a mixture layer or a bf16 output, resid_cols outside 1..n,
+ * ld_resid < resid_cols, a misaligned resid, or resid_cols / ld_resid without resid. */
 int b200nn_linear_create(const b200nn_linear_desc_t* desc, int32_t device, b200nn_linear_handle* out);
 int b200nn_linear_destroy(b200nn_linear_handle h);
 /* one launch on `stream` (CUDA-graph capturable) */

@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 # Pointer fields of the descriptor structs below carry the element type the header points at; native.fill refuses a tensor of any
@@ -26,6 +26,10 @@ class U8P(C.c_void_p):
 
 class U32P(C.c_void_p):
     pointee = C.c_uint32
+
+
+class F64P(C.c_void_p):
+    pointee = C.c_double
 
 
 class Model(C.Structure):
@@ -269,6 +273,27 @@ DEFAULT_BALL = dict(ball_mass=0.057, ball_inertia=4e-5, ball_radius=0.032, spin_
                     racket_head_halfthick=0.02125, racket_head_radius=0.15, racket_head_quat=(0.0, 0.0, 0.0, 1.0))
 
 
+class ImPolicy(C.Structure):
+    """b200_im_policy_t: the imitation policy's operand launch (b200env_im_policy_rows)"""
+    _fields_ = [
+        ("n", C.c_int32), ("num_obs", C.c_int32), ("num_frames", C.c_int32), ("feat_width", C.c_int32),
+        ("context_padding", C.c_int32), ("context_length", C.c_int32), ("ld", C.c_int32), ("clip_obs", C.c_float), ("clip", C.c_float),
+        ("pad_", C.c_int32),
+        ("obs_buf", F32P), ("context_feat", F32P), ("step", I64P), ("mean", F32P), ("rstd", F32P), ("x", C.c_void_p), ("resid", F32P),
+    ]
+    _nullable_, _defaults_ = ("mean", "rstd"), ("clip", "pad_")
+
+
+class PlayStats(C.Structure):
+    """b200_play_stats_t: ImitatorPlayer.run's bookkeeping of one step (b200env_play_stats)"""
+    _fields_ = [
+        ("n", C.c_int32), ("max_log", C.c_int32), ("n_games", C.c_int64),
+        ("rew", F32P), ("reset_buf", I64P), ("cr", F32P), ("steps", F32P), ("prev_dones", F32P), ("totals", F64P), ("log", F64P),
+        ("games", I64P), ("step", I64P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
 # ---------------------------------------------------------------- include/b200env_v2p.h
 class V2PState(C.Structure):
     _fields_ = [
@@ -441,6 +466,8 @@ SIGNATURES = {
     "b200env_obs_imitation_rows": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _f32, _p]),
     "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200env_motion_context": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _i32, _f32, _p, _p, _p]),
+    "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),
+    "b200env_play_stats": (C.c_int, [_p, _p]),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
     "b200env_set_hull_faces": (C.c_int, [_p, _p, _p, _p, _i32]),
     "b200env_kernel_form": (_i32, [_p]),

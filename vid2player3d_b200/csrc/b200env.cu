@@ -1749,8 +1749,12 @@ __host__ __device__ inline int obs_row_width(int nb, int nd, int shape_dim, bool
   return jpos ? 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 2 + nb * 3 + shape_dim
               : 1 + (nb - 1) * 3 + nb * 6 + nb * 3 + nb * 3 + nd + 1 + 6 + 2 + 2 + nd + nb * 3 + nb * 6 + shape_dim;
 }
-struct ObsStrides { int p_row, p_elem, q_row, q_elem, d_row, d_elem; };
-struct ObsBf16 { __nv_bfloat16* out; int ld; const float* mean; const float* rstd; float clamp; };
+// IM (b200env_im_policy_rows): the state comes from the raw observation rows obs_buf [n, num_obs] (every value clamped to +-clip_obs as it
+// is loaded), the targets from frame t_pad + (step[0] % t_len) of the context window (t_row floats per env, t_frame per frame; element
+// strides 3 / 4 / 1), motion_bodies from rows of mb_row floats; the float row is not written, the slot's target dof_pos goes to resid.
+struct ObsStrides { int p_row, p_elem, q_row, q_elem, d_row, d_elem; int t_row, t_frame, t_pad, t_len, mb_row; float clip_obs; };
+struct ObsBf16 { __nv_bfloat16* out; int ld; const float* mean; const float* rstd; float clamp; const int64_t* step; float* resid; };
+template <bool IM = false>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
 obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restrict__ body_pos, const float* __restrict__ body_rot,
                      const float* __restrict__ target_pos, const float* __restrict__ target_rot, const float* __restrict__ dof_pos,
@@ -1770,14 +1774,21 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
   float* srow = s_obs[warp];
   auto put = [&](int idx, float val) { srow[idx] = val; };
   const bool act = lane < nb;
+  // IM: the wrapper's clamp of the raw observation (torch.clamp keeps a NaN a NaN) and the first float of the target frame
+  auto in = [&](float x) {
+    if constexpr (IM) asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x) : "f"(st.clip_obs), "f"(-st.clip_obs));
+    return x;
+  };
+  int64_t toff = 0;
+  if constexpr (IM) toff = e * st.t_row + (int64_t)(st.t_pad + (int)(ob.step[0] % st.t_len)) * st.t_frame;
   float p[3] = {0, 0, 0}, q[4] = {0, 0, 0, 1}, v[3] = {0, 0, 0}, w[3] = {0, 0, 0}, tp[3] = {0, 0, 0}, tq[4] = {0, 0, 0, 1};
   if (act) {
-    const int64_t i3 = (e * nb + lane) * 3, i4 = (e * nb + lane) * 4;
+    const int64_t i3 = IM ? toff + lane * 3 : (e * nb + lane) * 3, i4 = IM ? toff + lane * 4 : (e * nb + lane) * 4;
     const int64_t s3 = e * st.p_row + (int64_t)lane * st.p_elem, s4 = e * st.q_row + (int64_t)lane * st.q_elem;   // state arrays: own strides
 #pragma unroll
-    for (int k = 0; k < 3; k++) { p[k] = body_pos[s3 + k]; v[k] = body_vel[s3 + k]; w[k] = body_ang_vel[s3 + k]; tp[k] = target_pos[i3 + k]; }
+    for (int k = 0; k < 3; k++) { p[k] = in(body_pos[s3 + k]); v[k] = in(body_vel[s3 + k]); w[k] = in(body_ang_vel[s3 + k]); tp[k] = target_pos[i3 + k]; }
 #pragma unroll
-    for (int k = 0; k < 4; k++) { q[k] = body_rot[s4 + k]; tq[k] = target_rot[i4 + k]; }
+    for (int k = 0; k < 4; k++) { q[k] = in(body_rot[s4 + k]); tq[k] = target_rot[i4 + k]; }
   }
   float rp[3], rq[4], trp[3], trq[4];
 #pragma unroll
@@ -1821,7 +1832,7 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
     for (int k = 0; k < 3; k++) put(off + nb * 3 + lane * 3 + k, l[k]);
   }
   off += nb * 6;
-  for (int k = lane; k < nd; k += 32) put(off + k, dof_vel[e * st.d_row + (int64_t)k * st.d_elem]);
+  for (int k = lane; k < nd; k += 32) put(off + k, in(dof_vel[e * st.d_row + (int64_t)k * st.d_elem]));
   off += nd;
   if (jpos) {
     if (lane == 0) {
@@ -1846,7 +1857,15 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
       put(off + 9, cosf(dh)); put(off + 10, sinf(dh));
     }
     off += 11;
-    for (int k = lane; k < nd; k += 32) put(off + k, target_dof_pos[e * nd + k] - dof_pos[e * st.d_row + (int64_t)k * st.d_elem]);
+    if constexpr (IM) {
+      for (int k = lane; k < nd; k += 32) {
+        const float td = target_dof_pos[toff + k];
+        put(off + k, td - in(dof_pos[e * st.d_row + (int64_t)k * st.d_elem]));
+        ob.resid[e * nd + k] = td;
+      }
+    } else {
+      for (int k = lane; k < nd; k += 32) put(off + k, target_dof_pos[e * nd + k] - dof_pos[e * st.d_row + (int64_t)k * st.d_elem]);
+    }
     off += nd;
   }
   if (act) {
@@ -1866,13 +1885,15 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
     }
     off += nb * 6;
   }
-  if (lane < shape_dim) put(off + lane, motion_bodies[e * shape_dim + lane]);
+  if (lane < shape_dim) put(off + lane, in(motion_bodies[IM ? e * st.mb_row + lane : e * shape_dim + lane]));
   __syncwarp();
-  float* orow = obs + e * W;
-  if ((((uintptr_t)orow) & 7) == 0 && (W & 1) == 0) {
-    for (int k = lane; k < W / 2; k += 32) reinterpret_cast<float2*>(orow)[k] = reinterpret_cast<const float2*>(srow)[k];
-  } else {
-    for (int k = lane; k < W; k += 32) orow[k] = srow[k];
+  if constexpr (!IM) {
+    float* orow = obs + e * W;
+    if ((((uintptr_t)orow) & 7) == 0 && (W & 1) == 0) {
+      for (int k = lane; k < W / 2; k += 32) reinterpret_cast<float2*>(orow)[k] = reinterpret_cast<const float2*>(srow)[k];
+    } else {
+      for (int k = lane; k < W; k += 32) orow[k] = srow[k];
+    }
   }
   if (ob.out) {
     __nv_bfloat16* brow = ob.out + e * (int64_t)ob.ld;
@@ -1888,6 +1909,51 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
       if (k + 1 < W) *reinterpret_cast<__nv_bfloat162*>(brow + k) = __floats2bfloat162_rn(x0, x1);   // the host checks: ld even, out 4-byte aligned
       else brow[k] = __float2bfloat16_rn(x0);
     }
+  }
+}
+
+// b200env_play_stats: ImitatorPlayer.run's bookkeeping of one step, one CTA; thread i takes envs i, i + PLAY_THREADS, ... and the partial
+// sums meet in a fixed tree, so a replay gives the same sums
+#define PLAY_THREADS 1024
+__global__ void __launch_bounds__(PLAY_THREADS) play_stats_kernel(b200_play_stats_t d) {
+  __shared__ float s_cr[PLAY_THREADS], s_st[PLAY_THREADS];
+  __shared__ int s_cnt[PLAY_THREADS];
+  if (d.games[1]) return;                           // stopped: the host has not started the next game yet
+  const int tid = threadIdx.x;
+  float scr = 0.f, sst = 0.f;
+  int cnt = 0;
+  for (int e = tid; e < d.n; e += PLAY_THREADS) {
+    const float done = d.reset_buf[e] != 0 ? 1.f : 0.f;
+    const float cr = d.cr[e] + d.rew[e], st = d.steps[e] + 1.f;
+    d.cr[e] = cr;
+    d.steps[e] = st;
+    if (done * (1.f - d.prev_dones[e]) != 0.f) { scr += cr; sst += st; cnt++; }
+  }
+  s_cr[tid] = scr; s_st[tid] = sst; s_cnt[tid] = cnt;
+  __syncthreads();
+  for (int w = PLAY_THREADS / 2; w > 0; w >>= 1) {
+    if (tid < w) { s_cr[tid] += s_cr[tid + w]; s_st[tid] += s_st[tid + w]; s_cnt[tid] += s_cnt[tid + w]; }
+    __syncthreads();
+  }
+  const int count = s_cnt[0];
+  for (int e = tid; e < d.n; e += PLAY_THREADS) {
+    const float done = d.reset_buf[e] != 0 ? 1.f : 0.f;
+    if (count > 0) { d.cr[e] = d.cr[e] * (1.f - done); d.steps[e] = d.steps[e] * (1.f - done); }
+    d.prev_dones[e] = done;
+  }
+  if (tid == 0) {
+    if (count > 0) {
+      d.totals[0] += (double)s_cr[0];
+      d.totals[1] += (double)s_st[0];
+      d.games[0] += count;
+      if (d.games[2] < d.max_log) {
+        double* row = d.log + d.games[2] * 3;
+        row[0] = count; row[1] = s_cr[0]; row[2] = s_st[0];
+      }
+      d.games[2] += 1;
+    }
+    d.games[1] = (d.games[0] >= d.n_games || d.reset_buf[0] != 0) ? 1 : 0;
+    d.step[0] += 1;
   }
 }
 
@@ -2596,7 +2662,7 @@ int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, co
   if (int rc = obs_row_check("b200env_obs_imitation", nbl, h->cfg.shape_dim, W)) return rc;
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-  obs_imitation_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(n, nbl, h->model.nd, h->cfg.shape_dim, body_pos, body_rot,
+  obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(n, nbl, h->model.nd, h->cfg.shape_dim, body_pos, body_rot,
                                                                               target_pos, target_rot, dof_pos, dof_vel, target_dof_pos,
                                                                               body_vel, body_ang_vel, motion_bodies, local_root_obs & 1,
                                                                               root_height_obs, obs, (local_root_obs >> 1) & 1,
@@ -2627,13 +2693,53 @@ int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_b
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
   const int nd = h->model.nd;
-  obs_imitation_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+  obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
       n, nbl, nd, h->cfg.shape_dim, rigid_body_state, rigid_body_state + 3, target_pos, target_rot, dof_state, dof_state + 1, target_dof_pos,
       rigid_body_state + 7, rigid_body_state + 10, motion_bodies, local_root_obs & 1, root_height_obs, obs, (local_root_obs >> 1) & 1,
       ObsStrides{bodies_per_env * 13, 13, bodies_per_env * 13, 13, nd * 2, 2},
       ObsBf16{reinterpret_cast<__nv_bfloat16*>(obs_bf16), ld_bf16, mean, rstd, clamp});
   CUDA_OK(cudaGetLastError());
   h->launches++;
+  return 0;
+}
+
+int b200env_im_policy_rows(b200env_handle h, const b200_im_policy_t* d, void* stream) {
+  if (!h || !d || !d->obs_buf || !d->context_feat || !d->step || !d->x || !d->resid) return fail(-1, "b200env_im_policy_rows: null argument%s");
+  if (d->n <= 0) return fail(-2, "b200env_im_policy_rows: n must be positive%s");
+  const int nbl = h->has_ml ? h->ml.num_lib_bodies : (h->model.fixed[h->model.nb - 1] ? h->model.nb - 1 : h->model.nb);
+  const int nd = h->model.nd, sd = h->cfg.shape_dim;
+  const int W = obs_row_width(nbl, nd, sd, false);
+  if (int rc = obs_row_check("b200env_im_policy_rows", nbl, sd, W)) return rc;
+  if (d->ld < W) return fail(-2, "b200env_im_policy_rows: ld is smaller than the observation row%s");
+  if (d->ld & 1) return fail(-2, "b200env_im_policy_rows: ld must be even%s");
+  if (reinterpret_cast<uintptr_t>(d->x) & 3) return fail(-2, "b200env_im_policy_rows: x must be 4-byte aligned%s");
+  if (d->num_obs < nbl * 13 + 2 * nd + sd) return fail(-2, "b200env_im_policy_rows: num_obs is narrower than the observation's named blocks%s");
+  if (d->feat_width < nbl * 7 + nd) return fail(-2, "b200env_im_policy_rows: feat_width is narrower than body_pos | body_rot | dof_pos%s");
+  if (d->context_padding < 0 || d->context_length < 1 || (int64_t)d->context_padding + d->context_length > d->num_frames)
+    return fail(-2, "b200env_im_policy_rows: the context slot lies outside the window (context_padding + context_length > num_frames)%s");
+  if ((d->mean == nullptr) != (d->rstd == nullptr)) return fail(-2, "b200env_im_policy_rows: mean and rstd go together%s");
+  if (d->mean && !(d->clip > 0.f)) return fail(-2, "b200env_im_policy_rows: the normaliser needs a positive clip%s");
+  cudaSetDevice(h->device);
+  const int grid = (d->n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
+  const float* o = d->obs_buf;   // obs_names order: body_pos | body_rot | dof_pos | dof_vel | body_vel | body_ang_vel | motion_bodies
+  const float* t = d->context_feat;
+  obs_imitation_kernel<true><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+      d->n, nbl, nd, sd, o, o + 3 * nbl, t, t + 3 * nbl, o + 7 * nbl, o + 7 * nbl + nd, t + 7 * nbl, o + 7 * nbl + 2 * nd, o + 10 * nbl + 2 * nd,
+      o + 13 * nbl + 2 * nd, 1, 1, nullptr, 0,
+      ObsStrides{d->num_obs, 3, d->num_obs, 4, d->num_obs, 1, d->num_frames * d->feat_width, d->feat_width, d->context_padding, d->context_length,
+                 d->num_obs, d->clip_obs},
+      ObsBf16{reinterpret_cast<__nv_bfloat16*>(d->x), d->ld, d->mean, d->rstd, d->mean ? d->clip : INFINITY, d->step, d->resid});
+  CUDA_OK(cudaGetLastError());
+  h->launches++;
+  return 0;
+}
+
+int b200env_play_stats(const b200_play_stats_t* d, void* stream) {
+  if (!d || !d->rew || !d->reset_buf || !d->cr || !d->steps || !d->prev_dones || !d->totals || !d->log || !d->games || !d->step)
+    return fail(-1, "b200env_play_stats: null argument%s");
+  if (d->n <= 0 || d->max_log < 1) return fail(-2, "b200env_play_stats: n and max_log must be positive%s");
+  play_stats_kernel<<<1, PLAY_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 

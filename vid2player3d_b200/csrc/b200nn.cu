@@ -212,6 +212,8 @@ struct LinearParams {
   int ldo, out_col0, rows, n, n_padded, k_padded, act, out_bf16;
   float out_min, out_max;
   int n_tiles, tiles;                              // output tiles across the columns, in all
+  const float* resid;                              // RES: x += resid[row * ld_resid + col] for col < resid_cols, before act and clamp
+  int ld_resid, resid_cols;
 };
 
 __device__ __forceinline__ float finish(float x, const LinearParams& p) {
@@ -251,7 +253,7 @@ __device__ __forceinline__ void quad_transpose(const uint32_t (&v)[4], int q, ui
 
 // Accumulator register i (of E * BN / 2) of this thread: expert i / (BN / 2), row row0 + 8 ((i / 2) % 2), column
 // 8 ((i % (BN / 2)) / 4) + 2 (lane % 4) + i % 2 of the tile (columns n0 ..).  Taken 32 columns at a time.
-template <int E, int BN>
+template <int E, int BN, bool RES>
 __device__ __forceinline__ void epilogue(const float* acc, const float (&coef)[2][E], const float* sbias, const LinearParams& p, int row0,
                                          int n0, int lane) {
   const int q = lane & 3;
@@ -269,6 +271,9 @@ __device__ __forceinline__ void epilogue(const float* acc, const float (&coef)[2
           float x;
           if (E == 1) {
             x = acc[i] + sbias[col];
+            if constexpr (RES) {
+              if (col < p.resid_cols && row < p.rows) x += __ldg(p.resid + (size_t)row * p.ld_resid + col);
+            }
           } else {
             x = 0.f;
 #pragma unroll
@@ -311,8 +316,10 @@ template <int E, int BN> __host__ __device__ constexpr int stage_bytes() { retur
 template <int E, int BN> __host__ __device__ constexpr int bias_offset() { return stages<E, BN>() * stage_bytes<E, BN>() + 16 * stages<E, BN>(); }
 template <int E, int BN> int smem_bytes(int n_padded) { return 1024 + bias_offset<E, BN>() + E * n_padded * 4; }
 
-template <int E, int BN>
-__global__ void __launch_bounds__(NUM_THREADS, ctas_per_sm<E>())
+// RES (residual epilogue, the policy's last layer): one CTA per SM - its register budget holds the residual's addressing without spilling,
+// and a layer as narrow as the policy's 75 actions has fewer tiles than SMs
+template <int E, int BN, bool RES = false>
+__global__ void __launch_bounds__(NUM_THREADS, RES ? 1 : ctas_per_sm<E>())
 linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const LinearParams p) {
   constexpr int ACC = E * BN;                          // accumulator columns = the N of every wgmma
   constexpr int STAGES = stages<E, BN>();
@@ -394,7 +401,7 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     }
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[prev]);
-    epilogue<E, BN>(acc, coef, sbias, p, row0, n0, lane);
+    epilogue<E, BN, RES>(acc, coef, sbias, p, row0, n0, lane);
   }
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
@@ -479,16 +486,16 @@ struct b200nn_linear {
 
 // prepare (at create, on the handle's device): the kernel's shared-memory size, and the grid = the CTA slots resident on the device
 // at once, at most one per tile.  Otherwise launch.
-template <int E, int BN> static int prepare_or_launch(b200nn_linear* h, cudaStream_t st, bool prepare) {
+template <int E, int BN, bool RES = false> static int prepare_or_launch(b200nn_linear* h, cudaStream_t st, bool prepare) {
   if (prepare) {
     // the attribute is per kernel, not per handle: allow the device's limit, so that handles of other widths launch too
     int sms = 0, per_sm = 0, limit = 0;
     CUDA_OK(cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
     if (smem_bytes<E, BN>(h->d.n_padded) > limit) return fail(-2, "b200nn_linear_create: n_padded too large for the bias in shared memory");
-    CUDA_OK(cudaFuncSetAttribute(linear_kernel<E, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit));
-    prefer_max_shared(linear_kernel<E, BN>);
+    CUDA_OK(cudaFuncSetAttribute(linear_kernel<E, BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit));
+    prefer_max_shared(linear_kernel<E, BN, RES>);
     CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_kernel<E, BN>, NUM_THREADS, smem_bytes<E, BN>(h->d.n_padded)));
+    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_kernel<E, BN, RES>, NUM_THREADS, smem_bytes<E, BN>(h->d.n_padded)));
     if (per_sm < 1) return fail(-3, "b200nn_linear_create: the GEMM kernel does not fit on an SM");
     h->grid = h->p.tiles < sms * per_sm ? h->p.tiles : sms * per_sm;
     return 0;
@@ -503,13 +510,15 @@ template <int E, int BN> static int prepare_or_launch(b200nn_linear* h, cudaStre
   attr[0].val.programmaticStreamSerializationAllowed = h->pdl ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  CUDA_OK(cudaLaunchKernelEx(&cfg, linear_kernel<E, BN>, h->tmA, h->tmW, h->p));
+  CUDA_OK(cudaLaunchKernelEx(&cfg, linear_kernel<E, BN, RES>, h->tmA, h->tmW, h->p));
   return 0;
 }
 
 static int dispatch(b200nn_linear* h, cudaStream_t st, bool prepare) {
   switch (h->d.num_experts) {
-    case 1: return h->bn == 64 ? prepare_or_launch<1, 64>(h, st, prepare) : prepare_or_launch<1, 128>(h, st, prepare);
+    case 1:
+      if (h->d.resid) return h->bn == 64 ? prepare_or_launch<1, 64, true>(h, st, prepare) : prepare_or_launch<1, 128, true>(h, st, prepare);
+      return h->bn == 64 ? prepare_or_launch<1, 64>(h, st, prepare) : prepare_or_launch<1, 128>(h, st, prepare);
     case 2: return prepare_or_launch<2, MOE_BN>(h, st, prepare);
     case 3: return prepare_or_launch<3, MOE_BN>(h, st, prepare);
     case 4: return prepare_or_launch<4, MOE_BN>(h, st, prepare);
@@ -540,6 +549,14 @@ int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_l
   if ((int64_t)d->ldo < (int64_t)d->out_col0 + d->n) return fail(-2, "b200nn_linear_create: ldo < out_col0 + n");
   if (d->act != B200NN_ACT_NONE && d->act != B200NN_ACT_RELU && d->act != B200NN_ACT_ELU) return fail(-2, "b200nn_linear_create: unknown activation");
   if (((uintptr_t)d->a | (uintptr_t)d->w | (uintptr_t)d->out) & 15) return fail(-2, "b200nn_linear_create: operands must be 16-byte aligned");
+  if (d->resid || d->resid_cols || d->ld_resid) {
+    if (!d->resid) return fail(-2, "b200nn_linear_create: resid_cols / ld_resid given without resid");
+    if (E > 1) return fail(-2, "b200nn_linear_create: a residual needs a single-expert layer (num_experts == 1)");
+    if (d->out_bf16) return fail(-2, "b200nn_linear_create: a residual needs a float output");
+    if (d->resid_cols < 1 || d->resid_cols > d->n) return fail(-2, "b200nn_linear_create: resid_cols must be in 1..n");
+    if (d->ld_resid < d->resid_cols) return fail(-2, "b200nn_linear_create: ld_resid < resid_cols");
+    if ((uintptr_t)d->resid & 3) return fail(-2, "b200nn_linear_create: resid must be 4-byte aligned");
+  }
   encode_tiled_fn enc = get_encode();
   if (!enc) return fail(-3, "b200nn_linear_create: cuTensorMapEncodeTiled not available (no CUDA driver)");
   CUDA_OK(cudaSetDevice(device));
@@ -570,7 +587,7 @@ int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_l
   }
   const int n_tiles = (d->n + h->bn - 1) / h->bn;
   h->p = LinearParams{d->bias, d->coef, d->out, d->ldo, d->out_col0, d->rows, d->n, d->n_padded, d->k_padded, d->act, d->out_bf16, d->out_min, d->out_max,
-                      n_tiles, rows_padded / BLOCK_M * n_tiles};
+                      n_tiles, rows_padded / BLOCK_M * n_tiles, d->resid, d->ld_resid, d->resid_cols};
   const int rc = dispatch(h, nullptr, true);
   if (rc) { delete h; return rc; }
   *out = h;

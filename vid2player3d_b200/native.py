@@ -48,7 +48,7 @@ def _layout(S):
     if lay is None:
         import torch
         dtypes = {abi.F32P: (torch.float32,), abi.I64P: (torch.int64,), abi.U8P: (torch.uint8, torch.bool),
-                  abi.U32P: (torch.int32, torch.uint32)}
+                  abi.U32P: (torch.int32, torch.uint32), abi.F64P: (torch.float64,)}
         scalars = [(name, ct._length_ if issubclass(ct, C.Array) else None) for name, ct in S._fields_ if not issubclass(ct, C.c_void_p)]
         ptrs = [(name, dtypes.get(ct)) for name, ct in S._fields_ if issubclass(ct, C.c_void_p)]
         lay = _layouts[S] = (scalars, ptrs)
@@ -97,6 +97,12 @@ def fill(S, scalars, tensors):
 def _stream():
     import torch
     return torch.cuda.current_stream().cuda_stream
+
+
+def play_stats(scalars, tensors):
+    """one step of ImitatorPlayer.run's bookkeeping on the device (include/b200env.h: b200env_play_stats); the fields of abi.PlayStats"""
+    d = fill(abi.PlayStats, scalars, tensors)
+    _check(lib().b200env_play_stats(C.byref(d), _stream()))
 
 
 def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):
@@ -264,6 +270,12 @@ class Env:
                                                 _ptr(target_pos), _ptr(target_rot), _ptr(target_dof_pos), _ptr(motion_bodies),
                                                 int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _ptr(obs_bf16),
                                                 obs_bf16.shape[1] if obs_bf16 is not None else 0, _ptr(mean), _ptr(rstd), clamp, _stream()))
+
+    def im_policy_rows(self, scalars, tensors):
+        """the imitation policy's bf16 operand rows and residual from obs_buf and the context slot of the device step counter
+        (include/b200env.h: b200env_im_policy_rows); scalars / tensors: the fields of abi.ImPolicy"""
+        d = fill(abi.ImPolicy, scalars, tensors)
+        _check(lib().b200env_im_policy_rows(self._h, C.byref(d), _stream()))
 
     def physics_only(self, root, dof_pos, dof_vel, pd_tar, ext_wrench, rb_out, contact_out, n_steps=1, ball=None, ball_hits=None,
                      dof_force=None):

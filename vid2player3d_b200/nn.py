@@ -21,14 +21,14 @@ from .build import LIB_NN
 ACT = {None: 0, "none": 0, "relu": 1, "elu": 2}
 _lib = None
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 
 class LinearDesc(C.Structure):
     _fields_ = [("a", C.c_void_p), ("lda", C.c_int32), ("w", C.c_void_p), ("ldw", C.c_int32), ("bias", C.c_void_p), ("coef", C.c_void_p),
                 ("out", C.c_void_p), ("ldo", C.c_int32), ("out_col0", C.c_int32), ("rows", C.c_int32), ("n", C.c_int32),
                 ("n_padded", C.c_int32), ("k_padded", C.c_int32), ("num_experts", C.c_int32), ("act", C.c_int32), ("out_bf16", C.c_int32),
-                ("out_min", C.c_float), ("out_max", C.c_float)]
+                ("out_min", C.c_float), ("out_max", C.c_float), ("resid", C.c_void_p), ("ld_resid", C.c_int32), ("resid_cols", C.c_int32)]
 
 
 # name -> (restype, argtypes) of every function include/b200nn.h declares; lib() applies all of them when it loads the library, so an
@@ -87,9 +87,11 @@ def padded_bf16(rows, cols, device):
 
 class Linear:
     """out[:, col0:col0+N] = act(sum_e coef[:, e] (a W_e^T + b_e)); one launch.  weight [E, N, K] or [N, K] float (torch layout:
-    out x in), bias [E, N] or [N]; `a` / `out` are buffers from padded_bf16 (out may also be a float [rows, N] tensor)."""
+    out x in), bias [E, N] or [N]; `a` / `out` are buffers from padded_bf16 (out may also be a float [rows, N] tensor).  residual = (float
+    tensor [rows, >= cols], cols): a single-expert layer with a float output adds resid[:, :cols] to its first cols outputs before the
+    activation and the clamp."""
 
-    def __init__(self, a, weight, bias, out, rows, act=None, coef=None, out_col0=0, out_clamp=None):
+    def __init__(self, a, weight, bias, out, rows, act=None, coef=None, out_col0=0, out_clamp=None, residual=None):
         dev = a.device
         if dev.type != "cuda":
             raise RuntimeError("b200nn runs on a CUDA device only (no CPU fallback)")
@@ -111,10 +113,16 @@ class Linear:
         assert out.shape[0] >= (padded_rows(rows) if out_bf16 else rows)
         if E > 1:
             assert coef is not None and coef.dtype == torch.float32 and coef.is_contiguous() and tuple(coef.shape) == (rows, E)
+        resid, cols = residual if residual is not None else (None, 0)
+        if resid is not None:
+            assert resid.dtype == torch.float32 and resid.stride(-1) == 1 and resid.device == dev and resid.shape[0] >= rows
+        self.residual = residual
         d = LinearDesc(a=a.data_ptr(), lda=a.shape[1], w=self.w.data_ptr(), ldw=self.k_padded, bias=self.b.data_ptr(),
                        coef=coef.data_ptr() if coef is not None else None, out=out.data_ptr(), ldo=out.shape[1], out_col0=out_col0,
                        rows=rows, n=N, n_padded=self.n_padded, k_padded=self.k_padded, num_experts=E, act=ACT[act], out_bf16=int(out_bf16),
-                       out_min=out_clamp[0] if out_clamp else 0.0, out_max=out_clamp[1] if out_clamp else 0.0)
+                       out_min=out_clamp[0] if out_clamp else 0.0, out_max=out_clamp[1] if out_clamp else 0.0,
+                       resid=resid.data_ptr() if resid is not None else None, ld_resid=resid.stride(0) if resid is not None else 0,
+                       resid_cols=int(cols))
         self._h = C.c_void_p()
         _check(lib().b200nn_linear_create(C.byref(d), dev.index or 0, C.byref(self._h)))
         self.flops = 2.0 * rows * N * K * E
@@ -143,9 +151,13 @@ class PolicyMLP:
     """mu = W4 relu(W3 relu(W2 relu(W1 x + b1) + b2) + b3) + b4 with x = clamp((obs - mean) / sqrt(var + eps), -5, 5)
     (im_network_builder.py:191-230 `actor_mlp` + `mu`, RunningMeanStd; im_player.py:187-202).  `layers` = [(weight [out, in],
     bias [out]), ...] in torch nn.Linear layout; the last layer has no activation.  clamp_actions = 1.0 folds
-    ImitatorPlayer's `torch.clamp(action, -1, 1)` (im_player.py:198) into the last layer's epilogue."""
+    ImitatorPlayer's `torch.clamp(action, -1, 1)` (im_player.py:198) into the last layer's epilogue.  obs_rstd: the normaliser's
+    1 / std given as it is (RunningNorm's 1 / (std + 1e-8)) instead of from obs_var.  residual = (float tensor [num_envs, >= cols], cols):
+    the last layer adds it to its first cols outputs before the action clamp (the embodied_pose imitation policy's residual action,
+    `mu[:, :69] += target_dof_pos`, im_network_builder.py:226-228)."""
 
-    def __init__(self, layers, num_envs, device, obs_mean=None, obs_var=None, eps=1e-5, clamp_obs=5.0, activation="relu", clamp_actions=None):
+    def __init__(self, layers, num_envs, device, obs_mean=None, obs_var=None, eps=1e-5, clamp_obs=5.0, activation="relu", clamp_actions=None,
+                 obs_rstd=None, residual=None):
         self.rows, self.device = num_envs, torch.device(device)
         self.in_dim = layers[0][0].shape[1]
         self.out_dim = layers[-1][0].shape[0]
@@ -153,6 +165,10 @@ class PolicyMLP:
         self.clamp_actions = clamp_actions
         self.mean = obs_mean.to(self.device, torch.float32).contiguous() if obs_mean is not None else None
         self.rstd = (1.0 / torch.sqrt(obs_var.to(self.device, torch.float32) + eps)).contiguous() if obs_var is not None else None
+        if obs_rstd is not None:
+            if obs_var is not None:
+                raise ValueError("obs_var and obs_rstd are two forms of the same statistic: give one")
+            self.rstd = obs_rstd.to(self.device, torch.float32).contiguous()
         if (self.mean is None) != (self.rstd is None):
             raise ValueError("obs_mean and obs_var go together")
         self.x = padded_bf16(num_envs, self.in_dim, self.device)
@@ -162,7 +178,8 @@ class PolicyMLP:
             last = i == len(layers) - 1
             o = self.out if last else padded_bf16(num_envs, w.shape[0], self.device)
             self.layers.append(Linear(a, w, b, o, num_envs, act=None if last else activation,
-                                      out_clamp=(-clamp_actions, clamp_actions) if (last and clamp_actions) else None))
+                                      out_clamp=(-clamp_actions, clamp_actions) if (last and clamp_actions) else None,
+                                      residual=residual if last else None))
             a = o
         self.flops = sum(l.flops for l in self.layers)
         self.launches_per_forward = 1 + len(self.layers)
@@ -245,21 +262,70 @@ def v2p_networks_from_checkpoint(checkpoint, obs_dim=None, normalize_input=True,
                 var = _prefix(torch.ones(D), rms["running_var"])
                 net["rstd"], net["clip"] = 1.0 / torch.sqrt(var + 1e-5), 5.0
         else:
-            mean, std, n = torch.zeros(D), torch.zeros(D), 0
-            if "running_obs.n" in model:
-                n = int(model["running_obs.n"])
-                _prefix(mean, model["running_obs.mean"])
-                _prefix(std, model["running_obs.std"])
-            elif "running_mean_std" in ck or "running_obs.running_mean" in model:
-                rms = ck["running_mean_std"] if "running_mean_std" in ck else \
-                    {k: model["running_obs." + k] for k in ("running_mean", "running_var", "count")}
-                n = int(rms["count"])
-                _prefix(mean, rms["running_mean"])
-                _prefix(std, torch.sqrt(rms["running_var"].float()))
-            if n > 0:
-                net["mean"], net["rstd"], net["clip"] = mean, 1.0 / (std + 1e-8), 5.0
+            net.update(_running_norm(ck, model, D))
         out.append(net)
     return out
+
+
+def _running_norm(ck, model, D, rlgame_fallback=True):
+    """{mean, rstd, clip} of a RunningNorm (`running_obs_type: ours`, embodied_pose/models/running_norm.py: y = clamp((x - mean) /
+    (std + 1e-8), -5, 5) while n > 0, the identity at n == 0), as the players load it: the model's `running_obs.{n,mean,std}`, or else
+    (rlgame_fallback: the load_rlgame_norm branch of ImitatorPlayer.load_pretrained / V2PPlayer.load_dual_cp) rl_games statistics of
+    the checkpoint's `running_mean_std` or of the model's `running_obs.{running_mean,running_var,count}` with std = sqrt(var).  A
+    statistic shorter than D fills a prefix and leaves mean 0, std 0 behind it (rstd 1e8).  The identity: mean / rstd None, clip inf."""
+    mean, std, n = torch.zeros(D), torch.zeros(D), 0
+    if "running_obs.n" in model:
+        n = int(model["running_obs.n"])
+        _prefix(mean, model["running_obs.mean"])
+        _prefix(std, model["running_obs.std"])
+    elif rlgame_fallback and ("running_mean_std" in ck or "running_obs.running_mean" in model):
+        rms = ck["running_mean_std"] if "running_mean_std" in ck else \
+            {k: model["running_obs." + k] for k in ("running_mean", "running_var", "count")}
+        n = int(rms["count"])
+        _prefix(mean, rms["running_mean"])
+        _prefix(std, torch.sqrt(rms["running_var"].float()))
+    if n > 0:
+        return dict(mean=mean, rstd=1.0 / (std + 1e-8), clip=5.0)
+    return dict(mean=None, rstd=None, clip=float("inf"))
+
+
+def im_networks_from_checkpoint(checkpoint, use_running_obs=True, running_obs_type="ours", normalize_input=False, use_ik=False,
+                                deterministic=True, obs_dim=734):
+    """What ImitatorPlayer.restore / load_pretrained (embodied_pose/players/im_player.py:43-94) read from an embodied_pose imitation
+    checkpoint, as one network dict: `layers` [(weight, bias)] x 4 (actor_mlp.{0,2,4} and mu of `model`, or of a Lightning checkpoint's
+    `state_dict`), `mean` / `rstd` [obs_dim] (None: no normaliser) and `clip` (the normaliser's clamp, inf for none).  The keyword
+    arguments are the network / player cfg entries of the same names (cfg/amass_im.yaml: use_running_obs True, running_obs_type ours).
+      running_obs_type ours:    RunningNorm (see _running_norm); a Lightning checkpoint loads only its own running_obs.* keys
+      running_obs_type rl_game: RunningMeanStd, rstd = 1 / sqrt(var + 1e-5), clamp 5, always applied: the model's
+                                running_obs.{running_mean,running_var}, else the fresh statistics (mean 0, var 1)
+    Refused, with the reason: normalize_input (the player's own RunningMeanStd over the raw obs), use_ik and a stochastic player.
+    checkpoint: a path or a loaded dict.  CPU tensors, float32."""
+    if normalize_input:
+        raise ValueError("normalize_input: True normalises the raw 461-wide observation before the network; the device operand launch "
+                         "reads obs_buf as the wrapper clamps it and does not implement that normaliser (neither shipped cfg sets it)")
+    if use_ik:
+        raise ValueError("use_ik: the network's inverse kinematics of the context (perform_ik) needs the SMPL model files and is not "
+                         "implemented on the device")
+    if not deterministic:
+        raise ValueError("the imitation policy serves the deterministic action (mu) only: the sampled action of a stochastic player "
+                         "(mu + sigma * N(0, 1)) is not implemented")
+    ck = _load(checkpoint)
+    lightning = "pytorch-lightning_version" in ck
+    if lightning:
+        model = dict(ck["state_dict"])
+    else:
+        model = {k[len("a2c_network."):]: v for k, v in ck["model"].items() if k.startswith("a2c_network.")}
+    layers = [(model[k + ".weight"].float(), model[k + ".bias"].float()) for k in V2P_ACTOR_KEYS]
+    net = dict(layers=layers, mean=None, rstd=None, clip=float("inf"))
+    if not use_running_obs:
+        return net
+    if running_obs_type == "rl_game":
+        mean = model.get("running_obs.running_mean", torch.zeros(obs_dim)).float()
+        var = model.get("running_obs.running_var", torch.ones(obs_dim)).float()
+        net.update(mean=mean.clone(), rstd=1.0 / torch.sqrt(var + 1e-5), clip=5.0)
+    else:
+        net.update(_running_norm({} if lightning else ck, model, obs_dim, rlgame_fallback=not lightning))
+    return net
 
 
 class V2PPolicy:

@@ -1,11 +1,13 @@
 """parse_task mirror (embodied_pose/utils/parse_task.py:19-42): same signature and error behaviour."""
 from .humanoid_smpl_im import HumanoidSMPLIM
+from .humanoid_smpl_im_vis import HumanoidSMPLIMVis
 from .humanoid_smpl_im_mvae import HumanoidSMPLIMMVAE, HumanoidSMPLIMMVAEDual
 from .mvae_controller_vis import MVAEControllerVis, MVAEControllerVisDual
 from .physics_mvae_controller import PhysicsMVAEController, PhysicsMVAEControllerDual
 from .vec_task import VecTaskPythonWrapper
 
-TASKS = {"HumanoidSMPLIM": HumanoidSMPLIM, "HumanoidSMPLIMMVAE": HumanoidSMPLIMMVAE, "HumanoidSMPLIMMVAEDual": HumanoidSMPLIMMVAEDual,
+TASKS = {"HumanoidSMPLIM": HumanoidSMPLIM, "HumanoidSMPLIMVis": HumanoidSMPLIMVis, "HumanoidSMPLIMMVAE": HumanoidSMPLIMMVAE,
+         "HumanoidSMPLIMMVAEDual": HumanoidSMPLIMMVAEDual,
          "PhysicsMVAEController": PhysicsMVAEController, "PhysicsMVAEControllerDual": PhysicsMVAEControllerDual,
          "MVAEControllerVis": MVAEControllerVis, "MVAEControllerVisDual": MVAEControllerVisDual}
 
