@@ -27,7 +27,7 @@ extern "C" {
 #define B200_MAX_BODIES 32
 #define B200_MAX_DOF 96
 #define B200_MAX_KEY 8
-#define B200_ABI_VERSION 10
+#define B200_ABI_VERSION 11
 
 /* Per-asset constant block produced by vid2player3d_b200/model_compiler.py from the MJCF/STL
  * assets (replaces gym.load_asset + create_actor + set_actor_dof_properties:
@@ -195,41 +195,63 @@ int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_
  * init_* may be NULL when ref_prob >= 1.  Rows whose mask is clear are not touched.
  * counter: [1] int64 device, advanced by 1 by every call; work: [num_envs + 2] int32 device, zero before the first call (each call
  * leaves its counters zero). */
-int b200env_reset_masked(b200env_handle h, const uint8_t* mask, int32_t sample_time, float truncate, float ref_prob, uint64_t seed,
-                         int64_t* counter, const float* init_root, const float* init_dof_pos, const float* init_dof_vel, float* reset_times,
-                         int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, int32_t* work,
-                         void* stream);
+typedef struct b200_reset_masked {
+  int32_t sample_time;     /* 0: ref-state init at t = 0, 1: at a drawn time */
+  float truncate, ref_prob;
+  int32_t num_frames, first_frame;
+  float dt;
+  uint64_t seed;
+  const uint8_t* mask;     /* [num_envs] */
+  int64_t* counter;        /* [1] */
+  const float *init_root, *init_dof_pos, *init_dof_vel; /* NULL when ref_prob >= 1 */
+  float* reset_times;      /* [num_envs] */
+  float* context_feat;     /* [num_envs, num_frames, W] */
+  uint8_t* context_mask;   /* [num_envs, num_frames] */
+  int32_t* work;           /* [num_envs + 2] */
+} b200_reset_masked_t;
+int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* stream);
 
 /* replaces MotionLib.get_motion_state(..., return_rigid_body=True, adjust_height=True)
  * (motion_lib.py:164-266) for arbitrary (id, time) pairs, e.g. _init_context
  * (humanoid_smpl_im.py:530-563).  Any output pointer may be NULL. */
-int b200env_motion_state(b200env_handle h, const int64_t* motion_ids, const float* motion_times, int32_t n,
-                         float* root_pos, float* root_rot, float* dof_pos, float* root_vel, float* root_ang_vel,
-                         float* dof_vel, float* key_pos, float* rb_pos, float* rb_rot, void* stream);
+typedef struct b200_motion_state {
+  int32_t n, pad_;
+  const int64_t* motion_ids;   /* [n] */
+  const float* motion_times;   /* [n] */
+  float *root_pos, *root_rot, *dof_pos, *root_vel, *root_ang_vel, *dof_vel, *key_pos, *rb_pos, *rb_rot;
+} b200_motion_state_t;
+int b200env_motion_state(b200env_handle h, const b200_motion_state_t* d, void* stream);
 
 /* replaces compute_humanoid_observations_imitation (humanoid_smpl_im.py:773-850 ==
- * models/im_network_builder.py:262-338): obs [n,1+..=734 for 24 bodies].  Bit 1 of `local_root_obs` selects the
- * 'joint_pos' variant compute_humanoid_observations_imitation_jpos (:853-915, 513 wide).  Returns -2 before any launch when the
- * row is wider than 768 columns or the humanoid has more than 32 bodies (one lane per body). */
-int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, const float* body_rot,
-                          const float* target_pos, const float* target_rot, const float* dof_pos, const float* dof_vel,
-                          const float* target_dof_pos, const float* body_vel, const float* body_ang_vel,
-                          const float* motion_bodies, int32_t local_root_obs, int32_t root_height_obs, float* obs,
-                          void* stream);
+ * models/im_network_builder.py:262-338): obs [n,1+..=734 for 24 bodies].  jpos != 0 selects the 'joint_pos' variant
+ * compute_humanoid_observations_imitation_jpos (:853-915, 513 wide).  Returns -2 before any launch when the row is wider than 768
+ * columns or the humanoid has more than 32 bodies (one lane per body). */
+typedef struct b200_obs_imitation {
+  int32_t n, local_root_obs, root_height_obs, jpos;
+  const float *body_pos, *body_rot, *target_pos, *target_rot, *dof_pos, *dof_vel, *target_dof_pos, *body_vel, *body_ang_vel;
+  const float* motion_bodies;
+  float* obs;
+} b200_obs_imitation_t;
+int b200env_obs_imitation(b200env_handle h, const b200_obs_imitation_t* d, void* stream);
 
 /* The same observation computed straight from the Isaac-layout state rows the env owns - rigid_body_state [n, bodies_per_env, 13]
  * (pos 0:3, rot 3:7, vel 7:10, ang vel 10:13; the first `humanoid bodies` rows of every env are used) and dof_state [n, nd, 2] -
  * instead of six contiguous gathers of them (what the reference's slicing + cat amounts to, humanoid_smpl_im_mvae.py:862-895).
  * obs_bf16 (may be NULL): additionally writes the policy's first-layer operand row, bf16(clamp((obs - mean) * rstd, -clamp, clamp)),
  * [n, ld_bf16] (RunningMeanStd + the +-5 clamp of ImitatorPlayer.run_one_step, vid2player/players/im_player.py:187-190; mean /
- * rstd NULL = no normalisation), so that the network forward (include/b200nn.h) starts without a cast launch.  Bit 1 of
- * `local_root_obs` selects the 'joint_pos' variant, as above.  Returns -2 before any launch on the refusals of
- * b200env_obs_imitation, and when obs_bf16 is given with ld_bf16 smaller than the row width, an odd ld_bf16 or an address that is not
- * 4-byte aligned (the row is stored as bf16 pairs). */
-int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_body_state, int32_t bodies_per_env, const float* dof_state,
-                               const float* target_pos, const float* target_rot, const float* target_dof_pos, const float* motion_bodies,
-                               int32_t local_root_obs, int32_t root_height_obs, float* obs, void* obs_bf16, int32_t ld_bf16, const float* mean,
-                               const float* rstd, float clamp, void* stream);
+ * rstd NULL = no normalisation), so that the network forward (include/b200nn.h) starts without a cast launch.  jpos selects the
+ * 'joint_pos' variant, as above.  Returns -2 before any launch on the refusals of b200env_obs_imitation, and when obs_bf16 is given
+ * with ld_bf16 smaller than the row width, an odd ld_bf16 or an address that is not 4-byte aligned (the row is stored as bf16 pairs). */
+typedef struct b200_obs_rows {
+  int32_t n, bodies_per_env, local_root_obs, root_height_obs, jpos, ld_bf16;
+  float clamp;
+  int32_t pad_;
+  const float *rigid_body_state, *dof_state, *target_pos, *target_rot, *target_dof_pos, *motion_bodies;
+  float* obs;
+  void* obs_bf16;                 /* NULL: no operand row */
+  const float *mean, *rstd;       /* NULL: no normalisation */
+} b200_obs_rows_t;
+int b200env_obs_imitation_rows(b200env_handle h, const b200_obs_rows_t* d, void* stream);
 
 /* The imitation policy's first-layer operand at test time (ImitatorBuilder.Network.preprocess_input, non-training branch, + running_obs,
  * embodied_pose/models/im_network_builder.py:117-189): the 734-wide observation of compute_humanoid_observations_imitation with
@@ -310,8 +332,16 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
  * j in [0, num_frames): t = motion_times[i] + dt + (first_frame + j) * dt; writes
  * context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos  ([N, num_frames, 2*(3B+D)+4B] row-major) and
  * context_mask[row, j] = t <= motion_length + 2 dt, with row = env_ids[i] (or i when env_ids is NULL). */
-int b200env_motion_context(b200env_handle h, const int64_t* env_ids, const int64_t* motion_ids, const float* motion_times, int32_t n,
-                           int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, void* stream);
+typedef struct b200_motion_context {
+  int32_t n, num_frames, first_frame;
+  float dt;
+  const int64_t* env_ids;      /* [n] or NULL */
+  const int64_t* motion_ids;   /* [n] */
+  const float* motion_times;   /* [n] */
+  float* context_feat;
+  uint8_t* context_mask;
+} b200_motion_context_t;
+int b200env_motion_context(b200env_handle h, const b200_motion_context_t* d, void* stream);
 
 /* Heterogeneous assets per env (dual mode: env 2k = player 0's asset, env 2k+1 = player 1's,
  * vid2player/env/tasks/humanoid_smpl_im_mvae.py:270-275 `motion_ids[1::2] = 1`): one handle per asset, all bound to the SAME

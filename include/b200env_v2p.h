@@ -17,25 +17,51 @@ const char* b200v2p_last_error(void);
  * root position of this call is stored there - `_save_prev_target_motion_state` (:741-750) and `self._target_root_pos = root_pos`
  * (:655) folded into the launch; prev_root_pos_update may be the same buffer as prev_root_pos.  only_mask (may be NULL): bool [n], the
  * envs whose entry is 0 are skipped (mask-driven reset: FK of the envs being reset only). */
-int b200v2p_smpl_to_sim(int32_t n, const float* root_pos, const float* joint_rotmat, const float* rest, int32_t num_rest,
-                        const int32_t* parents, const int32_t* smpl_2_mujoco, float dt, const float* prev_root_pos, const float* prev_rb_rot, float* root_rot,
-                        float* dof_pos, float* root_vel, float* root_ang_vel, float* dof_vel, float* rb_pos, float* rb_rot, float* prev_root_pos_update,
-                        float* target_root_pos_out, const uint8_t* only_mask, void* stream);
+typedef struct b200v2p_smpl {
+  int32_t n, num_rest;
+  float dt;
+  int32_t pad_;
+  const float *root_pos, *joint_rotmat, *rest; /* [n,3], [n,24,3,3], [num_rest,24,3] */
+  const int32_t *parents, *smpl_2_mujoco;      /* [24] */
+  const float *prev_root_pos, *prev_rb_rot;    /* NULL: zero velocities */
+  float *root_rot, *dof_pos, *root_vel, *root_ang_vel, *dof_vel, *rb_pos, *rb_rot;
+  float *prev_root_pos_update, *target_root_pos_out; /* NULL: not stored */
+  const uint8_t* only_mask;                    /* NULL: every env */
+} b200v2p_smpl_t;
+int b200v2p_smpl_to_sim(const b200v2p_smpl_t* d, void* stream);
 
 /* replaces the fix_head_orientation block of _set_target_motion_state (env/tasks/humanoid_smpl_im_mvae.py:605-634):
  * rb_pos/rb_rot [n,24,*] = FK of the uncorrected pose (MuJoCo order, head_body = 13); joint_rotmat [n,24,3,3] (SMPL order) is
  * corrected in place at SMPL joints Head (15) and Neck (12). */
-int b200v2p_fix_head(int32_t n, const float* rb_pos, const float* rb_rot, int32_t head_body, const float* ball_pos, const float* root_pos,
-                     float* joint_rotmat, void* stream);
+typedef struct b200v2p_head {
+  int32_t n, head_body;
+  const float *rb_pos, *rb_rot, *ball_pos, *root_pos;
+  float* joint_rotmat;
+} b200v2p_head_t;
+int b200v2p_fix_head(const b200v2p_head_t* d, void* stream);
 
 /* replaces apply_external_force_to_ball (env/tasks/humanoid_smpl_im_mvae.py:711-739): drag + Magnus lift, bounce flag */
-int b200v2p_ball_aero(int32_t n, const float* ball_states, int32_t stride, uint8_t* has_bounce, uint8_t* has_bounce_now, float* bounce_pos,
-                      float* force, int32_t substeps, float spin_scale, void* stream);
+typedef struct b200v2p_aero {
+  int32_t n, stride, substeps; /* stride: floats between consecutive envs' ball rows, >= 13 */
+  float spin_scale;
+  const float* ball_states;
+  uint8_t *has_bounce, *has_bounce_now;
+  float *bounce_pos, *force;
+} b200v2p_aero_t;
+int b200v2p_ball_aero(const b200v2p_aero_t* d, void* stream);
 
 /* replaces _reset_balls + TennisBallGeneratorOffline.generate (:503-524, utils/tennis_ball.py:435-456): pool [P,307] */
-int b200v2p_ball_reset(int32_t n, const int64_t* env_ids, const int64_t* pool_index, const float* pool, float* ball_states, int32_t stride,
-                       float* ball_pos, float* ball_vel, uint8_t* has_bounce, float* bounce_pos, uint8_t* has_contact, float* traj,
-                       void* stream);
+typedef struct b200v2p_breset {
+  int32_t n, stride;           /* stride: floats between consecutive envs' ball rows, >= 13 */
+  const int64_t *env_ids, *pool_index;
+  const float* pool;
+  float *ball_states, *ball_pos, *ball_vel;
+  uint8_t* has_bounce;
+  float* bounce_pos;
+  uint8_t* has_contact;
+  float* traj;
+} b200v2p_breset_t;
+int b200v2p_ball_reset(const b200v2p_breset_t* d, void* stream);
 
 /* replaces _update_state_from_sim (:799-860), substeps > 2 contact detector */
 typedef struct b200v2p_state {
@@ -140,8 +166,14 @@ int b200v2p_pre_step(const b200v2p_prestep_t* p, void* stream);
 
 /* the controller's own bookkeeping of a humanoid reset (env/tasks/physics_mvae_controller.py:176-181, 203-210) for the envs whose mask
  * is set: progress / reset / terminate / num_reset_reaction <- 0, distance <- 0, num_reset += 1 */
-int b200v2p_ctrl_reset(int32_t n, const uint8_t* mask, int64_t* progress_buf, int64_t* reset_buf, int64_t* terminate_buf, int64_t* num_reset_reaction,
-                       float* distance, int64_t* num_reset, void* stream);
+typedef struct b200v2p_creset {
+  int32_t n, pad_;
+  const uint8_t* mask;
+  int64_t *progress_buf, *reset_buf, *terminate_buf, *num_reset_reaction;
+  float* distance;
+  int64_t* num_reset;
+} b200v2p_creset_t;
+int b200v2p_ctrl_reset(const b200v2p_creset_t* d, void* stream);
 
 /* The resident kinematic target stream that stands in for the unreleased MVAE motion generator (SURVEY.md 8d, config 3): `frames`
  * frames of every field for all n envs are kept in HBM ([frames * n, ...], frame-major); env e reads frame (clock + advance +
@@ -170,8 +202,15 @@ int b200v2p_stream_gather(const b200v2p_stream_t* s, void* stream);
  * ball_states + contact_ids[i]*stride (the ball the opponent just hit) is snapped to the table grid; outputs the incoming
  * trajectory in the receiver's frame traj[n,50,3] and the snapped in / out ball states [n,13].  The caller scatters them
  * (states[ball_ids] = in, then states[contact_ids] = out).  table [rows,50,2]; params = HEIGHT, VEL_X, VEL_Y, VSPIN (lo,hi,step). */
-int b200v2p_ball_in_estimate(int32_t n, const int64_t* contact_ids, const float* ball_states, int32_t stride, const float* table,
-                             int64_t table_rows, const double* params, float* traj, float* states_in, float* states_out, void* stream);
+typedef struct b200v2p_inest {
+  int32_t n, stride;
+  int64_t table_rows;
+  double params[12];
+  const int64_t* contact_ids;
+  const float *ball_states, *table;
+  float *traj, *states_in, *states_out;
+} b200v2p_inest_t;
+int b200v2p_ball_in_estimate(const b200v2p_inest_t* d, void* stream);
 
 /* replaces the per-step task part of PhysicsMVAEController._reset_envs when no humanoid needs a reset
  * (env/tasks/physics_mvae_controller.py:173-201: _reset_balls for the reaction envs :503-524, _reset_recovery_tasks :242-245,

@@ -10,11 +10,14 @@ import torch
 import test_host
 from vid2player3d_b200 import abi, native
 
-C_NAMES = {C.c_float: "float", C.c_int64: "int64_t", C.c_uint8: "uint8_t", C.c_uint32: "uint32_t"}
+C_NAMES = {C.c_float: "float", C.c_int64: "int64_t", C.c_uint8: "uint8_t", C.c_uint32: "uint32_t", C.c_int32: "int32_t"}
 # the descriptors native.fill fills, and a dtype each typed pointer field must refuse
-FILLED = ("MotionLibView", "Buffers", "V2PState", "V2PCtrl", "V2PPreStep", "V2PStream", "V2PTaskReset", "V2PActorReset", "V2PRec", "V2PBest")
-DTYPE = {abi.F32P: torch.float32, abi.I64P: torch.int64, abi.U8P: torch.bool, abi.U32P: torch.int32, C.c_void_p: torch.bfloat16}
-WRONG = {abi.F32P: torch.float64, abi.I64P: torch.int32, abi.U8P: torch.int32, abi.U32P: torch.int64}
+FILLED = ("MotionLibView", "Buffers", "V2PState", "V2PCtrl", "V2PPreStep", "V2PStream", "V2PTaskReset", "V2PActorReset", "V2PRec", "V2PBest",
+          "ResetMasked", "MotionState", "MotionContext", "ObsImitation", "ObsRows", "V2PSmpl", "V2PHead", "V2PAero", "V2PBallReset",
+          "V2PCtrlReset", "V2PInEst")
+DTYPE = {abi.F32P: torch.float32, abi.I64P: torch.int64, abi.U8P: torch.bool, abi.U32P: torch.int32, abi.I32P: torch.int32,
+         C.c_void_p: torch.bfloat16}
+WRONG = {abi.F32P: torch.float64, abi.I64P: torch.int32, abi.U8P: torch.int32, abi.U32P: torch.int64, abi.I32P: torch.int64}
 
 
 def fields(kind):

@@ -471,20 +471,21 @@ def test_entry_points_and_layouts(handles, big_inputs, asset, jpos, lr, rh):
 
 
 @pytest.mark.gpu
-def test_jpos_rows_through_the_c_abi(handles, big_inputs):
-    """bit 1 of local_root_obs selects the 513-wide row on b200env_obs_imitation_rows, called through ctypes"""
+def test_jpos_field_through_the_c_abi(handles, big_inputs):
+    """the jpos field selects the 513-wide row on b200env_obs_imitation_rows, called through ctypes"""
     import torch
+    from vid2player3d_b200 import abi
     from vid2player3d_b200.native import lib
     env, bpe = handles["federer"]
     inp = {k: v[:MID] for k, v in big_inputs[0].items()}
     d = dev_inputs(inp, bpe)
     want = run_rows(env, d, MID, 1, 1, True)
     obs, op = sent_obs(MID, True), sent_op(MID, 768)
-    p = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
-    rc = lib().b200env_obs_imitation_rows(env._h, C.c_int32(MID), p(d["rbs"]), C.c_int32(bpe), p(d["dofs"]), p(d["target_pos"]),
-                                          p(d["target_rot"]), p(d["target_dof_pos"]), p(d["motion_bodies"]), C.c_int32(1 | 2), C.c_int32(1),
-                                          p(obs), p(op), C.c_int32(768), None, None, C.c_float(5.0),
-                                          C.c_void_p(torch.cuda.current_stream().cuda_stream))
+    desc = abi.ObsRows(n=MID, bodies_per_env=bpe, local_root_obs=1, root_height_obs=1, jpos=1, ld_bf16=768, clamp=5.0,
+                       rigid_body_state=d["rbs"].data_ptr(), dof_state=d["dofs"].data_ptr(), target_pos=d["target_pos"].data_ptr(),
+                       target_rot=d["target_rot"].data_ptr(), target_dof_pos=d["target_dof_pos"].data_ptr(),
+                       motion_bodies=d["motion_bodies"].data_ptr(), obs=obs.data_ptr(), obs_bf16=op.data_ptr())
+    rc = lib().b200env_obs_imitation_rows(env._h, C.byref(desc), C.c_void_p(torch.cuda.current_stream().cuda_stream))
     torch.cuda.synchronize()
     assert rc == 0, lib().b200env_last_error()
     assert torch.equal(bits(obs), bits(want))

@@ -669,7 +669,7 @@ def test_comparators_reject_mutated_oracles():
     rejects(compare(ref, bad, {"traj": "exact"}, rows=fin, limit=None), "traj", int(fin[0]))
 
 
-def test_entry_points_refuse_bad_arguments():
+def test_descriptor_entry_points_refuse_bad_arguments():
     """update_state (n < 0, strides below 13, racket / wrist bodies of either player outside [0, bodies_per_env)), ball_reset (stride
     below 13) and ball_in_estimate (stride below 13, a grid step <= 0 or NaN) refuse before any launch: fake, never dereferenced
     pointers reach every rule on a machine without a GPU"""
@@ -677,7 +677,6 @@ def test_entry_points_refuse_bad_arguments():
     from vid2player3d_b200.native import lib
     L = lib()
     L.b200v2p_last_error.restype = C.c_char_p
-    p = C.c_void_p(256)
 
     def state(**kw):
         s = abi.V2PState()
@@ -695,13 +694,13 @@ def test_entry_points_refuse_bad_arguments():
                              (dict(dual=1, wrist_body2=-1), -2, "racket and wrist"), (dict(bodies_per_env=24), -2, "racket and wrist")):
         rc, err = state(**kw)
         assert rc == rc_want and msg in err and "update_state" in err, (kw, rc, err)
-    rc = L.b200v2p_ball_reset(C.c_int32(4), p, p, p, p, C.c_int32(12), p, p, p, p, p, p, None)
+    fake = lambda S, **kw: S(**kw, **{f: 256 for f, ct in S._fields_ if issubclass(ct, C.c_void_p)})  # noqa: E731
+    rc = L.b200v2p_ball_reset(C.byref(fake(abi.V2PBallReset, n=4, stride=12)), None)
     assert rc == -1 and "ball_reset" in L.b200v2p_last_error().decode()
     good = [float(v) for v in IN_COARSE.reshape(-1)]
 
     def est(stride, params):
-        arr = (C.c_double * 12)(*params)
-        rc = L.b200v2p_ball_in_estimate(C.c_int32(4), p, p, C.c_int32(stride), p, C.c_int64(160), C.cast(arr, C.c_void_p), p, p, p, None)
+        rc = L.b200v2p_ball_in_estimate(C.byref(fake(abi.V2PInEst, n=4, stride=stride, table_rows=160, params=(C.c_double * 12)(*params))), None)
         return rc, L.b200v2p_last_error().decode()
     rc, err = est(12, good)
     assert rc == -1 and "ball_in_estimate" in err

@@ -24,7 +24,12 @@ STRUCT_MIRRORS = [("abi", "Model", "b200_model_t"), ("abi", "Cfg", "b200_cfg_t")
                   ("abi", "V2PPreStep", "b200v2p_prestep_t"), ("abi", "V2PStream", "b200v2p_stream_t"),
                   ("abi", "V2PTaskReset", "b200v2p_treset_t"), ("abi", "V2PActorReset", "b200v2p_areset_t"),
                   ("abi", "V2PRec", "b200v2p_rec_t"), ("abi", "V2PBest", "b200v2p_best_t"), ("abi", "V2PBhProb", "b200v2p_bhprob_t"),
-                  ("abi", "V2PBhFix", "b200v2p_bhfix_t"), ("ball_gen", "BallSim", "b200ball_sim_t"), ("nn", "LinearDesc", "b200nn_linear_desc_t")]
+                  ("abi", "V2PBhFix", "b200v2p_bhfix_t"), ("ball_gen", "BallSim", "b200ball_sim_t"), ("nn", "LinearDesc", "b200nn_linear_desc_t"),
+                  ("abi", "ResetMasked", "b200_reset_masked_t"), ("abi", "MotionState", "b200_motion_state_t"),
+                  ("abi", "MotionContext", "b200_motion_context_t"), ("abi", "ObsImitation", "b200_obs_imitation_t"),
+                  ("abi", "ObsRows", "b200_obs_rows_t"), ("abi", "V2PSmpl", "b200v2p_smpl_t"), ("abi", "V2PHead", "b200v2p_head_t"),
+                  ("abi", "V2PAero", "b200v2p_aero_t"), ("abi", "V2PBallReset", "b200v2p_breset_t"), ("abi", "V2PCtrlReset", "b200v2p_creset_t"),
+                  ("abi", "V2PInEst", "b200v2p_inest_t")]
 
 
 def header_prototypes(*headers):
@@ -92,18 +97,18 @@ def test_env_bindings_match_header_prototypes():
     assert L.b200env_abi_version() == abi.ABI_VERSION
 
 
-def test_signature_check_rejects_a_dropped_or_widened_parameter(monkeypatch):
+def test_signature_check_rejects_a_dropped_or_widened_positional_parameter(monkeypatch):
     """negative controls of the prototype check: a table with one parameter dropped, or one int32_t bound as int64"""
     from vid2player3d_b200 import abi
     table = dict(abi.SIGNATURES)
-    res, args = table["b200env_reset_masked"]
-    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200env_reset_masked=(res, args[:-1])))
-    assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == ["b200env_reset_masked: 17 parameters, header 18"]
-    res, args = table["b200v2p_ball_in_estimate"]
-    assert args[3] is C.c_int32                                   # the ball row stride; table_rows next to it is the int64_t
-    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200v2p_ball_in_estimate=(res, args[:3] + [C.c_int64] + args[4:])))
+    res, args = table["b200env_physics_only"]
+    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200env_physics_only=(res, args[:-1])))
+    assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == ["b200env_physics_only: 14 parameters, header 15"]
+    res, args = table["b200ball_simulate"]
+    assert args[2] is C.c_int32                                   # the precision flag; n next to it is the int64_t
+    monkeypatch.setattr(abi, "SIGNATURES", dict(table, b200ball_simulate=(res, args[:2] + [C.c_int64] + args[3:])))
     assert signature_mismatches(abi.SIGNATURES, ENV_HEADERS) == [
-        f"b200v2p_ball_in_estimate: parameter 3 is {C.c_int64.__name__}, header {C.c_int32.__name__}"]
+        f"b200ball_simulate: parameter 2 is {C.c_int64.__name__}, header {C.c_int32.__name__}"]
 
 
 def test_struct_layouts_match_header(tmp_path):

@@ -81,10 +81,10 @@ def test_loader_refusals(kw, msg):
         nn.im_networks_from_checkpoint(checkpoint("running"), **kw)
 
 
-def test_abi_versions_and_layouts(tmp_path):
-    assert abi.ABI_VERSION == 10 and nn.ABI_VERSION == 2
+def test_abi_version_11_and_layouts(tmp_path):
+    assert abi.ABI_VERSION == 11 and nn.ABI_VERSION == 2
     text = open(os.path.join(test_host.ROOT, "include", "b200env.h")).read()
-    assert "#define B200_ABI_VERSION 10" in text
+    assert "#define B200_ABI_VERSION 11" in text
     assert "#define B200NN_ABI_VERSION 2" in open(os.path.join(test_host.ROOT, "include", "b200nn.h")).read()
     mirrors = [(abi.ImPolicy, "b200_im_policy_t"), (abi.PlayStats, "b200_play_stats_t"), (nn.LinearDesc, "b200nn_linear_desc_t")]
     lines, want = [], []

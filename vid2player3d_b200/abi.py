@@ -5,7 +5,7 @@ import ctypes as C
 import numpy as np
 
 MAX_BODIES, MAX_DOF, MAX_KEY = 32, 96, 8
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 # Pointer fields of the descriptor structs below carry the element type the header points at; native.fill refuses a tensor of any
@@ -26,6 +26,10 @@ class U8P(C.c_void_p):
 
 class U32P(C.c_void_p):
     pointee = C.c_uint32
+
+
+class I32P(C.c_void_p):
+    pointee = C.c_int32
 
 
 class F64P(C.c_void_p):
@@ -294,7 +298,113 @@ class PlayStats(C.Structure):
     _nullable_, _defaults_ = (), ()
 
 
+class ResetMasked(C.Structure):
+    """b200_reset_masked_t: the mask-driven reset of the imitation task (b200env_reset_masked)"""
+    _fields_ = [
+        ("sample_time", C.c_int32), ("truncate", C.c_float), ("ref_prob", C.c_float), ("num_frames", C.c_int32),
+        ("first_frame", C.c_int32), ("dt", C.c_float), ("seed", C.c_uint64),
+        ("mask", U8P), ("counter", I64P), ("init_root", F32P), ("init_dof_pos", F32P), ("init_dof_vel", F32P), ("reset_times", F32P),
+        ("context_feat", F32P), ("context_mask", U8P), ("work", I32P),
+    ]
+    _nullable_, _defaults_ = ("init_root", "init_dof_pos", "init_dof_vel"), ()
+
+
+class MotionState(C.Structure):
+    """b200_motion_state_t: MoCap states of (id, time) pairs (b200env_motion_state)"""
+    _fields_ = [
+        ("n", C.c_int32), ("pad_", C.c_int32), ("motion_ids", I64P), ("motion_times", F32P),
+        ("root_pos", F32P), ("root_rot", F32P), ("dof_pos", F32P), ("root_vel", F32P), ("root_ang_vel", F32P), ("dof_vel", F32P),
+        ("key_pos", F32P), ("rb_pos", F32P), ("rb_rot", F32P),
+    ]
+    _nullable_ = ("root_pos", "root_rot", "dof_pos", "root_vel", "root_ang_vel", "dof_vel", "key_pos", "rb_pos", "rb_rot")
+    _defaults_ = ("pad_",)
+
+
+class MotionContext(C.Structure):
+    """b200_motion_context_t: the MoCap context window of listed envs (b200env_motion_context)"""
+    _fields_ = [
+        ("n", C.c_int32), ("num_frames", C.c_int32), ("first_frame", C.c_int32), ("dt", C.c_float),
+        ("env_ids", I64P), ("motion_ids", I64P), ("motion_times", F32P), ("context_feat", F32P), ("context_mask", U8P),
+    ]
+    _nullable_, _defaults_ = ("env_ids",), ()
+
+
+class ObsImitation(C.Structure):
+    """b200_obs_imitation_t: the imitation observation from contiguous gathers (b200env_obs_imitation)"""
+    _fields_ = [
+        ("n", C.c_int32), ("local_root_obs", C.c_int32), ("root_height_obs", C.c_int32), ("jpos", C.c_int32),
+        ("body_pos", F32P), ("body_rot", F32P), ("target_pos", F32P), ("target_rot", F32P), ("dof_pos", F32P), ("dof_vel", F32P),
+        ("target_dof_pos", F32P), ("body_vel", F32P), ("body_ang_vel", F32P), ("motion_bodies", F32P), ("obs", F32P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
+class ObsRows(C.Structure):
+    """b200_obs_rows_t: the imitation observation from the state rows, and the policy's bf16 operand row (b200env_obs_imitation_rows)"""
+    _fields_ = [
+        ("n", C.c_int32), ("bodies_per_env", C.c_int32), ("local_root_obs", C.c_int32), ("root_height_obs", C.c_int32),
+        ("jpos", C.c_int32), ("ld_bf16", C.c_int32), ("clamp", C.c_float), ("pad_", C.c_int32),
+        ("rigid_body_state", F32P), ("dof_state", F32P), ("target_pos", F32P), ("target_rot", F32P), ("target_dof_pos", F32P),
+        ("motion_bodies", F32P), ("obs", F32P), ("obs_bf16", C.c_void_p), ("mean", F32P), ("rstd", F32P),
+    ]
+    _nullable_, _defaults_ = ("obs_bf16", "mean", "rstd"), ("pad_",)
+
+
 # ---------------------------------------------------------------- include/b200env_v2p.h
+class V2PSmpl(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("num_rest", C.c_int32), ("dt", C.c_float), ("pad_", C.c_int32),
+        ("root_pos", F32P), ("joint_rotmat", F32P), ("rest", F32P), ("parents", I32P), ("smpl_2_mujoco", I32P),
+        ("prev_root_pos", F32P), ("prev_rb_rot", F32P),
+        ("root_rot", F32P), ("dof_pos", F32P), ("root_vel", F32P), ("root_ang_vel", F32P), ("dof_vel", F32P), ("rb_pos", F32P),
+        ("rb_rot", F32P), ("prev_root_pos_update", F32P), ("target_root_pos_out", F32P), ("only_mask", U8P),
+    ]
+    _nullable_ = ("prev_root_pos", "prev_rb_rot", "prev_root_pos_update", "target_root_pos_out", "only_mask")
+    _defaults_ = ("pad_",)
+
+
+class V2PHead(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("head_body", C.c_int32),
+        ("rb_pos", F32P), ("rb_rot", F32P), ("ball_pos", F32P), ("root_pos", F32P), ("joint_rotmat", F32P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
+class V2PAero(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("stride", C.c_int32), ("substeps", C.c_int32), ("spin_scale", C.c_float),
+        ("ball_states", F32P), ("has_bounce", U8P), ("has_bounce_now", U8P), ("bounce_pos", F32P), ("force", F32P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
+class V2PBallReset(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("stride", C.c_int32),
+        ("env_ids", I64P), ("pool_index", I64P), ("pool", F32P), ("ball_states", F32P), ("ball_pos", F32P), ("ball_vel", F32P),
+        ("has_bounce", U8P), ("bounce_pos", F32P), ("has_contact", U8P), ("traj", F32P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
+class V2PCtrlReset(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("pad_", C.c_int32),
+        ("mask", U8P), ("progress_buf", I64P), ("reset_buf", I64P), ("terminate_buf", I64P), ("num_reset_reaction", I64P),
+        ("distance", F32P), ("num_reset", I64P),
+    ]
+    _nullable_, _defaults_ = (), ("pad_",)
+
+
+class V2PInEst(C.Structure):
+    _fields_ = [
+        ("n", C.c_int32), ("stride", C.c_int32), ("table_rows", C.c_int64), ("params", C.c_double * 12),
+        ("contact_ids", I64P), ("ball_states", F32P), ("table", F32P), ("traj", F32P), ("states_in", F32P), ("states_out", F32P),
+    ]
+    _nullable_, _defaults_ = (), ()
+
+
 class V2PState(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("bodies_per_env", C.c_int32), ("ball_stride", C.c_int32), ("root_stride", C.c_int32),
@@ -449,7 +559,7 @@ def bhfix_scratch_bytes(Ts, scalar_bytes):
 # applies all of them when it loads the library, so an argument too many or too few, or one that does not convert to its C type,
 # raises ctypes.ArgumentError at the call instead of reaching the library as an undefined register.  Pointers and opaque handles
 # are c_void_p.  tests/test_host.py holds the table to the headers.
-_i32, _i64, _u64, _f32, _p = C.c_int32, C.c_int64, C.c_uint64, C.c_float, C.c_void_p
+_i32, _i64, _p = C.c_int32, C.c_int64, C.c_void_p
 SIGNATURES = {
     # include/b200env.h
     "b200env_abi_version": (C.c_int, []),
@@ -460,12 +570,12 @@ SIGNATURES = {
     "b200env_set_motion_lib": (C.c_int, [_p, _p]),
     "b200env_step": (C.c_int, [_p, _p, _p]),
     "b200env_reset": (C.c_int, [_p, _p, _p, _i32, _p]),
-    "b200env_reset_masked": (C.c_int, [_p, _p, _i32, _f32, _f32, _u64, _p, _p, _p, _p, _p, _i32, _i32, _f32, _p, _p, _p, _p]),
-    "b200env_motion_state": (C.c_int, [_p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
-    "b200env_obs_imitation": (C.c_int, [_p, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _i32, _p, _p]),
-    "b200env_obs_imitation_rows": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p, _p, _p, _i32, _i32, _p, _p, _i32, _p, _p, _f32, _p]),
+    "b200env_reset_masked": (C.c_int, [_p, _p, _p]),
+    "b200env_motion_state": (C.c_int, [_p, _p, _p]),
+    "b200env_obs_imitation": (C.c_int, [_p, _p, _p]),
+    "b200env_obs_imitation_rows": (C.c_int, [_p, _p, _p]),
     "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
-    "b200env_motion_context": (C.c_int, [_p, _p, _p, _p, _i32, _i32, _i32, _f32, _p, _p, _p]),
+    "b200env_motion_context": (C.c_int, [_p, _p, _p]),
     "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),
     "b200env_play_stats": (C.c_int, [_p, _p]),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
@@ -482,16 +592,16 @@ SIGNATURES = {
     "b200env_kernel_ms": (C.c_int, [_p, _p, _p]),
     # include/b200env_v2p.h
     "b200v2p_last_error": (C.c_char_p, []),
-    "b200v2p_smpl_to_sim": (C.c_int, [_i32, _p, _p, _p, _i32, _p, _p, _f32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
-    "b200v2p_fix_head": (C.c_int, [_i32, _p, _p, _i32, _p, _p, _p, _p]),
-    "b200v2p_ball_aero": (C.c_int, [_i32, _p, _i32, _p, _p, _p, _p, _i32, _f32, _p]),
-    "b200v2p_ball_reset": (C.c_int, [_i32, _p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "b200v2p_smpl_to_sim": (C.c_int, [_p, _p]),
+    "b200v2p_fix_head": (C.c_int, [_p, _p]),
+    "b200v2p_ball_aero": (C.c_int, [_p, _p]),
+    "b200v2p_ball_reset": (C.c_int, [_p, _p]),
     "b200v2p_update_state": (C.c_int, [_p, _p]),
     "b200v2p_controller_post": (C.c_int, [_p, _p]),
     "b200v2p_pre_step": (C.c_int, [_p, _p]),
-    "b200v2p_ctrl_reset": (C.c_int, [_i32, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200v2p_ctrl_reset": (C.c_int, [_p, _p]),
     "b200v2p_stream_gather": (C.c_int, [_p, _p]),
-    "b200v2p_ball_in_estimate": (C.c_int, [_i32, _p, _p, _i32, _p, _i64, _p, _p, _p, _p, _p]),
+    "b200v2p_ball_in_estimate": (C.c_int, [_p, _p]),
     "b200v2p_task_reset": (C.c_int, [_p, _p]),
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
     "b200v2p_eval_record": (C.c_int, [_p, _p]),

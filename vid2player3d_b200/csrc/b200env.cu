@@ -2576,64 +2576,62 @@ int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_
   return 0;
 }
 
-int b200env_reset_masked(b200env_handle h, const uint8_t* mask, int32_t sample_time, float truncate, float ref_prob, uint64_t seed,
-                         int64_t* counter, const float* init_root, const float* init_dof_pos, const float* init_dof_vel, float* reset_times,
-                         int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, int32_t* work,
-                         void* stream) {
+int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* stream) {
   if (!h) return fail(-1, "b200env_reset_masked: null handle%s");
-  if (!mask || !counter || !reset_times || !context_feat || !context_mask || !work || num_frames < 1)
+  if (!d || !d->mask || !d->counter || !d->reset_times || !d->context_feat || !d->context_mask || !d->work || d->num_frames < 1)
     return fail(-1, "b200env_reset_masked: bad arguments%s");
-  if (ref_prob < 1.0f && (!init_root || !init_dof_pos || !init_dof_vel))
+  if (d->ref_prob < 1.0f && (!d->init_root || !d->init_dof_pos || !d->init_dof_vel))
     return fail(-1, "b200env_reset_masked: ref_prob < 1 needs the initial root and dof buffers%s");
   if (!h->bound || !h->has_ml) return fail(-4, "b200env_reset_masked: bind buffers and a motion lib first%s");
   cudaSetDevice(h->device);
   const int n = h->num_envs;
   reset_masked_kernel<<<(n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
-      (const DevBlob*)h->d_blob, h->d_cfg, h->bufs, h->ml, n, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos,
-      init_dof_vel, reset_times, work);
+      (const DevBlob*)h->d_blob, h->d_cfg, h->bufs, h->ml, n, d->mask, d->sample_time, d->truncate, d->ref_prob, d->seed, d->counter,
+      d->init_root, d->init_dof_pos, d->init_dof_vel, d->reset_times, d->work);
   CUDA_OK(cudaGetLastError());
   int sms = 0;
   CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-  const int64_t warps = (int64_t)n * num_frames;
+  const int64_t warps = (int64_t)n * d->num_frames;
   const int grid = (int)std::min<int64_t>((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (int64_t)sms * 8);
   reset_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
-                                                                              reset_times, work, counter, num_frames, first_frame, dt,
-                                                                              (float)(2.0 * (double)dt), context_feat, context_mask);
+                                                                              d->reset_times, d->work, d->counter, d->num_frames, d->first_frame,
+                                                                              d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
   CUDA_OK(cudaGetLastError());
   h->launches += 2;
   return 0;
 }
 
-int b200env_motion_state(b200env_handle h, const int64_t* motion_ids, const float* motion_times, int32_t n, float* root_pos,
-                         float* root_rot, float* dof_pos, float* root_vel, float* root_ang_vel, float* dof_vel, float* key_pos,
-                         float* rb_pos, float* rb_rot, void* stream) {
+int b200env_motion_state(b200env_handle h, const b200_motion_state_t* d, void* stream) {
   if (!h) return fail(-1, "b200env_motion_state: null handle%s");
+  if (!d) return fail(-1, "b200env_motion_state: bad arguments%s");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (!motion_ids || !motion_times || n < 0) return fail(-1, "b200env_motion_state: bad arguments%s");
+  if (!d->motion_ids || !d->motion_times || n < 0) return fail(-1, "b200env_motion_state: bad arguments%s");
   if (!h->has_ml) return fail(-4, "b200env_motion_state: set a motion lib first%s");
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-  motion_state_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, motion_ids,
-                                                                             motion_times, n, root_pos, root_rot, dof_pos, root_vel,
-                                                                             root_ang_vel, dof_vel, key_pos, rb_pos, rb_rot);
+  motion_state_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, d->motion_ids,
+                                                                             d->motion_times, n, d->root_pos, d->root_rot, d->dof_pos, d->root_vel,
+                                                                             d->root_ang_vel, d->dof_vel, d->key_pos, d->rb_pos, d->rb_rot);
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;
 }
 
-int b200env_motion_context(b200env_handle h, const int64_t* env_ids, const int64_t* motion_ids, const float* motion_times, int32_t n,
-                           int32_t num_frames, int32_t first_frame, float dt, float* context_feat, uint8_t* context_mask, void* stream) {
+int b200env_motion_context(b200env_handle h, const b200_motion_context_t* d, void* stream) {
   if (!h) return fail(-1, "b200env_motion_context: null handle%s");
+  if (!d) return fail(-1, "b200env_motion_context: bad arguments%s");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (!motion_ids || !motion_times || !context_feat || !context_mask || n < 0 || num_frames < 1)
+  if (!d->motion_ids || !d->motion_times || !d->context_feat || !d->context_mask || n < 0 || d->num_frames < 1)
     return fail(-1, "b200env_motion_context: bad arguments%s");
   if (!h->has_ml) return fail(-4, "b200env_motion_context: set a motion lib first%s");
   cudaSetDevice(h->device);
-  const int64_t warps = (int64_t)n * num_frames;
+  const int64_t warps = (int64_t)n * d->num_frames;
   const int grid = (int)((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
-  motion_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, env_ids, motion_ids,
-                                                                               motion_times, n, num_frames, first_frame, dt,
-                                                                               (float)(2.0 * (double)dt), context_feat, context_mask);
+  motion_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, d->env_ids,
+                                                                               d->motion_ids, d->motion_times, n, d->num_frames, d->first_frame,
+                                                                               d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;
@@ -2648,56 +2646,56 @@ static int obs_row_check(const char* who, int nbl, int shape_dim, int W) {
   return 0;
 }
 
-int b200env_obs_imitation(b200env_handle h, int32_t n, const float* body_pos, const float* body_rot, const float* target_pos,
-                          const float* target_rot, const float* dof_pos, const float* dof_vel, const float* target_dof_pos,
-                          const float* body_vel, const float* body_ang_vel, const float* motion_bodies, int32_t local_root_obs,
-                          int32_t root_height_obs, float* obs, void* stream) {
+int b200env_obs_imitation(b200env_handle h, const b200_obs_imitation_t* d, void* stream) {
   if (!h) return fail(-1, "b200env_obs_imitation: null handle%s");
+  if (!d) return fail(-1, "b200env_obs_imitation: bad arguments%s");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (!body_pos || !body_rot || !target_pos || !target_rot || !dof_pos || !dof_vel || !target_dof_pos || !body_vel || !body_ang_vel ||
-      !motion_bodies || !obs || n < 0)
+  if (!d->body_pos || !d->body_rot || !d->target_pos || !d->target_rot || !d->dof_pos || !d->dof_vel || !d->target_dof_pos || !d->body_vel ||
+      !d->body_ang_vel || !d->motion_bodies || !d->obs || n < 0)
     return fail(-1, "b200env_obs_imitation: bad arguments%s");
   const int nbl = h->has_ml ? h->ml.num_lib_bodies : (h->model.fixed[h->model.nb - 1] ? h->model.nb - 1 : h->model.nb);
-  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, (local_root_obs >> 1) & 1);
+  const bool jpos = d->jpos != 0;
+  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, jpos);
   if (int rc = obs_row_check("b200env_obs_imitation", nbl, h->cfg.shape_dim, W)) return rc;
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-  obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(n, nbl, h->model.nd, h->cfg.shape_dim, body_pos, body_rot,
-                                                                              target_pos, target_rot, dof_pos, dof_vel, target_dof_pos,
-                                                                              body_vel, body_ang_vel, motion_bodies, local_root_obs & 1,
-                                                                              root_height_obs, obs, (local_root_obs >> 1) & 1,
+  obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(n, nbl, h->model.nd, h->cfg.shape_dim, d->body_pos,
+                                                                              d->body_rot, d->target_pos, d->target_rot, d->dof_pos, d->dof_vel,
+                                                                              d->target_dof_pos, d->body_vel, d->body_ang_vel, d->motion_bodies,
+                                                                              d->local_root_obs != 0, d->root_height_obs, d->obs, jpos,
                                                                               ObsStrides{nbl * 3, 3, nbl * 4, 4, h->model.nd, 1}, ObsBf16{nullptr, 0, nullptr, nullptr, 0.f});
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;
 }
 
-int b200env_obs_imitation_rows(b200env_handle h, int32_t n, const float* rigid_body_state, int32_t bodies_per_env, const float* dof_state,
-                               const float* target_pos, const float* target_rot, const float* target_dof_pos, const float* motion_bodies,
-                               int32_t local_root_obs, int32_t root_height_obs, float* obs, void* obs_bf16, int32_t ld_bf16, const float* mean,
-                               const float* rstd, float clamp, void* stream) {
-  if (!h || !rigid_body_state || !dof_state || !target_pos || !target_rot || !target_dof_pos || !motion_bodies || !obs)
+int b200env_obs_imitation_rows(b200env_handle h, const b200_obs_rows_t* d, void* stream) {
+  if (!h || !d || !d->rigid_body_state || !d->dof_state || !d->target_pos || !d->target_rot || !d->target_dof_pos || !d->motion_bodies || !d->obs)
     return fail(-1, "b200env_obs_imitation_rows: null argument%s");
+  const int n = d->n;
   if (n <= 0) return fail(-2, "b200env_obs_imitation_rows: n must be positive%s");
   const int nbl = h->has_ml ? h->ml.num_lib_bodies : (h->model.fixed[h->model.nb - 1] ? h->model.nb - 1 : h->model.nb);
-  if (bodies_per_env < nbl) return fail(-2, "b200env_obs_imitation_rows: bodies_per_env smaller than the humanoid%s");
-  if ((mean == nullptr) != (rstd == nullptr)) return fail(-2, "b200env_obs_imitation_rows: mean and rstd go together%s");
-  if (obs_bf16 && !(clamp > 0.f)) return fail(-2, "b200env_obs_imitation_rows: the bf16 row needs a positive clamp%s");
-  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, (local_root_obs >> 1) & 1);
+  if (d->bodies_per_env < nbl) return fail(-2, "b200env_obs_imitation_rows: bodies_per_env smaller than the humanoid%s");
+  if ((d->mean == nullptr) != (d->rstd == nullptr)) return fail(-2, "b200env_obs_imitation_rows: mean and rstd go together%s");
+  if (d->obs_bf16 && !(d->clamp > 0.f)) return fail(-2, "b200env_obs_imitation_rows: the bf16 row needs a positive clamp%s");
+  const bool jpos = d->jpos != 0;
+  const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, jpos);
   if (int rc = obs_row_check("b200env_obs_imitation_rows", nbl, h->cfg.shape_dim, W)) return rc;
-  if (obs_bf16) {   // the row goes out as bfloat162 pairs from column 0 of every row
-    if (ld_bf16 < W) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 is smaller than the observation row%s");
-    if (ld_bf16 & 1) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 must be even%s");
-    if (reinterpret_cast<uintptr_t>(obs_bf16) & 3) return fail(-2, "b200env_obs_imitation_rows: obs_bf16 must be 4-byte aligned%s");
+  if (d->obs_bf16) {   // the row goes out as bfloat162 pairs from column 0 of every row
+    if (d->ld_bf16 < W) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 is smaller than the observation row%s");
+    if (d->ld_bf16 & 1) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 must be even%s");
+    if (reinterpret_cast<uintptr_t>(d->obs_bf16) & 3) return fail(-2, "b200env_obs_imitation_rows: obs_bf16 must be 4-byte aligned%s");
   }
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-  const int nd = h->model.nd;
+  const int nd = h->model.nd, bpe = d->bodies_per_env;
+  const float* rbs = d->rigid_body_state;
   obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
-      n, nbl, nd, h->cfg.shape_dim, rigid_body_state, rigid_body_state + 3, target_pos, target_rot, dof_state, dof_state + 1, target_dof_pos,
-      rigid_body_state + 7, rigid_body_state + 10, motion_bodies, local_root_obs & 1, root_height_obs, obs, (local_root_obs >> 1) & 1,
-      ObsStrides{bodies_per_env * 13, 13, bodies_per_env * 13, 13, nd * 2, 2},
-      ObsBf16{reinterpret_cast<__nv_bfloat16*>(obs_bf16), ld_bf16, mean, rstd, clamp});
+      n, nbl, nd, h->cfg.shape_dim, rbs, rbs + 3, d->target_pos, d->target_rot, d->dof_state, d->dof_state + 1, d->target_dof_pos,
+      rbs + 7, rbs + 10, d->motion_bodies, d->local_root_obs != 0, d->root_height_obs, d->obs, jpos,
+      ObsStrides{bpe * 13, 13, bpe * 13, 13, nd * 2, 2},
+      ObsBf16{reinterpret_cast<__nv_bfloat16*>(d->obs_bf16), d->ld_bf16, d->mean, d->rstd, d->clamp});
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;

@@ -1237,61 +1237,67 @@ extern "C" {
 
 const char* b200v2p_last_error(void) { return g_verr; }
 
-int b200v2p_smpl_to_sim(int32_t n, const float* root_pos, const float* joint_rotmat, const float* rest, int32_t num_rest,
-                        const int32_t* parents, const int32_t* smpl_2_mujoco, float dt, const float* prev_root_pos, const float* prev_rb_rot, float* root_rot,
-                        float* dof_pos, float* root_vel, float* root_ang_vel, float* dof_vel, float* rb_pos, float* rb_rot, float* prev_root_pos_update,
-                        float* target_root_pos_out, const uint8_t* only_mask, void* stream) {
+int b200v2p_smpl_to_sim(const b200v2p_smpl_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_smpl_to_sim: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !root_pos || !joint_rotmat || !rest || !parents || !smpl_2_mujoco || !root_rot || !dof_pos || !root_vel || !root_ang_vel ||
-      !dof_vel || !rb_pos || !rb_rot)
+  if (n < 0 || !d->root_pos || !d->joint_rotmat || !d->rest || !d->parents || !d->smpl_2_mujoco || !d->root_rot || !d->dof_pos || !d->root_vel ||
+      !d->root_ang_vel || !d->dof_vel || !d->rb_pos || !d->rb_rot)
     return vfail(-1, "b200v2p_smpl_to_sim: bad arguments");
-  if (!(dt > 0)) return vfail(-2, "b200v2p_smpl_to_sim: dt must be positive");
-  if (num_rest < 1) return vfail(-2, "b200v2p_smpl_to_sim: num_rest must be >= 1");
+  if (!(d->dt > 0)) return vfail(-2, "b200v2p_smpl_to_sim: dt must be positive");
+  if (d->num_rest < 1) return vfail(-2, "b200v2p_smpl_to_sim: num_rest must be >= 1");
   smpl_to_sim_kernel<<<(n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      n, root_pos, joint_rotmat, rest, num_rest, parents, smpl_2_mujoco, dt, prev_root_pos, prev_rb_rot, root_rot, dof_pos, root_vel, root_ang_vel,
-      dof_vel, rb_pos, rb_rot, prev_root_pos_update, target_root_pos_out, only_mask);
+      n, d->root_pos, d->joint_rotmat, d->rest, d->num_rest, d->parents, d->smpl_2_mujoco, d->dt, d->prev_root_pos, d->prev_rb_rot, d->root_rot,
+      d->dof_pos, d->root_vel, d->root_ang_vel, d->dof_vel, d->rb_pos, d->rb_rot, d->prev_root_pos_update, d->target_root_pos_out, d->only_mask);
   V_CUDA_OK();
   return 0;
 }
 
-int b200v2p_fix_head(int32_t n, const float* rb_pos, const float* rb_rot, int32_t head_body, const float* ball_pos, const float* root_pos,
-                     float* joint_rotmat, void* stream) {
+int b200v2p_fix_head(const b200v2p_head_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_fix_head: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !rb_pos || !rb_rot || !ball_pos || !root_pos || !joint_rotmat || head_body < 0 || head_body > 23)
+  if (n < 0 || !d->rb_pos || !d->rb_rot || !d->ball_pos || !d->root_pos || !d->joint_rotmat || d->head_body < 0 || d->head_body > 23)
     return vfail(-1, "b200v2p_fix_head: bad arguments");
-  fix_head_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, rb_pos, rb_rot, head_body, ball_pos, root_pos, joint_rotmat);
+  fix_head_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, d->rb_pos, d->rb_rot, d->head_body, d->ball_pos, d->root_pos,
+                                                                     d->joint_rotmat);
   V_CUDA_OK();
   return 0;
 }
 
-int b200v2p_ball_aero(int32_t n, const float* ball_states, int32_t stride, uint8_t* has_bounce, uint8_t* has_bounce_now, float* bounce_pos,
-                      float* force, int32_t substeps, float spin_scale, void* stream) {
+int b200v2p_ball_aero(const b200v2p_aero_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_ball_aero: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !ball_states || !has_bounce || !has_bounce_now || !bounce_pos || !force || stride < 13) return vfail(-1, "b200v2p_ball_aero: bad arguments");
-  ball_aero_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, ball_states, stride, has_bounce, has_bounce_now, bounce_pos, force,
-                                                                     substeps, spin_scale);
+  if (n < 0 || !d->ball_states || !d->has_bounce || !d->has_bounce_now || !d->bounce_pos || !d->force || d->stride < 13)
+    return vfail(-1, "b200v2p_ball_aero: bad arguments");
+  ball_aero_kernel<<<(n + 127) / 128, 128, 0, (cudaStream_t)stream>>>(n, d->ball_states, d->stride, d->has_bounce, d->has_bounce_now,
+                                                                     d->bounce_pos, d->force, d->substeps, d->spin_scale);
   V_CUDA_OK();
   return 0;
 }
 
-int b200v2p_ball_reset(int32_t n, const int64_t* env_ids, const int64_t* pool_index, const float* pool, float* ball_states, int32_t stride,
-                       float* ball_pos, float* ball_vel, uint8_t* has_bounce, float* bounce_pos, uint8_t* has_contact, float* traj,
-                       void* stream) {
+int b200v2p_ball_reset(const b200v2p_breset_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_ball_reset: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !env_ids || !pool_index || !pool || !ball_states || !ball_pos || !ball_vel || !has_bounce || !bounce_pos || !has_contact || !traj ||
-      stride < 13)
+  if (n < 0 || !d->env_ids || !d->pool_index || !d->pool || !d->ball_states || !d->ball_pos || !d->ball_vel || !d->has_bounce || !d->bounce_pos ||
+      !d->has_contact || !d->traj || d->stride < 13)
     return vfail(-1, "b200v2p_ball_reset: bad arguments");
-  ball_reset_kernel<<<n, 64, 0, (cudaStream_t)stream>>>(n, env_ids, pool_index, pool, ball_states, stride, ball_pos, ball_vel, has_bounce,
-                                                        bounce_pos, has_contact, traj);
+  ball_reset_kernel<<<n, 64, 0, (cudaStream_t)stream>>>(n, d->env_ids, d->pool_index, d->pool, d->ball_states, d->stride, d->ball_pos,
+                                                        d->ball_vel, d->has_bounce, d->bounce_pos, d->has_contact, d->traj);
   V_CUDA_OK();
   return 0;
 }
 
-int b200v2p_ball_in_estimate(int32_t n, const int64_t* contact_ids, const float* ball_states, int32_t stride, const float* table,
-                             int64_t table_rows, const double* params, float* traj, float* states_in, float* states_out, void* stream) {
+int b200v2p_ball_in_estimate(const b200v2p_inest_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_ball_in_estimate: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !contact_ids || !ball_states || !table || table_rows < 1 || !params || !traj || !states_in || !states_out || stride < 13)
+  if (n < 0 || !d->contact_ids || !d->ball_states || !d->table || d->table_rows < 1 || !d->traj || !d->states_in || !d->states_out ||
+      d->stride < 13)
     return vfail(-1, "b200v2p_ball_in_estimate: bad arguments");
+  const double* params = d->params;
   for (int k = 0; k < 4; k++)
     if (!(params[k * 3 + 2] > 0)) return vfail(-2, "b200v2p_ball_in_estimate: grid steps must be positive");
   InParams P;
@@ -1303,7 +1309,7 @@ int b200v2p_ball_in_estimate(int32_t n, const int64_t* contact_ids, const float*
   }
   P.d1 = (float)dim[1]; P.d2 = (float)dim[2]; P.d3 = (float)dim[3];
   ball_in_estimate_kernel<<<(n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(
-      n, contact_ids, ball_states, stride, table, table_rows, P, traj, states_in, states_out);
+      n, d->contact_ids, d->ball_states, d->stride, d->table, d->table_rows, P, d->traj, d->states_in, d->states_out);
   V_CUDA_OK();
   return 0;
 }
@@ -1342,12 +1348,14 @@ int b200v2p_task_reset(const b200v2p_treset_t* r, void* stream) {
   return 0;
 }
 
-int b200v2p_ctrl_reset(int32_t n, const uint8_t* mask, int64_t* progress_buf, int64_t* reset_buf, int64_t* terminate_buf, int64_t* num_reset_reaction,
-                       float* distance, int64_t* num_reset, void* stream) {
+int b200v2p_ctrl_reset(const b200v2p_creset_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_ctrl_reset: bad arguments");
+  const int n = d->n;
   if (n == 0) return 0;
-  if (n < 0 || !mask || !progress_buf || !reset_buf || !terminate_buf || !num_reset_reaction || !distance || !num_reset)
+  if (n < 0 || !d->mask || !d->progress_buf || !d->reset_buf || !d->terminate_buf || !d->num_reset_reaction || !d->distance || !d->num_reset)
     return vfail(-1, "b200v2p_ctrl_reset: bad arguments");
-  ctrl_reset_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset);
+  ctrl_reset_kernel<<<(n + 255) / 256, 256, 0, (cudaStream_t)stream>>>(n, d->mask, d->progress_buf, d->reset_buf, d->terminate_buf,
+                                                                      d->num_reset_reaction, d->distance, d->num_reset);
   V_CUDA_OK();
   return 0;
 }

@@ -48,7 +48,7 @@ def _layout(S):
     if lay is None:
         import torch
         dtypes = {abi.F32P: (torch.float32,), abi.I64P: (torch.int64,), abi.U8P: (torch.uint8, torch.bool),
-                  abi.U32P: (torch.int32, torch.uint32), abi.F64P: (torch.float64,)}
+                  abi.U32P: (torch.int32, torch.uint32), abi.I32P: (torch.int32,), abi.F64P: (torch.float64,)}
         scalars = [(name, ct._length_ if issubclass(ct, C.Array) else None) for name, ct in S._fields_ if not issubclass(ct, C.c_void_p)]
         ptrs = [(name, dtypes.get(ct)) for name, ct in S._fields_ if issubclass(ct, C.c_void_p)]
         lay = _layouts[S] = (scalars, ptrs)
@@ -222,26 +222,24 @@ class Env:
     def reset_masked(self, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos, init_dof_vel, reset_times,
                      num_frames, first_frame, dt, feat, feat_mask, work):
         """reset of the envs whose mask [N] bool is set, context window included (include/b200env.h: b200env_reset_masked)"""
-        import torch
-        assert mask.dtype == torch.bool and counter.dtype == torch.int64 and work.dtype == torch.int32
         assert mask.shape[0] == self.num_envs and work.shape[0] >= self.num_envs + 2
-        for t in (mask, counter, init_root, init_dof_pos, init_dof_vel, reset_times, feat, feat_mask, work):
-            assert t is None or (t.is_cuda and t.is_contiguous())
-        _check(lib().b200env_reset_masked(self._h, _ptr(mask), int(bool(sample_time)), truncate, ref_prob, int(seed), _ptr(counter),
-                                          _ptr(init_root), _ptr(init_dof_pos), _ptr(init_dof_vel), _ptr(reset_times), num_frames, first_frame,
-                                          dt, _ptr(feat), _ptr(feat_mask), _ptr(work), _stream()))
+        d = fill(abi.ResetMasked, dict(sample_time=int(bool(sample_time)), truncate=truncate, ref_prob=ref_prob, num_frames=num_frames,
+                                       first_frame=first_frame, dt=dt, seed=int(seed)),
+                 dict(mask=mask, counter=counter, init_root=init_root, init_dof_pos=init_dof_pos, init_dof_vel=init_dof_vel,
+                      reset_times=reset_times, context_feat=feat, context_mask=feat_mask, work=work))
+        _check(lib().b200env_reset_masked(self._h, C.byref(d), _stream()))
 
     def motion_state(self, ids, times, out):
         """out: dict name -> tensor or None for root_pos, root_rot, dof_pos, root_vel, root_ang_vel, dof_vel, key_pos,
         rb_pos, rb_rot."""
-        names = ("root_pos", "root_rot", "dof_pos", "root_vel", "root_ang_vel", "dof_vel", "key_pos", "rb_pos", "rb_rot")
-        _check(lib().b200env_motion_state(self._h, _ptr(ids), _ptr(times), ids.shape[0], *[_ptr(out.get(k)) for k in names], _stream()))
+        d = fill(abi.MotionState, dict(n=ids.shape[0]), dict(out, motion_ids=ids, motion_times=times))
+        _check(lib().b200env_motion_state(self._h, C.byref(d), _stream()))
 
     def motion_context(self, env_ids, motion_ids, motion_times, num_frames, first_frame, dt, feat, mask):
         """feat [N, num_frames, W] float32, mask [N, num_frames] bool; rows env_ids (None: rows 0..n-1)"""
-        assert feat.is_cuda and feat.is_contiguous() and mask.is_contiguous() and motion_ids.is_contiguous() and motion_times.is_contiguous()
-        _check(lib().b200env_motion_context(self._h, _ptr(env_ids), _ptr(motion_ids), _ptr(motion_times), motion_ids.shape[0], num_frames,
-                                            first_frame, dt, _ptr(feat), _ptr(mask), _stream()))
+        d = fill(abi.MotionContext, dict(n=motion_ids.shape[0], num_frames=num_frames, first_frame=first_frame, dt=dt),
+                 dict(env_ids=env_ids, motion_ids=motion_ids, motion_times=motion_times, context_feat=feat, context_mask=mask))
+        _check(lib().b200env_motion_context(self._h, C.byref(d), _stream()))
 
     def obs_row_width(self, jpos=False):
         """columns of the row the observation launches write: 734 (513 with jpos) for the 24-body humanoid, 69 dofs, shape_dim 11"""
@@ -254,10 +252,10 @@ class Env:
                       body_ang_vel, motion_bodies, local_root_obs, root_height_obs, obs, jpos=False):
         n = int(body_pos.shape[0])
         assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == self.obs_row_width(jpos), (tuple(obs.shape), self.obs_row_width(jpos))
-        _check(lib().b200env_obs_imitation(self._h, n, _ptr(body_pos), _ptr(body_rot), _ptr(target_pos),
-                                           _ptr(target_rot), _ptr(dof_pos), _ptr(dof_vel), _ptr(target_dof_pos),
-                                           _ptr(body_vel), _ptr(body_ang_vel), _ptr(motion_bodies),
-                                           int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _stream()))
+        d = fill(abi.ObsImitation, dict(n=n, local_root_obs=int(bool(local_root_obs)), root_height_obs=int(root_height_obs), jpos=int(bool(jpos))),
+                 dict(body_pos=body_pos, body_rot=body_rot, target_pos=target_pos, target_rot=target_rot, dof_pos=dof_pos, dof_vel=dof_vel,
+                      target_dof_pos=target_dof_pos, body_vel=body_vel, body_ang_vel=body_ang_vel, motion_bodies=motion_bodies, obs=obs))
+        _check(lib().b200env_obs_imitation(self._h, C.byref(d), _stream()))
 
     def obs_imitation_rows(self, n, rigid_body_state, bodies_per_env, dof_state, target_pos, target_rot, target_dof_pos, motion_bodies,
                            local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0, jpos=False):
@@ -266,10 +264,12 @@ class Env:
         W = self.obs_row_width(jpos)
         assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == W, (tuple(obs.shape), W)
         assert obs_bf16 is None or (obs_bf16.dim() == 2 and obs_bf16.shape[0] >= n), tuple(obs_bf16.shape)
-        _check(lib().b200env_obs_imitation_rows(self._h, n, _ptr(rigid_body_state), bodies_per_env, _ptr(dof_state),
-                                                _ptr(target_pos), _ptr(target_rot), _ptr(target_dof_pos), _ptr(motion_bodies),
-                                                int(bool(local_root_obs)) | (2 if jpos else 0), int(root_height_obs), _ptr(obs), _ptr(obs_bf16),
-                                                obs_bf16.shape[1] if obs_bf16 is not None else 0, _ptr(mean), _ptr(rstd), clamp, _stream()))
+        d = fill(abi.ObsRows, dict(n=n, bodies_per_env=bodies_per_env, local_root_obs=int(bool(local_root_obs)),
+                                   root_height_obs=int(root_height_obs), jpos=int(bool(jpos)),
+                                   ld_bf16=obs_bf16.shape[1] if obs_bf16 is not None else 0, clamp=clamp),
+                 dict(rigid_body_state=rigid_body_state, dof_state=dof_state, target_pos=target_pos, target_rot=target_rot,
+                      target_dof_pos=target_dof_pos, motion_bodies=motion_bodies, obs=obs, obs_bf16=obs_bf16, mean=mean, rstd=rstd))
+        _check(lib().b200env_obs_imitation_rows(self._h, C.byref(d), _stream()))
 
     def im_policy_rows(self, scalars, tensors):
         """the imitation policy's bf16 operand rows and residual from obs_buf and the context slot of the device step counter

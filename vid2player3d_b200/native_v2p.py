@@ -24,29 +24,33 @@ def smpl_to_sim(root_pos, joint_rotmat, rest, parents, smpl_2_mujoco, dt, out, p
                 target_root_pos_out=None, only_mask=None):
     """out: dict with root_rot[n,4] dof_pos[n,69] root_vel[n,3] root_ang_vel[n,3] dof_vel[n,69] rb_pos[n,24,3] rb_rot[n,24,4];
     prev_root_pos_update / target_root_pos_out: the root position of this call is also stored there (may alias prev_root_pos)"""
-    n = int(root_pos.shape[0])
     num_rest = 1 if rest.dim() == 2 else int(rest.shape[0])      # rest [24,3] or [S,24,3]: env e uses shape e % S
-    assert rest.is_contiguous() and rest.shape[-2:] == (24, 3)
-    _check(lib().b200v2p_smpl_to_sim(n, _c(root_pos), _c(joint_rotmat), _c(rest), num_rest, _c(parents), _c(smpl_2_mujoco), dt,
-                                     _c(prev_root_pos), _c(prev_rb_rot), _c(out["root_rot"]), _c(out["dof_pos"]), _c(out["root_vel"]),
-                                     _c(out["root_ang_vel"]), _c(out["dof_vel"]), _c(out["rb_pos"]), _c(out["rb_rot"]), _c(prev_root_pos_update),
-                                     _c(target_root_pos_out), _c(only_mask), _stream()))
+    assert rest.shape[-2:] == (24, 3)
+    d = fill(abi.V2PSmpl, dict(n=root_pos.shape[0], num_rest=num_rest, dt=dt),
+             dict(out, root_pos=root_pos, joint_rotmat=joint_rotmat, rest=rest, parents=parents, smpl_2_mujoco=smpl_2_mujoco,
+                  prev_root_pos=prev_root_pos, prev_rb_rot=prev_rb_rot, prev_root_pos_update=prev_root_pos_update,
+                  target_root_pos_out=target_root_pos_out, only_mask=only_mask))
+    _check(lib().b200v2p_smpl_to_sim(C.byref(d), _stream()))
 
 
 def fix_head(rb_pos, rb_rot, ball_pos, root_pos, joint_rotmat, head_body=13):
-    _check(lib().b200v2p_fix_head(rb_pos.shape[0], _c(rb_pos), _c(rb_rot), head_body, _c(ball_pos), _c(root_pos), _c(joint_rotmat), _stream()))
+    d = fill(abi.V2PHead, dict(n=rb_pos.shape[0], head_body=head_body),
+             dict(rb_pos=rb_pos, rb_rot=rb_rot, ball_pos=ball_pos, root_pos=root_pos, joint_rotmat=joint_rotmat))
+    _check(lib().b200v2p_fix_head(C.byref(d), _stream()))
 
 
 def ball_aero(ball_states, has_bounce, has_bounce_now, bounce_pos, force, substeps, spin_scale, stride=None):
-    _check(lib().b200v2p_ball_aero(has_bounce.shape[0], _c(ball_states), stride or ball_states.stride(0), _c(has_bounce), _c(has_bounce_now),
-                                   _c(bounce_pos), _c(force), substeps, spin_scale, _stream()))
+    d = fill(abi.V2PAero, dict(n=has_bounce.shape[0], stride=stride or ball_states.stride(0), substeps=substeps, spin_scale=spin_scale),
+             dict(ball_states=ball_states, has_bounce=has_bounce, has_bounce_now=has_bounce_now, bounce_pos=bounce_pos, force=force))
+    _check(lib().b200v2p_ball_aero(C.byref(d), _stream()))
 
 
 def ball_reset(env_ids, pool_index, pool, ball_states, ball_pos, ball_vel, has_bounce, bounce_pos, has_contact, traj, stride=None):
     """ball_states: first ball row; `stride` floats between consecutive envs' ball rows (26 when the ball is actor 1 of 2)"""
-    _check(lib().b200v2p_ball_reset(env_ids.shape[0], _c(env_ids), _c(pool_index), _c(pool), _c(ball_states),
-                                    stride or ball_states.stride(0), _c(ball_pos), _c(ball_vel), _c(has_bounce), _c(bounce_pos),
-                                    _c(has_contact), _c(traj), _stream()))
+    d = fill(abi.V2PBallReset, dict(n=env_ids.shape[0], stride=stride or ball_states.stride(0)),
+             dict(env_ids=env_ids, pool_index=pool_index, pool=pool, ball_states=ball_states, ball_pos=ball_pos, ball_vel=ball_vel,
+                  has_bounce=has_bounce, bounce_pos=bounce_pos, has_contact=has_contact, traj=traj))
+    _check(lib().b200v2p_ball_reset(C.byref(d), _stream()))
 
 
 def update_state(n, bodies_per_env, rigid_body_state, root_states, root_stride, ball_states, ball_stride, t, grip='eastern',
@@ -65,15 +69,12 @@ def update_state(n, bodies_per_env, rigid_body_state, root_states, root_stride, 
 
 def ball_in_estimate(contact_ids, ball_states, stride, table, params, traj, states_in, states_out):
     """TennisBallInEstimator.estimate for the balls of envs `contact_ids`; params [4,3] float64 (HEIGHT, VEL_X, VEL_Y, VSPIN)"""
-    import numpy as np
     n = int(contact_ids.shape[0])
-    p = np.ascontiguousarray(np.asarray(params, np.float64).reshape(12))
-    for x in (contact_ids, table, traj, states_in, states_out):
-        assert x.is_cuda and x.is_contiguous()
     assert table.shape[1:] == (50, 2) and traj.shape == (n, 50, 3) and states_in.shape == (n, 13) and states_out.shape == (n, 13)
-    _check(lib().b200v2p_ball_in_estimate(n, _ptr(contact_ids), _ptr(ball_states), stride, _ptr(table),
-                                          table.shape[0], p.ctypes.data_as(C.c_void_p), _ptr(traj), _ptr(states_in),
-                                          _ptr(states_out), _stream()))
+    d = fill(abi.V2PInEst, dict(n=n, stride=stride, table_rows=table.shape[0],
+                                params=torch.as_tensor(params, dtype=torch.float64).reshape(12).tolist()),
+             dict(contact_ids=contact_ids, ball_states=ball_states, table=table, traj=traj, states_in=states_in, states_out=states_out))
+    _check(lib().b200v2p_ball_in_estimate(C.byref(d), _stream()))
 
 
 def controller_post(cfg, t):
@@ -163,7 +164,7 @@ def backhand_fix(problems, iters=BACKHAND_ITERS):
 
 
 def ctrl_reset(mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):
-    for x in (mask, progress_buf, reset_buf, terminate_buf, num_reset_reaction, distance, num_reset):
-        assert x.is_cuda and x.is_contiguous()
-    _check(lib().b200v2p_ctrl_reset(mask.shape[0], _ptr(mask), _ptr(progress_buf), _ptr(reset_buf), _ptr(terminate_buf),
-                                    _ptr(num_reset_reaction), _ptr(distance), _ptr(num_reset), _stream()))
+    d = fill(abi.V2PCtrlReset, dict(n=mask.shape[0]),
+             dict(mask=mask, progress_buf=progress_buf, reset_buf=reset_buf, terminate_buf=terminate_buf, num_reset_reaction=num_reset_reaction,
+                  distance=distance, num_reset=num_reset))
+    _check(lib().b200v2p_ctrl_reset(C.byref(d), _stream()))
