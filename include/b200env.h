@@ -245,13 +245,20 @@ int b200env_obs_imitation(b200env_handle h, const b200_obs_imitation_t* d, void*
 typedef struct b200_obs_rows {
   int32_t n, bodies_per_env, local_root_obs, root_height_obs, jpos, ld_bf16;
   float clamp;
-  int32_t pad_;
+  float clamp1;                   /* b200env_obs_imitation_rows_dual: player 1's clamp (clamp is player 0's); ignored otherwise */
   const float *rigid_body_state, *dof_state, *target_pos, *target_rot, *target_dof_pos, *motion_bodies;
   float* obs;
   void* obs_bf16;                 /* NULL: no operand row */
   const float *mean, *rstd;       /* NULL: no normalisation */
 } b200_obs_rows_t;
 int b200env_obs_imitation_rows(b200env_handle h, const b200_obs_rows_t* d, void* stream);
+/* The same launch for the two players of a rally (envs 2k and 2k+1), each with its own trained low-level policy
+ * (ImitatorBuilderDual.Network.eval_actor, vid2player/models/im_network_builder_dual.py:37-45): env e's operand row is
+ * (e & 1) * n/2 + (e >> 1), so each player's rows are one block, and player e & 1 uses row e & 1 of mean / rstd ([2, row width]) and
+ * clamp (player 0) or clamp1 (player 1); the float row stays in env order.  A clamp may be inf (RunningNorm at n == 0: no clamp).
+ * Returns -2 before any launch on the refusals of b200env_obs_imitation_rows, on an odd n and on a clamp or clamp1 that is not
+ * positive. */
+int b200env_obs_imitation_rows_dual(b200env_handle h, const b200_obs_rows_t* d, void* stream);
 
 /* The imitation policy's first-layer operand at test time (ImitatorBuilder.Network.preprocess_input, non-training branch, + running_obs,
  * embodied_pose/models/im_network_builder.py:117-189): the 734-wide observation of compute_humanoid_observations_imitation with

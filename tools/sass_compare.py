@@ -38,8 +38,9 @@ def demangle(names):
 
 def normalise_name(name, drops):
     for d in drops:
+        only = "<" + d + ">(" in name    # before the drop below, which turns f<false, false> into f<false> (not the only argument)
         name = name.replace(", " + d + ">", ">")
-        if "<" + d + ">(" in name:     # the only template argument: f<false>(...) of a kernel that was not a template before
+        if only:                         # the only template argument: f<false>(...) of a kernel that was not a template before
             name = re.sub(r"^void ", "", name.replace("<" + d + ">(", "("))
     return name
 

@@ -340,14 +340,15 @@ class ObsImitation(C.Structure):
 
 
 class ObsRows(C.Structure):
-    """b200_obs_rows_t: the imitation observation from the state rows, and the policy's bf16 operand row (b200env_obs_imitation_rows)"""
+    """b200_obs_rows_t: the imitation observation from the state rows, and the policy's bf16 operand row (b200env_obs_imitation_rows;
+    b200env_obs_imitation_rows_dual: one block of rows per player, clamp1 = player 1's clamp)"""
     _fields_ = [
         ("n", C.c_int32), ("bodies_per_env", C.c_int32), ("local_root_obs", C.c_int32), ("root_height_obs", C.c_int32),
-        ("jpos", C.c_int32), ("ld_bf16", C.c_int32), ("clamp", C.c_float), ("pad_", C.c_int32),
+        ("jpos", C.c_int32), ("ld_bf16", C.c_int32), ("clamp", C.c_float), ("clamp1", C.c_float),
         ("rigid_body_state", F32P), ("dof_state", F32P), ("target_pos", F32P), ("target_rot", F32P), ("target_dof_pos", F32P),
         ("motion_bodies", F32P), ("obs", F32P), ("obs_bf16", C.c_void_p), ("mean", F32P), ("rstd", F32P),
     ]
-    _nullable_, _defaults_ = ("obs_bf16", "mean", "rstd"), ("pad_",)
+    _nullable_, _defaults_ = ("obs_bf16", "mean", "rstd"), ("clamp1",)
 
 
 # ---------------------------------------------------------------- include/b200env_v2p.h
@@ -574,6 +575,7 @@ SIGNATURES = {
     "b200env_motion_state": (C.c_int, [_p, _p, _p]),
     "b200env_obs_imitation": (C.c_int, [_p, _p, _p]),
     "b200env_obs_imitation_rows": (C.c_int, [_p, _p, _p]),
+    "b200env_obs_imitation_rows_dual": (C.c_int, [_p, _p, _p]),
     "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200env_motion_context": (C.c_int, [_p, _p, _p]),
     "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),

@@ -1753,8 +1753,10 @@ __host__ __device__ inline int obs_row_width(int nb, int nd, int shape_dim, bool
 // is loaded), the targets from frame t_pad + (step[0] % t_len) of the context window (t_row floats per env, t_frame per frame; element
 // strides 3 / 4 / 1), motion_bodies from rows of mb_row floats; the float row is not written, the slot's target dof_pos goes to resid.
 struct ObsStrides { int p_row, p_elem, q_row, q_elem, d_row, d_elem; int t_row, t_frame, t_pad, t_len, mb_row; float clip_obs; };
-struct ObsBf16 { __nv_bfloat16* out; int ld; const float* mean; const float* rstd; float clamp; const int64_t* step; float* resid; };
-template <bool IM = false>
+// DUAL (b200env_obs_imitation_rows with dual): env e's bf16 row is (e & 1) * n/2 + (e >> 1), normalised by row e & 1 of mean / rstd
+// [2, W] and clamped to clamp (player 0) or clamp1 (player 1)
+struct ObsBf16 { __nv_bfloat16* out; int ld; const float* mean; const float* rstd; float clamp; const int64_t* step; float* resid; float clamp1; };
+template <bool IM = false, bool DUAL = false>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
 obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restrict__ body_pos, const float* __restrict__ body_rot,
                      const float* __restrict__ target_pos, const float* __restrict__ target_rot, const float* __restrict__ dof_pos,
@@ -1896,16 +1898,25 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
     }
   }
   if (ob.out) {
-    __nv_bfloat16* brow = ob.out + e * (int64_t)ob.ld;
+    int64_t row = e;
+    const float *mean = ob.mean, *rstd = ob.rstd;
+    float clamp = ob.clamp;
+    if constexpr (DUAL) {
+      const int p = (int)(e & 1);
+      row = p * (int64_t)(n >> 1) + (e >> 1);
+      if (mean) { mean += p * W; rstd += p * W; }
+      clamp = p ? ob.clamp1 : ob.clamp;
+    }
+    __nv_bfloat16* brow = ob.out + row * (int64_t)ob.ld;
     for (int k = 2 * lane; k < W; k += 64) {
       float x0 = srow[k], x1 = k + 1 < W ? srow[k + 1] : 0.f;
-      if (ob.mean) {
-        x0 = (x0 - __ldg(ob.mean + k)) * __ldg(ob.rstd + k);
-        if (k + 1 < W) x1 = (x1 - __ldg(ob.mean + k + 1)) * __ldg(ob.rstd + k + 1);
+      if (mean) {
+        x0 = (x0 - __ldg(mean + k)) * __ldg(rstd + k);
+        if (k + 1 < W) x1 = (x1 - __ldg(mean + k + 1)) * __ldg(rstd + k + 1);
       }
       // torch.clamp semantics: a NaN feature stays NaN in the operand (fminf / fmaxf would hide a blown-up env behind -clamp)
-      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x0) : "f"(ob.clamp), "f"(-ob.clamp));
-      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x1) : "f"(ob.clamp), "f"(-ob.clamp));
+      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x0) : "f"(clamp), "f"(-clamp));
+      asm("min.NaN.f32 %0, %0, %1;\n\tmax.NaN.f32 %0, %0, %2;" : "+f"(x1) : "f"(clamp), "f"(-clamp));
       if (k + 1 < W) *reinterpret_cast<__nv_bfloat162*>(brow + k) = __floats2bfloat162_rn(x0, x1);   // the host checks: ld even, out 4-byte aligned
       else brow[k] = __float2bfloat16_rn(x0);
     }
@@ -2670,35 +2681,52 @@ int b200env_obs_imitation(b200env_handle h, const b200_obs_imitation_t* d, void*
   return 0;
 }
 
-int b200env_obs_imitation_rows(b200env_handle h, const b200_obs_rows_t* d, void* stream) {
+// b200env_obs_imitation_rows (dual false) and b200env_obs_imitation_rows_dual (dual true): the same checks and launch; dual selects the
+// per-player operand placement, obs_imitation_kernel<false, true>
+static int obs_rows_launch(const char* who, b200env_handle h, const b200_obs_rows_t* d, bool dual, void* stream) {
   if (!h || !d || !d->rigid_body_state || !d->dof_state || !d->target_pos || !d->target_rot || !d->target_dof_pos || !d->motion_bodies || !d->obs)
-    return fail(-1, "b200env_obs_imitation_rows: null argument%s");
+    return fail(-1, "%s: null argument", who);
   const int n = d->n;
-  if (n <= 0) return fail(-2, "b200env_obs_imitation_rows: n must be positive%s");
+  if (n <= 0) return fail(-2, "%s: n must be positive", who);
   const int nbl = h->has_ml ? h->ml.num_lib_bodies : (h->model.fixed[h->model.nb - 1] ? h->model.nb - 1 : h->model.nb);
-  if (d->bodies_per_env < nbl) return fail(-2, "b200env_obs_imitation_rows: bodies_per_env smaller than the humanoid%s");
-  if ((d->mean == nullptr) != (d->rstd == nullptr)) return fail(-2, "b200env_obs_imitation_rows: mean and rstd go together%s");
-  if (d->obs_bf16 && !(d->clamp > 0.f)) return fail(-2, "b200env_obs_imitation_rows: the bf16 row needs a positive clamp%s");
+  if (d->bodies_per_env < nbl) return fail(-2, "%s: bodies_per_env smaller than the humanoid", who);
+  if ((d->mean == nullptr) != (d->rstd == nullptr)) return fail(-2, "%s: mean and rstd go together", who);
+  if (d->obs_bf16 && !(d->clamp > 0.f)) return fail(-2, "%s: the bf16 row needs a positive clamp", who);
+  if (dual && (n & 1)) return fail(-2, "%s: needs an even n (players are envs 2k and 2k+1)", who);
+  if (dual && !(d->clamp > 0.f && d->clamp1 > 0.f)) return fail(-2, "%s: needs two positive clamps", who);
   const bool jpos = d->jpos != 0;
   const int W = obs_row_width(nbl, h->model.nd, h->cfg.shape_dim, jpos);
-  if (int rc = obs_row_check("b200env_obs_imitation_rows", nbl, h->cfg.shape_dim, W)) return rc;
+  if (int rc = obs_row_check(who, nbl, h->cfg.shape_dim, W)) return rc;
   if (d->obs_bf16) {   // the row goes out as bfloat162 pairs from column 0 of every row
-    if (d->ld_bf16 < W) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 is smaller than the observation row%s");
-    if (d->ld_bf16 & 1) return fail(-2, "b200env_obs_imitation_rows: ld_bf16 must be even%s");
-    if (reinterpret_cast<uintptr_t>(d->obs_bf16) & 3) return fail(-2, "b200env_obs_imitation_rows: obs_bf16 must be 4-byte aligned%s");
+    if (d->ld_bf16 < W) return fail(-2, "%s: ld_bf16 is smaller than the observation row", who);
+    if (d->ld_bf16 & 1) return fail(-2, "%s: ld_bf16 must be even", who);
+    if (reinterpret_cast<uintptr_t>(d->obs_bf16) & 3) return fail(-2, "%s: obs_bf16 must be 4-byte aligned", who);
   }
   cudaSetDevice(h->device);
   const int grid = (n + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
   const int nd = h->model.nd, bpe = d->bodies_per_env;
   const float* rbs = d->rigid_body_state;
-  obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
-      n, nbl, nd, h->cfg.shape_dim, rbs, rbs + 3, d->target_pos, d->target_rot, d->dof_state, d->dof_state + 1, d->target_dof_pos,
-      rbs + 7, rbs + 10, d->motion_bodies, d->local_root_obs != 0, d->root_height_obs, d->obs, jpos,
-      ObsStrides{bpe * 13, 13, bpe * 13, 13, nd * 2, 2},
-      ObsBf16{reinterpret_cast<__nv_bfloat16*>(d->obs_bf16), d->ld_bf16, d->mean, d->rstd, d->clamp});
+  const ObsStrides st{bpe * 13, 13, bpe * 13, 13, nd * 2, 2};
+  const ObsBf16 ob{reinterpret_cast<__nv_bfloat16*>(d->obs_bf16), d->ld_bf16, d->mean, d->rstd, d->clamp, nullptr, nullptr, d->clamp1};
+  if (dual)
+    obs_imitation_kernel<false, true><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+        n, nbl, nd, h->cfg.shape_dim, rbs, rbs + 3, d->target_pos, d->target_rot, d->dof_state, d->dof_state + 1, d->target_dof_pos,
+        rbs + 7, rbs + 10, d->motion_bodies, d->local_root_obs != 0, d->root_height_obs, d->obs, jpos, st, ob);
+  else
+    obs_imitation_kernel<false><<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+        n, nbl, nd, h->cfg.shape_dim, rbs, rbs + 3, d->target_pos, d->target_rot, d->dof_state, d->dof_state + 1, d->target_dof_pos,
+        rbs + 7, rbs + 10, d->motion_bodies, d->local_root_obs != 0, d->root_height_obs, d->obs, jpos, st, ob);
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;
+}
+
+int b200env_obs_imitation_rows(b200env_handle h, const b200_obs_rows_t* d, void* stream) {
+  return obs_rows_launch("b200env_obs_imitation_rows", h, d, false, stream);
+}
+
+int b200env_obs_imitation_rows_dual(b200env_handle h, const b200_obs_rows_t* d, void* stream) {
+  return obs_rows_launch("b200env_obs_imitation_rows_dual", h, d, true, stream);
 }
 
 int b200env_im_policy_rows(b200env_handle h, const b200_im_policy_t* d, void* stream) {

@@ -258,18 +258,24 @@ class Env:
         _check(lib().b200env_obs_imitation(self._h, C.byref(d), _stream()))
 
     def obs_imitation_rows(self, n, rigid_body_state, bodies_per_env, dof_state, target_pos, target_rot, target_dof_pos, motion_bodies,
-                           local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0, jpos=False):
+                           local_root_obs, root_height_obs, obs, obs_bf16=None, mean=None, rstd=None, clamp=5.0, jpos=False, dual=False,
+                           clamp1=None):
         """the 734-d observation (513-d with jpos) straight from the state rows (no gathers); obs_bf16: padded bf16 operand buffer of
-        the policy's first layer, written in the same launch (normalised by mean / rstd when given, clamped to +-clamp)"""
+        the policy's first layer, written in the same launch (normalised by mean / rstd when given, clamped to +-clamp).  dual: the two
+        players' policies of a rally (b200env_obs_imitation_rows_dual) - env e's operand row is (e & 1) * n/2 + (e >> 1), with row
+        e & 1 of mean / rstd [2, W] and clamp (player 0) or clamp1 (player 1)"""
         W = self.obs_row_width(jpos)
         assert obs.dim() == 2 and obs.shape[0] >= n and obs.shape[1] == W, (tuple(obs.shape), W)
         assert obs_bf16 is None or (obs_bf16.dim() == 2 and obs_bf16.shape[0] >= n), tuple(obs_bf16.shape)
+        if dual and mean is not None:
+            assert tuple(mean.shape) == (2, W) and tuple(rstd.shape) == (2, W), (tuple(mean.shape), tuple(rstd.shape))
         d = fill(abi.ObsRows, dict(n=n, bodies_per_env=bodies_per_env, local_root_obs=int(bool(local_root_obs)),
                                    root_height_obs=int(root_height_obs), jpos=int(bool(jpos)),
-                                   ld_bf16=obs_bf16.shape[1] if obs_bf16 is not None else 0, clamp=clamp),
+                                   ld_bf16=obs_bf16.shape[1] if obs_bf16 is not None else 0, clamp=clamp, clamp1=clamp1),
                  dict(rigid_body_state=rigid_body_state, dof_state=dof_state, target_pos=target_pos, target_rot=target_rot,
                       target_dof_pos=target_dof_pos, motion_bodies=motion_bodies, obs=obs, obs_bf16=obs_bf16, mean=mean, rstd=rstd))
-        _check(lib().b200env_obs_imitation_rows(self._h, C.byref(d), _stream()))
+        fn = lib().b200env_obs_imitation_rows_dual if dual else lib().b200env_obs_imitation_rows
+        _check(fn(self._h, C.byref(d), _stream()))
 
     def im_policy_rows(self, scalars, tensors):
         """the imitation policy's bf16 operand rows and residual from obs_buf and the context slot of the device step counter

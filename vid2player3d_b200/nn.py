@@ -328,6 +328,62 @@ def im_networks_from_checkpoint(checkpoint, use_running_obs=True, running_obs_ty
     return net
 
 
+def low_level_networks_from_cfg(physics, num_obs, num_actions, dual):
+    """The tennis controller's trained low-level imitation policy, named by the controller cfg's `env.physics` block (PlayerBuilder,
+    vid2player/env/utils/player_builder.py:142-161; ImitatorPlayer.__init__, vid2player/players/im_player.py:32-42), as the network
+    dicts V2PPolicy takes; None when the block names no checkpoint.
+      single (physics.pretrained_model_cp): ImitatorPlayer.load_pretrained (:92-133), im_networks_from_checkpoint with tennis_im.yaml's
+              use_running_obs True, running_obs_type ours: one dict;
+      dual   (physics.dual_model_cp, one checkpoint per player): ImitatorPlayer.load_dual_cp (:54-90): each network's actor layers and
+              RunningNorm (see _running_norm) as they are - unlike V2PPlayer.load_dual_cp no zero-padded first layer, and the
+              statistics fill the whole row: two dicts, player 0 (even envs) first.
+    Refused with the reason (ValueError; nothing reaches the device): physics.checkpoint other than 'base' (the named restore reads
+    rl_games' network_path), a list of pretrained_model_cp files, the key of the other mode, a dual_model_cp that is not two
+    checkpoints, a first layer that does not take num_obs observations, a mu that does not give num_actions actions and (dual)
+    statistics of another width than num_obs.  CPU tensors, float32."""
+    single_cp, dual_cp = physics.get("pretrained_model_cp"), physics.get("dual_model_cp")
+    if not single_cp and not dual_cp:
+        return None
+    if physics.get("checkpoint", "base") != "base":
+        raise ValueError(f"physics.checkpoint = {physics['checkpoint']!r}: only 'base' (load the named pretrained_model_cp / "
+                         "dual_model_cp) is implemented; the named restore reads rl_games' network_path")
+    if dual and single_cp:
+        raise ValueError("physics.pretrained_model_cp on a dual-player task: a rally loads one network per player from dual_model_cp")
+    if not dual and dual_cp:
+        raise ValueError("physics.dual_model_cp on a single-player task: it loads from pretrained_model_cp")
+    if single_cp:
+        if isinstance(single_cp, (list, tuple)):
+            raise ValueError("physics.pretrained_model_cp is a list: loading several checkpoints in turn is not implemented "
+                             "(no shipped cfg uses it)")
+        nets = [im_networks_from_checkpoint(single_cp, use_running_obs=True, running_obs_type="ours", obs_dim=num_obs)]
+    else:
+        if not isinstance(dual_cp, (list, tuple)) or len(dual_cp) != 2:
+            raise ValueError("physics.dual_model_cp must name exactly two checkpoints, one per player")
+        nets = []
+        for p, cp in enumerate(dual_cp):
+            ck = _load(cp)
+            model = {k[len("a2c_network."):]: v for k, v in ck["model"].items() if k.startswith("a2c_network.")}
+            if "running_obs.n" in model:
+                stat = model["running_obs.mean"]
+            elif "running_mean_std" in ck:
+                stat = ck["running_mean_std"]["running_mean"]
+            else:
+                stat = model.get("running_obs.running_mean")
+            if stat is not None and stat.shape[0] != num_obs:
+                raise ValueError(f"dual_model_cp[{p}]: the observation statistics are {stat.shape[0]} wide, the env's observation "
+                                 f"{num_obs} (load_dual_cp fills the whole row)")
+            net = dict(layers=[(model[k + ".weight"].float(), model[k + ".bias"].float()) for k in V2P_ACTOR_KEYS])
+            net.update(_running_norm(ck, model, num_obs))
+            nets.append(net)
+    for p, net in enumerate(nets):
+        w0, mu = net["layers"][0][0], net["layers"][-1][0]
+        if w0.shape[1] != num_obs:
+            raise ValueError(f"low-level network {p}: the first layer takes {w0.shape[1]} observations, the env has {num_obs}")
+        if mu.shape[0] != num_actions:
+            raise ValueError(f"low-level network {p}: mu gives {mu.shape[0]} actions, the env takes {num_actions}")
+    return nets
+
+
 class V2PPolicy:
     """The tennis controller's trained high-level policy at test time (V2PPlayer.get_action with the deterministic `mu`,
     players/v2p_player.py:113-131; V2PBuilder.Network.eval_actor, models/v2p_network_builder.py:52-81): per network
@@ -336,6 +392,7 @@ class V2PPolicy:
     (V2PBuilderDual.Network.eval_actor, models/v2p_network_builder_dual.py:39-47): network p acts for envs p, p + 2, ...; its operand
     rows are one contiguous block (env e at row (e & 1) * N/2 + (e >> 1)) and its last layer writes rows p, p + 2, ... of `out`
     (ldo = 2 * actions, first column p * actions), so `out` is [N, actions] in env order.
+    It also serves the trained low-level imitation policy (low_level_networks_from_cfg; operand rows from b200env_obs_imitation_rows).
 
     The operand `x` is normally written by the controller's post launch (`operand()` gives it the fields of b200v2p_ctrl_t), and
     `forward_prepared()` runs the layers only; `forward(obs)` fills it from a float observation first.  bf16 operands, fp32 accumulation."""

@@ -259,11 +259,12 @@ class HumanoidSMPLIMMVAE(BaseTask):
 
     def _compute_observations(self):
         """:862-895 -> compute_humanoid_observations_imitation (:1046-1132) into obs_buf"""
-        op = self._obs_operand          # (bf16 operand buffer, mean, rstd, clamp) of a b200nn policy, or None
+        # (bf16 operand buffer, mean, rstd, clamp, dual, player 1's clamp) of a wgmma low-level policy, or None
+        op = self._obs_operand
         self._env.obs_imitation_rows(self.num_envs, self._rigid_body_state, 26, self._dof_state, self._target_rb_pos, self._target_rb_rot,
                                      self._target_dof_pos, self._reset_ref_motion_bodies, self._local_root_obs, self._root_height_obs, self.obs_buf,
                                      obs_bf16=op[0] if op else None, mean=op[1] if op else None, rstd=op[2] if op else None,
-                                     clamp=op[3] if op else 5.0)
+                                     clamp=op[3] if op else 5.0, dual=op[4] if op else False, clamp1=op[5] if op else None)
 
     def post_mvae_step(self):
         self._set_target_motion_state()

@@ -9,7 +9,8 @@ reference; PyTorch, stays PyTorch) and the physics player (low-level policy + Hu
 The MVAE checkpoints and the trained low-level policy are not released (README.md:13), so `SyntheticMotionPlayer` and a
 zero-residual policy stand in for tests and benchmarks; any object with the MVAEPlayer attribute surface
 (`_root_pos _joint_rotmat _phase_pred _swing_type _swing_type_cycle reset(ids) step(a, res)`) can be plugged in through
-cfg['env']['motion_player'], and any callable obs->action through cfg['env']['low_level_policy'].
+cfg['env']['motion_player'], and any callable obs->action through cfg['env']['low_level_policy'].  Without that key, the trained
+low-level imitation policy the cfg names (physics.pretrained_model_cp, dual: physics.dual_model_cp) drives the humanoid.
 """
 import math
 from types import SimpleNamespace
@@ -338,6 +339,15 @@ class PhysicsMVAEController:
         cls = HumanoidSMPLIMMVAEDual if self.cfg_v2p.get('dual_mode') else HumanoidSMPLIMMVAE
         task = cls(pcfg, self._sim_params, self._physics_engine, "cuda", self.device_id, True)
         policy = env.get("low_level_policy", None)
+        trained = None
+        if policy is None:
+            from .. import nn
+            nets = nn.low_level_networks_from_cfg(phys, task.num_obs, task.num_actions, dual=bool(self.cfg_v2p.get('dual_mode')))
+            if nets is not None:
+                # the trained imitation policy (ImitatorPlayer with tennis_im(_dual).yaml): both wrapper clamps are inf there, so the
+                # only clamp is each network's RunningNorm (+-5 while n > 0); dual: one chain of layers per player's row block
+                trained = policy = nn.V2PPolicy(nets, self.num_envs, self.device, clip_obs=float("inf"), clip_actions=None)
+                task._obs_operand = (policy.x, policy.mean, policy.rstd, policy.clip[0], policy.dual, policy.clip[-1])
         if policy is None:
             zeros = torch.zeros(self.num_envs, task.num_actions, device=self.device)
             policy = lambda obs: zeros  # noqa: E731  (zero residual: PD targets = kinematic targets)
@@ -349,14 +359,16 @@ class PhysicsMVAEController:
         self._low_level_policy = policy
         fused = getattr(policy, "clamp_obs", None) == 5.0 and getattr(policy, "clamp_actions", None) == 1.0 and hasattr(policy, "forward_prepared")
         if fused:     # the obs kernel writes the policy's normalised / clamped bf16 operand row itself: no cast launch
-            task._obs_operand = (policy.x, policy.mean, policy.rstd, policy.clamp_obs)
+            task._obs_operand = (policy.x, policy.mean, policy.rstd, policy.clamp_obs, False, None)
+        prepared = fused or trained is not None
 
         def run_one_step():   # ImitatorPlayer.run_one_step (players/im_player.py:187-202)
             # The reference clamps the raw observation to env.clip_obs, which player_builder.py:40 reads from `clip_observations`
             # (default inf; no imitation config sets it): the only observation clamp is the policy's own, after its running-mean-std
-            # normalisation.  Both branches give the policy the raw observation.
+            # normalisation.  Every branch gives the policy the raw observation; the trained policy's action is not clamped either
+            # (clip_actions_val, also inf).
             with torch.no_grad():
-                if fused:
+                if prepared:
                     task.step(self._low_level_policy.forward_prepared())
                 else:
                     action = self._low_level_policy(task.obs_buf)
