@@ -57,16 +57,29 @@ typedef struct b200nn_linear_desc {
   const float* resid; /* [rows, ld_resid] float, 4-byte aligned */
   int32_t ld_resid;   /* >= resid_cols */
   int32_t resid_cols; /* 1..n */
+  /* sampled action (single-expert layer, float output): out = clamp(act(acc + bias (+ resid) + noise_sigma[col] * eps)) with
+   * eps = N(0, 1) draw (row * ldo + out_col0 + col) of counter *noise_step under noise_seed (counter-based: splitmix64 + Box-Muller),
+   * i.e. `distr.sample()` of Normal(mu, sigma) (vid2player/models/v2p_models.py:26-43, embodied_pose/models/im_models.py:24-42) before
+   * the wrapper's action clamp.  The last CTA to finish adds 1 to *noise_step, so every launch (every CUDA graph replay) draws afresh.
+   * A column with sigma 0 keeps the deterministic value bit for bit.  noise_sigma NULL (and the other three 0 / NULL): no noise. */
+  const float* noise_sigma; /* [n] float, 4-byte aligned */
+  uint64_t noise_seed;
+  int64_t* noise_step;      /* [1] device step counter, 8-byte aligned */
+  uint32_t* noise_done;     /* [1] done ticket, 0 before the first launch; the last CTA re-arms it */
 } b200nn_linear_desc_t;
 
 int b200nn_abi_version(void);
+/* sizeof(b200nn_linear_desc_t) as the library was built: the descriptor grows by appended fields (the noise fields follow the
+ * residual), so a binding checks the size it passes against this and refuses a library built before the fields it fills */
+int32_t b200nn_linear_desc_size(void);
 const char* b200nn_last_error(void);
 
 /* builds the TMA tensor maps of the operands (host side, once); the device buffers must stay where they are.  Returns -2 (before any
  * driver call) for a descriptor the kernel cannot run: num_experts outside 1..6, K / lda / ldw not padded to 64, n_padded not a
  * multiple of the tile or n outside 1..n_padded, rows < 1, bf16 ldo / out_col0 not multiples of 8, operands not 16-byte aligned,
  * out_col0 < 0, ldo < out_col0 + n, an unknown act; and a residual on a mixture layer or a bf16 output, resid_cols outside 1..n,
- * ld_resid < resid_cols, a misaligned resid, or resid_cols / ld_resid without resid. */
+ * ld_resid < resid_cols, a misaligned resid, or resid_cols / ld_resid without resid; and noise on a mixture layer or a bf16 output,
+ * noise_sigma without noise_step or noise_done, noise_step / noise_done without noise_sigma, or a misaligned noise pointer. */
 int b200nn_linear_create(const b200nn_linear_desc_t* desc, int32_t device, b200nn_linear_handle* out);
 int b200nn_linear_destroy(b200nn_linear_handle h);
 /* one launch on `stream` (CUDA-graph capturable) */

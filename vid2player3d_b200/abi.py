@@ -288,6 +288,18 @@ class ImPolicy(C.Structure):
     _nullable_, _defaults_ = ("mean", "rstd"), ("clip", "pad_")
 
 
+class LinearDesc(C.Structure):
+    """b200nn_linear_desc_t (include/b200nn.h): one wgmma GEMM layer of libb200nn.so; nn.Linear fills it.  The noise fields (the
+    sampled action: sigma per output column, seed, device step counter, done ticket) are NULL / 0 for a deterministic layer."""
+    _fields_ = [("a", C.c_void_p), ("lda", C.c_int32), ("w", C.c_void_p), ("ldw", C.c_int32), ("bias", F32P), ("coef", F32P),
+                ("out", C.c_void_p), ("ldo", C.c_int32), ("out_col0", C.c_int32), ("rows", C.c_int32), ("n", C.c_int32),
+                ("n_padded", C.c_int32), ("k_padded", C.c_int32), ("num_experts", C.c_int32), ("act", C.c_int32), ("out_bf16", C.c_int32),
+                ("out_min", C.c_float), ("out_max", C.c_float), ("resid", F32P), ("ld_resid", C.c_int32), ("resid_cols", C.c_int32),
+                ("noise_sigma", F32P), ("noise_seed", C.c_uint64), ("noise_step", I64P), ("noise_done", U32P)]
+    _nullable_ = ("coef", "resid", "noise_sigma", "noise_step", "noise_done")
+    _defaults_ = ("out_min", "out_max", "ld_resid", "resid_cols", "noise_seed")
+
+
 class PlayStats(C.Structure):
     """b200_play_stats_t: ImitatorPlayer.run's bookkeeping of one step (b200env_play_stats)"""
     _fields_ = [

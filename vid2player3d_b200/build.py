@@ -10,7 +10,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.environ.get("B200ENV_LIB", os.path.join(LIB_DIR, "libb200env.so"))  # override: A/B kernel variants
 # the network forwards of SURVEY.md 8f-1 (wgmma GEMMs): a library of their own, include/b200nn.h
 SRCS_NN = [os.path.join(HERE, "csrc", "b200nn.cu")]
-HDRS_NN = [os.path.join(os.path.dirname(HERE), "include", "b200nn.h")]
+HDRS_NN = [os.path.join(os.path.dirname(HERE), "include", "b200nn.h"), os.path.join(HERE, "csrc", "counter_rng.cuh")]
 LIB_NN = os.environ.get("B200NN_LIB", os.path.join(LIB_DIR, "libb200nn.so"))
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "--shared",

@@ -608,7 +608,6 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
 }
 
 // ------------------------------------------------------------------------------------------ test-time rally recorder
-__device__ __forceinline__ void last_block_advance(int64_t* counter, unsigned int* done, int64_t inc);
 // render_vis's per-frame append (mvae_controller_vis.py:140-146, mvae_controller_vis_dual.py:156-162): one warp per env writes the
 // env's frame at row *row_counter (single; the last block advances the counter) or progress_buf[e] (dual); rows >= cap are dropped
 __global__ void __launch_bounds__(V2P_WARPS * 32) eval_record_kernel(b200v2p_rec_t r) {
@@ -1169,22 +1168,8 @@ __global__ void ctrl_reset_kernel(int n, const uint8_t* __restrict__ mask, int64
 // PhysicsMVAEController.pre_physics_step (:247-262) before the motion generator runs: the latent part of the action scaled by
 // vae_action_scale, replaced by clamp(N(0,1), -5, 5) for the envs in recovery (random_walk_in_recovery), the residual-dof part scaled
 // by residual_dof_scale.  The normal deviates come from a counter-based generator (splitmix64 of seed, step counter, element index +
-// Box-Muller) so that the step needs no separate RNG launch; the step counter lives on the device and is advanced by the last
-// block to finish, which keeps the launch replayable inside a CUDA graph.
-__device__ __forceinline__ float counter_normal(uint64_t seed, uint64_t step, uint64_t idx) {
-  const uint64_t h = counter_bits(seed, step, idx);
-  const float u1 = ((uint32_t)(h >> 40) + 1u) * (1.0f / 16777217.0f);     // (0, 1)
-  const float u2 = (uint32_t)((h >> 8) & 0xFFFFFFu) * (1.0f / 16777216.0f);
-  return sqrtf(-2.0f * logf(u1)) * cosf(6.283185307179586f * u2);
-}
-__device__ __forceinline__ void last_block_advance(int64_t* counter, unsigned int* done, int64_t inc) {
-  __shared__ bool last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) last = atomicAdd(done, 1u) == gridDim.x - 1;
-  __syncthreads();
-  if (last && threadIdx.x == 0) { counter[0] += inc; *done = 0u; __threadfence(); }
-}
+// Box-Muller, counter_rng.cuh) so that the step needs no separate RNG launch; the step counter lives on the device and is advanced
+// by the last block to finish, which keeps the launch replayable inside a CUDA graph.
 __global__ void pre_step_kernel(b200v2p_prestep_t p) {
   const int W = p.num_latent + p.num_res_dof;
   const int64_t step = p.step_counter[0];

@@ -12,7 +12,9 @@
 //                expert, so the A slice leaves shared memory once per k16 step), operands straight from the swizzled stages, fp32
 //                accumulators in registers.  One wgmma group stays in flight: after committing k block kb the warpgroup waits for kb - 1
 //                and releases that stage on its `empty` mbarrier.  Epilogue from the registers: bias, expert blend, activation, clamp;
-//                bf16 outputs leave as 16-byte stores (a quad shuffle gathers 8 consecutive columns of a row per thread).
+//                bf16 outputs leave as 16-byte stores (a quad shuffle gathers 8 consecutive columns of a row per thread).  The sampled
+//                action (NOISE, last policy layer) adds sigma[col] * N(0, 1) from the counter-based generator (counter_rng.cuh) before
+//                the clamp; the last CTA advances the device step counter, so a graph replay draws fresh noise.
 // E = 1: BN = 128 columns, or 64 when the layer has n <= 64.  E > 1 (mixture of experts, vid2player/motion_vae/model.py:237-252): the
 // tile is MOE_BN output columns x E experts = E * MOE_BN accumulator columns; the per-row softmax coefficients are applied in the
 // epilogue in fp32, so the per-env blended weight matrices of the reference never exist.
@@ -26,6 +28,7 @@
 #include <stdlib.h>
 
 #include "../../include/b200nn.h"
+#include "counter_rng.cuh"
 
 static thread_local char g_err[512] = "";
 static int fail(int code, const char* msg) {
@@ -214,6 +217,10 @@ struct LinearParams {
   int n_tiles, tiles;                              // output tiles across the columns, in all
   const float* resid;                              // RES: x += resid[row * ld_resid + col] for col < resid_cols, before act and clamp
   int ld_resid, resid_cols;
+  const float* noise_sigma;                        // NOISE: x += noise_sigma[col] * eps(seed, *noise_step, row * ldo + out_col0 + col),
+  uint64_t noise_seed;                             // after the residual, before act and clamp
+  int64_t* noise_step;
+  unsigned int* noise_done;
 };
 
 __device__ __forceinline__ float finish(float x, const LinearParams& p) {
@@ -253,9 +260,9 @@ __device__ __forceinline__ void quad_transpose(const uint32_t (&v)[4], int q, ui
 
 // Accumulator register i (of E * BN / 2) of this thread: expert i / (BN / 2), row row0 + 8 ((i / 2) % 2), column
 // 8 ((i % (BN / 2)) / 4) + 2 (lane % 4) + i % 2 of the tile (columns n0 ..).  Taken 32 columns at a time.
-template <int E, int BN, bool RES>
+template <int E, int BN, bool RES, bool NOISE>
 __device__ __forceinline__ void epilogue(const float* acc, const float (&coef)[2][E], const float* sbias, const LinearParams& p, int row0,
-                                         int n0, int lane) {
+                                         int n0, int lane, uint64_t step) {
   const int q = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; h++) {
@@ -273,6 +280,10 @@ __device__ __forceinline__ void epilogue(const float* acc, const float (&coef)[2
             x = acc[i] + sbias[col];
             if constexpr (RES) {
               if (col < p.resid_cols && row < p.rows) x += __ldg(p.resid + (size_t)row * p.ld_resid + col);
+            }
+            if constexpr (NOISE) {                 // sigma 0: no add at all, so the column keeps mu bit for bit (even -0)
+              const float s = (row < p.rows && col < p.n) ? __ldg(p.noise_sigma + col) : 0.f;
+              if (s != 0.f) x = fmaf(s, counter_normal(p.noise_seed, step, (uint64_t)row * p.ldo + p.out_col0 + col), x);
             }
           } else {
             x = 0.f;
@@ -317,9 +328,10 @@ template <int E, int BN> __host__ __device__ constexpr int bias_offset() { retur
 template <int E, int BN> int smem_bytes(int n_padded) { return 1024 + bias_offset<E, BN>() + E * n_padded * 4; }
 
 // RES (residual epilogue, the policy's last layer): one CTA per SM - its register budget holds the residual's addressing without spilling,
-// and a layer as narrow as the policy's 75 actions has fewer tiles than SMs
-template <int E, int BN, bool RES = false>
-__global__ void __launch_bounds__(NUM_THREADS, RES ? 1 : ctas_per_sm<E>())
+// and a layer as narrow as the policy's 75 actions has fewer tiles than SMs.  NOISE (sampled action, also only on the last layer): the
+// same budget for the counter-based normal; the last CTA to finish advances the step counter (producer and consumers both take part).
+template <int E, int BN, bool RES = false, bool NOISE = false>
+__global__ void __launch_bounds__(NUM_THREADS, (RES || NOISE) ? 1 : ctas_per_sm<E>())
 linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const LinearParams p) {
   constexpr int ACC = E * BN;                          // accumulator columns = the N of every wgmma
   constexpr int STAGES = stages<E, BN>();
@@ -366,12 +378,18 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       }
     }
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    if constexpr (NOISE) last_block_advance(p.noise_step, p.noise_done, 1);
     return;
   }
   // ---------------- consumers: warpgroup wg owns rows 64 wg .. + 63 of each tile
   const int wg = warp >> 2;
   const int t = threadIdx.x & 127;
   if (E > 1) asm volatile("griddepcontrol.wait;" ::: "memory");    // the coefficients come from the gate kernel before us
+  uint64_t step = 0;
+  if constexpr (NOISE) {                          // every launch before us is complete: the counter holds its final value
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    step = (uint64_t)__ldcg(p.noise_step);
+  }
   int s = 0;
   uint32_t ph = 0;
   for (int tile = blockIdx.x; tile < p.tiles; tile += gridDim.x) {
@@ -401,9 +419,10 @@ linear_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     }
     wgmma_wait<0>();
     if (t == 0) mbar_arrive(&empty[prev]);
-    epilogue<E, BN, RES>(acc, coef, sbias, p, row0, n0, lane);
+    epilogue<E, BN, RES, NOISE>(acc, coef, sbias, p, row0, n0, lane, step);
   }
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if constexpr (NOISE) last_block_advance(p.noise_step, p.noise_done, 1);
 }
 
 // ------------------------------------------------------------------------------------------ small SIMT kernels
@@ -486,16 +505,19 @@ struct b200nn_linear {
 
 // prepare (at create, on the handle's device): the kernel's shared-memory size, and the grid = the CTA slots resident on the device
 // at once, at most one per tile.  Otherwise launch.
-template <int E, int BN, bool RES = false> static int prepare_or_launch(b200nn_linear* h, cudaStream_t st, bool prepare) {
+template <int E, int BN, bool RES = false, bool NOISE = false> static int prepare_or_launch(b200nn_linear* h, cudaStream_t st, bool prepare) {
   if (prepare) {
     // the attribute is per kernel, not per handle: allow the device's limit, so that handles of other widths launch too
     int sms = 0, per_sm = 0, limit = 0;
     CUDA_OK(cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    cudaFuncAttributes fa;                         // the static shared memory (NOISE: the done flag) comes off the dynamic limit
+    CUDA_OK(cudaFuncGetAttributes(&fa, linear_kernel<E, BN, RES, NOISE>));
+    limit -= (int)fa.sharedSizeBytes;
     if (smem_bytes<E, BN>(h->d.n_padded) > limit) return fail(-2, "b200nn_linear_create: n_padded too large for the bias in shared memory");
-    CUDA_OK(cudaFuncSetAttribute(linear_kernel<E, BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit));
-    prefer_max_shared(linear_kernel<E, BN, RES>);
+    CUDA_OK(cudaFuncSetAttribute(linear_kernel<E, BN, RES, NOISE>, cudaFuncAttributeMaxDynamicSharedMemorySize, limit));
+    prefer_max_shared(linear_kernel<E, BN, RES, NOISE>);
     CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
-    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_kernel<E, BN, RES>, NUM_THREADS, smem_bytes<E, BN>(h->d.n_padded)));
+    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, linear_kernel<E, BN, RES, NOISE>, NUM_THREADS, smem_bytes<E, BN>(h->d.n_padded)));
     if (per_sm < 1) return fail(-3, "b200nn_linear_create: the GEMM kernel does not fit on an SM");
     h->grid = h->p.tiles < sms * per_sm ? h->p.tiles : sms * per_sm;
     return 0;
@@ -510,13 +532,17 @@ template <int E, int BN, bool RES = false> static int prepare_or_launch(b200nn_l
   attr[0].val.programmaticStreamSerializationAllowed = h->pdl ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  CUDA_OK(cudaLaunchKernelEx(&cfg, linear_kernel<E, BN, RES>, h->tmA, h->tmW, h->p));
+  CUDA_OK(cudaLaunchKernelEx(&cfg, linear_kernel<E, BN, RES, NOISE>, h->tmA, h->tmW, h->p));
   return 0;
 }
 
 static int dispatch(b200nn_linear* h, cudaStream_t st, bool prepare) {
   switch (h->d.num_experts) {
     case 1:
+      if (h->d.noise_sigma) {
+        if (h->d.resid) return h->bn == 64 ? prepare_or_launch<1, 64, true, true>(h, st, prepare) : prepare_or_launch<1, 128, true, true>(h, st, prepare);
+        return h->bn == 64 ? prepare_or_launch<1, 64, false, true>(h, st, prepare) : prepare_or_launch<1, 128, false, true>(h, st, prepare);
+      }
       if (h->d.resid) return h->bn == 64 ? prepare_or_launch<1, 64, true>(h, st, prepare) : prepare_or_launch<1, 128, true>(h, st, prepare);
       return h->bn == 64 ? prepare_or_launch<1, 64>(h, st, prepare) : prepare_or_launch<1, 128>(h, st, prepare);
     case 2: return prepare_or_launch<2, MOE_BN>(h, st, prepare);
@@ -531,6 +557,7 @@ static int dispatch(b200nn_linear* h, cudaStream_t st, bool prepare) {
 extern "C" {
 
 int b200nn_abi_version(void) { return B200NN_ABI_VERSION; }
+int32_t b200nn_linear_desc_size(void) { return (int32_t)sizeof(b200nn_linear_desc_t); }
 const char* b200nn_last_error(void) { return g_err; }
 
 int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_linear_handle* out) {
@@ -556,6 +583,15 @@ int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_l
     if (d->resid_cols < 1 || d->resid_cols > d->n) return fail(-2, "b200nn_linear_create: resid_cols must be in 1..n");
     if (d->ld_resid < d->resid_cols) return fail(-2, "b200nn_linear_create: ld_resid < resid_cols");
     if ((uintptr_t)d->resid & 3) return fail(-2, "b200nn_linear_create: resid must be 4-byte aligned");
+  }
+  if (d->noise_sigma || d->noise_step || d->noise_done) {
+    if (!d->noise_sigma) return fail(-2, "b200nn_linear_create: noise_step / noise_done given without noise_sigma");
+    if (E > 1) return fail(-2, "b200nn_linear_create: noise (the sampled action) needs a single-expert layer (num_experts == 1)");
+    if (d->out_bf16) return fail(-2, "b200nn_linear_create: noise (the sampled action) needs a float output");
+    if (!d->noise_step) return fail(-2, "b200nn_linear_create: noise_sigma needs the device step counter noise_step");
+    if (!d->noise_done) return fail(-2, "b200nn_linear_create: noise_sigma needs the done ticket noise_done");
+    if (((uintptr_t)d->noise_sigma & 3) || ((uintptr_t)d->noise_step & 7) || ((uintptr_t)d->noise_done & 3))
+      return fail(-2, "b200nn_linear_create: noise_sigma / noise_done must be 4-byte and noise_step 8-byte aligned");
   }
   encode_tiled_fn enc = get_encode();
   if (!enc) return fail(-3, "b200nn_linear_create: cuTensorMapEncodeTiled not available (no CUDA driver)");
@@ -587,7 +623,8 @@ int b200nn_linear_create(const b200nn_linear_desc_t* d, int32_t device, b200nn_l
   }
   const int n_tiles = (d->n + h->bn - 1) / h->bn;
   h->p = LinearParams{d->bias, d->coef, d->out, d->ldo, d->out_col0, d->rows, d->n, d->n_padded, d->k_padded, d->act, d->out_bf16, d->out_min, d->out_max,
-                      n_tiles, rows_padded / BLOCK_M * n_tiles, d->resid, d->ld_resid, d->resid_cols};
+                      n_tiles, rows_padded / BLOCK_M * n_tiles, d->resid, d->ld_resid, d->resid_cols,
+                      d->noise_sigma, d->noise_seed, d->noise_step, d->noise_done};
   const int rc = dispatch(h, nullptr, true);
   if (rc) { delete h; return rc; }
   *out = h;

@@ -16,6 +16,7 @@ import os
 
 import torch
 
+from . import abi, native
 from .build import LIB_NN
 
 ACT = {None: 0, "none": 0, "relu": 1, "elu": 2}
@@ -23,12 +24,7 @@ _lib = None
 
 ABI_VERSION = 2
 
-
-class LinearDesc(C.Structure):
-    _fields_ = [("a", C.c_void_p), ("lda", C.c_int32), ("w", C.c_void_p), ("ldw", C.c_int32), ("bias", C.c_void_p), ("coef", C.c_void_p),
-                ("out", C.c_void_p), ("ldo", C.c_int32), ("out_col0", C.c_int32), ("rows", C.c_int32), ("n", C.c_int32),
-                ("n_padded", C.c_int32), ("k_padded", C.c_int32), ("num_experts", C.c_int32), ("act", C.c_int32), ("out_bf16", C.c_int32),
-                ("out_min", C.c_float), ("out_max", C.c_float), ("resid", C.c_void_p), ("ld_resid", C.c_int32), ("resid_cols", C.c_int32)]
+LinearDesc = abi.LinearDesc   # b200nn_linear_desc_t, typed pointers: native.fill builds it
 
 
 # name -> (restype, argtypes) of every function include/b200nn.h declares; lib() applies all of them when it loads the library, so an
@@ -37,6 +33,7 @@ class LinearDesc(C.Structure):
 _i32, _f32, _p = C.c_int32, C.c_float, C.c_void_p
 SIGNATURES = {
     "b200nn_abi_version": (C.c_int, []),
+    "b200nn_linear_desc_size": (C.c_int32, []),
     "b200nn_last_error": (C.c_char_p, []),
     "b200nn_linear_create": (C.c_int, [_p, _i32, _p]),
     "b200nn_linear_destroy": (C.c_int, [_p]),
@@ -55,10 +52,16 @@ def lib():
             raise RuntimeError(f"{LIB_NN} not built - run `python -c 'import __graft_entry__ as g; g.build()'` (no fallback)")
         L = C.CDLL(LIB_NN)
         for name, (restype, argtypes) in SIGNATURES.items():
-            fn = getattr(L, name)
+            try:
+                fn = getattr(L, name)
+            except AttributeError:
+                raise RuntimeError(f"{LIB_NN} has no {name}: built from older sources - rebuild") from None
             fn.restype, fn.argtypes = restype, argtypes
         if L.b200nn_abi_version() != ABI_VERSION:
             raise RuntimeError("libb200nn.so ABI version mismatch - rebuild")
+        if L.b200nn_linear_desc_size() != C.sizeof(LinearDesc):   # the descriptor grows by appended fields within one version
+            raise RuntimeError(f"libb200nn.so takes a {L.b200nn_linear_desc_size()}-byte b200nn_linear_desc_t, the binding fills "
+                               f"{C.sizeof(LinearDesc)} bytes - rebuild")
         _lib = L
     return _lib
 
@@ -89,9 +92,11 @@ class Linear:
     """out[:, col0:col0+N] = act(sum_e coef[:, e] (a W_e^T + b_e)); one launch.  weight [E, N, K] or [N, K] float (torch layout:
     out x in), bias [E, N] or [N]; `a` / `out` are buffers from padded_bf16 (out may also be a float [rows, N] tensor).  residual = (float
     tensor [rows, >= cols], cols): a single-expert layer with a float output adds resid[:, :cols] to its first cols outputs before the
-    activation and the clamp."""
+    activation and the clamp.  noise = (sigma float [N], seed): the sampled action of the same kind of layer, out = clamp(act(x +
+    sigma[col] * eps)) after the residual, eps the counter-based N(0, 1) draw (seed, noise_step, row * ldo + out_col0 + col); the layer
+    owns its device step counter `noise_step`, which every launch advances."""
 
-    def __init__(self, a, weight, bias, out, rows, act=None, coef=None, out_col0=0, out_clamp=None, residual=None):
+    def __init__(self, a, weight, bias, out, rows, act=None, coef=None, out_col0=0, out_clamp=None, residual=None, noise=None):
         dev = a.device
         if dev.type != "cuda":
             raise RuntimeError("b200nn runs on a CUDA device only (no CPU fallback)")
@@ -117,12 +122,22 @@ class Linear:
         if resid is not None:
             assert resid.dtype == torch.float32 and resid.stride(-1) == 1 and resid.device == dev and resid.shape[0] >= rows
         self.residual = residual
-        d = LinearDesc(a=a.data_ptr(), lda=a.shape[1], w=self.w.data_ptr(), ldw=self.k_padded, bias=self.b.data_ptr(),
-                       coef=coef.data_ptr() if coef is not None else None, out=out.data_ptr(), ldo=out.shape[1], out_col0=out_col0,
-                       rows=rows, n=N, n_padded=self.n_padded, k_padded=self.k_padded, num_experts=E, act=ACT[act], out_bf16=int(out_bf16),
-                       out_min=out_clamp[0] if out_clamp else 0.0, out_max=out_clamp[1] if out_clamp else 0.0,
-                       resid=resid.data_ptr() if resid is not None else None, ld_resid=resid.stride(0) if resid is not None else 0,
-                       resid_cols=int(cols))
+        self.noise_sigma = self.noise_step = self.noise_done = None
+        seed = 0
+        if noise is not None:
+            sigma, seed = noise
+            self.noise_sigma = sigma.detach().to(dev, torch.float32).reshape(-1).contiguous()
+            if self.noise_sigma.shape[0] != N:
+                raise ValueError(f"noise: {self.noise_sigma.shape[0]} sigmas for a layer of {N} outputs")
+            self.noise_step = torch.zeros(1, device=dev, dtype=torch.int64)
+            self.noise_done = torch.zeros(1, device=dev, dtype=torch.int32)
+        d = native.fill(LinearDesc, dict(lda=a.shape[1], ldw=self.k_padded, ldo=out.shape[1], out_col0=out_col0, rows=rows, n=N,
+                                          n_padded=self.n_padded, k_padded=self.k_padded, num_experts=E, act=ACT[act], out_bf16=int(out_bf16),
+                                          out_min=out_clamp[0] if out_clamp else None, out_max=out_clamp[1] if out_clamp else None,
+                                          ld_resid=resid.stride(0) if resid is not None else None, resid_cols=int(cols),
+                                          noise_seed=int(seed) & (2 ** 64 - 1)),
+                        dict(a=a, w=self.w, bias=self.b, coef=coef, out=out, resid=resid, noise_sigma=self.noise_sigma,
+                             noise_step=self.noise_step, noise_done=self.noise_done))
         self._h = C.c_void_p()
         _check(lib().b200nn_linear_create(C.byref(d), dev.index or 0, C.byref(self._h)))
         self.flops = 2.0 * rows * N * K * E
@@ -154,10 +169,12 @@ class PolicyMLP:
     ImitatorPlayer's `torch.clamp(action, -1, 1)` (im_player.py:198) into the last layer's epilogue.  obs_rstd: the normaliser's
     1 / std given as it is (RunningNorm's 1 / (std + 1e-8)) instead of from obs_var.  residual = (float tensor [num_envs, >= cols], cols):
     the last layer adds it to its first cols outputs before the action clamp (the embodied_pose imitation policy's residual action,
-    `mu[:, :69] += target_dof_pos`, im_network_builder.py:226-228)."""
+    `mu[:, :69] += target_dof_pos`, im_network_builder.py:226-228).  noise_sigma (float [out_dim], the fixed sigma = exp(logstd)):
+    the sampled action mu + sigma * N(0, 1) of a stochastic player (im_models.py:24-42 `distr.sample()`), drawn in the last layer's
+    epilogue after the residual and before the action clamp from the counter-based generator under `seed`."""
 
     def __init__(self, layers, num_envs, device, obs_mean=None, obs_var=None, eps=1e-5, clamp_obs=5.0, activation="relu", clamp_actions=None,
-                 obs_rstd=None, residual=None):
+                 obs_rstd=None, residual=None, noise_sigma=None, seed=0):
         self.rows, self.device = num_envs, torch.device(device)
         self.in_dim = layers[0][0].shape[1]
         self.out_dim = layers[-1][0].shape[0]
@@ -179,8 +196,10 @@ class PolicyMLP:
             o = self.out if last else padded_bf16(num_envs, w.shape[0], self.device)
             self.layers.append(Linear(a, w, b, o, num_envs, act=None if last else activation,
                                       out_clamp=(-clamp_actions, clamp_actions) if (last and clamp_actions) else None,
-                                      residual=residual if last else None))
+                                      residual=residual if last else None,
+                                      noise=(noise_sigma, seed) if (last and noise_sigma is not None) else None))
             a = o
+        self.noise_step = self.layers[-1].noise_step     # None: the deterministic mu
         self.flops = sum(l.flops for l in self.layers)
         self.launches_per_forward = 1 + len(self.layers)
 
@@ -237,7 +256,19 @@ def _prefix(full, part):
     return full
 
 
-def v2p_networks_from_checkpoint(checkpoint, obs_dim=None, normalize_input=True, dual=False):
+def _fixed_sigma(model, what):
+    """sigma = exp(a2c_network.sigma) of a checkpoint's actor (`fixed_sigma: True`: the model's `sigma_act(self.sigma)` is the log std,
+    v2p_models.py:26 / im_models.py:24 take exp of it); refused with the reason for a learned sigma head or no sigma"""
+    if "sigma.weight" in model:
+        raise ValueError(f"{what}: the checkpoint has a learned sigma head (sigma.weight, fixed_sigma: False); the sampled action "
+                         "serves the fixed sigma parameter only (every shipped cfg sets fixed_sigma: True)")
+    if "sigma" not in model:
+        raise ValueError(f"{what}: deterministic=False samples mu + sigma * N(0, 1), but the checkpoint has no fixed sigma "
+                         "(a2c_network.sigma)")
+    return torch.exp(model["sigma"].float())
+
+
+def v2p_networks_from_checkpoint(checkpoint, obs_dim=None, normalize_input=True, dual=False, deterministic=True):
     """What V2PPlayer.restore (vid2player/players/v2p_player.py:71-111; dual: load_dual_cp :21-69) reads from the controller
     checkpoint(s), as one dict per network: `layers` [(weight, bias)] x 4 (actor_mlp.{0,2,4}, mu; the first zero-padded to obs_dim
     columns), `mean` / `rstd` [obs_dim] (None: no normaliser) and `clip` (the normaliser's clamp, inf for none).
@@ -246,15 +277,19 @@ def v2p_networks_from_checkpoint(checkpoint, obs_dim=None, normalize_input=True,
       dual:   each network's RunningNorm (running_obs_type 'ours'): `running_obs.{n,mean,std}` of the model, or else rl_games statistics
               of the checkpoint's `running_mean_std` or of the model's `running_obs.{running_mean,running_var,count}` with std = sqrt(var);
               a prefix leaves mean 0, std 0 behind it (rstd 1e8).  rstd = 1 / (std + 1e-8), clamp 5; identity while n == 0.
+    deterministic=False (a stochastic player): also `sigma` [actions] = exp(a2c_network.sigma) of each checkpoint (see _fixed_sigma).
     checkpoint: a path or a loaded dict (dual: a pair).  CPU tensors, float32."""
     out = []
-    for cp in (checkpoint if dual else [checkpoint]):
+    for p, cp in enumerate(checkpoint if dual else [checkpoint]):
         ck = _load(cp)
         model = {k[len("a2c_network."):]: v for k, v in ck["model"].items() if k.startswith("a2c_network.")}
+        sigma = None if deterministic else _fixed_sigma(model, f"checkpoint {p}" if dual else "checkpoint")
         layers = [(model[k + ".weight"].float(), model[k + ".bias"].float()) for k in V2P_ACTOR_KEYS]
         D = obs_dim or layers[0][0].shape[1]
         layers[0] = (_pad_first(layers[0][0], D), layers[0][1])
         net = dict(layers=layers, mean=None, rstd=None, clip=float("inf"))
+        if sigma is not None:
+            net["sigma"] = sigma
         if not dual:
             if normalize_input:
                 rms = ck["running_mean_std"]
@@ -298,25 +333,27 @@ def im_networks_from_checkpoint(checkpoint, use_running_obs=True, running_obs_ty
       running_obs_type ours:    RunningNorm (see _running_norm); a Lightning checkpoint loads only its own running_obs.* keys
       running_obs_type rl_game: RunningMeanStd, rstd = 1 / sqrt(var + 1e-5), clamp 5, always applied: the model's
                                 running_obs.{running_mean,running_var}, else the fresh statistics (mean 0, var 1)
-    Refused, with the reason: normalize_input (the player's own RunningMeanStd over the raw obs), use_ik and a stochastic player.
-    checkpoint: a path or a loaded dict.  CPU tensors, float32."""
+    deterministic=False (a stochastic player): also `sigma` [actions] = exp(sigma) of the actor (see _fixed_sigma), which
+    HumanoidSMPLIMVis.run_test then samples with.  Refused, with the reason: normalize_input (the player's own RunningMeanStd over the
+    raw obs), use_ik, and with deterministic=False a learned sigma head or a checkpoint without sigma.  checkpoint: a path or a loaded
+    dict.  CPU tensors, float32."""
     if normalize_input:
         raise ValueError("normalize_input: True normalises the raw 461-wide observation before the network; the device operand launch "
                          "reads obs_buf as the wrapper clamps it and does not implement that normaliser (neither shipped cfg sets it)")
     if use_ik:
         raise ValueError("use_ik: the network's inverse kinematics of the context (perform_ik) needs the SMPL model files and is not "
                          "implemented on the device")
-    if not deterministic:
-        raise ValueError("the imitation policy serves the deterministic action (mu) only: the sampled action of a stochastic player "
-                         "(mu + sigma * N(0, 1)) is not implemented")
     ck = _load(checkpoint)
     lightning = "pytorch-lightning_version" in ck
     if lightning:
         model = dict(ck["state_dict"])
     else:
         model = {k[len("a2c_network."):]: v for k, v in ck["model"].items() if k.startswith("a2c_network.")}
+    sigma = None if deterministic else _fixed_sigma(model, "imitation checkpoint")
     layers = [(model[k + ".weight"].float(), model[k + ".bias"].float()) for k in V2P_ACTOR_KEYS]
     net = dict(layers=layers, mean=None, rstd=None, clip=float("inf"))
+    if sigma is not None:
+        net["sigma"] = sigma
     if not use_running_obs:
         return net
     if running_obs_type == "rl_game":
@@ -395,9 +432,15 @@ class V2PPolicy:
     It also serves the trained low-level imitation policy (low_level_networks_from_cfg; operand rows from b200env_obs_imitation_rows).
 
     The operand `x` is normally written by the controller's post launch (`operand()` gives it the fields of b200v2p_ctrl_t), and
-    `forward_prepared()` runs the layers only; `forward(obs)` fills it from a float observation first.  bf16 operands, fp32 accumulation."""
+    `forward_prepared()` runs the layers only; `forward(obs)` fills it from a float observation first.  bf16 operands, fp32 accumulation.
 
-    def __init__(self, networks, num_envs, device, clip_obs=float("inf"), clip_actions=None, activation="relu"):
+    deterministic=False: the sampled action of a stochastic player (V2PPlayer.get_action's `res_dict['actions']`, the `distr.sample()`
+    of Normal(mu, sigma), v2p_models.py:26-43): every network dict carries `sigma` [actions] and network p's last layer adds
+    sigma_p[col] * N(0, 1) to its rows before the action clamp.  The normals come from the counter-based generator under `seed`, keyed
+    on the output element (env * actions + col) and each last layer's device step counter (`noise_steps`), so a graph replay draws
+    afresh: the distribution of the reference's torch draws, not their stream."""
+
+    def __init__(self, networks, num_envs, device, clip_obs=float("inf"), clip_actions=None, activation="relu", deterministic=True, seed=0):
         self.dual = len(networks) == 2
         if len(networks) not in (1, 2):
             raise ValueError("one network (single) or two (dual)")
@@ -408,6 +451,9 @@ class V2PPolicy:
         self.out_dim = networks[0]["layers"][-1][0].shape[0]
         self.clip_obs, self.clip_actions = float(clip_obs), clip_actions
         P, dev = len(networks), self.device
+        self.deterministic, self.seed = bool(deterministic), int(seed)
+        if not deterministic and any(n.get("sigma") is None for n in networks):
+            raise ValueError("deterministic=False needs every network's sigma (v2p_networks_from_checkpoint(..., deterministic=False))")
         if all(n["mean"] is None for n in networks):
             self.mean = self.rstd = None
         else:   # a network without a normaliser (RunningNorm with n == 0) is the identity: mean 0, rstd 1, no clamp
@@ -424,22 +470,22 @@ class V2PPolicy:
             for i, (w, b) in enumerate(net["layers"]):
                 last = i == len(net["layers"]) - 1
                 o = out_view if last else padded_bf16(H, w.shape[0], dev)
+                noise = (net["sigma"], seed) if (last and not deterministic) else None
                 self.layers.append(Linear(a, w, b, o, H, act=None if last else activation, out_col0=p * self.out_dim if last else 0,
-                                          out_clamp=(-clip_actions, clip_actions) if (last and clip_actions) else None))
+                                          out_clamp=(-clip_actions, clip_actions) if (last and clip_actions) else None, noise=noise))
                 a = o
+        self.noise_steps = [l.noise_step for l in self.layers if l.noise_step is not None]   # one per network; [] when deterministic
         self.flops = sum(l.flops for l in self.layers)
 
     @classmethod
     def from_checkpoint(cls, checkpoint, num_envs, device, obs_dim=None, normalize_input=True, clip_obs=float("inf"), clip_actions=None,
-                        deterministic=True):
+                        deterministic=True, seed=0):
         """checkpoint: a path or loaded dict (single, V2PPlayer.restore), or a pair of them (dual, load_dual_cp); clip_obs / clip_actions:
-        the wrapper's clamps (VecTaskPython.clip_obs / clip_actions)"""
-        if not deterministic:
-            raise ValueError("V2PPolicy serves the deterministic action (mu) only: the sampled action of a stochastic player "
-                             "(mu + sigma * N(0, 1)) is not implemented")
+        the wrapper's clamps (VecTaskPython.clip_obs / clip_actions); deterministic / seed: the player's `is_determenistic` and the
+        cfg's params.seed (offset by rank like the task's cfg["seed"]) for the sampled action"""
         dual = isinstance(checkpoint, (list, tuple))
-        nets = v2p_networks_from_checkpoint(checkpoint, obs_dim=obs_dim, normalize_input=normalize_input, dual=dual)
-        return cls(nets, num_envs, device, clip_obs=clip_obs, clip_actions=clip_actions)
+        nets = v2p_networks_from_checkpoint(checkpoint, obs_dim=obs_dim, normalize_input=normalize_input, dual=dual, deterministic=deterministic)
+        return cls(nets, num_envs, device, clip_obs=clip_obs, clip_actions=clip_actions, deterministic=deterministic, seed=seed)
 
     def operand(self):
         """(scalars, tensors) of b200v2p_ctrl_t's policy fields for native_v2p.controller_post"""

@@ -1,11 +1,13 @@
 """HumanoidSMPLIMVis mirror (embodied_pose/env/tasks/humanoid_smpl_im_vis.py): the task `run.py --test` builds from the imitation cfgs'
-`test_name`, and the test loop of ImitatorPlayer.run (embodied_pose/players/im_player.py:193-312) with the deterministic action.
+`test_name`, and the test loop of ImitatorPlayer.run (embodied_pose/players/im_player.py:193-312) with the deterministic action, or the
+sampled one of a stochastic player (a network dict with `sigma`, nn.im_networks_from_checkpoint(..., deterministic=False)).
 
 The loop runs on the device.  Per step, one CUDA graph replays four pieces:
   - the policy's operand launch (include/b200env.h: b200env_im_policy_rows): the network's 734-wide observation from obs_buf and the
     context slot of the device step counter, normalised and cast to bf16, and that slot's target dof_pos;
-  - the four wgmma layers of nn.PolicyMLP; the last one adds the target dof_pos (the residual action) and applies the wrapper's action
-    clamp in its epilogue;
+  - the four wgmma layers of nn.PolicyMLP; the last one adds the target dof_pos (the residual action), for a stochastic player then
+    sigma * N(0, 1) (counter-based, seeded by cfg["seed"], its step counter advanced by the launch itself), and applies the wrapper's
+    action clamp in its epilogue;
   - the env step;
   - the player's bookkeeping (b200env_play_stats): cumulative rewards and steps, finished games and the per-step statistics lines.
 The host only rebuilds the context window every context_length steps (it knows the step count) and reads the stop flag and the
@@ -42,8 +44,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
 
     # ------------------------------------------------------------------ test loop of ImitatorPlayer.run
     def set_policy(self, network, clip_obs=float("inf"), clip_actions=None, sync_every=None):
-        """network: a dict of nn.im_networks_from_checkpoint (layers, mean, rstd, clip); clip_obs / clip_actions: the wrapper's clamps
-        (VecTaskPython.clip_obs / clip_actions).  Allocates the operand, residual and statistics buffers; sync_every (default
+        """network: a dict of nn.im_networks_from_checkpoint (layers, mean, rstd, clip; with `sigma`: the sampled action, seeded by
+        cfg["seed"]); clip_obs / clip_actions: the wrapper's clamps (VecTaskPython.clip_obs / clip_actions).  Allocates the operand, residual and statistics buffers; sync_every (default
         context_length) sizes the statistics log the host drains."""
         N, dev, nd = self.num_envs, self.device, self.num_dof
         w = self._env.obs_row_width()
@@ -54,7 +56,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._im_step = torch.zeros(1, device=dev, dtype=torch.long)
         self._im_resid = torch.zeros(N, nd, device=dev)
         self._im_policy = nn.PolicyMLP(network["layers"], N, dev, obs_mean=network["mean"], obs_rstd=network["rstd"],
-                                       clamp_obs=network["clip"], clamp_actions=clip_actions, residual=(self._im_resid, nd))
+                                       clamp_obs=network["clip"], clamp_actions=clip_actions, residual=(self._im_resid, nd),
+                                       noise_sigma=network.get("sigma"), seed=int(self.cfg.get("seed", 10)))
         self._im_clip_obs, self._im_clip = float(clip_obs), float(network["clip"])
         cap = int(sync_every or self.context_length) + 1
         f = lambda *s: torch.zeros(*s, device=dev)  # noqa: E731
@@ -76,7 +79,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                  resid=self._im_resid))
 
     def act(self):
-        """operand launch + the four layers: the deterministic action (float [N, num_actions], a static buffer)"""
+        """operand launch + the four layers: the action, deterministic or sampled (float [N, num_actions], a static buffer)"""
         self.policy_rows()
         return self._im_policy.forward_prepared()
 
@@ -106,7 +109,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
 
     def run_test(self, policy, games_num, max_steps, n_game_life=1, print_stats=True, sync_every=None, clip_obs=float("inf"),
                  clip_actions=None, graph=True, history=None):
-        """ImitatorPlayer.run with the deterministic mu (im_player.py:193-312): per game a full reset(), then up to max_steps
+        """ImitatorPlayer.run (im_player.py:193-312) with the deterministic mu, or the sampled action when `policy` has a sigma: per game a full reset(), then up to max_steps
         test_step() calls; the host reads the stop flag and the statistics log every sync_every (default context_length) steps and at
         max_steps, and prints the reference's lines in order.  policy: a dict of nn.im_networks_from_checkpoint.  history: a list that
         receives, per game, the list of device copies (rew_buf, reset_buf) of every step run (for tests).  Returns dict(sum_rewards,

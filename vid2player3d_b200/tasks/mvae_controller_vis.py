@@ -132,7 +132,9 @@ class _EvalRecorder:
         self._test_graphs = None
 
     def run_test(self, policy, max_steps, graph=True):
-        """V2PPlayer.run with the deterministic action: reset, render_vis(init=True), then `max_steps` test_step() calls.  Ends like
+        """V2PPlayer.run with the policy's action (deterministic mu, or sampled for an nn.V2PPolicy built with deterministic=False: the
+        noise is drawn inside the policy's last layer, so the graphs replay it afresh): reset, render_vis(init=True), then `max_steps`
+        test_step() calls.  Ends like
         the reference, with SystemExit once num_rec_frames frames are recorded (with record)."""
         self.set_policy(policy)
         self.reset()
