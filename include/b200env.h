@@ -194,7 +194,9 @@ int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_
  * init_dof_vel[e] ([N,nd]), progress / reset / terminate = 0, raw obs from the new dofs and the rigid-body rows as they stand;
  * init_* may be NULL when ref_prob >= 1.  Rows whose mask is clear are not touched.
  * counter: [1] int64 device, advanced by 1 by every call; work: [num_envs + 2] int32 device, zero before the first call (each call
- * leaves its counters zero). */
+ * leaves its counters zero).
+ * The xf_* fields and feat_width are the transform program of the window (B200_XF_* below, as b200env_motion_context applies it);
+ * both launches read the same *counter, so its draws are those b200env_motion_context makes for (e, frame, body) at that counter. */
 typedef struct b200_reset_masked {
   int32_t sample_time;     /* 0: ref-state init at t = 0, 1: at a drawn time */
   float truncate, ref_prob;
@@ -208,6 +210,11 @@ typedef struct b200_reset_masked {
   float* context_feat;     /* [num_envs, num_frames, W] */
   uint8_t* context_mask;   /* [num_envs, num_frames] */
   int32_t* work;           /* [num_envs + 2] */
+  /* transform program, appended within ABI version 11; all zero = no transforms, rows W wide */
+  int32_t xf_ops[3];
+  uint32_t xf_joint_mask;
+  float xf_noisy_prob, xf_noise_std, xf_conf_std, xf_min_conf, xf_random_prob;
+  int32_t feat_width;
 } b200_reset_masked_t;
 int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* stream);
 
@@ -338,7 +345,26 @@ int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_st
 /* replaces HumanoidSMPLIM._init_context (embodied_pose/env/tasks/humanoid_smpl_im.py:530-563): for listed env i and frame
  * j in [0, num_frames): t = motion_times[i] + dt + (first_frame + j) * dt; writes
  * context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos  ([N, num_frames, 2*(3B+D)+4B] row-major) and
- * context_mask[row, j] = t <= motion_length + 2 dt, with row = env_ids[i] (or i when env_ids is NULL). */
+ * context_mask[row, j] = t <= motion_length + 2 dt, with row = env_ids[i] (or i when env_ids is NULL).
+ *
+ * Transform program (HumanoidSMPLIM._transform_target, humanoid_smpl_im.py:565-592, cfg.env.transform_specs): xf_ops[0..2] lists up
+ * to three of B200_XF_MASK_JOINTS / B200_XF_NOISY_JOINTS / B200_XF_MASK_RANDOM_JOINTS in the cfg's order, each at most once, ended by
+ * 0.  feat_width is the row width of context_feat: 0 or W = 2 (3 nb + nd) + 4 nb without a program, W + nb (the joint_conf block
+ * appended) with one.  Lane b of frame j of row e starts from pos = body_pos[b], conf = local = 1 and applies the ops in order:
+ *   MASK_JOINTS:   bit b of xf_joint_mask set: local = 0, and conf = 0 while no NOISY_JOINTS ran before; then pos *= local
+ *                  (the reference zeroes and multiplies by its local joint_conf tensor, which NOISY_JOINTS stops aliasing);
+ *   NOISY_JOINTS:  noise = z * (u0 < xf_noisy_prob ? xf_noise_std : 0), z = three N(0, 1) draws; pos += noise;
+ *                  conf = erfc(|noise| / (sqrt 3 xf_conf_std) / sqrt 2); conf < xf_min_conf: conf = 0, pos = 0;
+ *   MASK_RANDOM_JOINTS: b > 0 and u4 < xf_random_prob: conf = 0 (and local, while aliased), pos = 0.
+ * The row is body_pos (transformed) | body_rot | dof_pos | body_pos_gt | dof_pos_gt | conf; every frame is transformed whatever its
+ * mask.  Draws: bits(seed, *counter, 2 num_envs + ((e P + j) nb + b) 5 + k), u_k = (bits >> 40) 2^-24 for k = 0, 4 and z = the
+ * Box-Muller normal of counter_rng.cuh for k = 1..3; the offset 2 num_envs keeps them clear of b200env_reset_masked's 2e + k.  This
+ * launch reads *counter and does not advance it.  Returns -2 before any launch on a repeated or unknown op, an op after a 0, a prob
+ * outside [0, 1], xf_conf_std <= 0 or xf_noise_std < 0 with NOISY_JOINTS, a feat_width other than W or W + nb (W + nb with ops),
+ * and counter NULL with NOISY_JOINTS or MASK_RANDOM_JOINTS.  A zeroed program is the window without transforms. */
+#define B200_XF_MASK_JOINTS 1
+#define B200_XF_NOISY_JOINTS 2
+#define B200_XF_MASK_RANDOM_JOINTS 3
 typedef struct b200_motion_context {
   int32_t n, num_frames, first_frame;
   float dt;
@@ -347,8 +373,20 @@ typedef struct b200_motion_context {
   const float* motion_times;   /* [n] */
   float* context_feat;
   uint8_t* context_mask;
+  /* transform program, appended within ABI version 11; all zero = no transforms, rows W wide */
+  int32_t xf_ops[3];
+  uint32_t xf_joint_mask;
+  float xf_noisy_prob, xf_noise_std, xf_conf_std, xf_min_conf, xf_random_prob;
+  int32_t feat_width;
+  uint64_t seed;
+  const int64_t* counter;      /* [1], or NULL without draws */
 } b200_motion_context_t;
 int b200env_motion_context(b200env_handle h, const b200_motion_context_t* d, void* stream);
+
+/* sizeof(b200_reset_masked_t) and sizeof(b200_motion_context_t) as the library was built: both grew by appended fields within ABI
+ * version 11, and the binding refuses a library whose sizes differ from its own. */
+int32_t b200env_reset_masked_desc_size(void);
+int32_t b200env_motion_context_desc_size(void);
 
 /* Heterogeneous assets per env (dual mode: env 2k = player 0's asset, env 2k+1 = player 1's,
  * vid2player/env/tasks/humanoid_smpl_im_mvae.py:270-275 `motion_ids[1::2] = 1`): one handle per asset, all bound to the SAME

@@ -310,6 +310,49 @@ class PlayStats(C.Structure):
     _nullable_, _defaults_ = (), ()
 
 
+# the context window's transform program (include/b200env.h: b200_motion_context_t), appended to b200_reset_masked_t and
+# b200_motion_context_t; zero = no transforms
+XF_MASK_JOINTS, XF_NOISY_JOINTS, XF_MASK_RANDOM_JOINTS = 1, 2, 3
+_XF_FIELDS = [("xf_ops", C.c_int32 * 3), ("xf_joint_mask", C.c_uint32), ("xf_noisy_prob", C.c_float), ("xf_noise_std", C.c_float),
+              ("xf_conf_std", C.c_float), ("xf_min_conf", C.c_float), ("xf_random_prob", C.c_float), ("feat_width", C.c_int32)]
+_XF_DEFAULTS = tuple(name for name, _ in _XF_FIELDS)
+TRANSFORMS = {"mask_joints": XF_MASK_JOINTS, "noisy_joints": XF_NOISY_JOINTS, "mask_random_joints": XF_MASK_RANDOM_JOINTS}
+
+
+def transform_program(transform_specs, body_names, num_bodies):
+    """the xf_* fields of cfg.env.transform_specs (HumanoidSMPLIM._transform_target, humanoid_smpl_im.py:565-592), ops in the dict's
+    order; body_names[:num_bodies] are the bodies of joint_conf.  Raises ValueError on an unknown or repeated transform, a joint that
+    is not one of those bodies, a prob outside [0, 1], noise_std < 0, conf_std <= 0 or a missing key; the refusals of the C side."""
+    ops, p = [], dict(xf_joint_mask=0, xf_noisy_prob=0.0, xf_noise_std=0.0, xf_conf_std=0.0, xf_min_conf=0.0, xf_random_prob=0.0)
+    if num_bodies > 32:
+        raise ValueError(f"transform_specs: {num_bodies} bodies, the device transforms serve at most 32")
+    for name, specs in (transform_specs or {}).items():
+        if name not in TRANSFORMS:
+            raise ValueError(f"transform_specs: unknown transform {name!r} (known: {', '.join(TRANSFORMS)})")
+        ops.append(TRANSFORMS[name])
+        try:
+            if name == "mask_joints":
+                for j in specs["joints"]:
+                    if j not in body_names[:num_bodies]:
+                        raise ValueError(f"transform_specs.mask_joints: {j!r} is not a body of the humanoid")
+                    p["xf_joint_mask"] |= 1 << body_names.index(j)
+            elif name == "noisy_joints":
+                p.update(xf_noisy_prob=float(specs["prob"]), xf_noise_std=float(specs["noise_std"]), xf_conf_std=float(specs["conf_std"]),
+                         xf_min_conf=float(specs["min_conf"]))
+                if not p["xf_noise_std"] >= 0:
+                    raise ValueError(f"transform_specs.noisy_joints: noise_std {specs['noise_std']} < 0")
+                if not p["xf_conf_std"] > 0:
+                    raise ValueError(f"transform_specs.noisy_joints: conf_std {specs['conf_std']} must be > 0")
+            else:
+                p["xf_random_prob"] = float(specs["prob"])
+        except KeyError as ex:
+            raise ValueError(f"transform_specs.{name}: missing {ex.args[0]!r}") from None
+        prob = p["xf_noisy_prob"] if name == "noisy_joints" else p["xf_random_prob"]
+        if name != "mask_joints" and not 0.0 <= prob <= 1.0:
+            raise ValueError(f"transform_specs.{name}: prob {prob} outside [0, 1]")
+    return dict(p, xf_ops=ops + [0] * (3 - len(ops)))
+
+
 class ResetMasked(C.Structure):
     """b200_reset_masked_t: the mask-driven reset of the imitation task (b200env_reset_masked)"""
     _fields_ = [
@@ -317,8 +360,8 @@ class ResetMasked(C.Structure):
         ("first_frame", C.c_int32), ("dt", C.c_float), ("seed", C.c_uint64),
         ("mask", U8P), ("counter", I64P), ("init_root", F32P), ("init_dof_pos", F32P), ("init_dof_vel", F32P), ("reset_times", F32P),
         ("context_feat", F32P), ("context_mask", U8P), ("work", I32P),
-    ]
-    _nullable_, _defaults_ = ("init_root", "init_dof_pos", "init_dof_vel"), ()
+    ] + _XF_FIELDS
+    _nullable_, _defaults_ = ("init_root", "init_dof_pos", "init_dof_vel"), _XF_DEFAULTS
 
 
 class MotionState(C.Structure):
@@ -337,8 +380,8 @@ class MotionContext(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("num_frames", C.c_int32), ("first_frame", C.c_int32), ("dt", C.c_float),
         ("env_ids", I64P), ("motion_ids", I64P), ("motion_times", F32P), ("context_feat", F32P), ("context_mask", U8P),
-    ]
-    _nullable_, _defaults_ = ("env_ids",), ()
+    ] + _XF_FIELDS + [("seed", C.c_uint64), ("counter", I64P)]
+    _nullable_, _defaults_ = ("env_ids", "counter"), _XF_DEFAULTS + ("seed",)
 
 
 class ObsImitation(C.Structure):
@@ -590,6 +633,8 @@ SIGNATURES = {
     "b200env_obs_imitation_rows_dual": (C.c_int, [_p, _p, _p]),
     "b200env_physics_only": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "b200env_motion_context": (C.c_int, [_p, _p, _p]),
+    "b200env_reset_masked_desc_size": (_i32, []),
+    "b200env_motion_context_desc_size": (_i32, []),
     "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),
     "b200env_play_stats": (C.c_int, [_p, _p]),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),

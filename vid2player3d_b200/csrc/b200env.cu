@@ -1679,11 +1679,65 @@ motion_state_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restr
   if (dof_vel) for (int k = lane; k < nd; k += 32) dof_vel[i * nd + k] = ml.dvs[s.f0 * nd + k];
 }
 
+// transform program of the context window (include/b200env.h: b200_motion_context_t), passed by value to the launches that apply it
+struct ContextXf {
+  int32_t ops[3];
+  uint32_t joint_mask;
+  float noisy_prob, noise_std, conf_scale, min_conf, random_prob;   // conf_scale = sqrt(3) * conf_std
+  uint64_t seed;
+  const int64_t* counter;
+  int64_t num_envs;
+};
+
+// _transform_target (humanoid_smpl_im.py:565-592) on body `lane` of frame j of row e: transforms pos in place, returns joint_conf.
+// `local` is the reference's local joint_conf tensor (:567), which mask_joints zeroes and multiplies by; context_dict['joint_conf']
+// is that tensor until noisy_joints rebinds it to the noise confidence (alias false), so a later mask_joints zeroes its joints'
+// positions but leaves their conf and every other joint alone.  Float ops are the reference's, one rounding each (no contraction).
+__device__ __forceinline__ float context_transform(const ContextXf& xf, uint64_t c, int64_t e, int j, int P, int nbl, int lane, float pos[3]) {
+  const uint64_t base = 2 * (uint64_t)xf.num_envs + (((uint64_t)e * P + j) * nbl + lane) * 5;
+  float conf = 1.f, local = 1.f;
+  bool alias = true;
+#pragma unroll
+  for (int q = 0; q < 3; q++) {
+    const int op = xf.ops[q];
+    if (op == B200_XF_MASK_JOINTS) {
+      if ((xf.joint_mask >> lane) & 1u) {
+        local = 0.f;
+        if (alias) conf = 0.f;
+      }
+#pragma unroll
+      for (int k = 0; k < 3; k++) pos[k] = __fmul_rn(pos[k], local);
+    } else if (op == B200_XF_NOISY_JOINTS) {
+      const float sd = counter_uniform(xf.seed, c, base) < xf.noisy_prob ? xf.noise_std : 0.f;
+      float nz[3];
+#pragma unroll
+      for (int k = 0; k < 3; k++) nz[k] = __fmul_rn(counter_normal(xf.seed, c, base + 1 + k), sd);
+      const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(nz[0], nz[0]), __fmul_rn(nz[1], nz[1])), __fmul_rn(nz[2], nz[2])));
+      conf = erfcf(__fmul_rn(__fdiv_rn(nrm, xf.conf_scale), 0.70710678118654752f));
+      alias = false;
+      const bool occluded = conf < xf.min_conf;
+      if (occluded) conf = 0.f;
+#pragma unroll
+      for (int k = 0; k < 3; k++) pos[k] = occluded ? 0.f : __fadd_rn(pos[k], nz[k]);
+    } else if (op == B200_XF_MASK_RANDOM_JOINTS) {
+      if (lane > 0 && counter_uniform(xf.seed, c, base + 4) < xf.random_prob) {
+        conf = 0.f;
+        if (alias) local = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; k++) pos[k] = 0.f;
+      }
+    }
+  }
+  return conf;
+}
+
 // _init_context (humanoid_smpl_im.py:530-563): frame j of the P-frame MoCap window of motion mid starting at motion time time0, written
-// straight into context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos and context_mask[row, j]; one warp.
+// straight into context_feat[row, j, :] = rb_pos | rb_rot | dof_pos | rb_pos | dof_pos and context_mask[row, j]; one warp.  XF: the
+// transform program applied to the first rb_pos block and joint_conf appended (rows W + nbl wide), drawing at counter value c.
+template <bool XF>
 __device__ __forceinline__ void context_frame(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_motion_lib_t& ml,
                                               int64_t mid, float time0, int64_t row, int j, int P, int first, float dt, float two_dt,
-                                              float* __restrict__ feat, uint8_t* __restrict__ mask, int lane) {
+                                              float* __restrict__ feat, uint8_t* __restrict__ mask, int lane, const ContextXf& xf, uint64_t c) {
   const b200_model_t& M = gblob->m;
   const int nd = M.nd, nbl = ml.num_lib_bodies;
   const int dof0 = lane < M.nb ? M.dof_of_body[lane] : -1;
@@ -1691,10 +1745,17 @@ __device__ __forceinline__ void context_frame(const DevBlob* __restrict__ gblob,
   const float t = __fadd_rn(__fadd_rn(time0, dt), __fmul_rn((float)(first + j), dt));
   const MotionSample s = sample_motion(ml, M, mid, t, lane, gcfg->ground_tolerance);
   const int W = nbl * 3 + nbl * 4 + nd + nbl * 3 + nd;
-  float* o = feat + (row * P + j) * W;
+  float* o = feat + (row * P + j) * (XF ? W + nbl : W);
   if (lane < nbl) {
+    if constexpr (XF) {
+      float pos[3] = {s.rb_pos[0], s.rb_pos[1], s.rb_pos[2]};
+      o[W + lane] = context_transform(xf, c, row, j, P, nbl, lane, pos);
 #pragma unroll
-    for (int k = 0; k < 3; k++) { o[lane * 3 + k] = s.rb_pos[k]; o[nbl * 7 + nd + lane * 3 + k] = s.rb_pos[k]; }
+      for (int k = 0; k < 3; k++) { o[lane * 3 + k] = pos[k]; o[nbl * 7 + nd + lane * 3 + k] = s.rb_pos[k]; }
+    } else {
+#pragma unroll
+      for (int k = 0; k < 3; k++) { o[lane * 3 + k] = s.rb_pos[k]; o[nbl * 7 + nd + lane * 3 + k] = s.rb_pos[k]; }
+    }
 #pragma unroll
     for (int k = 0; k < 4; k++) o[nbl * 3 + lane * 4 + k] = s.rb_rot[k];
     if (dof0 >= 0) {
@@ -1706,38 +1767,67 @@ __device__ __forceinline__ void context_frame(const DevBlob* __restrict__ gblob,
 }
 
 // the window of each listed env; warp per (env, frame)
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
-motion_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
-                      const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids, const float* __restrict__ times, int n, int P,
-                      int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+template <bool XF>
+__device__ __forceinline__ void motion_context_body(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_motion_lib_t& ml,
+                                                    const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids,
+                                                    const float* __restrict__ times, int n, int P, int first, float dt, float two_dt,
+                                                    float* __restrict__ feat, uint8_t* __restrict__ mask, const ContextXf& xf) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp;
   if (w >= (int64_t)n * P) return;
   const int64_t i = w / P;
   const int j = (int)(w - i * P);
-  context_frame(gblob, gcfg, ml, ids[i], times[i], env_ids ? env_ids[i] : i, j, P, first, dt, two_dt, feat, mask, lane);
+  const uint64_t c = XF && xf.counter ? (uint64_t)xf.counter[0] : 0;
+  context_frame<XF>(gblob, gcfg, ml, ids[i], times[i], env_ids ? env_ids[i] : i, j, P, first, dt, two_dt, feat, mask, lane, xf, c);
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+motion_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                      const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids, const float* __restrict__ times, int n, int P,
+                      int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+  motion_context_body<false>(gblob, gcfg, ml, env_ids, ids, times, n, P, first, dt, two_dt, feat, mask, ContextXf{});
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+motion_context_xf_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                         const int64_t* __restrict__ env_ids, const int64_t* __restrict__ ids, const float* __restrict__ times, int n, int P,
+                         int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask, ContextXf xf) {
+  motion_context_body<true>(gblob, gcfg, ml, env_ids, ids, times, n, P, first, dt, two_dt, feat, mask, xf);
 }
 
 // b200env_reset_masked, second launch: the window of every env on the work list of reset_masked_kernel at its drawn time, warp per
 // (env, frame) over a grid of fixed size (the list's length is only known on the device).  The last block to finish clears the list
-// and advances the launch counter, so the pair of launches replays inside a CUDA graph with fresh draws every time.
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
-reset_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
-                     const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
-                     int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+// and advances the launch counter, so the pair of launches replays inside a CUDA graph with fresh draws every time.  XF: with the
+// transform program, drawing at the counter value both launches read.
+template <bool XF>
+__device__ __forceinline__ void reset_context_body(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_motion_lib_t& ml,
+                                                   const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work,
+                                                   int64_t* counter, int P, int first, float dt, float two_dt, float* __restrict__ feat,
+                                                   uint8_t* __restrict__ mask, const ContextXf& xf) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t total = (int64_t)work[0] * P;
+  const uint64_t c = XF ? (uint64_t)counter[0] : 0;
   for (int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp; w < total; w += (int64_t)gridDim.x * WARPS_PER_CTA) {
     const int64_t i = w / P;
     const int j = (int)(w - i * P);
     const int64_t e = work[2 + i];
-    context_frame(gblob, gcfg, ml, motion_ids[e], reset_times[e], e, j, P, first, dt, two_dt, feat, mask, lane);
+    context_frame<XF>(gblob, gcfg, ml, motion_ids[e], reset_times[e], e, j, P, first, dt, two_dt, feat, mask, lane, xf, c);
   }
   __shared__ bool last;
   __syncthreads();
   if (threadIdx.x == 0) last = atomicAdd(reinterpret_cast<unsigned int*>(&work[1]), 1u) == gridDim.x - 1;
   __syncthreads();
   if (last && threadIdx.x == 0) { counter[0] += 1; work[0] = 0; work[1] = 0; __threadfence(); }
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_context_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                     const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
+                     int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask) {
+  reset_context_body<false>(gblob, gcfg, ml, motion_ids, reset_times, work, counter, P, first, dt, two_dt, feat, mask, ContextXf{});
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_context_xf_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                        const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
+                        int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask, ContextXf xf) {
+  reset_context_body<true>(gblob, gcfg, ml, motion_ids, reset_times, work, counter, P, first, dt, two_dt, feat, mask, xf);
 }
 
 // compute_humanoid_observations_imitation (humanoid_smpl_im.py:773-850): warp per env, lane per body
@@ -2587,6 +2677,52 @@ int b200env_reset(b200env_handle h, const int64_t* env_ids, const float* motion_
   return 0;
 }
 
+// the transform program of a b200_reset_masked_t / b200_motion_context_t as the launch's ContextXf; *xf_on: launch the XF form (a
+// program, or rows W + nbl wide).  Refusals of include/b200env.h, before any launch.
+extern "C++" {
+template <class D>
+static int context_xf(const char* who, b200env_handle h, const D* d, const int64_t* counter, ContextXf* xf, bool* xf_on) {
+  const int nbl = h->ml.num_lib_bodies, nd = h->model.nd;
+  const int W = nbl * 3 + nbl * 4 + nd + nbl * 3 + nd;
+  int num_ops = 0;
+  bool seen[4] = {false, false, false, false}, ended = false;
+  for (int q = 0; q < 3; q++) {
+    const int op = d->xf_ops[q];
+    if (op == 0) { ended = true; continue; }
+    if (ended) return fail(-2, "%s: a transform op after the program's end (0)", who);
+    if (op < B200_XF_MASK_JOINTS || op > B200_XF_MASK_RANDOM_JOINTS) return fail(-2, "%s: unknown transform op", who);
+    if (seen[op]) return fail(-2, "%s: a transform op repeated", who);
+    seen[op] = true;
+    num_ops++;
+  }
+  const auto prob_ok = [](float p) { return p >= 0.f && p <= 1.f; };
+  if (!prob_ok(d->xf_noisy_prob) || !prob_ok(d->xf_random_prob)) return fail(-2, "%s: a transform prob outside [0, 1]", who);
+  if (seen[B200_XF_NOISY_JOINTS] && !(d->xf_conf_std > 0.f)) return fail(-2, "%s: noisy_joints needs conf_std > 0", who);
+  if (seen[B200_XF_NOISY_JOINTS] && !(d->xf_noise_std >= 0.f)) return fail(-2, "%s: noisy_joints needs noise_std >= 0", who);
+  const int fw = d->feat_width;
+  if (num_ops ? fw != W + nbl : (fw != 0 && fw != W && fw != W + nbl))
+    return fail(-2, "%s: context_feat row width must be W, or W + bodies (joint_conf) with a transform program", who);
+  if ((seen[B200_XF_NOISY_JOINTS] || seen[B200_XF_MASK_RANDOM_JOINTS]) && !counter)
+    return fail(-2, "%s: noisy_joints / mask_random_joints need the draw counter", who);
+  *xf_on = fw == W + nbl;
+  *xf = ContextXf{};
+  for (int q = 0; q < 3; q++) xf->ops[q] = d->xf_ops[q];
+  xf->joint_mask = d->xf_joint_mask;
+  xf->noisy_prob = d->xf_noisy_prob;
+  xf->noise_std = d->xf_noise_std;
+  xf->conf_scale = (float)(1.7320508075688772 * (double)d->xf_conf_std);
+  xf->min_conf = d->xf_min_conf;
+  xf->random_prob = d->xf_random_prob;
+  xf->seed = d->seed;
+  xf->counter = counter;
+  xf->num_envs = h->num_envs;
+  return 0;
+}
+}  // extern "C++"
+
+int32_t b200env_reset_masked_desc_size(void) { return (int32_t)sizeof(b200_reset_masked_t); }
+int32_t b200env_motion_context_desc_size(void) { return (int32_t)sizeof(b200_motion_context_t); }
+
 int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* stream) {
   if (!h) return fail(-1, "b200env_reset_masked: null handle%s");
   if (!d || !d->mask || !d->counter || !d->reset_times || !d->context_feat || !d->context_mask || !d->work || d->num_frames < 1)
@@ -2594,6 +2730,9 @@ int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* s
   if (d->ref_prob < 1.0f && (!d->init_root || !d->init_dof_pos || !d->init_dof_vel))
     return fail(-1, "b200env_reset_masked: ref_prob < 1 needs the initial root and dof buffers%s");
   if (!h->bound || !h->has_ml) return fail(-4, "b200env_reset_masked: bind buffers and a motion lib first%s");
+  ContextXf xf;
+  bool xf_on = false;
+  if (int rc = context_xf("b200env_reset_masked", h, d, d->counter, &xf, &xf_on)) return rc;
   cudaSetDevice(h->device);
   const int n = h->num_envs;
   reset_masked_kernel<<<(n + WARPS_PER_CTA - 1) / WARPS_PER_CTA, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
@@ -2604,9 +2743,15 @@ int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* s
   CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
   const int64_t warps = (int64_t)n * d->num_frames;
   const int grid = (int)std::min<int64_t>((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (int64_t)sms * 8);
-  reset_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
-                                                                              d->reset_times, d->work, d->counter, d->num_frames, d->first_frame,
-                                                                              d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
+  if (xf_on)
+    reset_context_xf_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
+                                                                                   d->reset_times, d->work, d->counter, d->num_frames,
+                                                                                   d->first_frame, d->dt, (float)(2.0 * (double)d->dt),
+                                                                                   d->context_feat, d->context_mask, xf);
+  else
+    reset_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
+                                                                                d->reset_times, d->work, d->counter, d->num_frames, d->first_frame,
+                                                                                d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
   CUDA_OK(cudaGetLastError());
   h->launches += 2;
   return 0;
@@ -2637,12 +2782,21 @@ int b200env_motion_context(b200env_handle h, const b200_motion_context_t* d, voi
   if (!d->motion_ids || !d->motion_times || !d->context_feat || !d->context_mask || n < 0 || d->num_frames < 1)
     return fail(-1, "b200env_motion_context: bad arguments%s");
   if (!h->has_ml) return fail(-4, "b200env_motion_context: set a motion lib first%s");
+  ContextXf xf;
+  bool xf_on = false;
+  if (int rc = context_xf("b200env_motion_context", h, d, d->counter, &xf, &xf_on)) return rc;
   cudaSetDevice(h->device);
   const int64_t warps = (int64_t)n * d->num_frames;
   const int grid = (int)((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA);
-  motion_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, d->env_ids,
-                                                                               d->motion_ids, d->motion_times, n, d->num_frames, d->first_frame,
-                                                                               d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
+  if (xf_on)
+    motion_context_xf_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, d->env_ids,
+                                                                                    d->motion_ids, d->motion_times, n, d->num_frames,
+                                                                                    d->first_frame, d->dt, (float)(2.0 * (double)d->dt),
+                                                                                    d->context_feat, d->context_mask, xf);
+  else
+    motion_context_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, d->env_ids,
+                                                                                 d->motion_ids, d->motion_times, n, d->num_frames, d->first_frame,
+                                                                                 d->dt, (float)(2.0 * (double)d->dt), d->context_feat, d->context_mask);
   CUDA_OK(cudaGetLastError());
   h->launches++;
   return 0;

@@ -26,6 +26,9 @@ def lib():
             fn.restype, fn.argtypes = restype, argtypes
         if L.b200env_abi_version() != abi.ABI_VERSION:
             raise RuntimeError("libb200env.so ABI version mismatch - rebuild")
+        for S, size in ((abi.ResetMasked, L.b200env_reset_masked_desc_size()), (abi.MotionContext, L.b200env_motion_context_desc_size())):
+            if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
+                raise RuntimeError(f"libb200env.so takes a {size}-byte {S.__name__} descriptor, the binding fills {C.sizeof(S)} - rebuild")
         _lib = L
     return _lib
 
@@ -220,10 +223,12 @@ class Env:
             _check(lib().b200env_reset(self._h, _ptr(env_ids), _ptr(motion_times), n, _stream()))
 
     def reset_masked(self, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos, init_dof_vel, reset_times,
-                     num_frames, first_frame, dt, feat, feat_mask, work):
-        """reset of the envs whose mask [N] bool is set, context window included (include/b200env.h: b200env_reset_masked)"""
+                     num_frames, first_frame, dt, feat, feat_mask, work, transforms=None):
+        """reset of the envs whose mask [N] bool is set, context window included (include/b200env.h: b200env_reset_masked);
+        transforms: the window's transform program (abi.transform_program), with feat rows W + bodies wide"""
         assert mask.shape[0] == self.num_envs and work.shape[0] >= self.num_envs + 2
-        d = fill(abi.ResetMasked, dict(sample_time=int(bool(sample_time)), truncate=truncate, ref_prob=ref_prob, num_frames=num_frames,
+        xf = dict(transforms, feat_width=int(feat.shape[-1])) if transforms is not None else {}
+        d = fill(abi.ResetMasked, dict(xf, sample_time=int(bool(sample_time)), truncate=truncate, ref_prob=ref_prob, num_frames=num_frames,
                                        first_frame=first_frame, dt=dt, seed=int(seed)),
                  dict(mask=mask, counter=counter, init_root=init_root, init_dof_pos=init_dof_pos, init_dof_vel=init_dof_vel,
                       reset_times=reset_times, context_feat=feat, context_mask=feat_mask, work=work))
@@ -235,10 +240,14 @@ class Env:
         d = fill(abi.MotionState, dict(n=ids.shape[0]), dict(out, motion_ids=ids, motion_times=times))
         _check(lib().b200env_motion_state(self._h, C.byref(d), _stream()))
 
-    def motion_context(self, env_ids, motion_ids, motion_times, num_frames, first_frame, dt, feat, mask):
-        """feat [N, num_frames, W] float32, mask [N, num_frames] bool; rows env_ids (None: rows 0..n-1)"""
-        d = fill(abi.MotionContext, dict(n=motion_ids.shape[0], num_frames=num_frames, first_frame=first_frame, dt=dt),
-                 dict(env_ids=env_ids, motion_ids=motion_ids, motion_times=motion_times, context_feat=feat, context_mask=mask))
+    def motion_context(self, env_ids, motion_ids, motion_times, num_frames, first_frame, dt, feat, mask, transforms=None, seed=0,
+                       counter=None):
+        """feat [N, num_frames, W] float32, mask [N, num_frames] bool; rows env_ids (None: rows 0..n-1).  transforms: the transform
+        program (abi.transform_program) with feat [N, num_frames, W + bodies], drawing from (seed, counter [1] int64, not advanced)"""
+        xf = dict(transforms, feat_width=int(feat.shape[-1]), seed=int(seed)) if transforms is not None else {}
+        d = fill(abi.MotionContext, dict(xf, n=motion_ids.shape[0], num_frames=num_frames, first_frame=first_frame, dt=dt),
+                 dict(env_ids=env_ids, motion_ids=motion_ids, motion_times=motion_times, context_feat=feat, context_mask=mask,
+                      counter=counter))
         _check(lib().b200env_motion_context(self._h, C.byref(d), _stream()))
 
     def obs_row_width(self, jpos=False):

@@ -125,6 +125,11 @@ class HumanoidSMPLIM(BaseTask):
         self._transform_specs = self.cfg['env'].get('transform_specs', None)
         if 'transform_specs' in self.cfg['env']:             # :202-204
             self.context_names.append('joint_conf')
+        # cfg.env.b200_device_transforms (addition): the context window's transforms run in the window launches (include/b200env.h:
+        # b200_motion_context_t), so reset_masked / reset_done and their graph serve transform_specs; the program is built here, once
+        self._xf_program = None
+        if self.cfg['env'].get('b200_device_transforms', False) and 'transform_specs' in self.cfg['env']:
+            self._xf_program = abi.transform_program(self._transform_specs, self.body_names, nb)
         self.context_shapes = [shape_dict[x] for x in self.context_names]
         self.context_dims = [int(np.prod(x)) for x in self.context_shapes]
         self.is_env_dim_setup = False
@@ -363,10 +368,12 @@ class HumanoidSMPLIM(BaseTask):
         bool, device) is set are reset by two launches (include/b200env.h: b200env_reset_masked) that make no host synchronisation,
         so the call can be captured in a CUDA graph.  Same state init, rows and context window as `reset(env_ids)`; the motion
         times and the Hybrid choice are drawn on the device from a counter-based generator seeded by cfg["seed"], a different stream
-        of the same distribution as the torch.rand / torch.bernoulli draws of `reset(env_ids)`.  Not with cfg.env.transform_specs
-        (its transforms of the window are torch ops on the reset rows): use `reset(env_ids)` there."""
-        if self._transform_specs is not None:
-            raise ValueError("reset_masked: cfg.env.transform_specs transforms the context window in torch - use reset(env_ids)")
+        of the same distribution as the torch.rand / torch.bernoulli draws of `reset(env_ids)`.  With cfg.env.transform_specs only under
+        cfg.env.b200_device_transforms (the window launch applies them, drawing at the same counter); otherwise the transforms are torch
+        ops on the reset rows: use `reset(env_ids)` there."""
+        if self._transform_specs is not None and self._xf_program is None:
+            raise ValueError("reset_masked: cfg.env.transform_specs transforms the context window in torch - use reset(env_ids), "
+                             "or set cfg.env.b200_device_transforms")
         modes = {"Start": (False, 1.0), "Random": (True, 1.0), "Hybrid": (True, min(float(self._hybrid_init_prob), 1.0)),
                  "Default": (False, 0.0)}
         if self._state_init not in modes:
@@ -377,14 +384,14 @@ class HumanoidSMPLIM(BaseTask):
         self._env.reset_masked(mask, sample_time, truncate, ref_prob, self.cfg.get("seed", 10), self._reset_rng,
                                self._initial_humanoid_root_states, self._initial_dof_pos, self._initial_dof_vel, self._reset_ref_motion_times,
                                self.context_length + self.context_padding * 2, -self.context_padding, self.dt, self.context_feat,
-                               self.context_mask, self._reset_work)
+                               self.context_mask, self._reset_work, transforms=self._xf_program)
         self._forward_context()
 
     def reset_done(self):
         """Addition: reset the envs whose reset_buf is set, from the device flags: the mask is taken with torch.ne and the reset is
         one replay of the reset graph when one was captured (VecTaskPython.enable_cuda_graph(reset_graph=True)), else `reset_masked`.
-        No host synchronisation.  With cfg.env.transform_specs: `reset(reset_buf.nonzero())`."""
-        if self._transform_specs is not None:
+        No host synchronisation.  With cfg.env.transform_specs and without cfg.env.b200_device_transforms: `reset(reset_buf.nonzero())`."""
+        if self._transform_specs is not None and self._xf_program is None:
             self.reset(self.reset_buf.nonzero(as_tuple=False).flatten())
             return
         torch.ne(self.reset_buf, 0, out=self._reset_mask)
@@ -395,8 +402,9 @@ class HumanoidSMPLIM(BaseTask):
 
     def _capture_reset_graph(self, tail=None):
         """capture `reset_masked(self._reset_mask)` and then `tail()` as the graph `reset_done` replays (warm-up: one eager call with an
-        empty mask, which only advances the draw counter); nothing with cfg.env.transform_specs.  Returns whether a graph was captured."""
-        if self._transform_specs is not None:
+        empty mask, which only advances the draw counter); nothing with cfg.env.transform_specs unless cfg.env.b200_device_transforms.
+        Returns whether a graph was captured."""
+        if self._transform_specs is not None and self._xf_program is None:
             return False
         self._reset_graph = None
         self._reset_mask.zero_()
@@ -424,13 +432,22 @@ class HumanoidSMPLIM(BaseTask):
         if not hasattr(self, "context_feat"):
             self.context_feat = torch.zeros(self.num_envs, P, W + (nbl if with_conf else 0), device=self.device)
             self.context_mask = torch.zeros(self.num_envs, P, device=self.device, dtype=torch.bool)
-            self._context_raw = torch.zeros(self.num_envs, P, W, device=self.device) if with_conf else self.context_feat
+            torch_xf = with_conf and self._xf_program is None        # the torch transforms read the raw rows of a W-wide buffer
+            self._context_raw = torch.zeros(self.num_envs, P, W, device=self.device) if torch_xf else self.context_feat
         return P, with_conf
 
     def _init_context(self, env_ids, motion_ids, motion_times):
-        """:530-563: 48-frame MoCap window per env -> context_feat / context_mask (one launch)."""
+        """:530-563: 48-frame MoCap window per env -> context_feat / context_mask (one launch).  Under cfg.env.b200_device_transforms
+        the launch also applies transform_specs, drawing at the masked reset's counter, which it then advances (a torch add)."""
         P, with_conf = self._context_buffers()
         env_ids = env_ids.to(self.device, dtype=torch.long).contiguous()
+        if self._xf_program is not None:
+            self._env.motion_context(env_ids, motion_ids.contiguous(), motion_times.contiguous(), P, -self.context_padding, self.dt,
+                                     self.context_feat, self.context_mask, transforms=self._xf_program, seed=self.cfg.get("seed", 10),
+                                     counter=self._reset_rng)
+            self._reset_rng.add_(1)
+            self._forward_context()
+            return
         self._env.motion_context(env_ids, motion_ids.contiguous(), motion_times.contiguous(),
                                  P, -self.context_padding, self.dt, self._context_raw, self.context_mask)
         if with_conf:

@@ -78,7 +78,8 @@ class VecTaskPython(VecTask):
         Valid while rl_device == the task's device and the task's step makes no host synchronisation (true for the env step).
         The warm-up runs a few real env steps: call it before the reset() that starts a rollout.
         reset_graph=True (tasks with `reset_masked`, e.g. HumanoidSMPLIM): also capture `task.reset_masked(mask of the finished envs)
-        -> clamp(obs)` as a second graph, which `reset_done()` replays (not with cfg.env.transform_specs: that reset stays eager)."""
+        -> clamp(obs)` as a second graph, which `reset_done()` replays (with cfg.env.transform_specs only under
+        cfg.env.b200_device_transforms, which applies them in the window launch; otherwise that reset stays eager)."""
         assert str(self.rl_device) == str(self.task.device), "graph capture needs rl_device == sim device"
         dev = self.task.device
         self._graph = None
@@ -120,7 +121,7 @@ class VecTaskPythonWrapper(VecTaskPython):
 
     def reset_done(self):
         """Addition: `reset(reset_buf.nonzero())` from the device flags (task.reset_done: no host synchronisation unless the task has
-        cfg.env.transform_specs).  Returns the clamped observations in a fixed buffer, overwritten by the next reset_done(); with
+        cfg.env.transform_specs without cfg.env.b200_device_transforms).  Returns the clamped observations in a fixed buffer, overwritten by the next reset_done(); with
         enable_cuda_graph(reset_graph=True) the reset and the clamp are one graph replay after the mask launch."""
         self.task.reset_done()
         if not getattr(self, "_reset_obs_in_graph", False):
