@@ -328,6 +328,48 @@ typedef struct b200_play_stats {
 
 int b200env_play_stats(const b200_play_stats_t* d, void* stream);
 
+/* One recorded frame of HumanoidSMPLIMVis._sync_ref_motion (embodied_pose/env/tasks/humanoid_smpl_im_vis.py:128-152) for every listed
+ * env: the qpos the reference's MuJoCo viewer shows, without the viewer.  One warp per recorded env i (row env_ids[i]); frame
+ * f = *frame.  With nq = 7 + nd and J = nd / 3, row (i, f) of qpos [n_rec, cap, 2, nq] gets
+ *   copy 0: rigid_body_state[e, 0] pos, its quaternion xyzw as wxyz, then the euler angles of dof_pos[e] (the dof_state column);
+ *   copy 1: init = 0: the root row of p_rb_pos / p_rb_rot and the euler angles of p_dof_pos[e]; init = 1: copy 0; then x += 1.
+ * The viewer's third copy (copy 0 with z += 1000) is left to the host.  The euler angles of a joint's rotation vector a are konia's
+ * angle_axis_to_quaternion (theta = sqrt(max(|a|^2, 1e-6)), k = sin(theta / 2) / theta, w = cos(theta / 2); |a| = 0: (1, 0, 0, 0))
+ * and ypr_euler_from_quat (atan2 with 1e-6 added to y when |y| and |x| are both below 1e-6, asin of the argument clamped to
+ * +-(1 - 1e-6)), computed in double from the float32 state and stored yaw, pitch, roll (the [2, 1, 0] reorder of its roll, pitch, yaw).  rec_motion_ids / rec_reset [n_rec, cap] get motion_ids[e] and reset_buf[e] (0 with init).
+ * The last CTA advances *frame by one (the ticket `done` is re-armed), so one CUDA graph capture replays every frame.
+ * games: b200_play_stats_t::games or NULL.  While games[1] (stop) is set, or *frame >= cap, the launch writes nothing and does not
+ * advance; the launch that writes frame cap - 1 sets games[1], so the bookkeeping of the same step changes nothing.  NULL: no stop flag.
+ * Returns -2 before any launch when n_rec, cap or num_envs is not positive, nd is not a positive multiple of 3, or num_bodies or
+ * num_lib_bodies is below 1.  env_ids must lie in [0, num_envs): the launch does not check them. */
+typedef struct b200_im_record {
+  int32_t n_rec;           /* recorded envs E */
+  int32_t num_envs;        /* rows of the state arrays */
+  int32_t num_bodies;      /* bodies per env of rigid_body_state */
+  int32_t num_lib_bodies;  /* bodies per env of p_rb_pos / p_rb_rot */
+  int32_t nd;              /* dofs: 3 per joint */
+  int32_t cap;             /* frames of the record buffers */
+  int32_t init;            /* 1: render_vis(init=True) */
+  int32_t pad_;
+  const int64_t* env_ids;          /* [n_rec] */
+  const float* rigid_body_state;   /* [num_envs, num_bodies, 13] */
+  const float* dof_state;          /* [num_envs, nd, 2] */
+  const float* p_dof_pos;          /* [num_envs, nd] */
+  const float* p_rb_pos;           /* [num_envs, num_lib_bodies, 3] */
+  const float* p_rb_rot;           /* [num_envs, num_lib_bodies, 4] */
+  const int64_t* reset_buf;        /* [num_envs] */
+  const int64_t* motion_ids;       /* [num_envs] */
+  float* qpos;                     /* [n_rec, cap, 2, 7 + nd] */
+  int64_t* rec_motion_ids;         /* [n_rec, cap] */
+  int64_t* rec_reset;              /* [n_rec, cap] */
+  int64_t* frame;                  /* [1] */
+  uint32_t* done;                  /* [1] ticket, 0 between launches */
+  int64_t* games;                  /* [3] or NULL */
+} b200_im_record_t;
+int b200env_im_record(const b200_im_record_t* d, void* stream);
+/* sizeof(b200_im_record_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_im_record_desc_size(void);
+
 /* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1): a separate test launch
  * (physics_kernel_packed; physics_kernel_tmem / physics_kernel for the other forms) that shares the control step
  * (control_step_packed) with b200env_step's physics launch, but not that launch's persistent hand-out of env batches,

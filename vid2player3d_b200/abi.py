@@ -310,6 +310,18 @@ class PlayStats(C.Structure):
     _nullable_, _defaults_ = (), ()
 
 
+class ImRecord(C.Structure):
+    """b200_im_record_t: one recorded viewer frame of HumanoidSMPLIMVis (b200env_im_record)"""
+    _fields_ = [
+        ("n_rec", C.c_int32), ("num_envs", C.c_int32), ("num_bodies", C.c_int32), ("num_lib_bodies", C.c_int32), ("nd", C.c_int32),
+        ("cap", C.c_int32), ("init", C.c_int32), ("pad_", C.c_int32),
+        ("env_ids", I64P), ("rigid_body_state", F32P), ("dof_state", F32P), ("p_dof_pos", F32P), ("p_rb_pos", F32P), ("p_rb_rot", F32P),
+        ("reset_buf", I64P), ("motion_ids", I64P), ("qpos", F32P), ("rec_motion_ids", I64P), ("rec_reset", I64P), ("frame", I64P),
+        ("done", U32P), ("games", I64P),
+    ]
+    _nullable_, _defaults_ = ("games",), ("pad_",)
+
+
 # the context window's transform program (include/b200env.h: b200_motion_context_t), appended to b200_reset_masked_t and
 # b200_motion_context_t; zero = no transforms
 XF_MASK_JOINTS, XF_NOISY_JOINTS, XF_MASK_RANDOM_JOINTS = 1, 2, 3
@@ -637,6 +649,8 @@ SIGNATURES = {
     "b200env_motion_context_desc_size": (_i32, []),
     "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),
     "b200env_play_stats": (C.c_int, [_p, _p]),
+    "b200env_im_record": (C.c_int, [_p, _p]),
+    "b200env_im_record_desc_size": (_i32, []),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
     "b200env_set_hull_faces": (C.c_int, [_p, _p, _p, _p, _i32]),
     "b200env_kernel_form": (_i32, [_p]),

@@ -2058,6 +2058,75 @@ __global__ void __launch_bounds__(PLAY_THREADS) play_stats_kernel(b200_play_stat
   }
 }
 
+// b200env_im_record: the euler angles the viewer gets for one joint's rotation vector (konia angle_axis_to_quaternion, then
+// ypr_euler_from_quat with eps 1e-6, reordered [2, 1, 0]).  theta >= 1e-3, so safe_zero_division never adds its eps.  In double: near
+// pitch +-pi/2 both atan2 arguments are rounding noise below eps, and float32 noise would turn yaw and roll into other angles.
+// sincospi needs no argument-reduction table, so the double kernels elsewhere in the library keep their code.
+__device__ __forceinline__ void rotvec_ypr(double a0, double a1, double a2, float* out) {
+  const double th2 = a0 * a0 + a1 * a1 + a2 * a2;
+  const double th = sqrt(fmax(th2, 1e-6));
+  double s, c;
+  sincospi(th * (0.5 / 3.14159265358979323846), &s, &c);
+  const double k = th2 > 0.0 ? s / th : 0.5, w = th2 > 0.0 ? c : 1.0;
+  const double x = a0 * k, y = a1 * k, z = a2 * k;
+  auto safe_atan2 = [](double yy, double xx) { return atan2((fabs(yy) < 1e-6 && fabs(xx) < 1e-6) ? yy + 1e-6 : yy, xx); };
+  out[0] = (float)safe_atan2(2.0 * (w * z + x * y), 1.0 - 2.0 * (y * y + z * z));
+  out[1] = (float)asin(fmin(fmax(2.0 * (w * y - x * z), -1.0 + 1e-6), 1.0 - 1e-6));
+  out[2] = (float)safe_atan2(2.0 * (w * x + y * z), 1.0 - 2.0 * (x * x + y * y));
+}
+
+// one warp per recorded env; task k < 2 (1 + J) of lane k, k + 32, ...: copy k / (1 + J), item k % (1 + J) (0: the root, else joint
+// item - 1).  The last CTA advances the frame counter (the ticket of last_block_advance) and sets the stop flag at the last frame.
+#define REC_WARPS 4
+__global__ void __launch_bounds__(REC_WARPS * 32) im_record_kernel(b200_im_record_t d) {
+  const int64_t f = d.frame[0];
+  if ((d.games && d.games[1]) || f >= d.cap) return;   // every CTA reads the same values: only the last CTA writes them
+  const int i = blockIdx.x * REC_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (i < d.n_rec) {
+    const int64_t e = d.env_ids[i];
+    const int nd = d.nd, J = nd / 3, nq = 7 + nd;
+    float* row = d.qpos + ((int64_t)i * d.cap + f) * 2 * nq;
+    for (int k = lane; k < 2 * (1 + J); k += 32) {
+      const int cp = k / (1 + J), item = k % (1 + J);
+      const bool sim = cp == 0 || d.init;
+      float* q = row + cp * nq;
+      if (item == 0) {
+        const float* p = sim ? d.rigid_body_state + e * d.num_bodies * 13 : d.p_rb_pos + e * d.num_lib_bodies * 3;
+        const float* r = sim ? p + 3 : d.p_rb_rot + e * d.num_lib_bodies * 4;
+        q[0] = cp ? p[0] + 1.0f : p[0];
+        q[1] = p[1]; q[2] = p[2];
+        q[3] = r[3]; q[4] = r[0]; q[5] = r[1]; q[6] = r[2];
+      } else {
+        const int j = item - 1;
+        float a[3];
+        if (sim) {
+          const float* s = d.dof_state + (e * nd + 3 * j) * 2;
+          a[0] = s[0]; a[1] = s[2]; a[2] = s[4];
+        } else {
+          const float* s = d.p_dof_pos + e * nd + 3 * j;
+          a[0] = s[0]; a[1] = s[1]; a[2] = s[2];
+        }
+        rotvec_ypr(a[0], a[1], a[2], q + 7 + 3 * j);
+      }
+    }
+    if (lane == 0) {
+      d.rec_motion_ids[(int64_t)i * d.cap + f] = d.motion_ids[e];
+      d.rec_reset[(int64_t)i * d.cap + f] = d.init ? 0 : d.reset_buf[e];
+    }
+  }
+  __shared__ bool last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) last = atomicAdd(d.done, 1u) == gridDim.x - 1;
+  __syncthreads();
+  if (last && threadIdx.x == 0) {
+    d.frame[0] = f + 1;
+    if (d.games && f == d.cap - 1) d.games[1] = 1;
+    *d.done = 0u;
+    __threadfence();
+  }
+}
+
 // physics-only entry used by the parity tests (float or double)
 template <typename T>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
@@ -2922,6 +2991,21 @@ int b200env_play_stats(const b200_play_stats_t* d, void* stream) {
   CUDA_OK(cudaGetLastError());
   return 0;
 }
+
+int b200env_im_record(const b200_im_record_t* d, void* stream) {
+  if (!d || !d->env_ids || !d->rigid_body_state || !d->dof_state || !d->p_dof_pos || !d->p_rb_pos || !d->p_rb_rot || !d->reset_buf ||
+      !d->motion_ids || !d->qpos || !d->rec_motion_ids || !d->rec_reset || !d->frame || !d->done)
+    return fail(-1, "b200env_im_record: null argument%s");
+  if (d->n_rec <= 0 || d->cap <= 0 || d->num_envs <= 0) return fail(-2, "b200env_im_record: n_rec, cap and num_envs must be positive%s");
+  if (d->nd <= 0 || d->nd % 3) return fail(-2, "b200env_im_record: nd must be a positive multiple of 3%s");
+  if (d->num_bodies < 1 || d->num_lib_bodies < 1) return fail(-2, "b200env_im_record: num_bodies and num_lib_bodies must be positive%s");
+  const int grid = (d->n_rec + REC_WARPS - 1) / REC_WARPS;
+  im_record_kernel<<<grid, REC_WARPS * 32, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int32_t b200env_im_record_desc_size(void) { return (int32_t)sizeof(b200_im_record_t); }
 
 int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_steps, void* root, void* dof_pos, void* dof_vel,
                          const void* pd_tar, const void* ext_wrench, void* rb_out, void* contact_out, void* ball, int32_t* ball_hits,

@@ -15,23 +15,133 @@ statistics log every `sync_every` steps.  The steps run after the stop flag was 
 next game's full reset discards their state, as the reference's `break` leaves it.
 
 Not served: the MuJoCo viewer (headless=False is refused) and the video (`record` is ignored: the reference opens a video file when
-headless but never writes a frame to it, since render_vis returns before rendering)."""
+headless but never writes a frame to it, since render_vis returns before rendering).
+
+Recording (cfg.env.b200_record_qpos, an addition): render_vis records, for the envs of cfg.env.b200_record_envs ([0] or "all"), the
+qpos the reference's viewer would show (_sync_ref_motion: the simulated humanoid, the target it tracked and the simulated one 1000 m
+up), one frame per call, on the device (include/b200env.h: b200env_im_record).  After num_rec_frames frames (the longest motion's
+frame count with args.rec_once) the frames go to an .npz (rec_fname with its extension replaced, or out/recording/qpos_<date>.npz)
+and SystemExit is raised, as the reference's render_vis quits.  run_test puts the record launch in the step graph, between the env
+step and the bookkeeping; a record launch that writes the last frame sets the bookkeeping's stop flag."""
+import os
+from datetime import datetime
+
+import numpy as np
 import torch
 
 from .. import native, nn
 from .humanoid_smpl_im import HumanoidSMPLIM
 
 
+def record_env_ids(spec, num_envs):
+    """cfg.env.b200_record_envs: a list of env ids or "all" -> the list of recorded envs"""
+    if isinstance(spec, str):
+        if spec != "all":
+            raise ValueError(f'b200_record_envs: {spec!r}; give a list of env ids or "all"')
+        return list(range(num_envs))
+    ids = [int(i) for i in spec]
+    if not ids:
+        raise ValueError("b200_record_envs is empty")
+    bad = [i for i in ids if not 0 <= i < num_envs]
+    if bad:
+        raise ValueError(f"b200_record_envs: env ids {bad} lie outside [0, {num_envs})")
+    if len(set(ids)) != len(ids):
+        raise ValueError(f"b200_record_envs: duplicate env ids {sorted({i for i in ids if ids.count(i) > 1})}")
+    return ids
+
+
+def record_frames(env, args, motion_num_frames):
+    """the frames to record: num_rec_frames (default 300), or the longest motion's frame count with args.rec_once"""
+    n = int(env.get("num_rec_frames", 300))
+    if getattr(args, "rec_once", False):
+        n = int(np.max(motion_num_frames))
+        print(f"Recording only {n} frames")
+    if n < 1:
+        raise ValueError(f"num_rec_frames must be at least 1, got {n}")
+    return n
+
+
+def record_path(env, now=None):
+    """rec_fname with its extension replaced by .npz, or out/recording/qpos_<date>.npz (next to the reference's video_<date>.mp4)"""
+    if env.get("rec_fname"):
+        return os.path.splitext(env["rec_fname"])[0] + ".npz"
+    now = now or datetime.now()
+    return os.path.join("out", "recording", "qpos_%s.npz" % now.strftime('%Y-%m-%d-%H:%M:%S'))
+
+
+def record_bytes(n_rec, cap, nq):
+    """device bytes of the qpos rows [n_rec, cap, 2, nq] float32"""
+    return n_rec * cap * 2 * nq * 4
+
+
+def assemble_qpos(rows):
+    """device rows [E, T, 2, nq] -> the viewer's qpos [E, T, 3 nq]: copy 0, copy 1, copy 0 with z += 1000"""
+    c2 = rows[:, :, 0].clone()
+    c2[..., 2] += 1000.0
+    return torch.cat([rows[:, :, 0], rows[:, :, 1], c2], -1)
+
+
 class HumanoidSMPLIMVis(HumanoidSMPLIM):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         if not headless:
             raise ValueError("HumanoidSMPLIMVis: there is no MuJoCo viewer; run headless")
+        env = cfg["env"]
+        self._rec = None
+        rec_ids = None
+        if env.get("b200_record_qpos", False):
+            rec_ids = record_env_ids(env.get("b200_record_envs", [0]), int(env["numEnvs"]))
+            if not getattr(cfg.get("args", None), "rec_once", False) and int(env.get("num_rec_frames", 300)) < 1:
+                raise ValueError(f"num_rec_frames must be at least 1, got {env['num_rec_frames']}")
         super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
                          headless=headless)
         self.headless = headless
         self.cam_inited = False
         self.vis_mode = getattr(self.args, "vis_mode", None)
         self._im_policy = None
+        if rec_ids is not None:
+            self._setup_record(rec_ids)
+
+    def _setup_record(self, ids):
+        """the recorder's device buffers, after the cfg checks and the free-memory check"""
+        env, dev = self.cfg["env"], self.device
+        cap, nq, E = record_frames(env, self.args, self._motion_lib.num_frames), 7 + self.num_dof, len(ids)
+        need, free = record_bytes(E, cap, nq), torch.cuda.mem_get_info(dev)[0]
+        if need > free:
+            raise ValueError(f"recording {E} envs x {cap} frames needs {need} bytes of device memory, {free} are free")
+        if "motion_assets" in env:
+            entries = env["motion_assets"]
+            name = lambda a: os.path.basename(str(a)) if isinstance(a, (str, os.PathLike)) else str(a["name"])  # noqa: E731
+            mids = self._reset_ref_motion_ids.cpu().numpy()
+            assets = [name(entries[mids[e]]) for e in ids]
+        else:
+            assets = [os.path.basename(env["asset"]["assetFileName"])] * E
+        i64 = lambda *s: torch.zeros(*s, device=dev, dtype=torch.long)  # noqa: E731
+        self._rec = dict(env_ids=torch.tensor(ids, device=dev, dtype=torch.long), qpos=torch.zeros(E, cap, 2, nq, device=dev),
+                         rec_motion_ids=i64(E, cap), rec_reset=i64(E, cap), frame=i64(1),
+                         done=torch.zeros(1, device=dev, dtype=torch.int32))
+        self._rec_cap, self._rec_assets, self._rec_path = cap, assets, record_path(env)
+        self.frame_index = 0
+
+    def _record_launch(self, init, games=None):
+        nb, nbl = self.num_bodies, self._num_lib_bodies
+        native.im_record(dict(n_rec=len(self._rec_assets), num_envs=self.num_envs, num_bodies=nb, num_lib_bodies=nbl, nd=self.num_dof,
+                              cap=self._rec_cap, init=int(init)),
+                         dict(self._rec, rigid_body_state=self._rigid_body_state, dof_state=self._dof_state,
+                              p_dof_pos=self._prev_target_dof_pos, p_rb_pos=self._prev_target_rb_pos, p_rb_rot=self._prev_target_rb_rot,
+                              reset_buf=self.reset_buf, motion_ids=self._reset_ref_motion_ids, games=games))
+
+    def export_recording(self):
+        """writes the frames recorded so far to the .npz; returns its path"""
+        T = min(int(self._rec["frame"]), self._rec_cap)
+        r = self._rec
+        path = self._rec_path
+        if os.path.dirname(path):
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+        np.savez(path, qpos=assemble_qpos(r["qpos"][:, :T]).cpu().numpy(), env_ids=r["env_ids"].cpu().numpy(),
+                 motion_ids=r["rec_motion_ids"][:, :T].cpu().numpy(), reset=r["rec_reset"][:, :T].cpu().numpy(),
+                 asset=np.array(self._rec_assets), fps=np.float64(1.0 / self.dt), nq=np.int64(7 + self.num_dof))
+        print(f"============ qpos of {T} frames written to {path} ============")
+        return path
 
     def create_sim(self):
         # humanoid_smpl_im_vis.py:35 sets max_episode_length = 3000; the step's reset rule reads it from the cfg struct made here
@@ -39,8 +149,15 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         super().create_sim()
 
     def render_vis(self, init=False):
-        """the reference's headless branch: nothing"""
-        return
+        """without b200_record_qpos the reference's headless branch: nothing.  With it: one frame of the recorded envs (init: after a
+        reset, the target copy is the simulated one); after num_rec_frames calls the .npz is written and SystemExit raised"""
+        if self._rec is None:
+            return
+        self._record_launch(init)
+        self.frame_index += 1
+        if self.frame_index >= self._rec_cap:
+            self.export_recording()
+            raise SystemExit
 
     # ------------------------------------------------------------------ test loop of ImitatorPlayer.run
     def set_policy(self, network, clip_obs=float("inf"), clip_actions=None, sync_every=None):
@@ -87,6 +204,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         with torch.no_grad():
             actions = self.act()
         self._env.step(actions)
+        if self._rec is not None:
+            self._record_launch(False, games=self._stats["games"])
         native.play_stats(dict(n=self.num_envs, max_log=self._stats_cap, n_games=self._n_games),
                           dict(self._stats, rew=self.rew_buf, reset_buf=self.reset_buf))
 
@@ -126,6 +245,11 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             for k in ("cr", "steps", "prev_dones", "step"):
                 st[k].zero_()
             st["games"][1:].zero_()            # stop flag and log rows; games_played and the totals run on
+            if self._rec is not None:          # render_vis(init=True): the host reads the frame counter once per game
+                self._record_launch(True, games=st["games"])
+                if int(self._rec["frame"]) >= self._rec_cap:
+                    self.export_recording()
+                    raise SystemExit
             game = [] if history is not None else None
             for n in range(max_steps):
                 self.test_step(n, graph)
@@ -138,6 +262,9 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                     if print_stats:
                         for count, r, s in rows:
                             print('reward:', r / count, 'steps:', s / count)
+                    if self._rec is not None and int(self._rec["frame"]) >= self._rec_cap:    # render_vis' quit()
+                        self.export_recording()
+                        raise SystemExit
                     if games[1]:
                         break
             if history is not None:
@@ -146,4 +273,6 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         games_played = int(st["games"][0])
         print(sum_rewards)
         print('av reward:', sum_rewards / games_played * n_game_life, 'av steps:', sum_steps / games_played * n_game_life)
+        if self._rec is not None:              # the games ended before the recorder filled: the frames so far
+            self.export_recording()
         return dict(sum_rewards=sum_rewards, sum_steps=sum_steps, games_played=games_played)
