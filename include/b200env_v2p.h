@@ -216,7 +216,10 @@ int b200v2p_ball_in_estimate(const b200v2p_inest_t* d, void* stream);
  * (env/tasks/physics_mvae_controller.py:173-201: _reset_balls for the reaction envs :503-524, _reset_recovery_tasks :242-245,
  * _reset_reaction_tasks :203-240), driven by the device-side masks instead of nonzero() id lists: no host sync.
  * Random draws come in as device tensors (torch RNG): pool_rand[n] in [0,P), side_rand[n] in [-1000,1000), frame_rand[n] in [-5,5),
- * target_seed: 3 floats (continuous mode) or n floats (discrete mode). */
+ * target_seed: 3 floats (continuous mode) or n floats (discrete mode).
+ * pool_cursor: NULL, or int64 [n] for the fixed test set (TennisBallGeneratorOffline with sample_random False, tennis_ball.py:444-447):
+ * a reaction env takes pool row pool_cursor[e] and moves its cursor to (pool_cursor[e] + 1) % pool_size; the ball's side is not looked
+ * at and pool_rand / side_rand are not read.  The cursor is only written here, so a graph replay advances it with no host work. */
 typedef struct b200v2p_treset {
   int32_t n, pool_size, ball_stride, bodies_per_env, reaction_nframes, target_mode; /* 0 none, 1 continuous, 2 discrete */
   float target_min[3], target_max[3];
@@ -231,8 +234,11 @@ typedef struct b200v2p_treset {
   int64_t *tar_time, *tar_time_total, *tar_action, *num_reset_reaction, *swing_type_cycle;
   float* ball_obs;       /* use_history_ball_obs (:213-214): rows of the reaction envs <- the new ball position repeated; NULL = off */
   int32_t obs_traj_len, pad_;
+  int64_t* pool_cursor;  /* appended field: a descriptor zeroed past obs_traj_len / pad_ keeps the random draw */
 } b200v2p_treset_t;
 int b200v2p_task_reset(const b200v2p_treset_t* r, void* stream);
+/* sizeof(b200v2p_treset_t) of the library, so that a binding refuses a library built before pool_cursor */
+int32_t b200v2p_task_reset_desc_size(void);
 
 /* replaces HumanoidSMPLIMMVAE._reset_actors + _set_env_state + _reset_env_tensors for an id list
  * (env/tasks/humanoid_smpl_im_mvae.py:463-501, 562-581): the FK of the motion generator's pose (b200v2p_smpl_to_sim over all

@@ -552,8 +552,9 @@ class V2PTaskReset(C.Structure):
         ("has_bounce", U8P), ("has_contact", U8P), ("bounce_in", U8P), ("est_bounce_in", U8P),
         ("tar_time", I64P), ("tar_time_total", I64P), ("tar_action", I64P), ("num_reset_reaction", I64P),
         ("swing_type_cycle", I64P), ("ball_obs", F32P), ("obs_traj_len", C.c_int32), ("pad_", C.c_int32),
+        ("pool_cursor", I64P),
     ]
-    _nullable_, _defaults_ = ("ball_obs",), ("obs_traj_len", "pad_")
+    _nullable_, _defaults_ = ("ball_obs", "pool_cursor"), ("obs_traj_len", "pad_")
 
 
 class V2PActorReset(C.Structure):
@@ -676,6 +677,7 @@ SIGNATURES = {
     "b200v2p_stream_gather": (C.c_int, [_p, _p]),
     "b200v2p_ball_in_estimate": (C.c_int, [_p, _p]),
     "b200v2p_task_reset": (C.c_int, [_p, _p]),
+    "b200v2p_task_reset_desc_size": (_i32, []),
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
     "b200v2p_eval_record": (C.c_int, [_p, _p]),
     "b200v2p_eval_best": (C.c_int, [_p, _p]),

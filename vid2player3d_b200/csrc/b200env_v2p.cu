@@ -1036,20 +1036,30 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) ball_in_estimate_kernel(int n,
 }
 
 // ------------------------------------------------------------------------------------------ mask-driven task reset
+// kSequential: the test-set branch of the offline pool (tennis_ball.py:444-447), row pool_cursor[e], then the cursor moves on
+template <bool kSequential>
 __global__ void __launch_bounds__(V2P_WARPS * 32) task_reset_kernel(b200v2p_treset_t r) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t e = (int64_t)blockIdx.x * V2P_WARPS + warp;
   if (e >= r.n) return;
   const bool rea = r.reset_reaction[e] != 0, rec = r.reset_recovery[e] != 0;
   if (!rea && !rec) return;
-  if (rea) {  // _reset_balls (:503-524) with the sample_random branch of the offline pool (tennis_ball.py:436-444)
-    int64_t idx = r.pool_rand[e];
-    if (r.ball_pos[e * 3 + 1] > 0.0f) {
-      idx = (int64_t)((r.ball_pos[e * 3] + 4.0f) / 8.0f * (float)r.pool_size) + r.side_rand[e];
-      idx = idx < 0 ? 0 : (idx > r.pool_size - 1 ? r.pool_size - 1 : idx);
+  if (rea) {  // _reset_balls (:503-524) with the offline pool's generate (tennis_ball.py:435-456)
+    int64_t idx;
+    if constexpr (kSequential) {
+      idx = r.pool_cursor[e];     // no start_pos remapping in this branch
+    } else {                      // sample_random (:436-444)
+      idx = r.pool_rand[e];
+      if (r.ball_pos[e * 3 + 1] > 0.0f) {
+        idx = (int64_t)((r.ball_pos[e * 3] + 4.0f) / 8.0f * (float)r.pool_size) + r.side_rand[e];
+        idx = idx < 0 ? 0 : (idx > r.pool_size - 1 ? r.pool_size - 1 : idx);
+      }
     }
     const float* row = r.pool + idx * 307;
-    __syncwarp();
+    __syncwarp();   // every lane has read the cursor before lane 0 moves it
+    if constexpr (kSequential) {
+      if (lane == 0) r.pool_cursor[e] = (idx + 1) % r.pool_size;
+    }
     if (r.ball_obs) {   // use_history_ball_obs: _ball_traj is left alone (:187-188), _ball_obs <- the launch position repeated (:213-214)
       for (int k = lane; k < r.obs_traj_len * 3; k += 32) r.ball_obs[e * r.obs_traj_len * 3 + k] = row[k % 3];
     } else {
@@ -1328,10 +1338,16 @@ int b200v2p_task_reset(const b200v2p_treset_t* r, void* stream) {
   if (!r) return vfail(-1, "b200v2p_task_reset: null");
   if (r->n == 0) return 0;
   if (r->pool_size < 1 || !r->pool || !r->reset_reaction || !r->reset_recovery) return vfail(-1, "b200v2p_task_reset: bad arguments");
-  task_reset_kernel<<<(r->n + V2P_WARPS - 1) / V2P_WARPS, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*r);
+  const unsigned grid = (r->n + V2P_WARPS - 1) / V2P_WARPS;
+  if (r->pool_cursor)
+    task_reset_kernel<true><<<grid, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*r);
+  else
+    task_reset_kernel<false><<<grid, V2P_WARPS * 32, 0, (cudaStream_t)stream>>>(*r);
   V_CUDA_OK();
   return 0;
 }
+
+int32_t b200v2p_task_reset_desc_size(void) { return (int32_t)sizeof(b200v2p_treset_t); }
 
 int b200v2p_ctrl_reset(const b200v2p_creset_t* d, void* stream) {
   if (!d) return vfail(-1, "b200v2p_ctrl_reset: bad arguments");

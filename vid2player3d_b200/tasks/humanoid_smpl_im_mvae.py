@@ -22,6 +22,41 @@ SMPL_NAMES = ["Pelvis", "L_Hip", "R_Hip", "Torso", "L_Knee", "R_Knee", "Spine", 
               "Neck", "L_Thorax", "R_Thorax", "Head", "L_Shoulder", "R_Shoulder", "L_Elbow", "R_Elbow", "L_Wrist", "R_Wrist",
               "L_Hand", "R_Hand"]
 SMPL_PARENTS = [-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21]
+TEST_MODES = ('random', 'single_cycle', 'multiple_cycle')
+
+
+def resolve_ball_pool(cfg_v2p, is_train):
+    """The incoming-ball pool of the single-player task and how it is drawn (:121-130): (pool [P, 307] float32 or None, sequential).
+
+    Training, or test_mode 'random' (the default): `ball_pool`, else the file `ball_traj_file`, else a synthetic pool; rows are drawn
+    at random.  At test time with test_mode 'single_cycle' or 'multiple_cycle' (set from env.ball_traj_file_test by
+    PhysicsMVAEController): `ball_pool_test`, else the file `ball_traj_file_test`; every env walks the rows in order (sequential).  A
+    missing test set is refused, since a random pool in its place would measure something else.  Dual mode builds no pool (None, False):
+    its incoming balls come from the in-estimator table, so the test-set keys are ignored there, as in the reference."""
+    if cfg_v2p.get('dual_mode', False):
+        return None, False
+    mode = cfg_v2p.get('test_mode', 'random')
+    if mode not in TEST_MODES:
+        raise ValueError(f"vid2player.test_mode {mode!r}: must be one of {', '.join(TEST_MODES)}")
+    if is_train or mode == 'random':
+        pool = cfg_v2p.get("ball_pool", None)
+        if pool is None:
+            path = cfg_v2p.get("ball_traj_file")
+            pool = np.load(path) if path and os.path.exists(path) else ball_data.synthetic_pool(2048, seed=10, spin_scale=cfg_v2p.get("spin_scale", 1.0))
+        return np.asarray(pool, np.float32), False
+    pool = cfg_v2p.get("ball_pool_test", None)
+    if pool is None:
+        path = cfg_v2p.get("ball_traj_file_test")
+        if not path:
+            raise ValueError(f"vid2player.test_mode {mode!r} evaluates on a fixed test set, but neither ball_traj_file_test nor "
+                             "ball_pool_test is given")
+        if not os.path.exists(path):
+            raise ValueError(f"vid2player.ball_traj_file_test {path!r} does not exist: the test set cannot be evaluated")
+        pool = np.load(path)
+    pool = np.asarray(pool, np.float32)
+    if pool.ndim != 2 or pool.shape[0] < 1 or pool.shape[1] != 307:
+        raise ValueError(f"the ball test set must be [P >= 1, 307] (launch pos, vel, vspin, 100 x 3 trajectory), got {list(pool.shape)}")
+    return pool, True
 
 
 class HumanoidSMPLIMMVAE(BaseTask):
@@ -220,12 +255,11 @@ class HumanoidSMPLIMMVAE(BaseTask):
         self._tmp = dict(root_rot=f(N, 4), dof_pos=f(N, D), root_vel=f(N, 3), root_ang_vel=f(N, 3), dof_vel=f(N, D), rb_pos=f(N, 24, 3),
                          rb_rot=f(N, 24, 4))
         # incoming-ball pool (TennisBallGeneratorOffline, utils/tennis_ball.py:422-456); dual mode has the in-estimator instead (:126-130)
-        if not self.cfg_v2p.get('dual_mode', False):
-            pool = self.cfg_v2p.get("ball_pool", None)
-            if pool is None:
-                path = self.cfg_v2p.get("ball_traj_file")
-                pool = np.load(path) if path and os.path.exists(path) else ball_data.synthetic_pool(2048, seed=10, spin_scale=self.cfg_v2p.get("spin_scale", 1.0))
-            self._ball_pool = torch.tensor(np.asarray(pool, np.float32), device=dev).contiguous()
+        pool, sequential = resolve_ball_pool(self.cfg_v2p, self._is_train)
+        if pool is not None:
+            self._ball_pool = torch.tensor(pool, device=dev).contiguous()
+        # the test set's per-env cursor (sample_idx, :433): only the ball resets move it, so it carries over humanoid resets
+        self._ball_pool_cursor = torch.zeros(N, device=dev, dtype=torch.long) if sequential else None
         self._ball_traj_buf = f(N, 100, 3)
         self.extras["terminate"] = self._terminate_buf
 
@@ -350,13 +384,18 @@ class HumanoidSMPLIMMVAE(BaseTask):
             reset_buf=self.reset_buf, terminate_buf=self._terminate_buf))
 
     def _reset_balls(self, env_ids):
-        """:503-524 with the random branch of TennisBallGeneratorOffline.generate (tennis_ball.py:436-444)"""
+        """:503-524 with TennisBallGeneratorOffline.generate (tennis_ball.py:435-456): the random branch (:436-444), or on a test set
+        the env's next row in order (:444-447)"""
         P = self._ball_pool.shape[0]
-        idx = torch.randint(0, P, (len(env_ids),), device=self.device)
-        other = self._ball_pos[env_ids, 1] > 0
-        if other.any():
-            j = ((self._ball_pos[env_ids, 0] + 4) / 8 * P).long() + torch.randint(-1000, 1000, (len(env_ids),), device=self.device)
-            idx = torch.where(other, torch.clamp(j, 0, P - 1), idx)
+        if self._ball_pool_cursor is not None:
+            idx = self._ball_pool_cursor[env_ids]
+            self._ball_pool_cursor[env_ids] = (idx + 1) % P
+        else:
+            idx = torch.randint(0, P, (len(env_ids),), device=self.device)
+            other = self._ball_pos[env_ids, 1] > 0
+            if other.any():
+                j = ((self._ball_pos[env_ids, 0] + 4) / 8 * P).long() + torch.randint(-1000, 1000, (len(env_ids),), device=self.device)
+                idx = torch.where(other, torch.clamp(j, 0, P - 1), idx)
         native_v2p.ball_reset(env_ids.contiguous(), idx.contiguous(), self._ball_pool, self._root_states[1:], self._ball_pos, self._ball_vel,
                               self._has_bounce, self._bounce_pos, self._has_racket_ball_contact, self._ball_traj_buf, stride=26)
         rbs = self._rigid_body_state.view(self.num_envs, 26, 13)

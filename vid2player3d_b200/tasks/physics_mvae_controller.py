@@ -33,6 +33,17 @@ SMPL_BETA = {
 BASE_ROTMAT = [[0.0, 0.0, 1.0], [1.0, 0.0, 0.0], [0.0, 1.0, 0.0]]  # quaternion (.5,.5,.5,.5): SMPL y-up -> world z-up
 
 
+def resolve_test_set(env, cfg_v2p):
+    """`run.py --test --ball_traj_file_test F` (player_builder.py:154-156): env.ball_traj_file_test is copied into the vid2player block,
+    with test_mode 'single_cycle' when the file name contains 'single', else 'multiple_cycle'.  Without the key nothing changes.  The
+    physics task then evaluates on that file's balls in order (humanoid_smpl_im_mvae.resolve_ball_pool); a plugged-in motion player can
+    read cfg_v2p['test_mode'] itself."""
+    path = env.get('ball_traj_file_test')
+    if path:
+        cfg_v2p['ball_traj_file_test'] = path
+        cfg_v2p['test_mode'] = 'single_cycle' if 'single' in str(path) else 'multiple_cycle'
+
+
 _SKEW = None
 
 
@@ -328,6 +339,7 @@ class PhysicsMVAEController:
     def create_sim(self):
         env = self.cfg["env"]
         phys = env.get("physics", {})
+        resolve_test_set(env, self.cfg_v2p)
         pcfg = {"env": dict(numEnvs=self.num_envs, episodeLength=self._max_episode_length, controlFrequencyInv=env.get("controlFrequencyInv", 2),
                             residual_force_scale=phys.get("residual_force_scale", 31.85), is_train=self._is_train,
                             localRootObs=phys.get("localRootObs", True), rootHeightObs=phys.get("rootHeightObs", True),   # tennis_im.yaml:17
@@ -441,7 +453,8 @@ class PhysicsMVAEController:
         native_v2p.task_reset(cfg, dict(
             reset_reaction=self._reset_reaction_buf, reset_recovery=self._reset_recovery_buf,
             pool_rand=torch.randint(0, P, (N,), device=dev), side_rand=torch.randint(-1000, 1000, (N,), device=dev),
-            frame_rand=torch.randint(-5, 5, (N,), device=dev), target_seed=seed, pool=t._ball_pool, ball_states=t._root_states[1:],
+            frame_rand=torch.randint(-5, 5, (N,), device=dev), target_seed=seed, pool=t._ball_pool, pool_cursor=t._ball_pool_cursor,
+            ball_states=t._root_states[1:],
             rigid_body_state=t._rigid_body_state, ball_pos=t._ball_pos, ball_vel=t._ball_vel, bounce_pos=t._bounce_pos,
             ball_traj=self._ball_traj, est_bounce_pos=self._est_bounce_pos, est_bounce_time=self._est_bounce_time,
             est_max_height=self._est_max_height, target_bounce_pos=self._target_bounce_pos, has_bounce=t._has_bounce,
