@@ -370,6 +370,43 @@ int b200env_im_record(const b200_im_record_t* d, void* stream);
 /* sizeof(b200_im_record_t) as the library was built; the binding refuses a library whose size differs from its own */
 int32_t b200env_im_record_desc_size(void);
 
+/* Per-motion meters of one test step (HumanoidSMPLIMVis.run_test with cfg.env.b200_motion_stats): the step's reward, its four
+ * sub-rewards (compute_humanoid_reward, embodied_pose/env/tasks/humanoid_smpl_im.py:919-955) and the body-position error, summed per
+ * game and folded, when the game ends, into the bucket of the env's motion.  Two launches in a fixed order, no float atomics, so a
+ * replay gives the same bits:
+ *   accumulate, one warp per env e: env_sums[e] += (rew, 1, sub_rewards[e, 0..3], err) in double, where err is the mean over the
+ *     num_lib_bodies bodies b of |rigid_body_state[e, b, 0:3] - target_rb_pos[e, b]| (metres, computed in double); then, with
+ *     done = reset_buf[e] != 0 (b200env_play_stats' rule), env_flags[e] = (done, ended), ended = done (1 - prev_done) ? 1 +
+ *     (terminate_buf[e] != 0) : 0;
+ *   fold, one CTA per motion m: over motion_envs[motion_start[m] .. motion_start[m + 1]), in that order, every env with ended != 0
+ *     adds (1, ended == 2) to counts[m] (games, falls) and env_sums[e] to sums[m], then its env_sums row and ended are zeroed.
+ * The caller zeroes env_sums and env_flags when a game starts, as b200env_play_stats' cr / steps / prev_dones.  games:
+ * b200_play_stats_t::games or NULL; while games[1] (stop) is set neither launch changes anything.  Each env must appear exactly once
+ * in motion_envs: the launch does not check the lists.  Returns -2 before any launch when n or num_motions is not positive or
+ * num_lib_bodies is not in [1, num_bodies]. */
+typedef struct b200_im_motion_stats {
+  int32_t n;                       /* envs */
+  int32_t num_motions;             /* M */
+  int32_t num_bodies;              /* bodies per env of rigid_body_state */
+  int32_t num_lib_bodies;          /* bodies compared: rows per env of target_rb_pos */
+  const float* rew;                /* [n] */
+  const float* sub_rewards;        /* [n, 4]: dof, vel, body_pos, body_rot */
+  const int64_t* reset_buf;        /* [n] */
+  const int64_t* terminate_buf;    /* [n]: 1 = the episode ended in a fall */
+  const float* rigid_body_state;   /* [n, num_bodies, 13] */
+  const float* target_rb_pos;      /* [n, num_lib_bodies, 3]: the targets the step's reward compared against (p_rb_pos) */
+  const int64_t* motion_start;     /* [M + 1] */
+  const int64_t* motion_envs;      /* [n]: the envs of each motion, grouped by motion, in env order within one */
+  double* env_sums;                /* [n, 7]: rew, steps, sub_rewards[4], err of the game so far */
+  int32_t* env_flags;              /* [n, 2]: prev_done, ended */
+  int64_t* counts;                 /* [M, 2]: games, falls */
+  double* sums;                    /* [M, 7]: the env_sums columns of the finished games */
+  const int64_t* games;            /* [3] or NULL */
+} b200_im_motion_stats_t;
+int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream);
+/* sizeof(b200_im_motion_stats_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_im_motion_stats_desc_size(void);
+
 /* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1): a separate test launch
  * (physics_kernel_packed; physics_kernel_tmem / physics_kernel for the other forms) that shares the control step
  * (control_step_packed) with b200env_step's physics launch, but not that launch's persistent hand-out of env batches,

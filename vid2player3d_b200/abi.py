@@ -322,6 +322,17 @@ class ImRecord(C.Structure):
     _nullable_, _defaults_ = ("games",), ("pad_",)
 
 
+class ImMotionStats(C.Structure):
+    """b200_im_motion_stats_t: the per-motion meters of one test step of HumanoidSMPLIMVis (b200env_im_motion_stats)"""
+    _fields_ = [
+        ("n", C.c_int32), ("num_motions", C.c_int32), ("num_bodies", C.c_int32), ("num_lib_bodies", C.c_int32),
+        ("rew", F32P), ("sub_rewards", F32P), ("reset_buf", I64P), ("terminate_buf", I64P), ("rigid_body_state", F32P),
+        ("target_rb_pos", F32P), ("motion_start", I64P), ("motion_envs", I64P), ("env_sums", F64P), ("env_flags", I32P),
+        ("counts", I64P), ("sums", F64P), ("games", I64P),
+    ]
+    _nullable_, _defaults_ = ("games",), ()
+
+
 # the context window's transform program (include/b200env.h: b200_motion_context_t), appended to b200_reset_masked_t and
 # b200_motion_context_t; zero = no transforms
 XF_MASK_JOINTS, XF_NOISY_JOINTS, XF_MASK_RANDOM_JOINTS = 1, 2, 3
@@ -652,6 +663,8 @@ SIGNATURES = {
     "b200env_play_stats": (C.c_int, [_p, _p]),
     "b200env_im_record": (C.c_int, [_p, _p]),
     "b200env_im_record_desc_size": (_i32, []),
+    "b200env_im_motion_stats": (C.c_int, [_p, _p]),
+    "b200env_im_motion_stats_desc_size": (_i32, []),
     "b200env_set_env_slice": (C.c_int, [_p, _i32, _i32]),
     "b200env_set_hull_faces": (C.c_int, [_p, _p, _p, _p, _i32]),
     "b200env_kernel_form": (_i32, [_p]),

@@ -2127,6 +2127,87 @@ __global__ void __launch_bounds__(REC_WARPS * 32) im_record_kernel(b200_im_recor
   }
 }
 
+// b200env_im_motion_stats: one warp per env accumulates the step; then one CTA per motion folds the games that ended, each thread a
+// contiguous run of the motion's env list and the runs meeting in a fixed tree, so every bucket has one writer and a fixed order
+#define MS_WARPS 8
+#define MS_FOLD_THREADS 256
+#define MS_COLS 7
+__global__ void __launch_bounds__(MS_WARPS * 32) im_motion_stats_acc_kernel(b200_im_motion_stats_t d) {
+  if (d.games && d.games[1]) return;
+  const int e = blockIdx.x * MS_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (e >= d.n) return;
+  double err = 0.0;
+  for (int b = lane; b < d.num_lib_bodies; b += 32) {
+    const float* p = d.rigid_body_state + ((int64_t)e * d.num_bodies + b) * 13;
+    const float* t = d.target_rb_pos + ((int64_t)e * d.num_lib_bodies + b) * 3;
+    const double x = (double)p[0] - t[0], y = (double)p[1] - t[1], z = (double)p[2] - t[2];
+    err += sqrt(x * x + y * y + z * z);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) err += __shfl_xor_sync(0xffffffffu, err, o);
+  if (lane == 0) {
+    double* s = d.env_sums + (int64_t)e * MS_COLS;
+    const float* sr = d.sub_rewards + (int64_t)e * 4;
+    s[0] += (double)d.rew[e];
+    s[1] += 1.0;
+#pragma unroll
+    for (int k = 0; k < 4; k++) s[2 + k] += (double)sr[k];
+    s[6] += err / d.num_lib_bodies;
+    int32_t* f = d.env_flags + 2 * (int64_t)e;
+    const int32_t done = d.reset_buf[e] != 0;
+    f[1] = (done && !f[0]) ? 1 + (d.terminate_buf[e] != 0) : 0;
+    f[0] = done;
+  }
+}
+
+__global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b200_im_motion_stats_t d) {
+  __shared__ double s_sum[MS_FOLD_THREADS / 32][MS_COLS];
+  __shared__ long long s_cnt[MS_FOLD_THREADS / 32][2];
+  if (d.games && d.games[1]) return;
+  const int m = blockIdx.x, tid = threadIdx.x;
+  const int64_t first = d.motion_start[m], last = d.motion_start[m + 1];
+  const int64_t run = (last - first + MS_FOLD_THREADS - 1) / MS_FOLD_THREADS;
+  const int64_t lo = first + tid * run, hi = min(lo + run, last);
+  double s[MS_COLS] = {};
+  long long games = 0, falls = 0;
+  for (int64_t i = lo; i < hi; i++) {
+    const int64_t e = d.motion_envs[i];
+    const int32_t ended = d.env_flags[2 * e + 1];
+    if (ended) {
+      games++;
+      falls += ended == 2;
+      double* es = d.env_sums + e * MS_COLS;
+#pragma unroll
+      for (int k = 0; k < MS_COLS; k++) { s[k] += es[k]; es[k] = 0.0; }
+      d.env_flags[2 * e + 1] = 0;
+    }
+  }
+  if (!__syncthreads_or(games != 0)) return;           // no game of this motion ended in this step
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int k = 0; k < MS_COLS; k++) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+    games += __shfl_xor_sync(0xffffffffu, games, o);
+    falls += __shfl_xor_sync(0xffffffffu, falls, o);
+  }
+  const int w = tid >> 5;
+  if ((tid & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < MS_COLS; k++) s_sum[w][k] = s[k];
+    s_cnt[w][0] = games; s_cnt[w][1] = falls;
+  }
+  __syncthreads();
+  if (tid < MS_COLS) {
+    double t = 0.0;
+    for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t += s_sum[j][tid];
+    d.sums[(int64_t)m * MS_COLS + tid] += t;
+  } else if (tid == 32 || tid == 33) {
+    long long t = 0;
+    for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t += s_cnt[j][tid - 32];
+    d.counts[2 * (int64_t)m + tid - 32] += t;
+  }
+}
+
 // physics-only entry used by the parity tests (float or double)
 template <typename T>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
@@ -3006,6 +3087,22 @@ int b200env_im_record(const b200_im_record_t* d, void* stream) {
 }
 
 int32_t b200env_im_record_desc_size(void) { return (int32_t)sizeof(b200_im_record_t); }
+
+int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream) {
+  if (!d || !d->rew || !d->sub_rewards || !d->reset_buf || !d->terminate_buf || !d->rigid_body_state || !d->target_rb_pos ||
+      !d->motion_start || !d->motion_envs || !d->env_sums || !d->env_flags || !d->counts || !d->sums)
+    return fail(-1, "b200env_im_motion_stats: null argument%s");
+  if (d->n <= 0 || d->num_motions <= 0) return fail(-2, "b200env_im_motion_stats: n and num_motions must be positive%s");
+  if (d->num_lib_bodies < 1 || d->num_lib_bodies > d->num_bodies)
+    return fail(-2, "b200env_im_motion_stats: num_lib_bodies must lie in [1, num_bodies]%s");
+  im_motion_stats_acc_kernel<<<(d->n + MS_WARPS - 1) / MS_WARPS, MS_WARPS * 32, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  im_motion_stats_fold_kernel<<<d->num_motions, MS_FOLD_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int32_t b200env_im_motion_stats_desc_size(void) { return (int32_t)sizeof(b200_im_motion_stats_t); }
 
 int b200env_physics_only(b200env_handle h, int32_t prec, int32_t n, int32_t n_steps, void* root, void* dof_pos, void* dof_vel,
                          const void* pd_tar, const void* ext_wrench, void* rb_out, void* contact_out, void* ball, int32_t* ball_hits,

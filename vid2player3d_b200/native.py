@@ -27,7 +27,8 @@ def lib():
         if L.b200env_abi_version() != abi.ABI_VERSION:
             raise RuntimeError("libb200env.so ABI version mismatch - rebuild")
         for S, size in ((abi.ResetMasked, L.b200env_reset_masked_desc_size()), (abi.MotionContext, L.b200env_motion_context_desc_size()),
-                        (abi.ImRecord, L.b200env_im_record_desc_size()), (abi.V2PTaskReset, L.b200v2p_task_reset_desc_size())):
+                        (abi.ImRecord, L.b200env_im_record_desc_size()), (abi.V2PTaskReset, L.b200v2p_task_reset_desc_size()),
+                        (abi.ImMotionStats, L.b200env_im_motion_stats_desc_size())):
             if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
                 raise RuntimeError(f"libb200env.so takes a {size}-byte {S.__name__} descriptor, the binding fills {C.sizeof(S)} - rebuild")
         _lib = L
@@ -113,6 +114,13 @@ def im_record(scalars, tensors):
     """one recorded viewer frame of HumanoidSMPLIMVis on the device (include/b200env.h: b200env_im_record); the fields of abi.ImRecord"""
     d = fill(abi.ImRecord, scalars, tensors)
     _check(lib().b200env_im_record(C.byref(d), _stream()))
+
+
+def im_motion_stats(scalars, tensors):
+    """the per-motion meters of one test step on the device (include/b200env.h: b200env_im_motion_stats); the fields of
+    abi.ImMotionStats"""
+    d = fill(abi.ImMotionStats, scalars, tensors)
+    _check(lib().b200env_im_motion_stats(C.byref(d), _stream()))
 
 
 def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):

@@ -25,6 +25,25 @@ def _sim_param(sim_params, name, default):
     return getattr(sim_params, name, default)
 
 
+def resolve_test_motion_file(cfg):
+    """humanoid_smpl_im.py:77-80: with args.test, cfg.env.test_motion_file replaces motion_file (and, with motion_assets, the test
+    library's own cfg.env.test_motion_assets replace them).  Returns the test file, or None when the key is absent or args.test unset.
+    A missing file, and motion_assets without test_motion_assets, are refused before anything is loaded."""
+    env, args = cfg["env"], cfg.get("args", None)
+    if args is None or not getattr(args, "test", False) or "test_motion_file" not in env:
+        return None
+    path = env["test_motion_file"]
+    if not os.path.exists(path):
+        raise FileNotFoundError(f"test_motion_file {path} does not exist")
+    if "motion_assets" in env:
+        if "test_motion_assets" not in env:
+            raise ValueError(f"motion_assets names one asset per motion of motion_file; test_motion_file {path} needs its own "
+                             "list in test_motion_assets")
+        env["motion_assets"] = env["test_motion_assets"]
+    env["motion_file"] = path
+    return path
+
+
 class HumanoidSMPLIM(BaseTask):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         self.cfg = cfg
@@ -48,6 +67,7 @@ class HumanoidSMPLIM(BaseTask):
         self._motion_sync_dt = control_freq_inv * self.sim_dt
         if self.args is not None and getattr(self.args, "test", False):
             env["stateInit"] = 'Start'
+        self._test_motion_file = resolve_test_motion_file(cfg)
         self._state_init = env.get("stateInit", "Hybrid")
         self._hybrid_init_prob = env.get("hybridInitProb", 1.0)
         self._pd_control = env.get("pdControl", True)
@@ -91,6 +111,10 @@ class HumanoidSMPLIM(BaseTask):
             flat = FlatMotionLib.from_reference(motion_file)
         else:
             raise TypeError(f"motion_lib / motion_file: expected a FlatMotionLib, a path or a reference MotionLib, got {type(motion_file)}")
+        env = self.cfg["env"]
+        if self._test_motion_file is not None and "motion_assets" in env and len(env["motion_assets"]) != flat.num_motions():
+            raise ValueError(f"test_motion_assets has {len(env['motion_assets'])} entries for the {flat.num_motions()} motions of "
+                             f"test_motion_file {self._test_motion_file}")
         self._motion_lib = flat
         dev = self.device
         self._ml_t = {k: torch.from_numpy(getattr(flat, k)).to(dev).contiguous() for k in FlatMotionLib.FIELDS}

@@ -22,7 +22,13 @@ qpos the reference's viewer would show (_sync_ref_motion: the simulated humanoid
 up), one frame per call, on the device (include/b200env.h: b200env_im_record).  After num_rec_frames frames (the longest motion's
 frame count with args.rec_once) the frames go to an .npz (rec_fname with its extension replaced, or out/recording/qpos_<date>.npz)
 and SystemExit is raised, as the reference's render_vis quits.  run_test puts the record launch in the step graph, between the env
-step and the bookkeeping; a record launch that writes the last frame sets the bookkeeping's stop flag."""
+step and the bookkeeping; a record launch that writes the last frame sets the bookkeeping's stop flag.
+
+Per-motion meters (cfg.env.b200_motion_stats, an addition): run_test also sums, per finished game, the reward, the steps, the four
+sub-rewards and the mean body-position error into the bucket of the env's motion, and counts games and falls per motion
+(include/b200env.h: b200env_im_motion_stats, in the step graph after the record launch and before the bookkeeping, so it stops with
+it).  When run_test ends (or the recorder quits) the buckets go to cfg.env.b200_motion_stats_file (default
+out/motion_stats/motion_stats_<date>.npz) and one summary line is printed."""
 import os
 from datetime import datetime
 
@@ -81,6 +87,33 @@ def assemble_qpos(rows):
     return torch.cat([rows[:, :, 0], rows[:, :, 1], c2], -1)
 
 
+def motion_stats_path(env, now=None):
+    """cfg.env.b200_motion_stats_file, or out/motion_stats/motion_stats_<date>.npz"""
+    if env.get("b200_motion_stats_file"):
+        return str(env["b200_motion_stats_file"])
+    now = now or datetime.now()
+    return os.path.join("out", "motion_stats", "motion_stats_%s.npz" % now.strftime('%Y-%m-%d-%H:%M:%S'))
+
+
+def motion_env_lists(motion_ids, num_motions):
+    """env -> motion map [N] -> (motion_start [M + 1], motion_envs [N]): the envs of motion m, in env order, are
+    motion_envs[motion_start[m]:motion_start[m + 1]]"""
+    ids = np.asarray(motion_ids.cpu() if torch.is_tensor(motion_ids) else motion_ids, np.int64)
+    start = np.zeros(num_motions + 1, np.int64)
+    start[1:] = np.cumsum(np.bincount(ids, minlength=num_motions))
+    return start, np.argsort(ids, kind="stable").astype(np.int64)
+
+
+def motion_stats_summary(counts, sums):
+    """the printed line of the per-motion buckets (counts [M, 2] games, falls; sums [M, 7] float64)"""
+    games, falls = counts[:, 0], counts[:, 1]
+    steps = sums[:, 1].sum()
+    ok = 1.0 - falls.sum() / games.sum() if games.sum() else float("nan")
+    per_step = (sums[:, 0].sum() / steps, sums[:, 6].sum() / steps) if steps else (float("nan"), float("nan"))
+    return (f"motions evaluated: {int((games > 0).sum())} of {len(games)}  games without a fall: {ok:.4f}  "
+            f"reward per step: {per_step[0]:.6f}  body position error: {per_step[1]:.6f} m")
+
+
 class HumanoidSMPLIMVis(HumanoidSMPLIM):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         if not headless:
@@ -98,6 +131,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self.cam_inited = False
         self.vis_mode = getattr(self.args, "vis_mode", None)
         self._im_policy = None
+        self._ms = None
         if rec_ids is not None:
             self._setup_record(rec_ids)
 
@@ -184,6 +218,37 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._stats_cap = cap
         self._n_games = 1 << 62            # run_test sets games_num * n_game_life
         self._im_graph = None
+        if self.cfg["env"].get("b200_motion_stats", False):
+            self._setup_motion_stats()
+
+    def _setup_motion_stats(self):
+        """the per-motion buckets and, from the env -> motion map the test run keeps, each motion's env list"""
+        N, M, dev = self.num_envs, self._motion_lib.num_motions(), self.device
+        start, envs = motion_env_lists(self._reset_ref_motion_ids, M)
+        self._ms = dict(motion_start=torch.from_numpy(start).to(dev), motion_envs=torch.from_numpy(envs).to(dev),
+                        env_sums=torch.zeros(N, 7, device=dev, dtype=torch.float64),
+                        env_flags=torch.zeros(N, 2, device=dev, dtype=torch.int32),
+                        counts=torch.zeros(M, 2, device=dev, dtype=torch.long), sums=torch.zeros(M, 7, device=dev, dtype=torch.float64))
+
+    def _motion_stats_launch(self, games=None):
+        native.im_motion_stats(dict(n=self.num_envs, num_motions=self._motion_lib.num_motions(), num_bodies=self.num_bodies,
+                                    num_lib_bodies=self._num_lib_bodies),
+                               dict(self._ms, rew=self.rew_buf, sub_rewards=self._sub_rewards, reset_buf=self.reset_buf,
+                                    terminate_buf=self._terminate_buf, rigid_body_state=self._rigid_body_state,
+                                    target_rb_pos=self._prev_target_rb_pos, games=games))
+
+    def export_motion_stats(self):
+        """writes the per-motion buckets to b200_motion_stats_file and prints the summary line; returns the file's path"""
+        counts, sums = self._ms["counts"].cpu().numpy(), self._ms["sums"].cpu().numpy()
+        path = motion_stats_path(self.cfg["env"])
+        if os.path.dirname(path):
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+        np.savez(path, games=counts[:, 0], falls=counts[:, 1], reward_sum=sums[:, 0], steps=sums[:, 1].astype(np.int64),
+                 sub_reward_sum=sums[:, 2:6], body_pos_err_sum=sums[:, 6], env_motion_ids=self._reset_ref_motion_ids.cpu().numpy(),
+                 test_motion_file=np.array(self._test_motion_file or ""))
+        print(motion_stats_summary(counts, sums))
+        print(f"============ per-motion statistics written to {path} ============")
+        return path
 
     def policy_rows(self):
         """the operand launch: policy.x and the residual from obs_buf and the context slot context_padding + step % context_length"""
@@ -206,6 +271,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._env.step(actions)
         if self._rec is not None:
             self._record_launch(False, games=self._stats["games"])
+        if self._ms is not None:
+            self._motion_stats_launch(games=self._stats["games"])
         native.play_stats(dict(n=self.num_envs, max_log=self._stats_cap, n_games=self._n_games),
                           dict(self._stats, rew=self.rew_buf, reset_buf=self.reset_buf))
 
@@ -226,6 +293,13 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                 self._test_launches()
             self._im_graph = g
 
+    def _quit_recording(self):
+        """render_vis' quit() inside run_test: the frames, the per-motion statistics of the games finished so far, SystemExit"""
+        self.export_recording()
+        if self._ms is not None:
+            self.export_motion_stats()
+        raise SystemExit
+
     def run_test(self, policy, games_num, max_steps, n_game_life=1, print_stats=True, sync_every=None, clip_obs=float("inf"),
                  clip_actions=None, graph=True, history=None):
         """ImitatorPlayer.run (im_player.py:193-312) with the deterministic mu, or the sampled action when `policy` has a sigma: per game a full reset(), then up to max_steps
@@ -245,11 +319,13 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             for k in ("cr", "steps", "prev_dones", "step"):
                 st[k].zero_()
             st["games"][1:].zero_()            # stop flag and log rows; games_played and the totals run on
+            if self._ms is not None:           # the games of the last run are folded; the buckets run on
+                self._ms["env_sums"].zero_()
+                self._ms["env_flags"].zero_()
             if self._rec is not None:          # render_vis(init=True): the host reads the frame counter once per game
                 self._record_launch(True, games=st["games"])
                 if int(self._rec["frame"]) >= self._rec_cap:
-                    self.export_recording()
-                    raise SystemExit
+                    self._quit_recording()
             game = [] if history is not None else None
             for n in range(max_steps):
                 self.test_step(n, graph)
@@ -263,8 +339,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                         for count, r, s in rows:
                             print('reward:', r / count, 'steps:', s / count)
                     if self._rec is not None and int(self._rec["frame"]) >= self._rec_cap:    # render_vis' quit()
-                        self.export_recording()
-                        raise SystemExit
+                        self._quit_recording()
                     if games[1]:
                         break
             if history is not None:
@@ -275,4 +350,6 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         print('av reward:', sum_rewards / games_played * n_game_life, 'av steps:', sum_steps / games_played * n_game_life)
         if self._rec is not None:              # the games ended before the recorder filled: the frames so far
             self.export_recording()
+        if self._ms is not None:
+            self.export_motion_stats()
         return dict(sum_rewards=sum_rewards, sum_steps=sum_steps, games_played=games_played)
