@@ -240,6 +240,41 @@ int b200v2p_task_reset(const b200v2p_treset_t* r, void* stream);
 /* sizeof(b200v2p_treset_t) of the library, so that a binding refuses a library built before pool_cursor */
 int32_t b200v2p_task_reset_desc_size(void);
 
+/* Per-row results of the fixed test set (MVAEControllerVis with cfg.env.b200_ball_stats).  No reference counterpart: the reference's
+ * _compute_stats (env/tasks/mvae_controller_vis.py:80-93) keeps per-env meters only.  Every flagged env adds to the bucket of the pool
+ * row r = (pool_cursor[e] + pool_size - 1) % pool_size, one behind its cursor: the cursor moves by one (mod pool_size) at each draw
+ * only, so r is the row of the env's last draw.  One launch, in one of two forms (exactly one of reset_reaction / reset_recovery):
+ *   draws   (reset_reaction, row_served), right after b200v2p_task_reset with pool_cursor: each env that just drew (reset_reaction set)
+ *           adds 1 to row_served[r], the row it took;
+ *   events  (reset_recovery and the fields after it), right after the eval post launch (b200v2p_controller_post with eval set),
+ *           before the next task reset: each recovery event (the events at which the meters update) adds (1, has_contact,
+ *           swing_type_cycle == 1, est_bounce_in, est_bounce_in ? q(|est_bounce_pos - target_bounce_pos|) : 0) to buckets[r], the
+ *           distance in float32 as meter 3 takes it.  A recovery needs tar_action 1, which only a reaction reset (a draw) sets, so r
+ *           is the row of the ball the env plays.
+ * Lanes of a warp that share a row are folded with __match_any_sync, and each row's leader adds the warp's totals with integer
+ * atomics, so the counts are the same bits on every run whatever the order.  q(v) = rint(v * 2^24): fixed point in units of 2^-24 m,
+ * exact for v >= 0.5 m (a float there has no bits below 2^-24), off by at most 2^-25 m below; a bounce-in error lies inside the court
+ * and target box (under 64 m = 2^30 units), so a row holds 2^33 events before the int64 can overflow.  The caller divides column 4 by
+ * 2^24 to get metres.  pool_cursor must lie in [0, pool_size), as the task reset leaves it. */
+#define B200V2P_BSTATS_COLS 5                 /* recoveries, hits, forehands, bounce_in, bounce-in error in 2^-24 m */
+#define B200V2P_BSTATS_FIX_SCALE 16777216.0   /* 2^24 */
+typedef struct b200v2p_bstats {
+  int32_t n, pool_size;
+  const int64_t* pool_cursor;        /* [n] */
+  const uint8_t* reset_reaction;     /* [n]: draws form, else NULL */
+  int64_t* row_served;               /* [pool_size]: draws form, else NULL */
+  const uint8_t* reset_recovery;     /* [n]: events form, else NULL; the events form needs every field below */
+  const uint8_t* has_contact;        /* [n] */
+  const int64_t* swing_type_cycle;   /* [n] */
+  const uint8_t* est_bounce_in;      /* [n] */
+  const float* est_bounce_pos;       /* [n, 3] */
+  const float* target_bounce_pos;    /* [n, 3] */
+  int64_t* buckets;                  /* [pool_size, B200V2P_BSTATS_COLS] */
+} b200v2p_bstats_t;
+int b200v2p_eval_ball_stats(const b200v2p_bstats_t* d, void* stream);
+/* sizeof(b200v2p_bstats_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200v2p_eval_ball_stats_desc_size(void);
+
 /* replaces HumanoidSMPLIMMVAE._reset_actors + _set_env_state + _reset_env_tensors for an id list
  * (env/tasks/humanoid_smpl_im_mvae.py:463-501, 562-581): the FK of the motion generator's pose (b200v2p_smpl_to_sim over all
  * envs, prev = NULL) is scattered into the simulation state of the listed envs; velocities zero. */

@@ -568,6 +568,23 @@ class V2PTaskReset(C.Structure):
     _nullable_, _defaults_ = ("ball_obs", "pool_cursor"), ("obs_traj_len", "pad_")
 
 
+BSTATS_COLS = 5                   # B200V2P_BSTATS_COLS: recoveries, hits, forehands, bounce_in, bounce-in error in 2^-24 m
+BSTATS_FIX_SCALE = float(1 << 24)  # B200V2P_BSTATS_FIX_SCALE
+
+
+class V2PBallStats(C.Structure):
+    """b200v2p_bstats_t: the per-row results of the fixed test set (b200v2p_eval_ball_stats), in its draws form (reset_reaction,
+    row_served) or its events form (reset_recovery and the fields after it); the entry point refuses a form with a field missing"""
+    _fields_ = [
+        ("n", C.c_int32), ("pool_size", C.c_int32), ("pool_cursor", I64P), ("reset_reaction", U8P), ("row_served", I64P),
+        ("reset_recovery", U8P), ("has_contact", U8P), ("swing_type_cycle", I64P), ("est_bounce_in", U8P), ("est_bounce_pos", F32P),
+        ("target_bounce_pos", F32P), ("buckets", I64P),
+    ]
+    _nullable_ = ("reset_reaction", "row_served", "reset_recovery", "has_contact", "swing_type_cycle", "est_bounce_in", "est_bounce_pos",
+                  "target_bounce_pos", "buckets")
+    _defaults_ = ()
+
+
 class V2PActorReset(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("num_dof", C.c_int32), ("bodies_per_env", C.c_int32), ("root_stride", C.c_int32),
@@ -691,6 +708,8 @@ SIGNATURES = {
     "b200v2p_ball_in_estimate": (C.c_int, [_p, _p]),
     "b200v2p_task_reset": (C.c_int, [_p, _p]),
     "b200v2p_task_reset_desc_size": (_i32, []),
+    "b200v2p_eval_ball_stats": (C.c_int, [_p, _p]),
+    "b200v2p_eval_ball_stats_desc_size": (_i32, []),
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
     "b200v2p_eval_record": (C.c_int, [_p, _p]),
     "b200v2p_eval_best": (C.c_int, [_p, _p]),

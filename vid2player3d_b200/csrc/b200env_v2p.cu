@@ -607,6 +607,61 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
   if (lane == 0 && c.obs_only && touched) { c.reset_reaction[e] = 0; c.reset_recovery[e] = 0; }   // tail of _reset_envs (:176-177) for the reset humanoids
 }
 
+// ------------------------------------------------------------------------------------------ per-row results of the test set
+// b200v2p_eval_ball_stats: one thread per env.  The flagged lanes of a warp are grouped by row (__match_any_sync); a group's counts are
+// popcounts of its ballots, its error the sum of its bounce-in lanes' fixed-point values; the group's lowest lane adds them.
+// kDraws: the draws form (reset_reaction -> row_served), else the events form (reset_recovery -> buckets)
+#define BSTATS_THREADS 256
+template <bool kDraws>
+__global__ void __launch_bounds__(BSTATS_THREADS) eval_ball_stats_kernel(b200v2p_bstats_t d) {
+  const int lane = threadIdx.x & 31;
+  const int64_t e = (int64_t)blockIdx.x * BSTATS_THREADS + threadIdx.x;
+  const bool ev = e < d.n && (kDraws ? d.reset_reaction[e] : d.reset_recovery[e]) != 0;
+  const unsigned evs = __ballot_sync(FULL, ev);
+  if (evs == 0) return;                       // warp-uniform
+  int64_t row = 0;
+  unsigned peers = 0;
+  if (ev) {
+    row = (d.pool_cursor[e] + d.pool_size - 1) % d.pool_size;
+    peers = __match_any_sync(evs, (unsigned long long)row);
+  }
+  if constexpr (kDraws) {
+    if (ev && lane == __ffs(peers) - 1)
+      atomicAdd(reinterpret_cast<unsigned long long*>(d.row_served + row), (unsigned long long)__popc(peers));
+    return;
+  }
+  bool hit = false, fh = false, bin = false;
+  long long q = 0;
+  if (ev) {
+    hit = d.has_contact[e] != 0;
+    fh = d.swing_type_cycle[e] == 1;
+    bin = d.est_bounce_in[e] != 0;
+    if (bin) {   // meter 3's value (eval_reset), then fixed point: v * 2^24 is exact in double, one rounding to the integer
+      float dd[3];
+#pragma unroll
+      for (int k = 0; k < 3; k++) dd[k] = __fsub_rn(d.est_bounce_pos[e * 3 + k], d.target_bounce_pos[e * 3 + k]);
+      const float v = sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(dd[0], dd[0]), __fmul_rn(dd[1], dd[1])), __fmul_rn(dd[2], dd[2])));
+      q = __double2ll_rn((double)v * B200V2P_BSTATS_FIX_SCALE);
+    }
+  }
+  const unsigned hits = __ballot_sync(FULL, hit), fhs = __ballot_sync(FULL, fh), bins = __ballot_sync(FULL, bin);
+  long long err = 0;
+  for (unsigned m = bins; m; m &= m - 1) {    // warp-uniform: every lane takes part in each shuffle
+    const int src = __ffs(m) - 1;
+    const long long t = __shfl_sync(FULL, q, src);
+    if ((peers >> src) & 1u) err += t;
+  }
+  if (!ev || lane != __ffs(peers) - 1) return;
+  unsigned long long* b = reinterpret_cast<unsigned long long*>(d.buckets + row * B200V2P_BSTATS_COLS);
+  atomicAdd(b, (unsigned long long)__popc(peers));
+  const unsigned long long c[3] = {(unsigned long long)__popc(peers & hits), (unsigned long long)__popc(peers & fhs),
+                                   (unsigned long long)__popc(peers & bins)};
+#pragma unroll
+  for (int k = 0; k < 3; k++)
+    if (c[k]) atomicAdd(b + 1 + k, c[k]);
+  if (err) atomicAdd(b + 4, (unsigned long long)err);
+}
+
 // ------------------------------------------------------------------------------------------ test-time rally recorder
 // render_vis's per-frame append (mvae_controller_vis.py:140-146, mvae_controller_vis_dual.py:156-162): one warp per env writes the
 // env's frame at row *row_counter (single; the last block advances the counter) or progress_buf[e] (dual); rows >= cap are dropped
@@ -1348,6 +1403,27 @@ int b200v2p_task_reset(const b200v2p_treset_t* r, void* stream) {
 }
 
 int32_t b200v2p_task_reset_desc_size(void) { return (int32_t)sizeof(b200v2p_treset_t); }
+
+int b200v2p_eval_ball_stats(const b200v2p_bstats_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_eval_ball_stats: null");
+  if (d->n == 0) return 0;
+  if (d->n < 0 || d->pool_size < 1 || !d->pool_cursor) return vfail(-1, "b200v2p_eval_ball_stats: bad arguments");
+  const bool draws = d->reset_reaction != nullptr;
+  if (draws == (d->reset_recovery != nullptr))
+    return vfail(-1, "b200v2p_eval_ball_stats: give reset_reaction (draws) or reset_recovery (events), not both or neither");
+  if (draws ? !d->row_served
+            : (!d->has_contact || !d->swing_type_cycle || !d->est_bounce_in || !d->est_bounce_pos || !d->target_bounce_pos || !d->buckets))
+    return vfail(-1, "b200v2p_eval_ball_stats: bad arguments");
+  const unsigned grid = (d->n + BSTATS_THREADS - 1) / BSTATS_THREADS;
+  if (draws)
+    eval_ball_stats_kernel<true><<<grid, BSTATS_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  else
+    eval_ball_stats_kernel<false><<<grid, BSTATS_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  V_CUDA_OK();
+  return 0;
+}
+
+int32_t b200v2p_eval_ball_stats_desc_size(void) { return (int32_t)sizeof(b200v2p_bstats_t); }
 
 int b200v2p_ctrl_reset(const b200v2p_creset_t* d, void* stream) {
   if (!d) return vfail(-1, "b200v2p_ctrl_reset: bad arguments");

@@ -97,6 +97,13 @@ def task_reset(cfg, t):
     _check(lib().b200v2p_task_reset(C.byref(fill(abi.V2PTaskReset, cfg, t)), _stream()))
 
 
+def eval_ball_stats(cfg, t):
+    """cfg: n, pool_size; t: pool_cursor and either the draws form - the task reset's reset_reaction, row_served (int64 [pool_size]) -
+    or the events form - the post launch's reset_recovery / has_contact / swing_type_cycle / est_bounce_in / est_bounce_pos /
+    target_bounce_pos and buckets (int64 [pool_size, abi.BSTATS_COLS]); see include/b200env_v2p.h b200v2p_bstats_t"""
+    _check(lib().b200v2p_eval_ball_stats(C.byref(fill(abi.V2PBallStats, cfg, t)), _stream()))
+
+
 def actor_reset(cfg, t):
     """cfg: scalars of abi.V2PActorReset; racket_offset2 (with racket_parent2, default racket_parent) sets dual"""
     two = cfg.get("racket_offset2") is not None

@@ -260,6 +260,7 @@ class HumanoidSMPLIMMVAE(BaseTask):
             self._ball_pool = torch.tensor(pool, device=dev).contiguous()
         # the test set's per-env cursor (sample_idx, :433): only the ball resets move it, so it carries over humanoid resets
         self._ball_pool_cursor = torch.zeros(N, device=dev, dtype=torch.long) if sequential else None
+        self._ball_row_served = None    # int64 [P] set by MVAEControllerVis (b200_ball_stats): every draw counts its row
         self._ball_traj_buf = f(N, 100, 3)
         self.extras["terminate"] = self._terminate_buf
 
@@ -390,6 +391,8 @@ class HumanoidSMPLIMMVAE(BaseTask):
         if self._ball_pool_cursor is not None:
             idx = self._ball_pool_cursor[env_ids]
             self._ball_pool_cursor[env_ids] = (idx + 1) % P
+            if self._ball_row_served is not None:
+                self._ball_row_served.index_add_(0, idx, torch.ones_like(idx))
         else:
             idx = torch.randint(0, P, (len(env_ids),), device=self.device)
             other = self._ball_pos[env_ids, 1] > 0

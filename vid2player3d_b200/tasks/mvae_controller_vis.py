@@ -6,6 +6,10 @@
                          num_rec_frames calls the chosen episodes are written as .npz files and SystemExit is raised like the
                          reference's exit()
   MVAEControllerVisDual  the best-episode list of finished rallies (:164-195), kept on the device (two launches per call)
+  MVAEControllerVis      with cfg.env.b200_ball_stats on a fixed test set (an addition): per pool row, the balls served and the
+                         recovery events with their hits, forehands, bounces in and bounce-in error, counted on the device inside
+                         the test loop's reset and step graphs and written by export_ball_stats when run_test ends or the
+                         recorder quits
 
 The renderer (SMPL meshes, video, HTML) is not part of this package: the .npz files hold exactly the arrays the reference's
 render_one_result is given, so they can be rendered with its visualizer.  Deliberate departures from the reference:
@@ -28,12 +32,13 @@ grows only when a candidate beats its current last entry, even while it holds fe
 import math
 import os
 import warnings
+from datetime import datetime
 
 import numpy as np
 import torch
 
-from .. import native_v2p
-from .physics_mvae_controller import PhysicsMVAEController, PhysicsMVAEControllerDual
+from .. import abi, native_v2p
+from .physics_mvae_controller import PhysicsMVAEController, PhysicsMVAEControllerDual, resolve_test_set
 
 METERS = ("hit_rate", "fh_ratio", "bounce_in_rate", "bounce_in_pos_error")   # rows of the meter arrays the post launch updates
 DUAL_CAPACITY = 1800                                                            # mvae_controller_vis_dual.py:51 "hardcode maximum length"
@@ -65,6 +70,40 @@ def _check_eval_cfg(cfg, headless):
     env["is_train"] = False          # utils/config.py:159 (--test); also makes the physics task export _joint_rot
 
 
+def _check_ball_stats_cfg(cfg, dual):
+    """b200_ball_stats counts results per row of a fixed test set, which only the single-player task walks in order: refuse it in
+    dual mode (no pool is built) and on random draws (test_mode random, the default without ball_traj_file_test: a drawn row keeps no
+    identity), before anything is allocated.  The test-time tasks never train (_check_eval_cfg), so the pool is the test set exactly
+    when resolve_ball_pool would take it."""
+    env = cfg["env"]
+    if not env.get("b200_ball_stats", False):
+        return
+    v2p = dict(env.get("vid2player", {}))
+    if dual or v2p.get("dual_mode"):
+        raise ValueError("b200_ball_stats: dual mode builds no ball pool, so there are no test-set rows to count results by")
+    resolve_test_set(env, v2p)          # on a copy: create_sim applies it to the task's own block
+    if v2p.get("test_mode", "random") == "random":
+        raise ValueError("b200_ball_stats needs a fixed test set (env.ball_traj_file_test, or vid2player.test_mode single_cycle / "
+                         "multiple_cycle with ball_pool_test): random draws keep no row identity")
+
+
+def ball_stats_path(env, now=None):
+    """cfg.env.b200_ball_stats_file, or out/ball_stats/ball_stats_<date>.npz"""
+    if env.get("b200_ball_stats_file"):
+        return str(env["b200_ball_stats_file"])
+    now = now or datetime.now()
+    return os.path.join("out", "ball_stats", "ball_stats_%s.npz" % now.strftime('%Y-%m-%d-%H:%M:%S'))
+
+
+def ball_stats_summary(a):
+    """the printed line of the per-row arrays of export_ball_stats: totals, the hit and bounce-in rates over the recovery events (as
+    the hit_rate and bounce_in_rate meters take them) and the rows no env ever hit"""
+    rec = int(a["recoveries"].sum())
+    rate = lambda k: int(a[k].sum()) / rec if rec else float("nan")  # noqa: E731
+    return (f"balls served: {int(a['served'].sum())}  recoveries: {rec}  hit rate: {rate('hits'):.4f}  "
+            f"bounce-in rate: {rate('bounce_in'):.4f}  rows never hit: {int((a['hits'] == 0).sum())} of {len(a['hits'])}")
+
+
 class _EvalRecorder:
     """host side shared by both tasks: frame counting, episode paths and the .npz export"""
 
@@ -80,6 +119,8 @@ class _EvalRecorder:
         self.exported = []
         self._fix_backhand = bool(self.cfg_v2p.get("fix_two_hand_backhand_post"))
         self.backhand_losses = {}
+        self._bstats = None              # per-row buckets of b200_ball_stats (MVAEControllerVis)
+        self._test_steps = 0
 
     def _episode_path(self, eg_id):
         return self._rec_fname or os.path.join("out", "episodes", f"{self._cfg_name}_{eg_id:03d}.npz")
@@ -116,6 +157,8 @@ class _EvalRecorder:
         self.frame_index += 1
         if self._record and self.frame_index >= self._num_rec_frames:
             self.export_episodes()
+            if self._bstats is not None:
+                self.export_ball_stats()
             raise SystemExit(0)
 
     # ------------------------------------------------------------------ test loop of V2PPlayer.run (players/v2p_player.py:133-156)
@@ -135,12 +178,16 @@ class _EvalRecorder:
         """V2PPlayer.run with the policy's action (deterministic mu, or sampled for an nn.V2PPolicy built with deterministic=False: the
         noise is drawn inside the policy's last layer, so the graphs replay it afresh): reset, render_vis(init=True), then `max_steps`
         test_step() calls.  Ends like
-        the reference, with SystemExit once num_rec_frames frames are recorded (with record)."""
+        the reference, with SystemExit once num_rec_frames frames are recorded (with record).  With b200_ball_stats the per-row
+        buckets are written when the run returns, or before that SystemExit; they count from the task's construction, so the first
+        reset's draws are in them whether it ran here or before."""
         self.set_policy(policy)
         self.reset()
         self.render_vis(init=True)
         for _ in range(max_steps):
             self.test_step(graph)
+        if self._bstats is not None:
+            self.export_ball_stats()
 
     def test_step(self, graph=True):
         """one iteration of V2PPlayer.run's loop: reset of the finished envs (mask-driven, from reset_buf), policy, env step,
@@ -160,6 +207,7 @@ class _EvalRecorder:
                 with torch.cuda.graph(sg, pool=rg.pool()):
                     self._test_launches()
                 self._test_graphs = (rg, sg)
+        self._test_steps += 1
         self._render_host()
 
     def _test_reset(self):
@@ -172,6 +220,8 @@ class _EvalRecorder:
         self.pre_physics_step(actions)
         self.physics_step()
         self.post_physics_step()
+        if self._bstats is not None:
+            self._ball_stats_launch()
         self._record_frame()
 
     def _rec_buffers(self, n, cap, fields):
@@ -184,6 +234,7 @@ class _EvalRecorder:
 class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         _check_eval_cfg(cfg, headless)
+        _check_ball_stats_cfg(cfg, dual=False)
         super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
                          headless=headless)
         self._init_eval(cfg)
@@ -201,6 +252,12 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
                                           ("joint_rot", "root_pos", "ball_pos", "target_pos", "phase", "swing_type"))
             self._rec_row = torch.zeros(1, device=dev, dtype=torch.long)
             self._rec_done = torch.zeros(1, device=dev, dtype=torch.int32)
+        if cfg["env"].get("b200_ball_stats", False):
+            task = self._physics_player.task
+            P = int(task._ball_pool.shape[0])
+            self._bstats = dict(served=torch.zeros(P, device=dev, dtype=torch.long),
+                                buckets=torch.zeros(P, abi.BSTATS_COLS, device=dev, dtype=torch.long))
+            task._ball_row_served = self._bstats["served"]      # both reset paths count their draws into it
 
     def _tensors(self):
         t = super()._tensors()
@@ -217,6 +274,30 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
             row_counter=self._rec_row, done_counter=self._rec_done, joint_rot=t._joint_rot, root_pos=t._root_pos, ball_pos=t._ball_pos,
             target_pos=self._target_bounce_pos, phase=p._phase_pred, swing_type=p._swing_type_cycle,
             **{"rec_" + k: v for k, v in self._rec.items()}))
+
+    def _ball_stats_launch(self):
+        """right after the post launch: every recovery event into the bucket of the row its env plays (b200v2p_eval_ball_stats)"""
+        t = self._physics_player.task
+        native_v2p.eval_ball_stats(dict(n=self.num_envs, pool_size=int(t._ball_pool.shape[0])), dict(
+            pool_cursor=t._ball_pool_cursor, reset_recovery=self._reset_recovery_buf, has_contact=t._has_racket_ball_contact,
+            swing_type_cycle=self._mvae_player._swing_type_cycle.contiguous(), est_bounce_in=self._est_bounce_in,
+            est_bounce_pos=self._est_bounce_pos, target_bounce_pos=self._target_bounce_pos, buckets=self._bstats["buckets"]))
+
+    def export_ball_stats(self):
+        """writes the per-row results of the test set to b200_ball_stats_file and prints the summary line; returns the file's path.
+        served, recoveries, hits, forehands, bounce_in: int64 [P]; bounce_err_sum: float64 [P], metres (the fixed-point sums over
+        2^24); ball_traj_file_test ('' for an in-memory ball_pool_test), num_envs, test_steps."""
+        b = self._bstats["buckets"].cpu().numpy()
+        a = dict(served=self._bstats["served"].cpu().numpy(), recoveries=b[:, 0].copy(), hits=b[:, 1].copy(), forehands=b[:, 2].copy(),
+                 bounce_in=b[:, 3].copy(), bounce_err_sum=b[:, 4] / abi.BSTATS_FIX_SCALE)
+        path = ball_stats_path(self.cfg["env"])
+        if os.path.dirname(path):
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+        np.savez(path, **a, ball_traj_file_test=np.array(str(self.cfg_v2p.get("ball_traj_file_test") or "")),
+                 num_envs=np.int64(self.num_envs), test_steps=np.int64(self._test_steps))
+        print(ball_stats_summary(a))
+        print(f"============ per-ball statistics written to {path} ============")
+        return path
 
     def select_candidates(self):
         """:152-159: with select_best the envs with bounce_in_rate.avg > 0.95 and fh_ratio.avg < 0.6, by distance travelled over the
@@ -250,6 +331,7 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
 class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless, capacity=DUAL_CAPACITY):
         _check_eval_cfg(cfg, headless)
+        _check_ball_stats_cfg(cfg, dual=True)
         super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
                          headless=headless)
         self._init_eval(cfg)

@@ -461,6 +461,9 @@ class PhysicsMVAEController:
             has_contact=t._has_racket_ball_contact, bounce_in=self._bounce_in, est_bounce_in=self._est_bounce_in, tar_time=self._tar_time,
             tar_time_total=self._tar_time_total, tar_action=self._tar_action, num_reset_reaction=self._num_reset_reaction,
             swing_type_cycle=self._mvae_player._swing_type_cycle, ball_obs=self._ball_obs if self._use_history else None))
+        if t._ball_row_served is not None:      # b200_ball_stats: the rows just drawn, one behind the moved cursors
+            native_v2p.eval_ball_stats(dict(n=N, pool_size=P), dict(pool_cursor=t._ball_pool_cursor, reset_reaction=self._reset_reaction_buf,
+                                                                    row_served=t._ball_row_served))
         if update_state:
             self._physics_player.task._update_state_from_sim(only_mask=humanoid_mask)   # :186-187 "setting the right fields to compute obs"
         post = dict(self._post_cfg)
