@@ -275,6 +275,51 @@ int b200v2p_eval_ball_stats(const b200v2p_bstats_t* d, void* stream);
 /* sizeof(b200v2p_bstats_t) as the library was built; the binding refuses a library whose size differs from its own */
 int32_t b200v2p_eval_ball_stats_desc_size(void);
 
+/* Rally results of the dual test run (MVAEControllerVisDual with cfg.env.b200_rally_stats).  No reference counterpart: the reference's
+ * MVAEControllerVisDual keeps no meters (env/tasks/mvae_controller_vis_dual.py:164-195 only sums _distance to choose what to render).
+ * Launched right after each full dual post launch (b200v2p_controller_post with dual, advance, not obs_only), one thread per pair k of
+ * the envs a = 2k (player 0) and b = 2k + 1 (player 1).  For player w on env i it takes the terms of the dual reset rule
+ * (physics_mvae_controller_dual.py:92-120) as the post launch computes them (a copy of its lines, which keeps the post kernel's SASS):
+ *   ta1, ta0 = tar_action[i] is 1 (to hit) / 0 (recovering); hc = has_contact[i]; hb = has_bounce[i]; bin = bounce_in[i] (as the post
+ *   launch has just updated it); behind = ball_y < root_y - 1; twice = hb && ball_z < 0.05;
+ *   rec[w] = ta1 && (hc || behind || twice)   the player meets a ball;
+ *   out[w] = ta0 && hb && !bin                 a ball the player hit bounced out.
+ * Counting, while the pair is open:
+ *   faced[w] += rec[w]; a rec is a hit when hc (a forehand when also swing_type_cycle[i] == 1), else a miss, caused by double_bounce
+ *   when twice, else behind.  The rally ends at the step where any player misses or has out, which is when the FSM sets reset_buf on the
+ *   pair: rallies += 1, ends[w][cause] += 1 for each player that caused it (causes behind, double_bounce, out; both players can count at
+ *   the same step), then this step's hits are added, the rally's hit total h (both players) goes to shots_hist[min(h, 64)] and
+ *   shots_sum, progress_buf[a] to frames_sum, and the pair closes.
+ *   A pair opens at the first post launch after its humanoids were reset (progress_buf[a] == 1), which zeroes its running hits
+ *   pair_hits[k]; events count only while it is open, so a host loop that steps a finished pair without resetting it counts its
+ *   ending once, and every reset path (masked, id list, the first reset) opens the rally without a hook of its own.  The serve is no
+ *   hit: a served ball that bounces out ends the rally as the server's out with 0 shots, as the FSM does.
+ * Invariants: faced[w] == hits[w] + misses[w]; hits[0] + hits[1] == shots_sum + the open pairs' running hits while pairs are reset
+ * only after their rally ended (as the test loop resets them, from reset_buf); sum(shots_hist) == rallies.  Per-warp aggregation (ballots and popcounts, __match_any_sync on the histogram bucket) and integer atomics only, so
+ * every run gives the same bits whatever the order.  n must be even; every pointer is required. */
+#define B200V2P_RSTATS_HIST 65      /* shots per rally 0..63, then 64 = 64 or more */
+#define B200V2P_RSTATS_CAUSES 3     /* behind, double_bounce, out */
+typedef struct b200v2p_rstats {
+  int32_t n, pad_;
+  const int64_t* tar_action;         /* [n] */
+  const uint8_t* has_contact;        /* [n] */
+  const uint8_t* has_bounce;         /* [n] */
+  const uint8_t* bounce_in;          /* [n] */
+  const float* ball_pos;             /* [n, 3] */
+  const float* root_pos;             /* [n, 3] */
+  const int64_t* swing_type_cycle;   /* [n] */
+  const int64_t* progress_buf;       /* [n] */
+  uint8_t* pair_open;                /* [n/2] state: the pair is in a rally */
+  int64_t* pair_hits;                /* [n/2, 2] state: the hits of each player in the pair's current (or last) rally */
+  int64_t* totals;                   /* [3] rallies, shots_sum, frames_sum */
+  int64_t* ends;                     /* [2, B200V2P_RSTATS_CAUSES] rallies ended by each player, by cause */
+  int64_t* player;                   /* [2, 3] faced, hits, forehands */
+  int64_t* shots_hist;               /* [B200V2P_RSTATS_HIST] */
+} b200v2p_rstats_t;
+int b200v2p_eval_rally_stats(const b200v2p_rstats_t* d, void* stream);
+/* sizeof(b200v2p_rstats_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200v2p_eval_rally_stats_desc_size(void);
+
 /* replaces HumanoidSMPLIMMVAE._reset_actors + _set_env_state + _reset_env_tensors for an id list
  * (env/tasks/humanoid_smpl_im_mvae.py:463-501, 562-581): the FK of the motion generator's pose (b200v2p_smpl_to_sim over all
  * envs, prev = NULL) is scattered into the simulation state of the listed envs; velocities zero. */

@@ -585,6 +585,23 @@ class V2PBallStats(C.Structure):
     _defaults_ = ()
 
 
+RSTATS_HIST = 65                  # B200V2P_RSTATS_HIST: shots per rally 0..63, then 64 or more
+RSTATS_CAUSES = ("behind", "double_bounce", "out")   # B200V2P_RSTATS_CAUSES, in the order of the ends columns
+RSTATS_PLAYER = ("faced", "hits", "forehands")       # columns of the player counts
+
+
+class V2PRallyStats(C.Structure):
+    """b200v2p_rstats_t: the rally results of the dual test run (b200v2p_eval_rally_stats): the post launch's flags, the per-pair state
+    and the int64 accumulators; every pointer is required"""
+    _fields_ = [
+        ("n", C.c_int32), ("pad_", C.c_int32), ("tar_action", I64P), ("has_contact", U8P), ("has_bounce", U8P), ("bounce_in", U8P),
+        ("ball_pos", F32P), ("root_pos", F32P), ("swing_type_cycle", I64P), ("progress_buf", I64P), ("pair_open", U8P),
+        ("pair_hits", I64P), ("totals", I64P), ("ends", I64P), ("player", I64P), ("shots_hist", I64P),
+    ]
+    _nullable_ = ()
+    _defaults_ = ("pad_",)
+
+
 class V2PActorReset(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("num_dof", C.c_int32), ("bodies_per_env", C.c_int32), ("root_stride", C.c_int32),
@@ -710,6 +727,8 @@ SIGNATURES = {
     "b200v2p_task_reset_desc_size": (_i32, []),
     "b200v2p_eval_ball_stats": (C.c_int, [_p, _p]),
     "b200v2p_eval_ball_stats_desc_size": (_i32, []),
+    "b200v2p_eval_rally_stats": (C.c_int, [_p, _p]),
+    "b200v2p_eval_rally_stats_desc_size": (_i32, []),
     "b200v2p_actor_reset": (C.c_int, [_p, _p]),
     "b200v2p_eval_record": (C.c_int, [_p, _p]),
     "b200v2p_eval_best": (C.c_int, [_p, _p]),

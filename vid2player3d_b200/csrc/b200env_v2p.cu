@@ -565,7 +565,7 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) controller_post_kernel(b200v2p
     if (lane == 0 && !c.obs_only) eval_reset(c, e, rp, bp, has_contact);
     return;
   }
-  if (lane == 0 && !c.obs_only && c.dual) {
+  if (lane == 0 && !c.obs_only && c.dual) {   // the terms below are restated by dual_terms (rally results): change both together
     const int64_t p = e ^ 1;
     bool rec[2], term[2];
     for (int w = 0; w < 2; w++) {
@@ -660,6 +660,97 @@ __global__ void __launch_bounds__(BSTATS_THREADS) eval_ball_stats_kernel(b200v2p
   for (int k = 0; k < 3; k++)
     if (c[k]) atomicAdd(b + 1 + k, c[k]);
   if (err) atomicAdd(b + 4, (unsigned long long)err);
+}
+
+// ------------------------------------------------------------------------------------------ rally results of the dual test run
+// b200v2p_eval_rally_stats: one thread per pair.  The per-pair state is the thread's own; the warp's counts are popcounts of ballots and
+// its shot / frame sums a shuffle reduction, added by lane 0; the ending lanes are grouped by histogram bucket (__match_any_sync) and
+// each group's lowest lane adds it.  Integer atomics only, so every run gives the same bits whatever the order.
+#define RSTATS_THREADS 256
+// the terms of the dual reset rule (physics_mvae_controller_dual.py:92-120) for player env i, as the dual block of
+// controller_post_kernel computes them.  A copy of those lines rather than a function both kernels call: moving them into a shared
+// function changes the post kernel's SASS, which is kept as shipped.  This launch runs after the post launch, so bounce_in[i] already
+// holds this step's value, which the post kernel recomputes for the partner's env.  rec: the player meets the ball (to hit, and it
+// touched it, is behind or bounced twice); out: a ball it hit bounced out
+struct DualTerms { bool rec, hc, twice, out; };
+__device__ __forceinline__ DualTerms dual_terms(const b200v2p_rstats_t& d, int64_t i) {
+  const bool ta1 = d.tar_action[i] == 1, ta0 = d.tar_action[i] == 0, hc = d.has_contact[i] != 0, hb = d.has_bounce[i] != 0;
+  const bool bin = d.bounce_in[i] != 0;
+  const bool miss_ball = d.ball_pos[i * 3 + 1] < d.root_pos[i * 3 + 1] - 1.0f;
+  const bool twice = hb && d.ball_pos[i * 3 + 2] < 0.05f;
+  DualTerms t;
+  t.rec = ta1 && (hc || miss_ball || twice);
+  t.hc = hc;
+  t.twice = twice;
+  t.out = ta0 && hb && !bin;
+  return t;
+}
+__device__ __forceinline__ long long warp_sum(long long v) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+  return v;
+}
+__global__ void __launch_bounds__(RSTATS_THREADS) eval_rally_stats_kernel(b200v2p_rstats_t d) {
+  const int lane = threadIdx.x & 31;
+  const int64_t k = (int64_t)blockIdx.x * RSTATS_THREADS + threadIdx.x;
+  bool faced[2] = {false, false}, hit[2] = {false, false}, fh[2] = {false, false};
+  bool cause[2][B200V2P_RSTATS_CAUSES] = {};
+  bool end = false;
+  long long shots = 0, frames = 0;
+  if (k < (d.n >> 1)) {
+    const int64_t a = 2 * k;
+    const int64_t progress = d.progress_buf[a];
+    const bool opening = progress == 1;      // the first post launch after the pair's reset opens its rally
+    if (opening || d.pair_open[k]) {
+      long long h[2] = {0, 0};
+      if (!opening) { h[0] = d.pair_hits[a]; h[1] = d.pair_hits[a + 1]; }
+#pragma unroll
+      for (int w = 0; w < 2; w++) {
+        const int64_t i = a + w;
+        const DualTerms t = dual_terms(d, i);
+        faced[w] = t.rec;
+        hit[w] = t.rec && t.hc;
+        fh[w] = hit[w] && d.swing_type_cycle[i] == 1;
+        cause[w][0] = t.rec && !t.hc && !t.twice;    // behind
+        cause[w][1] = t.rec && !t.hc && t.twice;     // double bounce
+        cause[w][2] = t.out;
+        h[w] += hit[w] ? 1 : 0;
+        end = end || cause[w][0] || cause[w][1] || cause[w][2];
+      }
+      if (opening || hit[0] || hit[1]) { d.pair_hits[a] = h[0]; d.pair_hits[a + 1] = h[1]; }
+      if (end) {
+        shots = h[0] + h[1];
+        frames = progress;
+      }
+      if (opening || end) d.pair_open[k] = end ? 0 : 1;    // open until the rally ends (the pair then waits for its reset)
+    }
+  }
+  const unsigned ends = __ballot_sync(FULL, end);
+  if (__ballot_sync(FULL, end || faced[0] || faced[1]) == 0) return;   // warp-uniform
+  if (end) {
+    const long long bucket = shots < B200V2P_RSTATS_HIST - 1 ? shots : B200V2P_RSTATS_HIST - 1;
+    const unsigned peers = __match_any_sync(ends, (unsigned long long)bucket);
+    if (lane == __ffs(peers) - 1)
+      atomicAdd(reinterpret_cast<unsigned long long*>(d.shots_hist + bucket), (unsigned long long)__popc(peers));
+  }
+  unsigned long long v[15];
+  v[0] = __popc(ends);
+  v[1] = ends ? (unsigned long long)warp_sum(shots) : 0ull;
+  v[2] = ends ? (unsigned long long)warp_sum(frames) : 0ull;
+#pragma unroll
+  for (int w = 0; w < 2; w++) {
+#pragma unroll
+    for (int c = 0; c < B200V2P_RSTATS_CAUSES; c++) v[3 + w * B200V2P_RSTATS_CAUSES + c] = __popc(__ballot_sync(FULL, cause[w][c]));
+    v[9 + w * 3] = __popc(__ballot_sync(FULL, faced[w]));
+    v[10 + w * 3] = __popc(__ballot_sync(FULL, hit[w]));
+    v[11 + w * 3] = __popc(__ballot_sync(FULL, fh[w]));
+  }
+  if (lane != 0) return;
+  unsigned long long* const dst[3] = {reinterpret_cast<unsigned long long*>(d.totals), reinterpret_cast<unsigned long long*>(d.ends),
+                                      reinterpret_cast<unsigned long long*>(d.player)};
+#pragma unroll
+  for (int j = 0; j < 15; j++)
+    if (v[j]) atomicAdd(j < 3 ? dst[0] + j : (j < 9 ? dst[1] + (j - 3) : dst[2] + (j - 9)), v[j]);
 }
 
 // ------------------------------------------------------------------------------------------ test-time rally recorder
@@ -1424,6 +1515,28 @@ int b200v2p_eval_ball_stats(const b200v2p_bstats_t* d, void* stream) {
 }
 
 int32_t b200v2p_eval_ball_stats_desc_size(void) { return (int32_t)sizeof(b200v2p_bstats_t); }
+
+int b200v2p_eval_rally_stats(const b200v2p_rstats_t* d, void* stream) {
+  if (!d) return vfail(-1, "b200v2p_eval_rally_stats: null");
+  if (d->n < 0 || (d->n & 1)) return vfail(-1, "b200v2p_eval_rally_stats: n must be even and >= 0 (the pairs 2k, 2k+1)");
+  const struct { const void* p; const char* name; } fields[] = {
+      {d->tar_action, "tar_action"}, {d->has_contact, "has_contact"}, {d->has_bounce, "has_bounce"}, {d->bounce_in, "bounce_in"},
+      {d->ball_pos, "ball_pos"}, {d->root_pos, "root_pos"}, {d->swing_type_cycle, "swing_type_cycle"}, {d->progress_buf, "progress_buf"},
+      {d->pair_open, "pair_open"}, {d->pair_hits, "pair_hits"}, {d->totals, "totals"}, {d->ends, "ends"}, {d->player, "player"},
+      {d->shots_hist, "shots_hist"}};
+  for (const auto& f : fields)
+    if (!f.p) {
+      snprintf(g_verr, sizeof(g_verr), "b200v2p_eval_rally_stats: %s is NULL", f.name);
+      return -1;
+    }
+  if (d->n == 0) return 0;
+  const int64_t pairs = d->n >> 1;
+  eval_rally_stats_kernel<<<(unsigned)((pairs + RSTATS_THREADS - 1) / RSTATS_THREADS), RSTATS_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  V_CUDA_OK();
+  return 0;
+}
+
+int32_t b200v2p_eval_rally_stats_desc_size(void) { return (int32_t)sizeof(b200v2p_rstats_t); }
 
 int b200v2p_ctrl_reset(const b200v2p_creset_t* d, void* stream) {
   if (!d) return vfail(-1, "b200v2p_ctrl_reset: bad arguments");

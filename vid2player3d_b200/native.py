@@ -29,7 +29,8 @@ def lib():
         for S, size in ((abi.ResetMasked, L.b200env_reset_masked_desc_size()), (abi.MotionContext, L.b200env_motion_context_desc_size()),
                         (abi.ImRecord, L.b200env_im_record_desc_size()), (abi.V2PTaskReset, L.b200v2p_task_reset_desc_size()),
                         (abi.ImMotionStats, L.b200env_im_motion_stats_desc_size()),
-                        (abi.V2PBallStats, L.b200v2p_eval_ball_stats_desc_size())):
+                        (abi.V2PBallStats, L.b200v2p_eval_ball_stats_desc_size()),
+                        (abi.V2PRallyStats, L.b200v2p_eval_rally_stats_desc_size())):
             if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
                 raise RuntimeError(f"libb200env.so takes a {size}-byte {S.__name__} descriptor, the binding fills {C.sizeof(S)} - rebuild")
         _lib = L

@@ -104,6 +104,13 @@ def eval_ball_stats(cfg, t):
     _check(lib().b200v2p_eval_ball_stats(C.byref(fill(abi.V2PBallStats, cfg, t)), _stream()))
 
 
+def eval_rally_stats(cfg, t):
+    """cfg: n (even); t: the dual post launch's tar_action / has_contact / has_bounce / bounce_in / ball_pos / root_pos /
+    swing_type_cycle / progress_buf, the pair state pair_open (bool [n/2]) / pair_hits (int64 [n/2, 2]) and the int64 accumulators
+    totals [3], ends [2, 3], player [2, 3], shots_hist [abi.RSTATS_HIST]; see include/b200env_v2p.h b200v2p_rstats_t"""
+    _check(lib().b200v2p_eval_rally_stats(C.byref(fill(abi.V2PRallyStats, cfg, t)), _stream()))
+
+
 def actor_reset(cfg, t):
     """cfg: scalars of abi.V2PActorReset; racket_offset2 (with racket_parent2, default racket_parent) sets dual"""
     two = cfg.get("racket_offset2") is not None

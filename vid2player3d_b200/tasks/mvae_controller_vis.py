@@ -10,6 +10,10 @@
                          recovery events with their hits, forehands, bounces in and bounce-in error, counted on the device inside
                          the test loop's reset and step graphs and written by export_ball_stats when run_test ends or the
                          recorder quits
+  MVAEControllerVisDual  with cfg.env.b200_rally_stats (an addition): the rallies of the pairs - shots per rally, how each rally
+                         ends and which player ended it, each player's balls faced, hits and forehands - counted on the device right
+                         after every post launch (inside the step graph) and written by export_rally_stats when run_test ends or
+                         the recorder quits
 
 The renderer (SMPL meshes, video, HTML) is not part of this package: the .npz files hold exactly the arrays the reference's
 render_one_result is given, so they can be rendered with its visualizer.  Deliberate departures from the reference:
@@ -87,12 +91,22 @@ def _check_ball_stats_cfg(cfg, dual):
                          "multiple_cycle with ball_pool_test): random draws keep no row identity")
 
 
+def _stats_path(env, kind, now):
+    """cfg.env.b200_<kind>_file, or out/<kind>/<kind>_<date>.npz"""
+    if env.get(f"b200_{kind}_file"):
+        return str(env[f"b200_{kind}_file"])
+    now = now or datetime.now()
+    return os.path.join("out", kind, "%s_%s.npz" % (kind, now.strftime('%Y-%m-%d-%H:%M:%S')))
+
+
 def ball_stats_path(env, now=None):
     """cfg.env.b200_ball_stats_file, or out/ball_stats/ball_stats_<date>.npz"""
-    if env.get("b200_ball_stats_file"):
-        return str(env["b200_ball_stats_file"])
-    now = now or datetime.now()
-    return os.path.join("out", "ball_stats", "ball_stats_%s.npz" % now.strftime('%Y-%m-%d-%H:%M:%S'))
+    return _stats_path(env, "ball_stats", now)
+
+
+def rally_stats_path(env, now=None):
+    """cfg.env.b200_rally_stats_file, or out/rally_stats/rally_stats_<date>.npz"""
+    return _stats_path(env, "rally_stats", now)
 
 
 def ball_stats_summary(a):
@@ -102,6 +116,26 @@ def ball_stats_summary(a):
     rate = lambda k: int(a[k].sum()) / rec if rec else float("nan")  # noqa: E731
     return (f"balls served: {int(a['served'].sum())}  recoveries: {rec}  hit rate: {rate('hits'):.4f}  "
             f"bounce-in rate: {rate('bounce_in'):.4f}  rows never hit: {int((a['hits'] == 0).sum())} of {len(a['hits'])}")
+
+
+def _check_rally_stats_cfg(cfg, dual):
+    """b200_rally_stats counts the rallies of the two-player task: refuse it on the single-player one, before anything is allocated"""
+    if cfg["env"].get("b200_rally_stats", False) and not dual:
+        raise ValueError("b200_rally_stats counts the rallies of MVAEControllerVisDual; the single-player task's per-ball results are "
+                         "b200_ball_stats")
+
+
+def rally_stats_summary(a):
+    """the printed line of export_rally_stats: rallies, mean shots per rally, and per player the hit rate hits / faced and the share
+    of all rallies it ended by each cause (both players can end the same rally)"""
+    R = int(a["rallies"])
+    nan = float("nan")
+    line = f"rallies: {R}  shots per rally: {int(a['shots_sum']) / R if R else nan:.2f}"
+    for w in range(2):
+        faced = int(a["faced"][w])
+        ends = " ".join(f"{c} {int(a['ends'][w, j]) / R if R else nan:.4f}" for j, c in enumerate(abi.RSTATS_CAUSES))
+        line += f"  player {w} ({a['players'][w]}): hit rate {int(a['hits'][w]) / faced if faced else nan:.4f}, ended {ends}"
+    return line
 
 
 class _EvalRecorder:
@@ -120,6 +154,7 @@ class _EvalRecorder:
         self._fix_backhand = bool(self.cfg_v2p.get("fix_two_hand_backhand_post"))
         self.backhand_losses = {}
         self._bstats = None              # per-row buckets of b200_ball_stats (MVAEControllerVis)
+        self._rstats = None              # pair state and counts of b200_rally_stats (MVAEControllerVisDual)
         self._test_steps = 0
 
     def _episode_path(self, eg_id):
@@ -157,9 +192,14 @@ class _EvalRecorder:
         self.frame_index += 1
         if self._record and self.frame_index >= self._num_rec_frames:
             self.export_episodes()
-            if self._bstats is not None:
-                self.export_ball_stats()
+            self._export_stats()
             raise SystemExit(0)
+
+    def _export_stats(self):
+        if self._bstats is not None:
+            self.export_ball_stats()
+        if self._rstats is not None:
+            self.export_rally_stats()
 
     # ------------------------------------------------------------------ test loop of V2PPlayer.run (players/v2p_player.py:133-156)
     def set_policy(self, policy):
@@ -180,14 +220,14 @@ class _EvalRecorder:
         test_step() calls.  Ends like
         the reference, with SystemExit once num_rec_frames frames are recorded (with record).  With b200_ball_stats the per-row
         buckets are written when the run returns, or before that SystemExit; they count from the task's construction, so the first
-        reset's draws are in them whether it ran here or before."""
+        reset's draws are in them whether it ran here or before.  b200_rally_stats' counts are written at the same points; they count
+        every post launch since the task's construction, step() included."""
         self.set_policy(policy)
         self.reset()
         self.render_vis(init=True)
         for _ in range(max_steps):
             self.test_step(graph)
-        if self._bstats is not None:
-            self.export_ball_stats()
+        self._export_stats()
 
     def test_step(self, graph=True):
         """one iteration of V2PPlayer.run's loop: reset of the finished envs (mask-driven, from reset_buf), policy, env step,
@@ -235,6 +275,7 @@ class MVAEControllerVis(_EvalRecorder, PhysicsMVAEController):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         _check_eval_cfg(cfg, headless)
         _check_ball_stats_cfg(cfg, dual=False)
+        _check_rally_stats_cfg(cfg, dual=False)
         super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
                          headless=headless)
         self._init_eval(cfg)
@@ -332,10 +373,16 @@ class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless, capacity=DUAL_CAPACITY):
         _check_eval_cfg(cfg, headless)
         _check_ball_stats_cfg(cfg, dual=True)
+        _check_rally_stats_cfg(cfg, dual=True)
         super().__init__(cfg=cfg, sim_params=sim_params, physics_engine=physics_engine, device_type=device_type, device_id=device_id,
                          headless=headless)
         self._init_eval(cfg)
         self._cap = int(capacity)
+        if cfg["env"].get("b200_rally_stats", False):
+            i64 = lambda *s: torch.zeros(*s, device=self.device, dtype=torch.long)  # noqa: E731
+            K = self.num_envs // 2
+            self._rstats = dict(pair_open=torch.zeros(K, device=self.device, dtype=torch.bool), pair_hits=i64(K, 2), totals=i64(3),
+                                ends=i64(2, len(abi.RSTATS_CAUSES)), player=i64(2, len(abi.RSTATS_PLAYER)), shots_hist=i64(abi.RSTATS_HIST))
         if self._record:
             N, E, dev = self.num_envs, self._num_eg, self.device
             fields = ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action")
@@ -358,6 +405,40 @@ class MVAEControllerVisDual(_EvalRecorder, PhysicsMVAEControllerDual):
         native_v2p.eval_best(self.num_envs, self._cap, self._num_eg, dict(
             reset_buf=self.reset_buf, progress_buf=self.progress_buf, distance=self._distance, **self._list, **rec,
             **{"best_" + k: v for k, v in self._best.items()}))
+
+    def post_physics_step(self):
+        """the step's post launch, then with b200_rally_stats the pairs' rally results from its flags (b200v2p_eval_rally_stats), so that
+        step(), its graph and run_test's step graph all count"""
+        super().post_physics_step()
+        if self._rstats is not None:
+            t = self._physics_player.task
+            native_v2p.eval_rally_stats(dict(n=self.num_envs), dict(
+                tar_action=self._tar_action, has_contact=t._has_racket_ball_contact, has_bounce=t._has_bounce, bounce_in=self._bounce_in,
+                ball_pos=t._ball_pos, root_pos=t._root_pos, swing_type_cycle=self._mvae_player._swing_type_cycle.contiguous(),
+                progress_buf=self.progress_buf, **self._rstats))
+
+    def rally_players(self):
+        """the cfg's players of a pair: the `player` pair in dual_mode different, else the one player twice"""
+        v = self.cfg_v2p
+        return [str(p) for p in v["player"]] if v.get("dual_mode") == "different" else [str(v.get("player"))] * 2
+
+    def export_rally_stats(self):
+        """writes the rally results to b200_rally_stats_file and prints the summary line; returns the file's path.  int64: rallies,
+        shots_sum, frames_sum, shots_hist [65] (shots per rally 0..63, then 64 or more), ends [2, 3] by end_causes, faced, hits,
+        forehands [2], open_rallies and open_hits [open, 2] (the pairs still in a rally), num_envs, test_steps; players [2]."""
+        r = {k: v.cpu().numpy() for k, v in self._rstats.items()}
+        pl = r["player"]
+        a = dict(rallies=r["totals"][0], shots_sum=r["totals"][1], frames_sum=r["totals"][2], shots_hist=r["shots_hist"], ends=r["ends"],
+                 end_causes=np.array(abi.RSTATS_CAUSES), **{k: pl[:, j].copy() for j, k in enumerate(abi.RSTATS_PLAYER)},
+                 open_rallies=np.int64(r["pair_open"].sum()), open_hits=r["pair_hits"][r["pair_open"]],
+                 players=np.array(self.rally_players()), num_envs=np.int64(self.num_envs), test_steps=np.int64(self._test_steps))
+        path = rally_stats_path(self.cfg["env"])
+        if os.path.dirname(path):
+            os.makedirs(os.path.dirname(path), exist_ok=True)
+        np.savez(path, **a)
+        print(rally_stats_summary(a))
+        print(f"============ rally statistics written to {path} ============")
+        return path
 
     def best_list(self):
         """the list in rank order: (slot, even env of the pair, distance, frames) per entry"""
