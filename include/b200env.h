@@ -383,25 +383,54 @@ int32_t b200env_im_record_desc_size(void);
  * The caller zeroes env_sums and env_flags when a game starts, as b200env_play_stats' cr / steps / prev_dones.  games:
  * b200_play_stats_t::games or NULL; while games[1] (stop) is set neither launch changes anything.  Each env must appear exactly once
  * in motion_envs: the launch does not check the lists.  Returns -2 before any launch when n or num_motions is not positive or
- * num_lib_bodies is not in [1, num_bodies]. */
-typedef struct b200_im_motion_stats {
-  int32_t n;                       /* envs */
-  int32_t num_motions;             /* M */
-  int32_t num_bodies;              /* bodies per env of rigid_body_state */
-  int32_t num_lib_bodies;          /* bodies compared: rows per env of target_rb_pos */
-  const float* rew;                /* [n] */
-  const float* sub_rewards;        /* [n, 4]: dof, vel, body_pos, body_rot */
-  const int64_t* reset_buf;        /* [n] */
-  const int64_t* terminate_buf;    /* [n]: 1 = the episode ended in a fall */
-  const float* rigid_body_state;   /* [n, num_bodies, 13] */
-  const float* target_rb_pos;      /* [n, num_lib_bodies, 3]: the targets the step's reward compared against (p_rb_pos) */
-  const int64_t* motion_start;     /* [M + 1] */
-  const int64_t* motion_envs;      /* [n]: the envs of each motion, grouped by motion, in env order within one */
-  double* env_sums;                /* [n, 7]: rew, steps, sub_rewards[4], err of the game so far */
-  int32_t* env_flags;              /* [n, 2]: prev_done, ended */
-  int64_t* counts;                 /* [M, 2]: games, falls */
-  double* sums;                    /* [M, 7]: the env_sums columns of the finished games */
+ * num_lib_bodies is not in [1, num_bodies].
+ *
+ * Pose metrics (cfg.env.b200_pose_metrics; all five pose pointers set, or all NULL for the meters alone): with p_b the simulated and
+ * r_b the target position of body b < num_lib_bodies (body 0 the root), the accumulate launch also adds, per frame, the means over
+ * the bodies of
+ *   l   = |(p_b - p_0) - (r_b - r_0)|                                          root-relative MPJPE
+ *   pa  = |s R (p_b - mean p) + mean r - r_b|                                  PA-MPJPE: s, R the similarity of HMR/SPIN's
+ *         compute_similarity_transform (proper rotation), s = 0 when the simulated bodies have no spread (var1 = 0)
+ *   vel = |(p_t - p_t-1) - (r_t - r_t-1)|                                      from the game's second frame on
+ *   acc = |(p_t - 2 p_t-1 + p_t-2) - (r_t - 2 r_t-1 + r_t-2)|                  from the game's third frame on
+ * in double to env_pose[e] (with the frame counts of vel and acc), and keeps in env_pose[e, 6] the game's largest err (the
+ * body-position error above), NaN once a frame has a non-finite error.  The previous two frames are kept in pose_hist (float, as
+ * the positions arrive) with pose_fill frames valid; a game's end (ended != 0) empties it.  The fold adds the env_pose sums of the
+ * finished games to pose_sums[m], takes the largest of their maxima into pose_sums[m, 6] (NaN if one is NaN), counts in success[m]
+ * the games whose maximum is <= success_threshold (so not NaN), and zeroes the env's row.  The caller zeroes env_pose and pose_fill
+ * when a game starts.  One warp per env with lane b on body b: returns -2 when num_lib_bodies > 32 or success_threshold is not a
+ * finite positive number, and -1 when only some pose pointers are NULL, all after the checks above. */
+#define B200_IM_MOTION_METERS_FIELDS                                                                                              \
+  int32_t n;                       /* envs */                                                                                       \
+  int32_t num_motions;             /* M */                                                                                          \
+  int32_t num_bodies;              /* bodies per env of rigid_body_state */                                                         \
+  int32_t num_lib_bodies;          /* bodies compared: rows per env of target_rb_pos */                                             \
+  const float* rew;                /* [n] */                                                                                        \
+  const float* sub_rewards;        /* [n, 4]: dof, vel, body_pos, body_rot */                                                       \
+  const int64_t* reset_buf;        /* [n] */                                                                                        \
+  const int64_t* terminate_buf;    /* [n]: 1 = the episode ended in a fall */                                                       \
+  const float* rigid_body_state;   /* [n, num_bodies, 13] */                                                                        \
+  const float* target_rb_pos;      /* [n, num_lib_bodies, 3]: the targets the step's reward compared against (p_rb_pos) */          \
+  const int64_t* motion_start;     /* [M + 1] */                                                                                    \
+  const int64_t* motion_envs;      /* [n]: the envs of each motion, grouped by motion, in env order within one */                   \
+  double* env_sums;                /* [n, 7]: rew, steps, sub_rewards[4], err of the game so far */                                 \
+  int32_t* env_flags;              /* [n, 2]: prev_done, ended */                                                                   \
+  int64_t* counts;                 /* [M, 2]: games, falls */                                                                       \
+  double* sums;                    /* [M, 7]: the env_sums columns of the finished games */                                         \
   const int64_t* games;            /* [3] or NULL */
+/* the meters' fields alone: the parameter of the meters' kernels.  A by-value kernel parameter over 128 bytes is read through its
+ * address instead of being loaded up front, so the meters' kernels take these 120 bytes and not the whole descriptor. */
+typedef struct b200_im_motion_stats {
+  B200_IM_MOTION_METERS_FIELDS
+} b200_im_motion_meters_t;
+typedef struct b200_im_motion_stats_desc {
+  B200_IM_MOTION_METERS_FIELDS
+  double* env_pose;                /* [n, 7] or NULL: l, pa, vel, acc sums, vel frames, acc frames, largest err of the game so far */
+  float* pose_hist;                /* [n, 2, 2, num_lib_bodies, 3] or NULL: frames t-1, t-2 of (simulated, target) positions */
+  int32_t* pose_fill;              /* [n] or NULL: frames of pose_hist that hold this game's positions, 0..2 */
+  double* pose_sums;               /* [M, 7] or NULL: the env_pose columns of the finished games, column 6 their largest err */
+  int64_t* success;                /* [M] or NULL: finished games whose largest err is <= success_threshold */
+  double success_threshold;        /* metres */
 } b200_im_motion_stats_t;
 int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream);
 /* sizeof(b200_im_motion_stats_t) as the library was built; the binding refuses a library whose size differs from its own */

@@ -329,8 +329,11 @@ class ImMotionStats(C.Structure):
         ("rew", F32P), ("sub_rewards", F32P), ("reset_buf", I64P), ("terminate_buf", I64P), ("rigid_body_state", F32P),
         ("target_rb_pos", F32P), ("motion_start", I64P), ("motion_envs", I64P), ("env_sums", F64P), ("env_flags", I32P),
         ("counts", I64P), ("sums", F64P), ("games", I64P),
+        ("env_pose", F64P), ("pose_hist", F32P), ("pose_fill", I32P), ("pose_sums", F64P), ("success", I64P),
+        ("success_threshold", C.c_double),
     ]
-    _nullable_, _defaults_ = ("games",), ()
+    _nullable_ = ("games", "env_pose", "pose_hist", "pose_fill", "pose_sums", "success")
+    _defaults_ = ("success_threshold",)
 
 
 # the context window's transform program (include/b200env.h: b200_motion_context_t), appended to b200_reset_masked_t and

@@ -2132,7 +2132,154 @@ __global__ void __launch_bounds__(REC_WARPS * 32) im_record_kernel(b200_im_recor
 #define MS_WARPS 8
 #define MS_FOLD_THREADS 256
 #define MS_COLS 7
-__global__ void __launch_bounds__(MS_WARPS * 32) im_motion_stats_acc_kernel(b200_im_motion_stats_t d) {
+#define MS_POSE_COLS 7       // env_pose / pose_sums: l, pa, vel, acc, vel frames, acc frames, largest err
+#define MS_JACOBI_SWEEPS 6   // cyclic sweeps on Horn's 4x4 matrix: 5 reach double rounding on random and near-exact poses
+
+__device__ __forceinline__ double ms_warp_sum(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// the larger of two errors, NaN if either is NaN: the same value in any order
+__device__ __forceinline__ double ms_max(double a, double b) { return (a != a || b > a || b != b) ? (a != a ? a : b) : a; }
+
+// PA-MPJPE's rotation: the proper rotation R maximising tr(R k), k = sum_b x_b y_b^T (x simulated, y target, both centred), from
+// Horn's quaternion, the eigenvector of the largest eigenvalue of his symmetric 4x4 matrix, by a fixed number of cyclic Jacobi sweeps
+__device__ __forceinline__ void ms_horn_rotation(const double k[3][3], double r[3][3]) {
+  double a[4][4] = {{k[0][0] + k[1][1] + k[2][2], k[1][2] - k[2][1], k[2][0] - k[0][2], k[0][1] - k[1][0]},
+                    {k[1][2] - k[2][1], k[0][0] - k[1][1] - k[2][2], k[0][1] + k[1][0], k[2][0] + k[0][2]},
+                    {k[2][0] - k[0][2], k[0][1] + k[1][0], -k[0][0] + k[1][1] - k[2][2], k[1][2] + k[2][1]},
+                    {k[0][1] - k[1][0], k[2][0] + k[0][2], k[1][2] + k[2][1], -k[0][0] - k[1][1] + k[2][2]}};
+  double v[4][4] = {{1.0, 0.0, 0.0, 0.0}, {0.0, 1.0, 0.0, 0.0}, {0.0, 0.0, 1.0, 0.0}, {0.0, 0.0, 0.0, 1.0}};
+  for (int sweep = 0; sweep < MS_JACOBI_SWEEPS; sweep++) {
+#pragma unroll
+    for (int p = 0; p < 3; p++) {
+#pragma unroll
+      for (int q = p + 1; q < 4; q++) {
+        const double apq = a[p][q];
+        if (apq == 0.0) continue;
+        const double theta = (a[q][q] - a[p][p]) / (2.0 * apq);
+        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = rsqrt(t * t + 1.0), s = t * c;
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          if (i == p || i == q) continue;
+          const double aip = a[i][p], aiq = a[i][q];
+          a[i][p] = a[p][i] = c * aip - s * aiq;
+          a[i][q] = a[q][i] = s * aip + c * aiq;
+        }
+        a[p][p] -= t * apq;
+        a[q][q] += t * apq;
+        a[p][q] = a[q][p] = 0.0;
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+          const double vip = v[i][p], viq = v[i][q];
+          v[i][p] = c * vip - s * viq;
+          v[i][q] = s * vip + c * viq;
+        }
+      }
+    }
+  }
+  double w = v[0][0], x = v[1][0], y = v[2][0], z = v[3][0], best = a[0][0];
+#pragma unroll
+  for (int j = 1; j < 4; j++)
+    if (a[j][j] > best) { best = a[j][j]; w = v[0][j]; x = v[1][j]; y = v[2][j]; z = v[3][j]; }
+  const double inv = 1.0 / (w * w + x * x + y * y + z * z);
+  r[0][0] = (w * w + x * x - y * y - z * z) * inv; r[0][1] = 2.0 * (x * y - w * z) * inv; r[0][2] = 2.0 * (x * z + w * y) * inv;
+  r[1][0] = 2.0 * (x * y + w * z) * inv; r[1][1] = (w * w - x * x + y * y - z * z) * inv; r[1][2] = 2.0 * (y * z - w * x) * inv;
+  r[2][0] = 2.0 * (x * z - w * y) * inv; r[2][1] = 2.0 * (y * z + w * x) * inv; r[2][2] = (w * w - x * x - y * y + z * z) * inv;
+}
+
+// the pose fields of b200_im_motion_stats_t: the second parameter of the pose forms of the meters' kernels
+struct MsPose {
+  double* env_pose;
+  float* hist;
+  int32_t* fill;
+  double* sums;
+  int64_t* success;
+  double threshold;
+};
+__device__ __forceinline__ const MsPose& ms_pose(const MsPose& q) { return q; }
+
+// the pose metrics of one frame of env e, by every lane of its warp (lane b on body b < num_lib_bodies <= 32).  Every lane holds the
+// same butterfly sums, so every lane solves the same rotation: no lane waits for another's solve and no broadcast follows.
+// g: the frame's body-position error.  Runs after the meters' lane 0 set this step's ended flag, which empties the history
+__device__ __forceinline__ void ms_pose_frame(const b200_im_motion_meters_t& d, const MsPose& q, int e, int lane, double g) {
+  const int nb = d.num_lib_bodies;
+  const bool own = lane < nb;
+  float p[3] = {0.f, 0.f, 0.f}, r[3] = {0.f, 0.f, 0.f};
+  if (own) {
+    const float* ps = d.rigid_body_state + ((int64_t)e * d.num_bodies + lane) * 13;
+    const float* rs = d.target_rb_pos + ((int64_t)e * nb + lane) * 3;
+#pragma unroll
+    for (int c = 0; c < 3; c++) { p[c] = ps[c]; r[c] = rs[c]; }
+  }
+  double l = 0.0, x[3], y[3];
+#pragma unroll
+  for (int c = 0; c < 3; c++) {
+    const float p0 = __shfl_sync(0xffffffffu, p[c], 0), r0 = __shfl_sync(0xffffffffu, r[c], 0);
+    const double dl = ((double)p[c] - p0) - ((double)r[c] - r0);
+    l += dl * dl;
+    const double mp = ms_warp_sum(p[c]) / nb, mr = ms_warp_sum(r[c]) / nb;
+    x[c] = own ? (double)p[c] - mp : 0.0;
+    y[c] = own ? (double)r[c] - mr : 0.0;
+  }
+  l = ms_warp_sum(own ? sqrt(l) : 0.0) / nb;
+  const double var1 = ms_warp_sum(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);
+  double k[3][3], rot[3][3];
+#pragma unroll
+  for (int i = 0; i < 3; i++)
+#pragma unroll
+    for (int j = 0; j < 3; j++) k[i][j] = ms_warp_sum(x[i] * y[j]);
+  ms_horn_rotation(k, rot);
+  double lam = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; i++)
+#pragma unroll
+    for (int j = 0; j < 3; j++) lam += rot[i][j] * k[j][i];
+  const double s = var1 > 0.0 ? lam / var1 : 0.0;
+  double pa = 0.0;
+#pragma unroll
+  for (int i = 0; i < 3; i++) {
+    const double a = s * (rot[i][0] * x[0] + rot[i][1] * x[1] + rot[i][2] * x[2]) - y[i];
+    pa += a * a;
+  }
+  pa = ms_warp_sum(own ? sqrt(pa) : 0.0) / nb;
+  // velocity and acceleration against the previous two frames of this game
+  const int fill = q.fill[e];
+  float* h = q.hist + (int64_t)e * 12 * nb + lane * 3;      // [frame t-1, t-2][simulated, target][nb][3]
+  double vel = 0.0, acc = 0.0;
+  if (own) {
+#pragma unroll
+    for (int c = 0; c < 3; c++) {
+      const float p1 = h[c], r1 = h[3 * nb + c], p2 = h[6 * nb + c], r2 = h[9 * nb + c];
+      const double dv = ((double)p[c] - p1) - ((double)r[c] - r1);
+      const double da = ((double)p[c] - 2.0 * p1 + p2) - ((double)r[c] - 2.0 * r1 + r2);
+      vel += dv * dv;
+      acc += da * da;
+      h[6 * nb + c] = p1; h[9 * nb + c] = r1; h[c] = p[c]; h[3 * nb + c] = r[c];
+    }
+  }
+  vel = ms_warp_sum(own ? sqrt(vel) : 0.0) / nb;       // the history's stale frames count only from pose_fill on
+  acc = ms_warp_sum(own ? sqrt(acc) : 0.0) / nb;
+  if (fill < 1) vel = 0.0;
+  if (fill < 2) acc = 0.0;
+  if (lane == 0) {
+    double* ep = q.env_pose + (int64_t)e * MS_POSE_COLS;
+    ep[0] += l;
+    ep[1] += pa;
+    if (fill >= 1) { ep[2] += vel; ep[4] += 1.0; }
+    if (fill >= 2) { ep[3] += acc; ep[5] += 1.0; }
+    const bool finite = isfinite(l) && isfinite(pa) && isfinite(vel) && isfinite(acc);
+    ep[6] = ms_max(ep[6], finite ? g : __longlong_as_double(0x7ff8000000000000ll));
+    q.fill[e] = d.env_flags[2 * (int64_t)e + 1] ? 0 : min(fill + 1, 2);
+  }
+}
+
+// Pose: empty for the meters alone, MsPose for the pose forms
+template <bool POSE, typename... Pose>
+__global__ void __launch_bounds__(MS_WARPS * 32) im_motion_stats_acc_kernel(b200_im_motion_meters_t d, Pose... pose) {
   if (d.games && d.games[1]) return;
   const int e = blockIdx.x * MS_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (e >= d.n) return;
@@ -2158,18 +2305,23 @@ __global__ void __launch_bounds__(MS_WARPS * 32) im_motion_stats_acc_kernel(b200
     f[1] = (done && !f[0]) ? 1 + (d.terminate_buf[e] != 0) : 0;
     f[0] = done;
   }
+  if constexpr (POSE) ms_pose_frame(d, ms_pose(pose...), e, lane, err / d.num_lib_bodies);
 }
 
-__global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b200_im_motion_stats_t d) {
-  __shared__ double s_sum[MS_FOLD_THREADS / 32][MS_COLS];
-  __shared__ long long s_cnt[MS_FOLD_THREADS / 32][2];
+// POSE: the env_pose columns ride behind the meters' (the largest err by ms_max, the rest summed), and the successes behind the counts
+template <bool POSE, typename... Pose>
+__global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b200_im_motion_meters_t d, Pose... pose) {
+  static constexpr int W = MS_COLS + (POSE ? MS_POSE_COLS : 0), MAXC = MS_COLS + MS_POSE_COLS - 1, NC = POSE ? 3 : 2;
+  __shared__ double s_sum[MS_FOLD_THREADS / 32][W];
+  __shared__ long long s_cnt[MS_FOLD_THREADS / 32][NC];
   if (d.games && d.games[1]) return;
   const int m = blockIdx.x, tid = threadIdx.x;
   const int64_t first = d.motion_start[m], last = d.motion_start[m + 1];
   const int64_t run = (last - first + MS_FOLD_THREADS - 1) / MS_FOLD_THREADS;
   const int64_t lo = first + tid * run, hi = min(lo + run, last);
-  double s[MS_COLS] = {};
+  double s[W] = {};
   long long games = 0, falls = 0;
+  long long succ = 0;                                   // POSE: the games under the threshold
   for (int64_t i = lo; i < hi; i++) {
     const int64_t e = d.motion_envs[i];
     const int32_t ended = d.env_flags[2 * e + 1];
@@ -2179,6 +2331,15 @@ __global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b
       double* es = d.env_sums + e * MS_COLS;
 #pragma unroll
       for (int k = 0; k < MS_COLS; k++) { s[k] += es[k]; es[k] = 0.0; }
+      if constexpr (POSE) {
+        const MsPose& q = ms_pose(pose...);
+        double* ep = q.env_pose + e * MS_POSE_COLS;
+#pragma unroll
+        for (int k = 0; k < MS_POSE_COLS - 1; k++) { s[MS_COLS + k] += ep[k]; ep[k] = 0.0; }
+        succ += ep[MS_POSE_COLS - 1] <= q.threshold;
+        s[MAXC] = ms_max(s[MAXC], ep[MS_POSE_COLS - 1]);
+        ep[MS_POSE_COLS - 1] = 0.0;
+      }
       d.env_flags[2 * e + 1] = 0;
     }
   }
@@ -2186,15 +2347,20 @@ __global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-    for (int k = 0; k < MS_COLS; k++) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+    for (int k = 0; k < W; k++) {
+      const double t = __shfl_xor_sync(0xffffffffu, s[k], o);
+      s[k] = (POSE && k == MAXC) ? ms_max(s[k], t) : s[k] + t;
+    }
     games += __shfl_xor_sync(0xffffffffu, games, o);
     falls += __shfl_xor_sync(0xffffffffu, falls, o);
+    if constexpr (POSE) succ += __shfl_xor_sync(0xffffffffu, succ, o);
   }
   const int w = tid >> 5;
   if ((tid & 31) == 0) {
 #pragma unroll
-    for (int k = 0; k < MS_COLS; k++) s_sum[w][k] = s[k];
+    for (int k = 0; k < W; k++) s_sum[w][k] = s[k];
     s_cnt[w][0] = games; s_cnt[w][1] = falls;
+    if constexpr (POSE) s_cnt[w][2] = succ;
   }
   __syncthreads();
   if (tid < MS_COLS) {
@@ -2205,6 +2371,24 @@ __global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b
     long long t = 0;
     for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t += s_cnt[j][tid - 32];
     d.counts[2 * (int64_t)m + tid - 32] += t;
+  }
+  if constexpr (POSE) {
+    const MsPose& q = ms_pose(pose...);
+    if (tid >= MS_COLS && tid < W) {
+      double* ps = q.sums + (int64_t)m * MS_POSE_COLS + tid - MS_COLS;
+      double t = 0.0;
+      if (tid == MAXC) {
+        for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t = ms_max(t, s_sum[j][tid]);
+        *ps = ms_max(*ps, t);
+      } else {
+        for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t += s_sum[j][tid];
+        *ps += t;
+      }
+    } else if (tid == 34) {
+      long long t = 0;
+      for (int j = 0; j < MS_FOLD_THREADS / 32; j++) t += s_cnt[j][2];
+      q.success[m] += t;
+    }
   }
 }
 
@@ -3095,9 +3279,27 @@ int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream) {
   if (d->n <= 0 || d->num_motions <= 0) return fail(-2, "b200env_im_motion_stats: n and num_motions must be positive%s");
   if (d->num_lib_bodies < 1 || d->num_lib_bodies > d->num_bodies)
     return fail(-2, "b200env_im_motion_stats: num_lib_bodies must lie in [1, num_bodies]%s");
-  im_motion_stats_acc_kernel<<<(d->n + MS_WARPS - 1) / MS_WARPS, MS_WARPS * 32, 0, (cudaStream_t)stream>>>(*d);
-  CUDA_OK(cudaGetLastError());
-  im_motion_stats_fold_kernel<<<d->num_motions, MS_FOLD_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  const bool pose = d->env_pose || d->pose_hist || d->pose_fill || d->pose_sums || d->success;
+  if (pose && (!d->env_pose || !d->pose_hist || !d->pose_fill || !d->pose_sums || !d->success))
+    return fail(-1, "b200env_im_motion_stats: the pose pointers must be all set or all NULL%s");
+  if (pose && d->num_lib_bodies > 32) return fail(-2, "b200env_im_motion_stats: the pose metrics take at most 32 bodies%s");
+  if (pose && !(d->success_threshold > 0.0 && isfinite(d->success_threshold)))
+    return fail(-2, "b200env_im_motion_stats: success_threshold must be a finite positive number of metres%s");
+  static_assert(offsetof(b200_im_motion_stats_t, env_pose) == sizeof(b200_im_motion_meters_t), "the meters' fields lead");
+  b200_im_motion_meters_t m;
+  memcpy(&m, d, sizeof m);
+  const int acc_blocks = (d->n + MS_WARPS - 1) / MS_WARPS;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (pose) {
+    const MsPose q = {d->env_pose, d->pose_hist, d->pose_fill, d->pose_sums, d->success, d->success_threshold};
+    im_motion_stats_acc_kernel<true><<<acc_blocks, MS_WARPS * 32, 0, st>>>(m, q);
+    CUDA_OK(cudaGetLastError());
+    im_motion_stats_fold_kernel<true><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m, q);
+  } else {
+    im_motion_stats_acc_kernel<false><<<acc_blocks, MS_WARPS * 32, 0, st>>>(m);
+    CUDA_OK(cudaGetLastError());
+    im_motion_stats_fold_kernel<false><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m);
+  }
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -28,7 +28,12 @@ Per-motion meters (cfg.env.b200_motion_stats, an addition): run_test also sums, 
 sub-rewards and the mean body-position error into the bucket of the env's motion, and counts games and falls per motion
 (include/b200env.h: b200env_im_motion_stats, in the step graph after the record launch and before the bookkeeping, so it stops with
 it).  When run_test ends (or the recorder quits) the buckets go to cfg.env.b200_motion_stats_file (default
-out/motion_stats/motion_stats_<date>.npz) and one summary line is printed."""
+out/motion_stats/motion_stats_<date>.npz) and one summary line is printed.
+
+Pose metrics (cfg.env.b200_pose_metrics, an addition; needs b200_motion_stats): the same launch also sums, per finished game, the
+metrics motion-imitation work compares policies on - root-relative and Procrustes-aligned MPJPE, velocity and acceleration error - and
+counts the games whose largest body-position error (global MPJPE) stays within cfg.env.b200_pose_success_threshold (default 0.5 m).
+The file then also holds those sums, their frame counts, the successes and each motion's largest error, and a second line is printed."""
 import os
 from datetime import datetime
 
@@ -104,6 +109,35 @@ def motion_env_lists(motion_ids, num_motions):
     return start, np.argsort(ids, kind="stable").astype(np.int64)
 
 
+def pose_metrics_threshold(env):
+    """cfg.env.b200_pose_metrics -> None when off, else the success threshold in metres (b200_pose_success_threshold, default 0.5);
+    refuses the key without b200_motion_stats and a threshold that is not a finite number above 0"""
+    if not env.get("b200_pose_metrics", False):
+        return None
+    if not env.get("b200_motion_stats", False):
+        raise ValueError("b200_pose_metrics extends the per-motion meters: set b200_motion_stats: True as well")
+    t = env.get("b200_pose_success_threshold", 0.5)
+    try:
+        t = float(t)
+    except (TypeError, ValueError):
+        raise ValueError(f"b200_pose_success_threshold must be a number of metres, got {t!r}") from None
+    if not (np.isfinite(t) and t > 0):
+        raise ValueError(f"b200_pose_success_threshold must be a finite number of metres above 0, got {t!r}")
+    return t
+
+
+def pose_metrics_summary(counts, sums, pose_sums, success):
+    """the printed line of the pose metrics (counts [M, 2], sums [M, 7], pose_sums [M, 7], success [M]): success rate, the MPJPEs in
+    mm and the velocity and acceleration errors in mm/frame and mm/frame^2 over the finished games"""
+    games, steps = counts[:, 0].sum(), sums[:, 1].sum()
+    vf, af = pose_sums[:, 4].sum(), pose_sums[:, 5].sum()
+    mm = lambda x, n: 1000.0 * x / n if n else float("nan")  # noqa: E731
+    rate = success.sum() / games if games else float("nan")
+    return (f"success rate: {rate:.4f}  MPJPE-g: {mm(sums[:, 6].sum(), steps):.2f} mm  MPJPE-l: {mm(pose_sums[:, 0].sum(), steps):.2f} mm"
+            f"  PA-MPJPE: {mm(pose_sums[:, 1].sum(), steps):.2f} mm  velocity error: {mm(pose_sums[:, 2].sum(), vf):.2f} mm/frame"
+            f"  acceleration error: {mm(pose_sums[:, 3].sum(), af):.2f} mm/frame^2")
+
+
 def motion_stats_summary(counts, sums):
     """the printed line of the per-motion buckets (counts [M, 2] games, falls; sums [M, 7] float64)"""
     games, falls = counts[:, 0], counts[:, 1]
@@ -121,6 +155,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         env = cfg["env"]
         self._rec = None
         rec_ids = None
+        self._pose_threshold = pose_metrics_threshold(env)
         if env.get("b200_record_qpos", False):
             rec_ids = record_env_ids(env.get("b200_record_envs", [0]), int(env["numEnvs"]))
             if not getattr(cfg.get("args", None), "rec_once", False) and int(env.get("num_rec_frames", 300)) < 1:
@@ -229,10 +264,17 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                         env_sums=torch.zeros(N, 7, device=dev, dtype=torch.float64),
                         env_flags=torch.zeros(N, 2, device=dev, dtype=torch.int32),
                         counts=torch.zeros(M, 2, device=dev, dtype=torch.long), sums=torch.zeros(M, 7, device=dev, dtype=torch.float64))
+        if self._pose_threshold is not None:    # one warp per env, a lane per body
+            nbl = self._num_lib_bodies
+            if nbl > 32:
+                raise ValueError(f"b200_pose_metrics compares at most 32 bodies, the motion library has {nbl}")
+            self._ms.update(env_pose=torch.zeros(N, 7, device=dev, dtype=torch.float64), pose_hist=torch.zeros(N, 2, 2, nbl, 3, device=dev),
+                            pose_fill=torch.zeros(N, device=dev, dtype=torch.int32),
+                            pose_sums=torch.zeros(M, 7, device=dev, dtype=torch.float64), success=torch.zeros(M, device=dev, dtype=torch.long))
 
     def _motion_stats_launch(self, games=None):
         native.im_motion_stats(dict(n=self.num_envs, num_motions=self._motion_lib.num_motions(), num_bodies=self.num_bodies,
-                                    num_lib_bodies=self._num_lib_bodies),
+                                    num_lib_bodies=self._num_lib_bodies, success_threshold=self._pose_threshold),
                                dict(self._ms, rew=self.rew_buf, sub_rewards=self._sub_rewards, reset_buf=self.reset_buf,
                                     terminate_buf=self._terminate_buf, rigid_body_state=self._rigid_body_state,
                                     target_rb_pos=self._prev_target_rb_pos, games=games))
@@ -245,10 +287,27 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             os.makedirs(os.path.dirname(path), exist_ok=True)
         np.savez(path, games=counts[:, 0], falls=counts[:, 1], reward_sum=sums[:, 0], steps=sums[:, 1].astype(np.int64),
                  sub_reward_sum=sums[:, 2:6], body_pos_err_sum=sums[:, 6], env_motion_ids=self._reset_ref_motion_ids.cpu().numpy(),
-                 test_motion_file=np.array(self._test_motion_file or ""))
+                 test_motion_file=np.array(self._test_motion_file or ""), **self._pose_metrics_keys())
         print(motion_stats_summary(counts, sums))
+        if self._pose_threshold is not None:
+            print(pose_metrics_summary(counts, sums, self._ms["pose_sums"].cpu().numpy(), self._ms["success"].cpu().numpy()))
         print(f"============ per-motion statistics written to {path} ============")
         return path
+
+    def _pose_metrics_keys(self):
+        """the pose metrics' keys of the file (none without b200_pose_metrics)"""
+        if self._pose_threshold is None:
+            return {}
+        ps = self._ms["pose_sums"].cpu().numpy()
+        return dict(mpjpe_l_sum=ps[:, 0], mpjpe_pa_sum=ps[:, 1], vel_err_sum=ps[:, 2], acc_err_sum=ps[:, 3],
+                    vel_frames=ps[:, 4].astype(np.int64), acc_frames=ps[:, 5].astype(np.int64), success=self._ms["success"].cpu().numpy(),
+                    max_body_pos_err=ps[:, 6], success_threshold=np.float64(self._pose_threshold), dt=np.float64(self.dt))
+
+    def clear_motion_stats_games(self):
+        """a game starts: the per-env sums, flags and pose history start again; the per-motion buckets run on"""
+        for k in ("env_sums", "env_flags", "env_pose", "pose_fill"):
+            if k in self._ms:
+                self._ms[k].zero_()
 
     def policy_rows(self):
         """the operand launch: policy.x and the residual from obs_buf and the context slot context_padding + step % context_length"""
@@ -320,8 +379,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                 st[k].zero_()
             st["games"][1:].zero_()            # stop flag and log rows; games_played and the totals run on
             if self._ms is not None:           # the games of the last run are folded; the buckets run on
-                self._ms["env_sums"].zero_()
-                self._ms["env_flags"].zero_()
+                self.clear_motion_stats_games()
             if self._rec is not None:          # render_vis(init=True): the host reads the frame counter once per game
                 self._record_launch(True, games=st["games"])
                 if int(self._rec["frame"]) >= self._rec_cap:
