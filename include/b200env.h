@@ -215,6 +215,14 @@ typedef struct b200_reset_masked {
   uint32_t xf_joint_mask;
   float xf_noisy_prob, xf_noise_std, xf_conf_std, xf_min_conf, xf_random_prob;
   int32_t feat_width;
+  /* window offset of a game restarted mid-run (b200env_im_motion_queue), appended within ABI version 11; step NULL = the window above.
+   * With step set, s = step[0] % context_length and the window of env e is the one b200env_motion_context writes for (e, motion_ids[e],
+   * reset_times[e], num_frames, first_frame - s, dt): frame j at t = reset_times[e] + dt + (first_frame - s + j) dt.  The policy reads
+   * slot context_padding + step % context_length (b200env_im_policy_rows), so the restarted game's next step reads the frame at
+   * reset_times[e] + dt, bit for bit the frame a game the full reset started reads at step 0.  Frames before time 0 clamp to frame 0. */
+  const int64_t* step;     /* [1] b200_play_stats_t::step, or NULL */
+  int32_t context_length;  /* >= 1 when step is set */
+  int32_t pad_;
 } b200_reset_masked_t;
 int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* stream);
 
@@ -310,7 +318,9 @@ int b200env_im_policy_rows(b200env_handle h, const b200_im_policy_t* d, void* st
  * When any step_done is set: totals += (sum cr, sum steps) over them (double), games[0] += their count, cr *= 1 - done,
  * steps *= 1 - done, and (count, sum cr, sum steps) is appended to log [max_log, 3] at row games[2] (games[2] += 1; a full log keeps
  * counting but writes nothing).  The float sums are summed in float32, like the reference's cr[done].sum().  Then prev_done = done,
- * games[1] (stop) = games[0] >= n_games or done of env 0, and step[0] += 1.  While games[1] is set the call changes nothing. */
+ * games[1] (stop) = games[0] >= n_games or done of env 0, and step[0] += 1.  While games[1] is set the call changes nothing.
+ * Queue form (queue_games > 0, b200env_im_motion_queue): games[1] = games[0] >= queue_games instead; env 0's done does not stop the
+ * run, since a finished env takes the next queued game. */
 typedef struct b200_play_stats {
   int32_t n;
   int32_t max_log;
@@ -324,9 +334,53 @@ typedef struct b200_play_stats {
   double* log;             /* [max_log, 3] */
   int64_t* games;          /* [3]: games_played, stop, log rows */
   int64_t* step;           /* [1] */
+  int64_t queue_games;     /* appended within ABI version 11: 0 = the rule above, else the queued games of the run (R M) */
 } b200_play_stats_t;
 
 int b200env_play_stats(const b200_play_stats_t* d, void* stream);
+/* sizeof(b200_play_stats_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_play_stats_desc_size(void);
+
+/* The motion queue of an imitation test run over a library larger than the env count (HumanoidSMPLIMVis with
+ * cfg.env.b200_motion_queue; an addition, the reference's ImitatorPlayer.run never resets an env mid-game).  The queue holds the
+ * entries q = r M + m (r < R rounds, m < M motions) in that order; entries below *cursor are taken.  One CTA walks the envs in env
+ * order, in chunks of its threads: the k-th env (k = 0, 1, ...) whose reset_buf is set and whose idle byte is clear gets entry
+ * q = *cursor + k when q < queue_len, and then
+ *   motion_ids[e] = q % M, entry[e] = q, motion_bodies[e] = lib_motion_bodies[q % M], game_env[q] = e, game_start_step[q] = step[0]
+ *   (the step counter b200env_play_stats advanced: the index of the new game's first step), mask[e] = 1, and the done memory of
+ *   the new game is cleared, prev_dones[e] = 0 (b200_play_stats_t) and env_flags[e, 0] = 0 (b200_im_motion_stats_t, when given),
+ *   as the host clears them before a full reset, so a game that ends on its first step is counted too;
+ * otherwise (the queue is empty) idle[e] = 1: the env is never reset again and its reset_buf stays set (the step keeps a done env
+ * done), so the bookkeeping counts its last game once.  mask[e] = 0 for every other env, and *cursor advances once, by the entries
+ * taken.  No atomics: the same flags give the same assignment.  The caller then resets the masked envs (b200env_reset_masked with
+ * its step field, so each restarted window is aligned with the policy's slot).  games: b200_play_stats_t::games or NULL; while
+ * games[1] (stop) is set the launch clears the mask and changes nothing else.  Returns -1 on a NULL pointer but games and env_flags,
+ * -2 before
+ * any launch when n, num_motions or queue_len is not positive, or shape_dim is outside [0, 32]. */
+typedef struct b200_im_motion_queue {
+  int32_t n;                       /* envs */
+  int32_t num_motions;             /* M */
+  int64_t queue_len;               /* R M */
+  int32_t shape_dim;               /* columns of motion_bodies */
+  int32_t pad_;
+  const int64_t* reset_buf;        /* [n] */
+  const float* lib_motion_bodies;  /* [M, shape_dim] */
+  int64_t* motion_ids;             /* [n] */
+  float* motion_bodies;            /* [n, shape_dim] */
+  int64_t* entry;                  /* [n]: the entry each env plays */
+  uint8_t* mask;                   /* [n]: the envs to reset */
+  uint8_t* idle;                   /* [n] */
+  int64_t* cursor;                 /* [1] */
+  int64_t* game_env;               /* [queue_len] */
+  int64_t* game_start_step;        /* [queue_len] */
+  const int64_t* step;             /* [1] b200_play_stats_t::step */
+  const int64_t* games;            /* [3] or NULL */
+  float* prev_dones;               /* [n] b200_play_stats_t::prev_dones */
+  int32_t* env_flags;              /* [n, 2] b200_im_motion_stats_t::env_flags, or NULL */
+} b200_im_motion_queue_t;
+int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream);
+/* sizeof(b200_im_motion_queue_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_im_motion_queue_desc_size(void);
 
 /* One recorded frame of HumanoidSMPLIMVis._sync_ref_motion (embodied_pose/env/tasks/humanoid_smpl_im_vis.py:128-152) for every listed
  * env: the qpos the reference's MuJoCo viewer shows, without the viewer.  One warp per recorded env i (row env_ids[i]); frame
@@ -435,6 +489,19 @@ typedef struct b200_im_motion_stats_desc {
 int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream);
 /* sizeof(b200_im_motion_stats_t) as the library was built; the binding refuses a library whose size differs from its own */
 int32_t b200env_im_motion_stats_desc_size(void);
+
+/* The same meters with the motion queue (b200env_im_motion_queue): the rows of counts, sums, pose_sums and success are the queue's
+ * entries (meters.num_motions = R M rows) and meters.motion_start / motion_envs are not read (may be NULL).  The accumulate launch is
+ * the one above; the fold, one thread per env, adds each game that ended in this step to row env_entry[e], which must lie in
+ * [0, R M), with the column rules above.  Every entry is played once, so every row has one writer and needs no atomics.  Refusals of
+ * b200env_im_motion_stats, and -1 when env_entry is NULL. */
+typedef struct b200_im_motion_queue_stats {
+  b200_im_motion_stats_t meters;
+  const int64_t* env_entry;        /* [n]: the entry each env plays */
+} b200_im_motion_queue_stats_t;
+int b200env_im_motion_queue_stats(const b200_im_motion_queue_stats_t* d, void* stream);
+/* sizeof(b200_im_motion_queue_stats_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_im_motion_queue_stats_desc_size(void);
 
 /* Physics-only control step on caller-provided arrays, float (prec=0) or double (prec=1): a separate test launch
  * (physics_kernel_packed; physics_kernel_tmem / physics_kernel for the other forms) that shares the control step

@@ -305,9 +305,20 @@ class PlayStats(C.Structure):
     _fields_ = [
         ("n", C.c_int32), ("max_log", C.c_int32), ("n_games", C.c_int64),
         ("rew", F32P), ("reset_buf", I64P), ("cr", F32P), ("steps", F32P), ("prev_dones", F32P), ("totals", F64P), ("log", F64P),
-        ("games", I64P), ("step", I64P),
+        ("games", I64P), ("step", I64P), ("queue_games", C.c_int64),
     ]
-    _nullable_, _defaults_ = (), ()
+    _nullable_, _defaults_ = (), ("queue_games",)
+
+
+class ImMotionQueue(C.Structure):
+    """b200_im_motion_queue_t: the motion queue of an imitation test run (b200env_im_motion_queue)"""
+    _fields_ = [
+        ("n", C.c_int32), ("num_motions", C.c_int32), ("queue_len", C.c_int64), ("shape_dim", C.c_int32), ("pad_", C.c_int32),
+        ("reset_buf", I64P), ("lib_motion_bodies", F32P), ("motion_ids", I64P), ("motion_bodies", F32P), ("entry", I64P), ("mask", U8P),
+        ("idle", U8P), ("cursor", I64P), ("game_env", I64P), ("game_start_step", I64P), ("step", I64P), ("games", I64P),
+        ("prev_dones", F32P), ("env_flags", I32P),
+    ]
+    _nullable_, _defaults_ = ("games", "env_flags"), ("pad_",)
 
 
 class ImRecord(C.Structure):
@@ -334,6 +345,14 @@ class ImMotionStats(C.Structure):
     ]
     _nullable_ = ("games", "env_pose", "pose_hist", "pose_fill", "pose_sums", "success")
     _defaults_ = ("success_threshold",)
+
+
+class ImMotionQueueStats(C.Structure):
+    """b200_im_motion_queue_stats_t: the per-motion meters folded by queue entry (b200env_im_motion_queue_stats); the fields of
+    b200_im_motion_stats_t (its first member) and env_entry"""
+    _fields_ = ImMotionStats._fields_ + [("env_entry", I64P)]
+    _nullable_ = ImMotionStats._nullable_ + ("motion_start", "motion_envs")
+    _defaults_ = ImMotionStats._defaults_
 
 
 # the context window's transform program (include/b200env.h: b200_motion_context_t), appended to b200_reset_masked_t and
@@ -386,8 +405,8 @@ class ResetMasked(C.Structure):
         ("first_frame", C.c_int32), ("dt", C.c_float), ("seed", C.c_uint64),
         ("mask", U8P), ("counter", I64P), ("init_root", F32P), ("init_dof_pos", F32P), ("init_dof_vel", F32P), ("reset_times", F32P),
         ("context_feat", F32P), ("context_mask", U8P), ("work", I32P),
-    ] + _XF_FIELDS
-    _nullable_, _defaults_ = ("init_root", "init_dof_pos", "init_dof_vel"), _XF_DEFAULTS
+    ] + _XF_FIELDS + [("step", I64P), ("context_length", C.c_int32), ("pad_", C.c_int32)]
+    _nullable_, _defaults_ = ("init_root", "init_dof_pos", "init_dof_vel", "step"), _XF_DEFAULTS + ("context_length", "pad_")
 
 
 class MotionState(C.Structure):
@@ -698,6 +717,11 @@ SIGNATURES = {
     "b200env_motion_context_desc_size": (_i32, []),
     "b200env_im_policy_rows": (C.c_int, [_p, _p, _p]),
     "b200env_play_stats": (C.c_int, [_p, _p]),
+    "b200env_play_stats_desc_size": (_i32, []),
+    "b200env_im_motion_queue": (C.c_int, [_p, _p]),
+    "b200env_im_motion_queue_desc_size": (_i32, []),
+    "b200env_im_motion_queue_stats": (C.c_int, [_p, _p]),
+    "b200env_im_motion_queue_stats_desc_size": (_i32, []),
     "b200env_im_record": (C.c_int, [_p, _p]),
     "b200env_im_record_desc_size": (_i32, []),
     "b200env_im_motion_stats": (C.c_int, [_p, _p]),

@@ -1796,15 +1796,17 @@ motion_context_xf_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __
 // b200env_reset_masked, second launch: the window of every env on the work list of reset_masked_kernel at its drawn time, warp per
 // (env, frame) over a grid of fixed size (the list's length is only known on the device).  The last block to finish clears the list
 // and advances the launch counter, so the pair of launches replays inside a CUDA graph with fresh draws every time.  XF: with the
-// transform program, drawing at the counter value both launches read.
-template <bool XF>
+// transform program, drawing at the counter value both launches read.  OFS: the window of a game restarted at step counter s starts
+// s % context_length frames earlier (include/b200env.h: b200_reset_masked_t::step).
+template <bool XF, bool OFS = false>
 __device__ __forceinline__ void reset_context_body(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, const b200_motion_lib_t& ml,
                                                    const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work,
                                                    int64_t* counter, int P, int first, float dt, float two_dt, float* __restrict__ feat,
-                                                   uint8_t* __restrict__ mask, const ContextXf& xf) {
+                                                   uint8_t* __restrict__ mask, const ContextXf& xf, const int64_t* step = nullptr, int len = 1) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t total = (int64_t)work[0] * P;
   const uint64_t c = XF ? (uint64_t)counter[0] : 0;
+  if constexpr (OFS) first -= (int)(step[0] % len);
   for (int64_t w = (int64_t)blockIdx.x * WARPS_PER_CTA + warp; w < total; w += (int64_t)gridDim.x * WARPS_PER_CTA) {
     const int64_t i = w / P;
     const int j = (int)(w - i * P);
@@ -1828,6 +1830,21 @@ reset_context_xf_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __r
                         const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
                         int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask, ContextXf xf) {
   reset_context_body<true>(gblob, gcfg, ml, motion_ids, reset_times, work, counter, P, first, dt, two_dt, feat, mask, xf);
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_context_ofs_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                         const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter, int P,
+                         int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask, const int64_t* __restrict__ step,
+                         int len) {
+  reset_context_body<false, true>(gblob, gcfg, ml, motion_ids, reset_times, work, counter, P, first, dt, two_dt, feat, mask, ContextXf{}, step,
+                                  len);
+}
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
+reset_context_ofs_xf_kernel(const DevBlob* __restrict__ gblob, const b200_cfg_t* __restrict__ gcfg, b200_motion_lib_t ml,
+                            const int64_t* __restrict__ motion_ids, const float* __restrict__ reset_times, int32_t* work, int64_t* counter,
+                            int P, int first, float dt, float two_dt, float* __restrict__ feat, uint8_t* __restrict__ mask, ContextXf xf,
+                            const int64_t* __restrict__ step, int len) {
+  reset_context_body<true, true>(gblob, gcfg, ml, motion_ids, reset_times, work, counter, P, first, dt, two_dt, feat, mask, xf, step, len);
 }
 
 // compute_humanoid_observations_imitation (humanoid_smpl_im.py:773-850): warp per env, lane per body
@@ -2016,6 +2033,7 @@ obs_imitation_kernel(int n, int nb, int nd, int shape_dim, const float* __restri
 // b200env_play_stats: ImitatorPlayer.run's bookkeeping of one step, one CTA; thread i takes envs i, i + PLAY_THREADS, ... and the partial
 // sums meet in a fixed tree, so a replay gives the same sums
 #define PLAY_THREADS 1024
+template <bool QUEUE>   // QUEUE: the stop rule of the motion queue (b200_play_stats_t::queue_games)
 __global__ void __launch_bounds__(PLAY_THREADS) play_stats_kernel(b200_play_stats_t d) {
   __shared__ float s_cr[PLAY_THREADS], s_st[PLAY_THREADS];
   __shared__ int s_cnt[PLAY_THREADS];
@@ -2053,7 +2071,8 @@ __global__ void __launch_bounds__(PLAY_THREADS) play_stats_kernel(b200_play_stat
       }
       d.games[2] += 1;
     }
-    d.games[1] = (d.games[0] >= d.n_games || d.reset_buf[0] != 0) ? 1 : 0;
+    if constexpr (QUEUE) d.games[1] = d.games[0] >= d.queue_games ? 1 : 0;
+    else d.games[1] = (d.games[0] >= d.n_games || d.reset_buf[0] != 0) ? 1 : 0;
     d.step[0] += 1;
   }
 }
@@ -2390,6 +2409,83 @@ __global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_stats_fold_kernel(b
       q.success[m] += t;
     }
   }
+}
+
+// the fold of the motion queue (b200_im_motion_stats_t::env_entry): one thread per env adds the game that ended in this step to the row
+// of its entry; each entry is played once, so each row has one writer and the sums need no atomics
+template <bool POSE, typename... Pose>
+__global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_queue_fold_kernel(b200_im_motion_meters_t d, const int64_t* __restrict__ entry,
+                                                                              Pose... pose) {
+  if (d.games && d.games[1]) return;
+  const int64_t e = (int64_t)blockIdx.x * MS_FOLD_THREADS + threadIdx.x;
+  if (e >= d.n) return;
+  const int32_t ended = d.env_flags[2 * e + 1];
+  if (!ended) return;
+  const int64_t row = entry[e];
+  d.counts[2 * row] += 1;
+  d.counts[2 * row + 1] += ended == 2;
+  double* es = d.env_sums + e * MS_COLS;
+#pragma unroll
+  for (int k = 0; k < MS_COLS; k++) { d.sums[row * MS_COLS + k] += es[k]; es[k] = 0.0; }
+  if constexpr (POSE) {
+    const MsPose& q = ms_pose(pose...);
+    double* ep = q.env_pose + e * MS_POSE_COLS;
+    double* ps = q.sums + row * MS_POSE_COLS;
+#pragma unroll
+    for (int k = 0; k < MS_POSE_COLS - 1; k++) { ps[k] += ep[k]; ep[k] = 0.0; }
+    q.success[row] += ep[MS_POSE_COLS - 1] <= q.threshold;
+    ps[MS_POSE_COLS - 1] = ms_max(ps[MS_POSE_COLS - 1], ep[MS_POSE_COLS - 1]);
+    ep[MS_POSE_COLS - 1] = 0.0;
+  }
+  d.env_flags[2 * e + 1] = 0;
+}
+
+// b200env_im_motion_queue: one CTA walks the envs in chunks of QUEUE_THREADS; a block-wide exclusive count (ballots, then the warp
+// totals in shared memory) gives each finished env its rank k in env order, so the assignment depends on the flags alone
+#define QUEUE_THREADS 1024
+__global__ void __launch_bounds__(QUEUE_THREADS) im_motion_queue_kernel(b200_im_motion_queue_t d) {
+  __shared__ int s_warp[QUEUE_THREADS / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool stopped = d.games && d.games[1];
+  const int64_t cursor = d.cursor[0], step = d.step[0];
+  int64_t base = 0;                                      // finished envs before this chunk
+  for (int64_t c0 = 0; c0 < d.n; c0 += QUEUE_THREADS) {
+    const int64_t e = c0 + tid;
+    const bool fin = !stopped && e < d.n && d.reset_buf[e] != 0 && !d.idle[e];
+    const unsigned bal = __ballot_sync(0xffffffffu, fin);
+    if (lane == 0) s_warp[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll 8
+    for (int w = 0; w < QUEUE_THREADS / 32; w++) {
+      const int c = s_warp[w];
+      before += w < warp ? c : 0;
+      total += c;
+    }
+    __syncthreads();                                     // s_warp is rewritten by the next chunk
+    if (e < d.n) {
+      uint8_t m = 0;
+      if (fin) {
+        const int64_t q = cursor + base + before + __popc(bal & ((1u << lane) - 1u));
+        if (q < d.queue_len) {
+          const int64_t mid = q % d.num_motions;
+          d.motion_ids[e] = mid;
+          d.entry[e] = q;
+          for (int k = 0; k < d.shape_dim; k++) d.motion_bodies[e * d.shape_dim + k] = d.lib_motion_bodies[mid * d.shape_dim + k];
+          d.game_env[q] = e;
+          d.game_start_step[q] = step;
+          d.prev_dones[e] = 0.f;
+          if (d.env_flags) d.env_flags[2 * e] = 0;
+          m = 1;
+        } else {
+          d.idle[e] = 1;
+        }
+      }
+      d.mask[e] = m;
+    }
+    base += total;
+  }
+  if (tid == 0 && !stopped) d.cursor[0] = min(cursor + base, d.queue_len);
 }
 
 // physics-only entry used by the parity tests (float or double)
@@ -3064,6 +3160,7 @@ int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* s
   if (d->ref_prob < 1.0f && (!d->init_root || !d->init_dof_pos || !d->init_dof_vel))
     return fail(-1, "b200env_reset_masked: ref_prob < 1 needs the initial root and dof buffers%s");
   if (!h->bound || !h->has_ml) return fail(-4, "b200env_reset_masked: bind buffers and a motion lib first%s");
+  if (d->step && d->context_length < 1) return fail(-2, "b200env_reset_masked: the window offset needs context_length >= 1%s");
   ContextXf xf;
   bool xf_on = false;
   if (int rc = context_xf("b200env_reset_masked", h, d, d->counter, &xf, &xf_on)) return rc;
@@ -3077,7 +3174,16 @@ int b200env_reset_masked(b200env_handle h, const b200_reset_masked_t* d, void* s
   CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
   const int64_t warps = (int64_t)n * d->num_frames;
   const int grid = (int)std::min<int64_t>((warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA, (int64_t)sms * 8);
-  if (xf_on)
+  const float two_dt = (float)(2.0 * (double)d->dt);
+  if (d->step && xf_on)
+    reset_context_ofs_xf_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+        (const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids, d->reset_times, d->work, d->counter, d->num_frames, d->first_frame,
+        d->dt, two_dt, d->context_feat, d->context_mask, xf, d->step, d->context_length);
+  else if (d->step)
+    reset_context_ofs_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>(
+        (const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids, d->reset_times, d->work, d->counter, d->num_frames, d->first_frame,
+        d->dt, two_dt, d->context_feat, d->context_mask, d->step, d->context_length);
+  else if (xf_on)
     reset_context_xf_kernel<<<grid, WARPS_PER_CTA * 32, 0, (cudaStream_t)stream>>>((const DevBlob*)h->d_blob, h->d_cfg, h->ml, h->bufs.motion_ids,
                                                                                    d->reset_times, d->work, d->counter, d->num_frames,
                                                                                    d->first_frame, d->dt, (float)(2.0 * (double)d->dt),
@@ -3252,10 +3358,30 @@ int b200env_play_stats(const b200_play_stats_t* d, void* stream) {
   if (!d || !d->rew || !d->reset_buf || !d->cr || !d->steps || !d->prev_dones || !d->totals || !d->log || !d->games || !d->step)
     return fail(-1, "b200env_play_stats: null argument%s");
   if (d->n <= 0 || d->max_log < 1) return fail(-2, "b200env_play_stats: n and max_log must be positive%s");
-  play_stats_kernel<<<1, PLAY_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  if (d->queue_games < 0) return fail(-2, "b200env_play_stats: queue_games must not be negative%s");
+  if (d->queue_games > 0)
+    play_stats_kernel<true><<<1, PLAY_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  else
+    play_stats_kernel<false><<<1, PLAY_THREADS, 0, (cudaStream_t)stream>>>(*d);
   CUDA_OK(cudaGetLastError());
   return 0;
 }
+
+int32_t b200env_play_stats_desc_size(void) { return (int32_t)sizeof(b200_play_stats_t); }
+
+int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream) {
+  if (!d || !d->reset_buf || !d->lib_motion_bodies || !d->motion_ids || !d->motion_bodies || !d->entry || !d->mask || !d->idle || !d->cursor ||
+      !d->game_env || !d->game_start_step || !d->step || !d->prev_dones)
+    return fail(-1, "b200env_im_motion_queue: null argument%s");
+  if (d->n <= 0 || d->num_motions <= 0 || d->queue_len <= 0)
+    return fail(-2, "b200env_im_motion_queue: n, num_motions and queue_len must be positive%s");
+  if (d->shape_dim < 0 || d->shape_dim > 32) return fail(-2, "b200env_im_motion_queue: shape_dim must lie in [0, 32]%s");
+  im_motion_queue_kernel<<<1, QUEUE_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int32_t b200env_im_motion_queue_desc_size(void) { return (int32_t)sizeof(b200_im_motion_queue_t); }
 
 int b200env_im_record(const b200_im_record_t* d, void* stream) {
   if (!d || !d->env_ids || !d->rigid_body_state || !d->dof_state || !d->p_dof_pos || !d->p_rb_pos || !d->p_rb_rot || !d->reset_buf ||
@@ -3272,37 +3398,57 @@ int b200env_im_record(const b200_im_record_t* d, void* stream) {
 
 int32_t b200env_im_record_desc_size(void) { return (int32_t)sizeof(b200_im_record_t); }
 
-int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream) {
+// b200env_im_motion_stats (env_entry NULL) and b200env_im_motion_queue_stats: the same checks and accumulate launch, then the fold by
+// motion or by entry
+static int motion_stats_launch(const char* who, const b200_im_motion_stats_t* d, const int64_t* env_entry, void* stream) {
   if (!d || !d->rew || !d->sub_rewards || !d->reset_buf || !d->terminate_buf || !d->rigid_body_state || !d->target_rb_pos ||
-      !d->motion_start || !d->motion_envs || !d->env_sums || !d->env_flags || !d->counts || !d->sums)
-    return fail(-1, "b200env_im_motion_stats: null argument%s");
-  if (d->n <= 0 || d->num_motions <= 0) return fail(-2, "b200env_im_motion_stats: n and num_motions must be positive%s");
+      (!env_entry && (!d->motion_start || !d->motion_envs)) || !d->env_sums || !d->env_flags || !d->counts || !d->sums)
+    return fail(-1, "%s: null argument", who);
+  if (d->n <= 0 || d->num_motions <= 0) return fail(-2, "%s: n and num_motions must be positive", who);
   if (d->num_lib_bodies < 1 || d->num_lib_bodies > d->num_bodies)
-    return fail(-2, "b200env_im_motion_stats: num_lib_bodies must lie in [1, num_bodies]%s");
+    return fail(-2, "%s: num_lib_bodies must lie in [1, num_bodies]", who);
   const bool pose = d->env_pose || d->pose_hist || d->pose_fill || d->pose_sums || d->success;
   if (pose && (!d->env_pose || !d->pose_hist || !d->pose_fill || !d->pose_sums || !d->success))
-    return fail(-1, "b200env_im_motion_stats: the pose pointers must be all set or all NULL%s");
-  if (pose && d->num_lib_bodies > 32) return fail(-2, "b200env_im_motion_stats: the pose metrics take at most 32 bodies%s");
+    return fail(-1, "%s: the pose pointers must be all set or all NULL", who);
+  if (pose && d->num_lib_bodies > 32) return fail(-2, "%s: the pose metrics take at most 32 bodies", who);
   if (pose && !(d->success_threshold > 0.0 && isfinite(d->success_threshold)))
-    return fail(-2, "b200env_im_motion_stats: success_threshold must be a finite positive number of metres%s");
+    return fail(-2, "%s: success_threshold must be a finite positive number of metres", who);
   static_assert(offsetof(b200_im_motion_stats_t, env_pose) == sizeof(b200_im_motion_meters_t), "the meters' fields lead");
   b200_im_motion_meters_t m;
   memcpy(&m, d, sizeof m);
   const int acc_blocks = (d->n + MS_WARPS - 1) / MS_WARPS;
   cudaStream_t st = (cudaStream_t)stream;
+  const int queue_blocks = (d->n + MS_FOLD_THREADS - 1) / MS_FOLD_THREADS;
   if (pose) {
     const MsPose q = {d->env_pose, d->pose_hist, d->pose_fill, d->pose_sums, d->success, d->success_threshold};
     im_motion_stats_acc_kernel<true><<<acc_blocks, MS_WARPS * 32, 0, st>>>(m, q);
     CUDA_OK(cudaGetLastError());
-    im_motion_stats_fold_kernel<true><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m, q);
+    if (env_entry)
+      im_motion_queue_fold_kernel<true><<<queue_blocks, MS_FOLD_THREADS, 0, st>>>(m, env_entry, q);
+    else
+      im_motion_stats_fold_kernel<true><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m, q);
   } else {
     im_motion_stats_acc_kernel<false><<<acc_blocks, MS_WARPS * 32, 0, st>>>(m);
     CUDA_OK(cudaGetLastError());
-    im_motion_stats_fold_kernel<false><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m);
+    if (env_entry)
+      im_motion_queue_fold_kernel<false><<<queue_blocks, MS_FOLD_THREADS, 0, st>>>(m, env_entry);
+    else
+      im_motion_stats_fold_kernel<false><<<d->num_motions, MS_FOLD_THREADS, 0, st>>>(m);
   }
   CUDA_OK(cudaGetLastError());
   return 0;
 }
+
+int b200env_im_motion_stats(const b200_im_motion_stats_t* d, void* stream) {
+  return motion_stats_launch("b200env_im_motion_stats", d, nullptr, stream);
+}
+
+int b200env_im_motion_queue_stats(const b200_im_motion_queue_stats_t* d, void* stream) {
+  if (!d || !d->env_entry) return fail(-1, "b200env_im_motion_queue_stats: null argument%s");
+  return motion_stats_launch("b200env_im_motion_queue_stats", &d->meters, d->env_entry, stream);
+}
+
+int32_t b200env_im_motion_queue_stats_desc_size(void) { return (int32_t)sizeof(b200_im_motion_queue_stats_t); }
 
 int32_t b200env_im_motion_stats_desc_size(void) { return (int32_t)sizeof(b200_im_motion_stats_t); }
 

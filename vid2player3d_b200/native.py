@@ -29,6 +29,8 @@ def lib():
         for S, size in ((abi.ResetMasked, L.b200env_reset_masked_desc_size()), (abi.MotionContext, L.b200env_motion_context_desc_size()),
                         (abi.ImRecord, L.b200env_im_record_desc_size()), (abi.V2PTaskReset, L.b200v2p_task_reset_desc_size()),
                         (abi.ImMotionStats, L.b200env_im_motion_stats_desc_size()),
+                        (abi.PlayStats, L.b200env_play_stats_desc_size()), (abi.ImMotionQueue, L.b200env_im_motion_queue_desc_size()),
+                        (abi.ImMotionQueueStats, L.b200env_im_motion_queue_stats_desc_size()),
                         (abi.V2PBallStats, L.b200v2p_eval_ball_stats_desc_size()),
                         (abi.V2PRallyStats, L.b200v2p_eval_rally_stats_desc_size())):
             if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
@@ -123,6 +125,19 @@ def im_motion_stats(scalars, tensors):
     abi.ImMotionStats"""
     d = fill(abi.ImMotionStats, scalars, tensors)
     _check(lib().b200env_im_motion_stats(C.byref(d), _stream()))
+
+
+def im_motion_queue_stats(scalars, tensors):
+    """the per-motion meters of one test step folded by queue entry (include/b200env.h: b200env_im_motion_queue_stats); the fields of
+    abi.ImMotionQueueStats"""
+    d = fill(abi.ImMotionQueueStats, scalars, tensors)
+    _check(lib().b200env_im_motion_queue_stats(C.byref(d), _stream()))
+
+
+def im_motion_queue(scalars, tensors):
+    """one assignment of the motion queue on the device (include/b200env.h: b200env_im_motion_queue); the fields of abi.ImMotionQueue"""
+    d = fill(abi.ImMotionQueue, scalars, tensors)
+    _check(lib().b200env_im_motion_queue(C.byref(d), _stream()))
 
 
 def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):
@@ -240,15 +255,16 @@ class Env:
             _check(lib().b200env_reset(self._h, _ptr(env_ids), _ptr(motion_times), n, _stream()))
 
     def reset_masked(self, mask, sample_time, truncate, ref_prob, seed, counter, init_root, init_dof_pos, init_dof_vel, reset_times,
-                     num_frames, first_frame, dt, feat, feat_mask, work, transforms=None):
+                     num_frames, first_frame, dt, feat, feat_mask, work, transforms=None, step=None, context_length=None):
         """reset of the envs whose mask [N] bool is set, context window included (include/b200env.h: b200env_reset_masked);
-        transforms: the window's transform program (abi.transform_program), with feat rows W + bodies wide"""
+        transforms: the window's transform program (abi.transform_program), with feat rows W + bodies wide; step ([1] int64, the
+        bookkeeping's step counter) with context_length: each window starts step % context_length frames earlier"""
         assert mask.shape[0] == self.num_envs and work.shape[0] >= self.num_envs + 2
         xf = dict(transforms, feat_width=int(feat.shape[-1])) if transforms is not None else {}
         d = fill(abi.ResetMasked, dict(xf, sample_time=int(bool(sample_time)), truncate=truncate, ref_prob=ref_prob, num_frames=num_frames,
-                                       first_frame=first_frame, dt=dt, seed=int(seed)),
+                                       first_frame=first_frame, dt=dt, seed=int(seed), context_length=context_length),
                  dict(mask=mask, counter=counter, init_root=init_root, init_dof_pos=init_dof_pos, init_dof_vel=init_dof_vel,
-                      reset_times=reset_times, context_feat=feat, context_mask=feat_mask, work=work))
+                      reset_times=reset_times, context_feat=feat, context_mask=feat_mask, work=work, step=step))
         _check(lib().b200env_reset_masked(self._h, C.byref(d), _stream()))
 
     def motion_state(self, ids, times, out):

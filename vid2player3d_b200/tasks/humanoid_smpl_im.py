@@ -115,9 +115,13 @@ class HumanoidSMPLIM(BaseTask):
         if self._test_motion_file is not None and "motion_assets" in env and len(env["motion_assets"]) != flat.num_motions():
             raise ValueError(f"test_motion_assets has {len(env['motion_assets'])} entries for the {flat.num_motions()} motions of "
                              f"test_motion_file {self._test_motion_file}")
+        self._check_motion_lib(flat)
         self._motion_lib = flat
         dev = self.device
         self._ml_t = {k: torch.from_numpy(getattr(flat, k)).to(dev).contiguous() for k in FlatMotionLib.FIELDS}
+
+    def _check_motion_lib(self, flat):
+        """refusals that need the loaded library, before it goes to the device (none here)"""
 
     def _load_asset(self):
         name = os.path.splitext(os.path.basename(self.cfg["env"]["asset"]["assetFileName"]))[0]
@@ -387,14 +391,15 @@ class HumanoidSMPLIM(BaseTask):
         self._reset_ref_env_ids = env_ids
         self._init_context(env_ids, motion_ids, motion_times)
 
-    def reset_masked(self, mask):
+    def reset_masked(self, mask, step=None):
         """Addition (not in the reference): `reset(mask.nonzero())` without the id list - the envs whose entry of `mask` ([num_envs]
         bool, device) is set are reset by two launches (include/b200env.h: b200env_reset_masked) that make no host synchronisation,
         so the call can be captured in a CUDA graph.  Same state init, rows and context window as `reset(env_ids)`; the motion
         times and the Hybrid choice are drawn on the device from a counter-based generator seeded by cfg["seed"], a different stream
         of the same distribution as the torch.rand / torch.bernoulli draws of `reset(env_ids)`.  With cfg.env.transform_specs only under
         cfg.env.b200_device_transforms (the window launch applies them, drawing at the same counter); otherwise the transforms are torch
-        ops on the reset rows: use `reset(env_ids)` there."""
+        ops on the reset rows: use `reset(env_ids)` there.  step: a device step counter ([1] int64) the policy reads its context slot
+        from; each window then starts step % context_length frames earlier, so the next slot read is the new game's first frame."""
         if self._transform_specs is not None and self._xf_program is None:
             raise ValueError("reset_masked: cfg.env.transform_specs transforms the context window in torch - use reset(env_ids), "
                              "or set cfg.env.b200_device_transforms")
@@ -408,7 +413,8 @@ class HumanoidSMPLIM(BaseTask):
         self._env.reset_masked(mask, sample_time, truncate, ref_prob, self.cfg.get("seed", 10), self._reset_rng,
                                self._initial_humanoid_root_states, self._initial_dof_pos, self._initial_dof_vel, self._reset_ref_motion_times,
                                self.context_length + self.context_padding * 2, -self.context_padding, self.dt, self.context_feat,
-                               self.context_mask, self._reset_work, transforms=self._xf_program)
+                               self.context_mask, self._reset_work, transforms=self._xf_program, step=step,
+                               context_length=self.context_length if step is not None else None)
         self._forward_context()
 
     def reset_done(self):

@@ -33,7 +33,14 @@ out/motion_stats/motion_stats_<date>.npz) and one summary line is printed.
 Pose metrics (cfg.env.b200_pose_metrics, an addition; needs b200_motion_stats): the same launch also sums, per finished game, the
 metrics motion-imitation work compares policies on - root-relative and Procrustes-aligned MPJPE, velocity and acceleration error - and
 counts the games whose largest body-position error (global MPJPE) stays within cfg.env.b200_pose_success_threshold (default 0.5 m).
-The file then also holds those sums, their frame counts, the successes and each motion's largest error, and a second line is printed."""
+The file then also holds those sums, their frame counts, the successes and each motion's largest error, and a second line is printed.
+
+Motion queue (cfg.env.b200_motion_queue, an addition; the reference never resets an env mid-game): a library larger than the env count
+is scored in one run.  The queue holds every motion once per round, R = cfg.env.b200_motion_queue_repeats rounds (default 1), entry
+q = r M + m; env e starts on entry e, and when its game ends it takes the next unplayed entry inside the step graph (include/b200env.h:
+b200env_im_motion_queue, then the masked reset with the window aligned to the policy's slot), with no host synchronisation.  An env
+that finishes once the queue is empty stays done.  run_test then runs one full reset and steps until every queued game has finished
+or max_steps steps have run; the per-motion meters fold each game into the row of its entry, and the file sums a motion's R rows."""
 import os
 from datetime import datetime
 
@@ -148,7 +155,45 @@ def motion_stats_summary(counts, sums):
             f"reward per step: {per_step[0]:.6f}  body position error: {per_step[1]:.6f} m")
 
 
+def motion_queue_rounds(cfg):
+    """cfg.env.b200_motion_queue -> None when off, else the rounds R of the queue (b200_motion_queue_repeats, default 1); refuses R
+    that is not an int >= 1, several assets (motion_assets), transform_specs without b200_device_transforms (the queue restarts
+    games through the masked reset) and a state init other than Start (every queued game starts at its motion's first frame)"""
+    env = cfg["env"]
+    if not env.get("b200_motion_queue", False):
+        return None
+    R = env.get("b200_motion_queue_repeats", 1)
+    if isinstance(R, bool) or not isinstance(R, (int, np.integer)) or R < 1:
+        raise ValueError(f"b200_motion_queue_repeats must be an int >= 1, got {R!r}")
+    if "motion_assets" in env:
+        raise ValueError("b200_motion_queue serves a handle of one asset; motion_assets (several assets) is not supported")
+    if "transform_specs" in env and not env.get("b200_device_transforms", False):
+        raise ValueError("b200_motion_queue restarts games through the masked reset: with transform_specs set b200_device_transforms")
+    args = cfg.get("args", None)
+    state_init = "Start" if args is not None and getattr(args, "test", False) else env.get("stateInit", "Hybrid")
+    if state_init != "Start":
+        raise ValueError(f"b200_motion_queue starts every game at its motion's first frame: needs args.test or stateInit: Start, "
+                         f"got {state_init!r}")
+    return int(R)
+
+
+def queue_fold(rows, R, M, max_col=None):
+    """the queue's per-entry rows [R M, ...] -> per motion [M, ...]: the R rows of motion m (entries r M + m) added in r order; column
+    max_col (the largest error) takes the largest instead, NaN if one is NaN"""
+    rows = np.asarray(rows).reshape(R, M, *np.shape(rows)[1:])
+    out = rows[0].copy()
+    for r in range(1, R):
+        if max_col is None:
+            out += rows[r]
+        else:
+            keep = out[..., max_col].copy()
+            out += rows[r]
+            out[..., max_col] = np.maximum(keep, rows[r][..., max_col])
+    return out
+
+
 class HumanoidSMPLIMVis(HumanoidSMPLIM):
+    _q = None               # the motion queue's device state (cfg.env.b200_motion_queue), set by set_policy
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         if not headless:
             raise ValueError("HumanoidSMPLIMVis: there is no MuJoCo viewer; run headless")
@@ -156,6 +201,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._rec = None
         rec_ids = None
         self._pose_threshold = pose_metrics_threshold(env)
+        self._queue_rounds = motion_queue_rounds(cfg)
         if env.get("b200_record_qpos", False):
             rec_ids = record_env_ids(env.get("b200_record_envs", [0]), int(env["numEnvs"]))
             if not getattr(cfg.get("args", None), "rec_once", False) and int(env.get("num_rec_frames", 300)) < 1:
@@ -169,6 +215,50 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._ms = None
         if rec_ids is not None:
             self._setup_record(rec_ids)
+
+    def _check_motion_lib(self, flat):
+        N = int(self.cfg["env"]["numEnvs"])
+        if self._queue_rounds is not None and N > flat.num_motions() * self._queue_rounds:
+            raise ValueError(f"b200_motion_queue: {N} envs for a queue of {flat.num_motions()} motions x {self._queue_rounds} rounds; every "
+                             "env starts on its own entry, so give at most as many envs as queued games")
+
+    def _sample_motion_ids(self):
+        """with the queue env e starts on entry e, motion e % M; else humanoid_smpl_im.py:247-254"""
+        if self._queue_rounds is None:
+            return super()._sample_motion_ids()
+        return torch.arange(self.num_envs, device=self.device) % self._motion_lib.num_motions()
+
+    def _setup_queue(self):
+        """the queue's device state: each env's entry, the idle flags, the cursor and, per entry, its env and first step"""
+        N, Q, dev = self.num_envs, self._motion_lib.num_motions() * self._queue_rounds, self.device
+        i64 = lambda n: torch.zeros(n, device=dev, dtype=torch.long)  # noqa: E731
+        self._q = dict(entry=i64(N), idle=torch.zeros(N, device=dev, dtype=torch.uint8), cursor=i64(1), game_env=i64(Q),
+                       game_start_step=i64(Q))
+
+    def _start_queue(self):
+        """before the run's full reset: env e on entry e, the rest of the queue unplayed"""
+        q, N = self._q, self.num_envs
+        e = torch.arange(N, device=self.device)
+        self._reset_ref_motion_ids.copy_(self._sample_motion_ids())
+        self._reset_ref_motion_bodies.copy_(self._ml_t["motion_bodies"][self._reset_ref_motion_ids])
+        q["entry"].copy_(e)
+        q["idle"].zero_()
+        q["cursor"].fill_(N)
+        q["game_env"].fill_(-1)
+        q["game_env"][:N] = e
+        q["game_start_step"].fill_(-1)
+        q["game_start_step"][:N] = 0
+
+    def _queue_launches(self):
+        """the assignment of the finished envs' next entries, then their masked reset with the window aligned to the step counter"""
+        M = self._motion_lib.num_motions()
+        native.im_motion_queue(dict(n=self.num_envs, num_motions=M, queue_len=M * self._queue_rounds,
+                                    shape_dim=self._reset_ref_motion_bodies.shape[1]),
+                               dict(self._q, reset_buf=self.reset_buf, lib_motion_bodies=self._ml_t["motion_bodies"],
+                                    motion_ids=self._reset_ref_motion_ids, motion_bodies=self._reset_ref_motion_bodies, mask=self._reset_mask,
+                                    step=self._im_step, games=self._stats["games"], prev_dones=self._stats["prev_dones"],
+                                    env_flags=self._ms["env_flags"] if self._ms is not None else None))
+        self.reset_masked(self._reset_mask, step=self._im_step)
 
     def _setup_record(self, ids):
         """the recorder's device buffers, after the cfg checks and the free-memory check"""
@@ -253,15 +343,22 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         self._stats_cap = cap
         self._n_games = 1 << 62            # run_test sets games_num * n_game_life
         self._im_graph = None
+        if self._queue_rounds is not None:
+            self._setup_queue()
         if self.cfg["env"].get("b200_motion_stats", False):
             self._setup_motion_stats()
 
     def _setup_motion_stats(self):
-        """the per-motion buckets and, from the env -> motion map the test run keeps, each motion's env list"""
+        """the per-motion buckets and, from the env -> motion map the test run keeps, each motion's env list; with the queue one row
+        per queued game, folded by its entry"""
         N, M, dev = self.num_envs, self._motion_lib.num_motions(), self.device
-        start, envs = motion_env_lists(self._reset_ref_motion_ids, M)
-        self._ms = dict(motion_start=torch.from_numpy(start).to(dev), motion_envs=torch.from_numpy(envs).to(dev),
-                        env_sums=torch.zeros(N, 7, device=dev, dtype=torch.float64),
+        if self._q is None:
+            start, envs = motion_env_lists(self._reset_ref_motion_ids, M)
+            self._ms = dict(motion_start=torch.from_numpy(start).to(dev), motion_envs=torch.from_numpy(envs).to(dev))
+        else:
+            M *= self._queue_rounds
+            self._ms = dict(env_entry=self._q["entry"])
+        self._ms.update(env_sums=torch.zeros(N, 7, device=dev, dtype=torch.float64),
                         env_flags=torch.zeros(N, 2, device=dev, dtype=torch.int32),
                         counts=torch.zeros(M, 2, device=dev, dtype=torch.long), sums=torch.zeros(M, 7, device=dev, dtype=torch.float64))
         if self._pose_threshold is not None:    # one warp per env, a lane per body
@@ -273,34 +370,46 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                             pose_sums=torch.zeros(M, 7, device=dev, dtype=torch.float64), success=torch.zeros(M, device=dev, dtype=torch.long))
 
     def _motion_stats_launch(self, games=None):
-        native.im_motion_stats(dict(n=self.num_envs, num_motions=self._motion_lib.num_motions(), num_bodies=self.num_bodies,
-                                    num_lib_bodies=self._num_lib_bodies, success_threshold=self._pose_threshold),
-                               dict(self._ms, rew=self.rew_buf, sub_rewards=self._sub_rewards, reset_buf=self.reset_buf,
-                                    terminate_buf=self._terminate_buf, rigid_body_state=self._rigid_body_state,
-                                    target_rb_pos=self._prev_target_rb_pos, games=games))
+        rows = self._motion_lib.num_motions() * (self._queue_rounds or 1)
+        launch = native.im_motion_stats if self._q is None else native.im_motion_queue_stats
+        launch(dict(n=self.num_envs, num_motions=rows, num_bodies=self.num_bodies, num_lib_bodies=self._num_lib_bodies,
+                    success_threshold=self._pose_threshold),
+               dict(self._ms, rew=self.rew_buf, sub_rewards=self._sub_rewards, reset_buf=self.reset_buf, terminate_buf=self._terminate_buf,
+                    rigid_body_state=self._rigid_body_state, target_rb_pos=self._prev_target_rb_pos, games=games))
 
     def export_motion_stats(self):
         """writes the per-motion buckets to b200_motion_stats_file and prints the summary line; returns the file's path"""
         counts, sums = self._ms["counts"].cpu().numpy(), self._ms["sums"].cpu().numpy()
+        pose = (self._ms["pose_sums"].cpu().numpy(), self._ms["success"].cpu().numpy()) if self._pose_threshold is not None else None
+        env_motion_ids, queue = self._reset_ref_motion_ids.cpu().numpy(), {}
+        if self._q is not None:
+            R, M = self._queue_rounds, self._motion_lib.num_motions()
+            queue = dict(game_env=self._q["game_env"].cpu().numpy().reshape(R, M),
+                         game_start_step=self._q["game_start_step"].cpu().numpy().reshape(R, M),
+                         unfinished=np.flatnonzero(counts[:, 0] == 0).astype(np.int64))
+            counts, sums = queue_fold(counts, R, M), queue_fold(sums, R, M)
+            if pose is not None:
+                pose = queue_fold(pose[0], R, M, max_col=6), queue_fold(pose[1], R, M)
+            env_motion_ids = self._sample_motion_ids().cpu().numpy()
         path = motion_stats_path(self.cfg["env"])
         if os.path.dirname(path):
             os.makedirs(os.path.dirname(path), exist_ok=True)
         np.savez(path, games=counts[:, 0], falls=counts[:, 1], reward_sum=sums[:, 0], steps=sums[:, 1].astype(np.int64),
-                 sub_reward_sum=sums[:, 2:6], body_pos_err_sum=sums[:, 6], env_motion_ids=self._reset_ref_motion_ids.cpu().numpy(),
-                 test_motion_file=np.array(self._test_motion_file or ""), **self._pose_metrics_keys())
+                 sub_reward_sum=sums[:, 2:6], body_pos_err_sum=sums[:, 6], env_motion_ids=env_motion_ids,
+                 test_motion_file=np.array(self._test_motion_file or ""), **self._pose_metrics_keys(pose), **queue)
         print(motion_stats_summary(counts, sums))
-        if self._pose_threshold is not None:
-            print(pose_metrics_summary(counts, sums, self._ms["pose_sums"].cpu().numpy(), self._ms["success"].cpu().numpy()))
+        if pose is not None:
+            print(pose_metrics_summary(counts, sums, *pose))
         print(f"============ per-motion statistics written to {path} ============")
         return path
 
-    def _pose_metrics_keys(self):
-        """the pose metrics' keys of the file (none without b200_pose_metrics)"""
-        if self._pose_threshold is None:
+    def _pose_metrics_keys(self, pose):
+        """the pose metrics' keys of the file from (pose_sums [M, 7], success [M]) (none without b200_pose_metrics)"""
+        if pose is None:
             return {}
-        ps = self._ms["pose_sums"].cpu().numpy()
+        ps, success = pose
         return dict(mpjpe_l_sum=ps[:, 0], mpjpe_pa_sum=ps[:, 1], vel_err_sum=ps[:, 2], acc_err_sum=ps[:, 3],
-                    vel_frames=ps[:, 4].astype(np.int64), acc_frames=ps[:, 5].astype(np.int64), success=self._ms["success"].cpu().numpy(),
+                    vel_frames=ps[:, 4].astype(np.int64), acc_frames=ps[:, 5].astype(np.int64), success=success,
                     max_body_pos_err=ps[:, 6], success_threshold=np.float64(self._pose_threshold), dt=np.float64(self.dt))
 
     def clear_motion_stats_games(self):
@@ -332,8 +441,11 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             self._record_launch(False, games=self._stats["games"])
         if self._ms is not None:
             self._motion_stats_launch(games=self._stats["games"])
-        native.play_stats(dict(n=self.num_envs, max_log=self._stats_cap, n_games=self._n_games),
+        queue_games = self._motion_lib.num_motions() * self._queue_rounds if self._q is not None else 0
+        native.play_stats(dict(n=self.num_envs, max_log=self._stats_cap, n_games=self._n_games, queue_games=queue_games),
                           dict(self._stats, rew=self.rew_buf, reset_buf=self.reset_buf))
+        if self._q is not None:
+            self._queue_launches()
 
     def test_step(self, n, graph=True):
         """step n (0-based) of a game: the context rebuild of all envs when n > 0 and n % context_length == 0, then the operand launch,
@@ -363,17 +475,20 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                  clip_actions=None, graph=True, history=None):
         """ImitatorPlayer.run (im_player.py:193-312) with the deterministic mu, or the sampled action when `policy` has a sigma: per game a full reset(), then up to max_steps
         test_step() calls; the host reads the stop flag and the statistics log every sync_every (default context_length) steps and at
-        max_steps, and prints the reference's lines in order.  policy: a dict of nn.im_networks_from_checkpoint.  history: a list that
-        receives, per game, the list of device copies (rew_buf, reset_buf) of every step run (for tests).  Returns dict(sum_rewards,
-        sum_steps, games_played)."""
+        max_steps, and prints the reference's lines in order.  With cfg.env.b200_motion_queue: one full reset, then up to max_steps
+        steps in all, until every queued game has finished; games_played counts the finished queued games.  policy: a dict of
+        nn.im_networks_from_checkpoint.  history: a list that receives, per game, the list of device copies (rew_buf, reset_buf) of
+        every step run (for tests).  Returns dict(sum_rewards, sum_steps, games_played)."""
         sync_every = int(sync_every or self.context_length)
         self.set_policy(policy, clip_obs=clip_obs, clip_actions=clip_actions, sync_every=sync_every)
         n_games = games_num * n_game_life
         self._n_games = n_games
         st = self._stats
-        for _ in range(n_games):
+        for _ in range(n_games if self._q is None else 1):
             if int(st["games"][0]) >= n_games:
                 break
+            if self._q is not None:
+                self._start_queue()
             self.reset()
             for k in ("cr", "steps", "prev_dones", "step"):
                 st[k].zero_()
