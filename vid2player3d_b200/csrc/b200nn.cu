@@ -327,8 +327,8 @@ template <int E, int BN> __host__ __device__ constexpr int stage_bytes() { retur
 template <int E, int BN> __host__ __device__ constexpr int bias_offset() { return stages<E, BN>() * stage_bytes<E, BN>() + 16 * stages<E, BN>(); }
 template <int E, int BN> int smem_bytes(int n_padded) { return 1024 + bias_offset<E, BN>() + E * n_padded * 4; }
 
-// RES (residual epilogue, the policy's last layer): one CTA per SM - its register budget holds the residual's addressing without spilling,
-// and a layer as narrow as the policy's 75 actions has fewer tiles than SMs.  NOISE (sampled action, also only on the last layer): the
+// RES (residual epilogue, the policy's last layer): launch bounds of one CTA per SM, a register budget that holds the residual's addressing
+// without spilling; a layer with more tiles than CTA slots walks several tiles per CTA like any other.  NOISE (sampled action, also only on the last layer): the
 // same budget for the counter-based normal; the last CTA to finish advances the step counter (producer and consumers both take part).
 template <int E, int BN, bool RES = false, bool NOISE = false>
 __global__ void __launch_bounds__(NUM_THREADS, (RES || NOISE) ? 1 : ctas_per_sm<E>())
