@@ -137,62 +137,98 @@ class FakeVisDual(VD.MVAEControllerVisDual):
         pass
 
 
-d = FakeVisDual()
-d.cfg = {"env": {"record": True, "num_rec_frames": TD + 1, "num_eg": EGD, "start_eg_id": 1}}
-d.headless, d.num_envs, d.frame_index, d.num_best = True, ND, 0, EGD
-d.joint_rot_all = torch.zeros((ND, CAP, 24, 3))
-d.root_pos_all = torch.zeros((ND, CAP, 3))
-d.ball_pos_all = torch.zeros((ND, CAP, 3))
-d.target_pos_all = torch.zeros((ND, CAP, 3))
-d.phase_all = torch.zeros((ND, CAP))
-d.swing_type_all = torch.zeros((ND, CAP), dtype=torch.int64)
-d.tar_action_all = torch.zeros((ND, CAP), dtype=torch.int64)
-d.distance_best_all, d.joint_rot_best_all, d.root_pos_best_all, d.ball_pos_best_all = [], [], [], []
-d.phase_best_all, d.swing_type_best_all, d.tar_action_best_all = [], [], []
-d._mvae_player = SimpleNamespace()
-captured = []
-d.render_one_result = lambda best_idx, eg_id: captured.append((best_idx, eg_id))
+def render_dual(schedule, seed, steps):
+    """MVAEControllerVisDual.render_vis over steps + 1 scripted steps: schedule {step: {pair: (distance of player 0, of player 1)}}
+    flags those pairs; other distances are random.  Returns the per-step inputs, the final list and the render_one_result indices."""
+    d = FakeVisDual()
+    d.cfg = {"env": {"record": True, "num_rec_frames": steps + 1, "num_eg": EGD, "start_eg_id": 1}}
+    d.headless, d.num_envs, d.frame_index, d.num_best = True, ND, 0, EGD
+    d.joint_rot_all = torch.zeros((ND, CAP, 24, 3))
+    d.root_pos_all = torch.zeros((ND, CAP, 3))
+    d.ball_pos_all = torch.zeros((ND, CAP, 3))
+    d.target_pos_all = torch.zeros((ND, CAP, 3))
+    d.phase_all = torch.zeros((ND, CAP))
+    d.swing_type_all = torch.zeros((ND, CAP), dtype=torch.int64)
+    d.tar_action_all = torch.zeros((ND, CAP), dtype=torch.int64)
+    d.distance_best_all, d.joint_rot_best_all, d.root_pos_best_all, d.ball_pos_best_all = [], [], [], []
+    d.phase_best_all, d.swing_type_best_all, d.tar_action_best_all = [], [], []
+    d._mvae_player = SimpleNamespace()
+    captured = []
+    d.render_one_result = lambda best_idx, eg_id: captured.append((best_idx, eg_id))
+    gd = torch.Generator().manual_seed(seed)
+    progress = torch.zeros(ND, dtype=torch.long)
+    keys = ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action", "progress", "reset", "distance")
+    dual_in = {k: [] for k in keys}
+    flagged_prev = torch.zeros(ND, dtype=torch.bool)
+    done = False
+    for step in range(steps + 1):
+        if step > 0:
+            progress[flagged_prev] = 0                # env_reset of the previous step's finished pairs, then the step counts one
+            progress += 1
+        reset = torch.zeros(ND, dtype=torch.long)
+        distance = (torch.rand(ND, generator=gd) * 4.0).float()
+        for p, (d0, d1) in schedule.get(step, {}).items():
+            reset[2 * p] = reset[2 * p + 1] = 1
+            distance[2 * p], distance[2 * p + 1] = d0, d1
+        fr = dict(joint_rot=torch.randn(ND, 24, 3, generator=gd), root_pos=torch.randn(ND, 3, generator=gd),
+                  ball_pos=torch.randn(ND, 3, generator=gd), phase=torch.rand(ND, generator=gd) * 6.0,
+                  swing_type=torch.randint(-1, 4, (ND,), generator=gd), tar_action=torch.randint(0, 2, (ND,), generator=gd))
+        d._joint_rot, d._root_pos, d._ball_pos, d._tar_action = fr["joint_rot"], fr["root_pos"], fr["ball_pos"], fr["tar_action"]
+        d._mvae_player._phase_pred, d._mvae_player._swing_type_cycle = fr["phase"], fr["swing_type"]
+        d.progress_buf, d.reset_buf, d._distance = progress.clone(), reset, distance
+        for k, x in dict(fr, progress=progress, reset=reset, distance=distance).items():
+            dual_in[k].append(x.numpy().copy())
+        try:
+            d.render_vis(init=(step == 0))
+        except SystemExit:
+            done = True
+        flagged_prev = reset.bool()
+    assert done
+    out = {"dual_" + k: np.stack(x) for k, x in dual_in.items()}
+    out["dual_best_distance"] = np.array([float(x) for x in d.distance_best_all], np.float32)
+    out["dual_best_nframes"] = np.array([x.shape[1] for x in d.root_pos_best_all])
+    for k in ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action"):
+        lst = getattr(d, k + "_best_all")
+        out["dual_best_" + k] = np.concatenate([x.numpy() for x in lst], 1)    # entries concatenated along the frame axis
+    return out, captured
+
+
 # pair -> pair distance by step: same-step pairs, equal distances, a refused insertion while short, the capacity rally
 SCHEDULE = {3: {0: 5.0, 1: 7.0}, 5: {0: 3.0}, 7: {1: 9.0, 2: 9.0}, 9: {0: 8.0}, 11: {3: 10.0}, 13: {0: 8.5, 2: 2.0}}
-gd = torch.Generator().manual_seed(13)
-progress = torch.zeros(ND, dtype=torch.long)
-keys = ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action", "progress", "reset", "distance")
-dual_in = {k: [] for k in keys}
-flagged_prev = torch.zeros(ND, dtype=torch.bool)
-done = False
-for step in range(TD + 1):
-    if step > 0:
-        progress[flagged_prev] = 0                # env_reset of the previous step's finished pairs, then the step counts one
-        progress += 1
-    reset = torch.zeros(ND, dtype=torch.long)
-    distance = (torch.rand(ND, generator=gd) * 4.0).float()
-    for p, dist in SCHEDULE.get(step, {}).items():
-        reset[2 * p] = reset[2 * p + 1] = 1
-        distance[2 * p], distance[2 * p + 1] = 0.25 * dist, 0.75 * dist
-    fr = dict(joint_rot=torch.randn(ND, 24, 3, generator=gd), root_pos=torch.randn(ND, 3, generator=gd),
-              ball_pos=torch.randn(ND, 3, generator=gd), phase=torch.rand(ND, generator=gd) * 6.0,
-              swing_type=torch.randint(-1, 4, (ND,), generator=gd), tar_action=torch.randint(0, 2, (ND,), generator=gd))
-    d._joint_rot, d._root_pos, d._ball_pos, d._tar_action = fr["joint_rot"], fr["root_pos"], fr["ball_pos"], fr["tar_action"]
-    d._mvae_player._phase_pred, d._mvae_player._swing_type_cycle = fr["phase"], fr["swing_type"]
-    d.progress_buf, d.reset_buf, d._distance = progress.clone(), reset, distance
-    for k, x in dict(fr, progress=progress, reset=reset, distance=distance).items():
-        dual_in[k].append(x.numpy().copy())
-    try:
-        d.render_vis(init=(step == 0))
-    except SystemExit:
-        done = True
-    flagged_prev = reset.bool()
-assert done and int(np.max(dual_in["progress"])) == CAP - 1     # one rally fills the buffer
-for k, x in dual_in.items():
-    OUT["dual_" + k] = np.stack(x)
+dual, captured = render_dual({s: {p: (0.25 * x, 0.75 * x) for p, x in sch.items()} for s, sch in SCHEDULE.items()}, 13, TD)
+OUT.update(dual)
+assert int(np.max(OUT["dual_progress"])) == CAP - 1     # one rally fills the buffer
 OUT["dual_capacity"] = np.int64(CAP)
 OUT["dual_num_eg"] = np.int64(EGD)
-OUT["dual_best_distance"] = np.array([float(x) for x in d.distance_best_all], np.float32)
-OUT["dual_best_nframes"] = np.array([x.shape[1] for x in d.root_pos_best_all])
-for k in ("joint_rot", "root_pos", "ball_pos", "phase", "swing_type", "tar_action"):
-    lst = getattr(d, k + "_best_all")
-    OUT["dual_best_" + k] = np.concatenate([x.numpy() for x in lst], 1)    # entries concatenated along the frame axis
 assert [i for i, _ in captured] == list(range(EGD))
 
 np.savez_compressed(os.path.join(HERE, "v2p_eval.npz"), **OUT)
 print("v2p_eval.npz", {k: v.shape for k, v in OUT.items()})
+
+# ------------------------------------------------------------------ dual: NaN pair distances (v2p_eval_nonfinite.npz)
+# A pair's distance is NaN once its root velocity is.  distance.max() is then NaN and torch.argmax (CPU) returns the first NaN; the
+# insertion's max_dist > last is false for a NaN, so a NaN pair enters only an empty list, and a NaN in the list stops it growing.
+# Scenario i is stored under "s{i}_" with the keys of the dual_ fixture above.
+NAN, INF = float("nan"), float("inf")
+NONFINITE = [
+    # into the empty list: three NaN pairs (one player NaN, both, Inf - Inf) and a larger finite pair on one step -> the first NaN,
+    # then a larger finite pair and another NaN pair are refused
+    {2: {0: (1.0, 2.0), 1: (NAN, 1.0), 2: (INF, -INF), 3: (0.5, NAN)}, 5: {0: (50.0, 50.0)}, 8: {2: (NAN, NAN), 3: (9.0, 9.0)}},
+    # into a short list: a NaN pair with a larger finite pair is refused, a larger finite pair alone enters
+    {2: {0: (2.0, 3.0)}, 5: {1: (NAN, 0.0), 2: (40.0, 1.0)}, 8: {3: (6.0, 1.0)}, 10: {2: (0.0, NAN)}},
+    # into the full list: a NaN pair beside a larger finite pair is refused, +Inf enters at the head, a NaN pair beside a +Inf pair is
+    # refused, a larger finite pair enters behind the +Inf
+    {1: {0: (1.0, 1.0)}, 2: {1: (2.0, 2.0)}, 3: {2: (3.0, 3.0)}, 5: {3: (NAN, 9.0), 0: (10.0, 10.0)}, 7: {1: (INF, 1.0)},
+     9: {2: (NAN, NAN), 3: (INF, 0.0)}, 11: {0: (20.0, 20.0)}},
+    # the first flag of the run is a lone NaN pair: the list holds it and refuses everything after
+    {1: {3: (NAN, 2.0)}, 4: {0: (1.0, 1.0)}, 6: {1: (INF, INF)}, 9: {2: (NAN, 0.0)}},
+]
+NF = {}
+for i, sch in enumerate(NONFINITE):
+    out, captured = render_dual(sch, 17 + i, CAP - 1)
+    assert [j for j, _ in captured] == list(range(EGD))
+    NF.update({f"s{i}_" + k[5:]: v for k, v in out.items()})
+NF["capacity"], NF["num_eg"], NF["scenarios"] = np.int64(CAP), np.int64(EGD), np.int64(len(NONFINITE))
+assert np.isnan(NF["s0_best_distance"]).all() and len(NF["s0_best_distance"]) == 1 and len(NF["s2_best_distance"]) == EGD
+np.savez_compressed(os.path.join(HERE, "v2p_eval_nonfinite.npz"), **NF)
+print("v2p_eval_nonfinite.npz", {k: v.shape for k, v in NF.items()})

@@ -8,6 +8,10 @@ p_rb_rot, p_dof_pos; the target root is the root row of p_rb_*) and, per env, th
 (qpos_init0) and True (qpos_init1).  The reference syncs env 0, so env e is synced as env 0 of its own slice.  Joints of the random
 state are overwritten with the edge cases: a zero rotation vector, |theta| near pi, pitch at and near +-pi/2 (where the yaw and roll
 arguments both fall below eps), and rotations of pi about x and z (the +-pi branch cut of atan2).
+
+Also tests/golden/im_record_nonfinite.npz, the same keys for the joints and roots of a failing policy: rotation vectors with NaN in one,
+two or three components, +-Inf and +-1e30 (finite, but its square overflows float32), a NaN root position and an Inf root quaternion.
+The reference's torch.clamp keeps a NaN pitch.
 """
 import os
 import sys
@@ -38,6 +42,11 @@ EDGES = [(0.0, 0.0, 0.0), (PI - 1e-7, 0.0, 0.0), (0.0, 0.0, -(PI - 1e-6)), tuple
          (0.0, 0.0, PI), (0.0, 0.0, -PI), (1e-5, 0.0, 0.0), (3e-4, -2e-4, 1e-4)]
 
 
+NAN, INF = float("nan"), float("inf")
+NONFINITE = [(NAN, 0.3, -0.2), (0.1, NAN, 0.0), (NAN, NAN, 0.5), (NAN, NAN, NAN), (INF, 0.0, 0.0), (0.0, -INF, 0.0), (INF, -INF, 1.0),
+             (0.0, 0.0, NAN), (1e30, 0.0, 0.0), (0.0, -1e30, 0.0), (1e30, 1e30, -1e30)]
+
+
 def state(seed):
     g = np.random.default_rng(seed)
     rb_pos = g.normal(0, 1.5, (N, NB, 3))
@@ -47,9 +56,9 @@ def state(seed):
     return rb_pos, rb_rot, dof
 
 
-def with_edges(dof, shift):
+def with_edges(dof, shift, edges=EDGES):
     dof = dof.copy().reshape(N, ND // 3, 3)
-    for k, a in enumerate(EDGES):
+    for k, a in enumerate(edges):
         dof[(k + shift) % N, (3 * k + shift) % (ND // 3)] = a
     return dof.reshape(N, ND)
 
@@ -75,6 +84,17 @@ def main():
         out[f"qpos_init{int(init)}"] = np.stack([sync(st, e, init) for e in range(N)])
     np.savez_compressed(os.path.join(HERE, "im_record.npz"), **out)
     print("im_record.npz", {k: v.shape for k, v in out.items()})
+
+    rb_pos, rb_rot, dof = state(3)
+    p_rb_pos, p_rb_rot, p_dof = state(4)
+    rb_pos[1, 0, 2], rb_rot[2, 0, 0], p_rb_pos[5, 0, 0], p_rb_rot[6, 0, 3] = NAN, INF, NAN, -INF
+    st = (rb_pos, rb_rot, with_edges(dof, 0, NONFINITE), p_rb_pos, p_rb_rot, with_edges(p_dof, 5, NONFINITE))
+    out = {k: v for k, v in zip(("rb_pos", "rb_rot", "dof_pos", "p_rb_pos", "p_rb_rot", "p_dof_pos"), st)}
+    for init in (False, True):
+        out[f"qpos_init{int(init)}"] = np.stack([sync(st, e, init) for e in range(N)])
+    assert np.isnan(out["qpos_init0"]).any() and np.isfinite(out["qpos_init0"]).any()
+    np.savez_compressed(os.path.join(HERE, "im_record_nonfinite.npz"), **out)
+    print("im_record_nonfinite.npz", {k: v.shape for k, v in out.items()})
 
 
 if __name__ == "__main__":

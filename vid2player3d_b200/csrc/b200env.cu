@@ -2081,16 +2081,19 @@ __global__ void __launch_bounds__(PLAY_THREADS) play_stats_kernel(b200_play_stat
 // ypr_euler_from_quat with eps 1e-6, reordered [2, 1, 0]).  theta >= 1e-3, so safe_zero_division never adds its eps.  In double: near
 // pitch +-pi/2 both atan2 arguments are rounding noise below eps, and float32 noise would turn yaw and roll into other angles.
 // sincospi needs no argument-reduction table, so the double kernels elsewhere in the library keep their code.
+// The max of theta and the clamp of the pitch keep a NaN (torch.clamp, np.maximum); fmin / fmax would drop it and record a finite
+// pitch for a NaN joint.
 __device__ __forceinline__ void rotvec_ypr(double a0, double a1, double a2, float* out) {
   const double th2 = a0 * a0 + a1 * a1 + a2 * a2;
-  const double th = sqrt(fmax(th2, 1e-6));
+  const double th = sqrt(th2 < 1e-6 ? 1e-6 : th2);
   double s, c;
   sincospi(th * (0.5 / 3.14159265358979323846), &s, &c);
   const double k = th2 > 0.0 ? s / th : 0.5, w = th2 > 0.0 ? c : 1.0;
   const double x = a0 * k, y = a1 * k, z = a2 * k;
   auto safe_atan2 = [](double yy, double xx) { return atan2((fabs(yy) < 1e-6 && fabs(xx) < 1e-6) ? yy + 1e-6 : yy, xx); };
   out[0] = (float)safe_atan2(2.0 * (w * z + x * y), 1.0 - 2.0 * (y * y + z * z));
-  out[1] = (float)asin(fmin(fmax(2.0 * (w * y - x * z), -1.0 + 1e-6), 1.0 - 1e-6));
+  const double sp = 2.0 * (w * y - x * z);
+  out[1] = (float)asin(sp < -1.0 + 1e-6 ? -1.0 + 1e-6 : (sp > 1.0 - 1e-6 ? 1.0 - 1e-6 : sp));
   out[2] = (float)safe_atan2(2.0 * (w * x + y * z), 1.0 - 2.0 * (x * x + y * y));
 }
 

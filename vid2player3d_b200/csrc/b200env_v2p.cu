@@ -778,20 +778,27 @@ __global__ void __launch_bounds__(V2P_WARPS * 32) eval_record_kernel(b200v2p_rec
 }
 
 // ------------------------------------------------------------------------------------------ dual best-episode list
-// mvae_controller_vis_dual.py:164-195 on one CTA: first argmax over the flagged pairs, then the insertion rule on the slot order
+// mvae_controller_vis_dual.py:164-195 on one CTA: first argmax over the flagged pairs, then the insertion rule on the slot order.
+// The argmax is torch.argmax's: a NaN ranks above every number and the first NaN wins, so the pair taken is the same whatever the
+// thread and shuffle order.  The insertion rule's > is false for a NaN, as in the reference: a NaN pair enters only an empty list,
+// and once it is there nothing passes it.
 __global__ void __launch_bounds__(1024) eval_best_select_kernel(b200v2p_best_t b) {
   __shared__ float sd[32];
   __shared__ int64_t sk[32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   float d = 0.0f;
-  int64_t k = -1;   // a thread walks its pairs in increasing order, so a strict > keeps the first of equal distances
+  int64_t k = -1;   // a thread walks its pairs in increasing order, so a strict rank keeps the first of equal distances or NaNs
   for (int64_t p = threadIdx.x; p < b.n / 2; p += blockDim.x) {
     if (b.reset_buf[2 * p] == 0) continue;
     const float v = __fadd_rn(b.distance[2 * p], b.distance[2 * p + 1]);
-    if (k < 0 || v > d) { d = v; k = p; }
+    if (k < 0 || (d == d && (v != v || v > d))) { d = v; k = p; }
   }
-  // (d, k) beats (od, ok) when it is valid and either the other is not, or its distance is larger, or equal with a lower pair
-  const auto take = [](float od, int64_t ok, float d, int64_t k) { return ok >= 0 && (k < 0 || od > d || (od == d && ok < k)); };
+  // (d, k) beats (od, ok) when it is valid and either the other is not, or its distance ranks higher (NaN above every number), or
+  // ranks the same (equal, or both NaN) with a lower pair
+  const auto take = [](float od, int64_t ok, float d, int64_t k) {
+    const bool onan = od != od, dnan = d != d;
+    return ok >= 0 && (k < 0 || (onan && !dnan) || (!dnan && od > d) || ((od == d || (onan && dnan)) && ok < k));
+  };
 #pragma unroll
   for (int s = 16; s > 0; s >>= 1) {
     const float od = __shfl_down_sync(FULL, d, s);
