@@ -356,7 +356,11 @@ int32_t b200env_play_stats_desc_size(void);
  * its step field, so each restarted window is aligned with the policy's slot).  games: b200_play_stats_t::games or NULL; while
  * games[1] (stop) is set the launch clears the mask and changes nothing else.  Returns -1 on a NULL pointer but games and env_flags,
  * -2 before
- * any launch when n, num_motions or queue_len is not positive, or shape_dim is outside [0, 32]. */
+ * any launch when n, num_motions or queue_len is not positive, or shape_dim is outside [0, 32].
+ * Bodies (motion_asset and env_asset, appended within ABI version 11; both NULL = the launch above): an env that takes entry q also
+ * gets env_asset[e] = motion_asset[q % M], the asset of its next motion; an idle env and a stopped run change nothing.  The caller
+ * then re-points the handle's asset table (b200env_set_env_assets) before the masked reset, so the next physics launch steps each
+ * restarted env with its new motion's body.  -1 when only one of the two is set. */
 typedef struct b200_im_motion_queue {
   int32_t n;                       /* envs */
   int32_t num_motions;             /* M */
@@ -377,6 +381,8 @@ typedef struct b200_im_motion_queue {
   const int64_t* games;            /* [3] or NULL */
   float* prev_dones;               /* [n] b200_play_stats_t::prev_dones */
   int32_t* env_flags;              /* [n, 2] b200_im_motion_stats_t::env_flags, or NULL */
+  const int32_t* motion_asset;     /* [M]: the asset of each motion, or NULL */
+  int32_t* env_asset;              /* [n]: the asset each env is simulated with, or NULL */
 } b200_im_motion_queue_t;
 int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream);
 /* sizeof(b200_im_motion_queue_t) as the library was built; the binding refuses a library whose size differs from its own */
@@ -589,8 +595,9 @@ int b200env_physics_launch_shape(b200env_handle h, int32_t* envs_per_batch, int3
 
 /* Several assets of one topology in one handle (replaces the per-env actors of HumanoidSMPLIM._create_envs, each built from its
  * motion's body: embodied_pose/env/tasks/humanoid_smpl_im.py:231-351, PD gains scaled by that actor's mass :356-389).  models [num_assets]
- * and verts [num_assets] (verts[a]: [nb][models[a].vmax][3]) are HOST arrays; env e is simulated with asset env_asset[e] for the
- * handle's lifetime.  Every asset must have asset 0's topology (nb, nd, max_depth, parent, depth, fixed, dof_of_body); vmax, the
+ * and verts [num_assets] (verts[a]: [nb][models[a].vmax][3]) are HOST arrays; env e is simulated with asset env_asset[e], for the
+ * handle's lifetime unless the handle is fixed to the mixed plan (b200env_fix_mixed_plan), whose b200env_set_env_assets moves envs to
+ * other assets of the handle on the device.  Every asset must have asset 0's topology (nb, nd, max_depth, parent, depth, fixed, dof_of_body); vmax, the
  * vertices and every numeric field may differ.  The physics launch runs one of two plans:
  *  - grouped (b200env_plan_assets): batches of at most 32 envs of one asset each; a CTA re-stages the asset's header in shared memory
  *    when it moves to a batch of another asset;
@@ -624,9 +631,33 @@ int b200env_choose_asset_plan(const int32_t* env_asset, int32_t num_envs, int32_
 
 /* The plan a handle of b200env_create_assets runs (batch b runs in round b / grid of b200env_physics_launch_shape); *mixed = 1 for
  * the mixed plan, 0 for the grouped one.  Array arguments and mixed may be NULL (query the sizes first: rows has num_envs entries,
- * the batch arrays *num_batches).  Fails on a handle of b200env_create. */
+ * the batch arrays *num_batches).  Fails on a handle of b200env_create.  batch_asset describes the env_asset of b200env_create_assets:
+ * after b200env_set_env_assets a mixed batch's envs may run other assets. */
 int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batches, int32_t* rows, int32_t* batch_asset,
                        int32_t* batch_first, int32_t* batch_count, int32_t* mixed);
+
+/* Setup call on a handle of b200env_create_assets, before its first step: the handle runs the mixed plan for its lifetime, whatever
+ * the rule (or B200ENV_ASSET_PLAN) chose, so that b200env_set_env_assets may re-point its envs' assets on the device (the mixed plan's
+ * batches do not depend on the assignment; the grouped plan's do).  Host work and one device allocation, like create: the env ->
+ * asset-header table of the mixed plan when the grouped plan had been chosen.  Both plans give bit-identical results.  Afterwards
+ * b200env_asset_plan reports mixed = 1 and the mixed batches of the creation-time assignment.  Returns -2 on a handle of
+ * b200env_create (one asset); calling it twice is allowed. */
+int b200env_fix_mixed_plan(b200env_handle h);
+
+/* Re-point the assets of the envs of a handle fixed to the mixed plan, on the device: one thread per env sets env e's entry of the
+ * asset-header table to asset env_asset[e] (an index into the models of b200env_create_assets), read by every physics launch from the
+ * next one on.  An index outside [0, num_assets) leaves that env's asset as it was and, when *error is 0, sets *error = e + 1 (the
+ * first such env the launch met; the word keeps it until the caller clears it).  No allocation, no host synchronisation: graph-safe.
+ * Returns -1 on a NULL pointer, -2 before any launch on a handle not fixed to the mixed plan or when n is not the handle's env count. */
+typedef struct b200_set_env_assets {
+  int32_t n;                       /* envs: the handle's num_envs */
+  int32_t pad_;
+  const int32_t* env_asset;        /* [n] */
+  int32_t* error;                  /* [1] */
+} b200_set_env_assets_t;
+int b200env_set_env_assets(b200env_handle h, const b200_set_env_assets_t* d, void* stream);
+/* sizeof(b200_set_env_assets_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_set_env_assets_desc_size(void);
 
 /* number of kernels launched by this handle so far (bench.py "gpu_launches") */
 int64_t b200env_launch_count(b200env_handle h);

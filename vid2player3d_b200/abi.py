@@ -316,9 +316,15 @@ class ImMotionQueue(C.Structure):
         ("n", C.c_int32), ("num_motions", C.c_int32), ("queue_len", C.c_int64), ("shape_dim", C.c_int32), ("pad_", C.c_int32),
         ("reset_buf", I64P), ("lib_motion_bodies", F32P), ("motion_ids", I64P), ("motion_bodies", F32P), ("entry", I64P), ("mask", U8P),
         ("idle", U8P), ("cursor", I64P), ("game_env", I64P), ("game_start_step", I64P), ("step", I64P), ("games", I64P),
-        ("prev_dones", F32P), ("env_flags", I32P),
+        ("prev_dones", F32P), ("env_flags", I32P), ("motion_asset", I32P), ("env_asset", I32P),
     ]
-    _nullable_, _defaults_ = ("games", "env_flags"), ("pad_",)
+    _nullable_, _defaults_ = ("games", "env_flags", "motion_asset", "env_asset"), ("pad_",)
+
+
+class SetEnvAssets(C.Structure):
+    """b200_set_env_assets_t: the assets of a mixed-plan handle's envs, re-pointed on the device (b200env_set_env_assets)"""
+    _fields_ = [("n", C.c_int32), ("pad_", C.c_int32), ("env_asset", I32P), ("error", I32P)]
+    _nullable_, _defaults_ = (), ("pad_",)
 
 
 class ImRecord(C.Structure):
@@ -735,6 +741,9 @@ SIGNATURES = {
     "b200env_plan_assets_mixed": (C.c_int, [_p, _i32, _i32, _i32, _p, _p, _p, _p, _p]),
     "b200env_choose_asset_plan": (C.c_int, [_p, _i32, _i32, _i32, _p]),
     "b200env_asset_plan": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, _p]),
+    "b200env_fix_mixed_plan": (C.c_int, [_p]),
+    "b200env_set_env_assets": (C.c_int, [_p, _p, _p]),
+    "b200env_set_env_assets_desc_size": (_i32, []),
     "b200env_launch_count": (_i64, [_p]),
     "b200env_set_kernel_timing": (C.c_int, [_p, _i32]),
     "b200env_kernel_ms": (C.c_int, [_p, _p, _p]),

@@ -96,6 +96,7 @@ struct b200env {
   // the mixed plan (b200env_plan_assets_mixed, PhysForm::Mixed): batches of consecutive envs whatever their assets;
   // d_env_blob[e] = env e's asset header in d_assets (d_rows / d_batches stay unset)
   const DevBlob** d_env_blob;
+  bool fixed_mixed;                    // b200env_fix_mixed_plan: the mixed plan for the handle's lifetime, d_env_blob re-pointable
 };
 
 static thread_local char g_err[512] = "";
@@ -2444,8 +2445,10 @@ __global__ void __launch_bounds__(MS_FOLD_THREADS) im_motion_queue_fold_kernel(b
 }
 
 // b200env_im_motion_queue: one CTA walks the envs in chunks of QUEUE_THREADS; a block-wide exclusive count (ballots, then the warp
-// totals in shared memory) gives each finished env its rank k in env order, so the assignment depends on the flags alone
+// totals in shared memory) gives each finished env its rank k in env order, so the assignment depends on the flags alone.  ASSET:
+// each restarted env also takes its next motion's asset (b200_im_motion_queue_t::motion_asset / env_asset)
 #define QUEUE_THREADS 1024
+template <bool ASSET>
 __global__ void __launch_bounds__(QUEUE_THREADS) im_motion_queue_kernel(b200_im_motion_queue_t d) {
   __shared__ int s_warp[QUEUE_THREADS / 32];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -2479,6 +2482,7 @@ __global__ void __launch_bounds__(QUEUE_THREADS) im_motion_queue_kernel(b200_im_
           d.game_start_step[q] = step;
           d.prev_dones[e] = 0.f;
           if (d.env_flags) d.env_flags[2 * e] = 0;
+          if constexpr (ASSET) d.env_asset[e] = d.motion_asset[mid];
           m = 1;
         } else {
           d.idle[e] = 1;
@@ -2489,6 +2493,19 @@ __global__ void __launch_bounds__(QUEUE_THREADS) im_motion_queue_kernel(b200_im_
     base += total;
   }
   if (tid == 0 && !stopped) d.cursor[0] = min(cursor + base, d.queue_len);
+}
+
+// b200env_set_env_assets: one thread per env re-points its entry of the mixed plan's asset-header table; a bad index keeps the old
+// entry and records the first env that had one
+#define SET_ASSET_THREADS 256
+__global__ void __launch_bounds__(SET_ASSET_THREADS) set_env_assets_kernel(int n, int num_assets, const int32_t* __restrict__ env_asset,
+                                                                            const DevBlob* const* __restrict__ asset_ptr,
+                                                                            const DevBlob** __restrict__ env_blob, int32_t* error) {
+  const int e = blockIdx.x * SET_ASSET_THREADS + threadIdx.x;
+  if (e >= n) return;
+  const int32_t a = env_asset[e];
+  if (a >= 0 && a < num_assets) env_blob[e] = asset_ptr[a];
+  else atomicCAS(error, 0, e + 1);
 }
 
 // physics-only entry used by the parity tests (float or double)
@@ -2942,6 +2959,53 @@ int b200env_asset_plan(b200env_handle h, int32_t* num_assets, int32_t* num_batch
   return 0;
 }
 
+int b200env_fix_mixed_plan(b200env_handle h) {
+  if (!h) return fail(-1, "b200env_fix_mixed_plan: null argument%s");
+  if (!h->num_assets) return fail(-2, "b200env_fix_mixed_plan: not a handle of b200env_create_assets (one asset)%s");
+  h->fixed_mixed = true;
+  if (h->form == PhysForm::Mixed) return 0;
+  // the creation-time assignment from the grouped plan (rows of batch i run asset batch_asset[i]), then the mixed plan and its table
+  const int32_t n = h->num_envs, nb = h->num_batches;
+  const int32_t* P = h->plan->data();
+  std::vector<int32_t> env_asset(n);
+  for (int i = 0; i < nb; i++)
+    for (int p = P[n + nb + i]; p < P[n + nb + i] + P[n + 2 * nb + i]; p++) env_asset[P[p]] = P[n + i];
+  std::vector<int32_t> plan;
+  int32_t nbat = 0;
+  if (int rc = make_asset_plan(b200env_plan_assets_mixed, env_asset.data(), n, h->num_assets, plan, &nbat)) return rc;
+  CUDA_OK(cudaSetDevice(h->device));
+  std::vector<const DevBlob*> ptr(h->num_assets), eb(n);
+  CUDA_OK(cudaMemcpy(ptr.data(), h->d_asset_ptr, sizeof(const DevBlob*) * h->num_assets, cudaMemcpyDeviceToHost));
+  for (int e = 0; e < n; e++) eb[e] = ptr[env_asset[e]];
+  const DevBlob** d_eb = nullptr;
+  CUDA_OK(cudaMalloc(&d_eb, sizeof(const DevBlob*) * n));
+  if (cudaMemcpy(d_eb, eb.data(), sizeof(const DevBlob*) * n, cudaMemcpyHostToDevice) != cudaSuccess) {
+    cudaFree(d_eb);
+    return fail(-10, "CUDA error: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  cudaFree(h->d_rows); cudaFree(h->d_batches);
+  h->d_rows = nullptr; h->d_batches = nullptr;
+  h->d_env_blob = d_eb;
+  *h->plan = std::move(plan);
+  h->num_batches = nbat;
+  h->form = PhysForm::Mixed;
+  h->step_slots = 0;    // the grid of the mixed launch, computed at the next step
+  return 0;
+}
+
+int b200env_set_env_assets(b200env_handle h, const b200_set_env_assets_t* d, void* stream) {
+  if (!h || !d || !d->env_asset || !d->error) return fail(-1, "b200env_set_env_assets: null argument%s");
+  if (!h->fixed_mixed) return fail(-2, "b200env_set_env_assets: the handle is not fixed to the mixed plan (b200env_fix_mixed_plan)%s");
+  if (d->n != h->num_envs) return fail(-2, "b200env_set_env_assets: n must be the handle's env count%s");
+  set_env_assets_kernel<<<(d->n + SET_ASSET_THREADS - 1) / SET_ASSET_THREADS, SET_ASSET_THREADS, 0, (cudaStream_t)stream>>>(
+      d->n, h->num_assets, d->env_asset, h->d_asset_ptr, h->d_env_blob, d->error);
+  CUDA_OK(cudaGetLastError());
+  h->launches++;
+  return 0;
+}
+
+int32_t b200env_set_env_assets_desc_size(void) { return (int32_t)sizeof(b200_set_env_assets_t); }
+
 int b200env_set_hull_faces(b200env_handle h, const float* planes, const uint8_t* tris, const int32_t* ntris, int32_t tmax) {
   if (!h || !planes || !tris || !ntris) return fail(-1, "b200env_set_hull_faces: null argument%s");
   if (tmax < 1 || tmax > 255) return fail(-2, "b200env_set_hull_faces: tmax must be in 1..255%s");
@@ -3379,7 +3443,11 @@ int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream) {
   if (d->n <= 0 || d->num_motions <= 0 || d->queue_len <= 0)
     return fail(-2, "b200env_im_motion_queue: n, num_motions and queue_len must be positive%s");
   if (d->shape_dim < 0 || d->shape_dim > 32) return fail(-2, "b200env_im_motion_queue: shape_dim must lie in [0, 32]%s");
-  im_motion_queue_kernel<<<1, QUEUE_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  if (!d->motion_asset != !d->env_asset) return fail(-1, "b200env_im_motion_queue: motion_asset and env_asset must be both set or both NULL%s");
+  if (d->env_asset)
+    im_motion_queue_kernel<true><<<1, QUEUE_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  else
+    im_motion_queue_kernel<false><<<1, QUEUE_THREADS, 0, (cudaStream_t)stream>>>(*d);
   CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -31,6 +31,7 @@ def lib():
                         (abi.ImMotionStats, L.b200env_im_motion_stats_desc_size()),
                         (abi.PlayStats, L.b200env_play_stats_desc_size()), (abi.ImMotionQueue, L.b200env_im_motion_queue_desc_size()),
                         (abi.ImMotionQueueStats, L.b200env_im_motion_queue_stats_desc_size()),
+                        (abi.SetEnvAssets, L.b200env_set_env_assets_desc_size()),
                         (abi.V2PBallStats, L.b200v2p_eval_ball_stats_desc_size()),
                         (abi.V2PRallyStats, L.b200v2p_eval_rally_stats_desc_size())):
             if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
@@ -369,6 +370,18 @@ class Env:
         na, nb, m = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         _check(lib().b200env_asset_plan(self._h, C.byref(na), C.byref(nb), None, None, None, None, C.byref(m)))
         return bool(m.value)
+
+    def fix_mixed_plan(self):
+        """a handle of several assets runs the mixed plan for its lifetime, so set_env_assets may move envs to other assets
+        (include/b200env.h: b200env_fix_mixed_plan; setup work, before the first step)"""
+        _check(lib().b200env_fix_mixed_plan(self._h))
+
+    def set_env_assets(self, env_asset, error):
+        """env e is simulated with asset env_asset[e] ([N] int32, device) from the next physics launch on; an index outside the
+        handle's assets keeps the env's asset and sets error ([1] int32, device) to env + 1 when it is 0 (include/b200env.h:
+        b200env_set_env_assets; graph-safe, no host synchronisation)"""
+        d = fill(abi.SetEnvAssets, dict(n=self.num_envs), dict(env_asset=env_asset, error=error))
+        _check(lib().b200env_set_env_assets(self._h, C.byref(d), _stream()))
 
     @property
     def launch_count(self):

@@ -185,15 +185,18 @@ class HumanoidSMPLIM(BaseTask):
         if len(entries) != self._motion_lib.num_motions():
             raise ValueError(f"motion_assets has {len(entries)} entries for {self._motion_lib.num_motions()} motions")
         models, keys, of_motion = [], {}, []
+        resolved = {}    # file name or id of a model dict -> asset index: a library of thousands of motions loads each file once
         for entry in entries:
-            if isinstance(entry, (str, os.PathLike)):
-                entry = model_compiler.load_compiled(os.path.splitext(os.path.basename(str(entry)))[0])
-            ms, verts = self._pack(entry)
-            key = bytes(ms) + verts.tobytes()
-            if key not in keys:
-                keys[key] = len(models)
-                models.append(entry)
-            of_motion.append(keys[key])
+            ref = os.path.splitext(os.path.basename(str(entry)))[0] if isinstance(entry, (str, os.PathLike)) else id(entry)
+            if ref not in resolved:
+                model = model_compiler.load_compiled(ref) if isinstance(ref, str) else entry
+                ms, verts = self._pack(model)
+                key = bytes(ms) + verts.tobytes()
+                if key not in keys:
+                    keys[key] = len(models)
+                    models.append(model)
+                resolved[ref] = keys[key]
+            of_motion.append(resolved[ref])
         return models, np.asarray(of_motion, np.int64)
 
     def create_sim(self):
@@ -207,7 +210,7 @@ class HumanoidSMPLIM(BaseTask):
             self._reset_ref_motion_ids = self._sample_motion_ids()
             models, of_motion = self._motion_asset_models()
             self._env_asset = of_motion[self._reset_ref_motion_ids.cpu().numpy()]
-            self._asset_models = models
+            self._asset_models, self._motion_asset = models, of_motion
             packed = [self._pack(m) for m in models]
             structs, verts = [p[0] for p in packed], [p[1] for p in packed]
             self.humanoid_masses = np.array([float(m["mass"].sum()) for m in models])[self._env_asset]     # :370-371

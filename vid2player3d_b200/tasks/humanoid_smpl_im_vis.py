@@ -40,7 +40,14 @@ is scored in one run.  The queue holds every motion once per round, R = cfg.env.
 q = r M + m; env e starts on entry e, and when its game ends it takes the next unplayed entry inside the step graph (include/b200env.h:
 b200env_im_motion_queue, then the masked reset with the window aligned to the policy's slot), with no host synchronisation.  An env
 that finishes once the queue is empty stays done.  run_test then runs one full reset and steps until every queued game has finished
-or max_steps steps have run; the per-motion meters fold each game into the row of its entry, and the file sums a motion's R rows."""
+or max_steps steps have run; the per-motion meters fold each game into the row of its entry, and the file sums a motion's R rows.
+
+Motion queue with a body per motion (cfg.env.motion_assets with test_motion_assets, the reference's per-motion actors): the handle holds
+every distinct asset of the library, runs the mixed plan for its lifetime (include/b200env.h: b200env_fix_mixed_plan), and env e
+starts on the asset of motion e % M.  When an env takes its next entry, the queue launch also writes that motion's asset, and
+b200env_set_env_assets re-points the env's asset before the masked reset, so the restarted game is stepped with its own body.  The
+recording's `asset` is then [E, T], each recorded env's body per frame.  humanoid_masses (host, informational) keeps the
+creation-time assignment."""
 import os
 from datetime import datetime
 
@@ -157,16 +164,18 @@ def motion_stats_summary(counts, sums):
 
 def motion_queue_rounds(cfg):
     """cfg.env.b200_motion_queue -> None when off, else the rounds R of the queue (b200_motion_queue_repeats, default 1); refuses R
-    that is not an int >= 1, several assets (motion_assets), transform_specs without b200_device_transforms (the queue restarts
-    games through the masked reset) and a state init other than Start (every queued game starts at its motion's first frame)"""
+    that is not an int >= 1, motion_assets without test_motion_assets (several assets are served for the held-out library of a test
+    run), transform_specs without b200_device_transforms (the queue restarts games through the masked reset) and a state init other
+    than Start (every queued game starts at its motion's first frame)"""
     env = cfg["env"]
     if not env.get("b200_motion_queue", False):
         return None
     R = env.get("b200_motion_queue_repeats", 1)
     if isinstance(R, bool) or not isinstance(R, (int, np.integer)) or R < 1:
         raise ValueError(f"b200_motion_queue_repeats must be an int >= 1, got {R!r}")
-    if "motion_assets" in env:
-        raise ValueError("b200_motion_queue serves a handle of one asset; motion_assets (several assets) is not supported")
+    if "motion_assets" in env and "test_motion_assets" not in env:
+        raise ValueError("b200_motion_queue with several assets scores a held-out library: give its bodies in test_motion_assets "
+                         "(with test_motion_file); motion_assets alone is not supported")
     if "transform_specs" in env and not env.get("b200_device_transforms", False):
         raise ValueError("b200_motion_queue restarts games through the masked reset: with transform_specs set b200_device_transforms")
     args = cfg.get("args", None)
@@ -233,7 +242,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         N, Q, dev = self.num_envs, self._motion_lib.num_motions() * self._queue_rounds, self.device
         i64 = lambda n: torch.zeros(n, device=dev, dtype=torch.long)  # noqa: E731
         self._q = dict(entry=i64(N), idle=torch.zeros(N, device=dev, dtype=torch.uint8), cursor=i64(1), game_env=i64(Q),
-                       game_start_step=i64(Q))
+                       game_start_step=i64(Q), **self._queue_assets())
 
     def _start_queue(self):
         """before the run's full reset: env e on entry e, the rest of the queue unplayed"""
@@ -248,6 +257,10 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
         q["game_env"][:N] = e
         q["game_start_step"].fill_(-1)
         q["game_start_step"][:N] = 0
+        if "env_asset" in q:                   # every env back on its start body
+            q["env_asset"].copy_(q["start_env_asset"])
+            q["asset_error"].zero_()
+            self._env.set_env_assets(q["env_asset"], q["asset_error"])
 
     def _queue_launches(self):
         """the assignment of the finished envs' next entries, then their masked reset with the window aligned to the step counter"""
@@ -258,6 +271,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                                     motion_ids=self._reset_ref_motion_ids, motion_bodies=self._reset_ref_motion_bodies, mask=self._reset_mask,
                                     step=self._im_step, games=self._stats["games"], prev_dones=self._stats["prev_dones"],
                                     env_flags=self._ms["env_flags"] if self._ms is not None else None))
+        if "env_asset" in self._q:             # the restarted envs' new bodies, read by the next physics launch
+            self._env.set_env_assets(self._q["env_asset"], self._q["asset_error"])
         self.reset_masked(self._reset_mask, step=self._im_step)
 
     def _setup_record(self, ids):
@@ -272,6 +287,8 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             name = lambda a: os.path.basename(str(a)) if isinstance(a, (str, os.PathLike)) else str(a["name"])  # noqa: E731
             mids = self._reset_ref_motion_ids.cpu().numpy()
             assets = [name(entries[mids[e]]) for e in ids]
+            if self._queue_rounds is not None:     # bodies change with the motion: the export names them per frame
+                self._rec_motion_asset = np.array([name(x) for x in entries])
         else:
             assets = [os.path.basename(env["asset"]["assetFileName"])] * E
         i64 = lambda *s: torch.zeros(*s, device=dev, dtype=torch.long)  # noqa: E731
@@ -298,14 +315,41 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             os.makedirs(os.path.dirname(path), exist_ok=True)
         np.savez(path, qpos=assemble_qpos(r["qpos"][:, :T]).cpu().numpy(), env_ids=r["env_ids"].cpu().numpy(),
                  motion_ids=r["rec_motion_ids"][:, :T].cpu().numpy(), reset=r["rec_reset"][:, :T].cpu().numpy(),
-                 asset=np.array(self._rec_assets), fps=np.float64(1.0 / self.dt), nq=np.int64(7 + self.num_dof))
+                 asset=self._recorded_assets(T), fps=np.float64(1.0 / self.dt), nq=np.int64(7 + self.num_dof))
         print(f"============ qpos of {T} frames written to {path} ============")
         return path
+
+    def _recorded_assets(self, T):
+        """the recording's `asset`: each recorded env's body name [E], or per frame [E, T] from the recorded motion ids when the queue
+        changes bodies"""
+        if getattr(self, "_rec_motion_asset", None) is None:
+            return np.array(self._rec_assets)
+        return self._rec_motion_asset[self._rec["rec_motion_ids"][:, :T].cpu().numpy()]
 
     def create_sim(self):
         # humanoid_smpl_im_vis.py:35 sets max_episode_length = 3000; the step's reset rule reads it from the cfg struct made here
         self.max_episode_length = 3000
         super().create_sim()
+        if self._queue_rounds is not None and "motion_assets" in self.cfg["env"]:
+            self._env.fix_mixed_plan()         # envs change body as their games end
+
+    def _queue_assets(self):
+        """with motion_assets: the asset of each motion [M], each env's asset [N] (started as at create) and the error word of
+        b200env_set_env_assets, all int32 on the device; else {}"""
+        if "motion_assets" not in self.cfg["env"]:
+            return {}
+        dev, i32 = self.device, torch.int32
+        start = torch.as_tensor(self._env_asset, dtype=i32, device=dev)
+        return dict(motion_asset=torch.as_tensor(self._motion_asset, dtype=i32, device=dev), env_asset=start.clone(), start_env_asset=start,
+                    asset_error=torch.zeros(1, device=dev, dtype=i32))
+
+    def _check_asset_error(self):
+        """the host's check of b200env_set_env_assets' error word, at the run's sync points"""
+        if self._q is not None and "asset_error" in self._q:
+            e = int(self._q["asset_error"])
+            if e:
+                raise ValueError(f"b200env_set_env_assets: env {e - 1} was given an asset index outside the handle's "
+                                 f"{len(self._asset_models)} assets; its body was left unchanged")
 
     def render_vis(self, init=False):
         """without b200_record_qpos the reference's headless branch: nothing.  With it: one frame of the recorded envs (init: after a
@@ -506,6 +550,7 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
                     game.append((self.rew_buf.clone(), self.reset_buf.clone()))
                 if (n + 1) % sync_every == 0 or n + 1 == max_steps:
                     games = st["games"].tolist()
+                    self._check_asset_error()
                     rows = st["log"][:games[2]].tolist()    # at most sync_every rows since the last read
                     st["games"][2].zero_()
                     if print_stats:
