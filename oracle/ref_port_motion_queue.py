@@ -7,11 +7,13 @@ step, after the env step:
     (its motion id, entry and reset mask are set, its done memory is cleared, and the entry records the env and the step
     counter), and becomes idle otherwise;
     the cursor moves by the entries taken.  While stopped it sets no mask and changes nothing.
-QueueRun composes it with ref_port_motion_stats.MotionStats, whose buckets are then the entries: a game is folded into the row of the
-entry it played.  Test infrastructure: the device launches and the task's export are held to it."""
+QueueRun composes it with ref_port_motion_stats.MotionStats, or with ref_port_pose_metrics.PoseMetrics for the pose metrics, whose
+buckets are then the entries: a game is folded into the row of the entry it played.  Test infrastructure: the device launches and the
+task's export are held to it."""
 import numpy as np
 
 from .ref_port_motion_stats import MotionStats
+from .ref_port_pose_metrics import PoseMetrics, nan_max
 
 
 class MotionQueue:
@@ -58,11 +60,13 @@ class MotionQueue:
 
 
 class QueueRun:
-    """the queue with the per-entry meters: step() takes one step's inputs as the device sees them before the queue's reset"""
+    """the queue with the per-entry meters: step() takes one step's inputs as the device sees them before the queue's reset.
+    pose_threshold: with a success threshold the stats are PoseMetrics (pose_sums and success per entry as well)"""
 
-    def __init__(self, num_envs, num_motions, rounds):
+    def __init__(self, num_envs, num_motions, rounds, pose_threshold=None):
         self.queue = MotionQueue(num_envs, num_motions, rounds)
-        self.stats = MotionStats(np.zeros(num_envs, np.int64), self.queue.Q)
+        ids = np.zeros(num_envs, np.int64)
+        self.stats = MotionStats(ids, self.queue.Q) if pose_threshold is None else PoseMetrics(ids, self.queue.Q, pose_threshold)
         self.stats.motion_ids = self.queue.entry                    # the rows are the entries, read at the fold
 
     def step(self, rew, sub_rewards, reset_buf, terminate_buf, body_pos, target_pos):
@@ -74,12 +78,22 @@ class QueueRun:
         self.stats.prev_done[mask] = False
         return mask
 
-    def per_motion(self):
-        """(counts [M, 2], sums [M, 7]): the R rows of each motion added in round order"""
+    def fold(self, rows, max_col=None):
+        """rows [R M, ...] -> [M, ...]: the R rows of each motion added in round order; column max_col by the NaN-propagating max"""
         R, M = self.queue.Q // self.queue.M, self.queue.M
-        c, s = self.stats.counts.reshape(R, M, 2), self.stats.sums.reshape(R, M, -1)
-        counts, sums = c[0].copy(), s[0].copy()
-        for r in range(1, R):
-            counts += c[r]
-            sums += s[r]
-        return counts, sums
+        r = rows.reshape((R, M) + rows.shape[1:])
+        out = r[0].copy()
+        for k in range(1, R):
+            top = out[:, max_col].copy() if max_col is not None else None
+            out += r[k]
+            if max_col is not None:
+                out[:, max_col] = nan_max(top, r[k][:, max_col])
+        return out
+
+    def per_motion(self):
+        """(counts [M, 2], sums [M, 7]) per motion"""
+        return self.fold(self.stats.counts), self.fold(self.stats.sums)
+
+    def per_motion_pose(self):
+        """(pose_sums [M, 7], success [M]) per motion, the largest error (column 6) by the NaN-propagating max"""
+        return self.fold(self.stats.pose_sums, max_col=6), self.fold(self.stats.success)

@@ -121,6 +121,72 @@ def test_the_meters_fold_each_game_into_its_entry():
     assert counts.tolist() == [[2, 1], [2, 0]] and sums[:, 0].tolist() == [5.5 + 40.0, 2.25 + 16.0]
 
 
+def pose_game(run, frames):
+    """one env (N = 1) with two bodies, both at (a, 0, 0) against targets at the origin, for each a of frames; the game ends on the
+    last frame and the queue restarts the env on its next entry.  Per frame: body-position error |a|, root-relative and PA errors 0
+    (no spread), velocity error |a - a'|, acceleration error |a - 2 a' + a''| over the game's own earlier frames"""
+    rb, z = np.zeros(1, np.int64), np.zeros((1, 4))
+    for k, a in enumerate(frames):
+        rb[0] = int(k == len(frames) - 1)
+        bp = np.zeros((1, 2, 3))
+        bp[0, :, 0] = a
+        mask = run.step(np.zeros(1), z, rb, np.zeros(1, np.int64), bp, np.zeros((1, 2, 3)))
+        rb[mask] = 0
+    return mask
+
+
+def test_a_restarted_envs_first_frame_adds_no_velocity_or_acceleration_frame():
+    run = Q.QueueRun(1, 2, 1, pose_threshold=5.0)       # env 0 plays entry 0, then entry 1
+    assert pose_game(run, [1.0, 2.0, 4.0]).tolist() == [True]
+    pose_game(run, [10.0, 11.0])
+    ps = run.stats.pose_sums
+    assert ps[:, 0].tolist() == [0.0, 0.0] and ps[:, 1].tolist() == [0.0, 0.0]
+    assert ps[0, 2:].tolist() == [1.0 + 2.0, 1.0, 2, 1, 4.0]               # vel, acc, vel frames, acc frames, largest error
+    assert ps[1, 2:].tolist() == [1.0, 0.0, 1, 0, 11.0]                    # no frame against entry 0's last two
+    assert run.stats.success.tolist() == [1, 0] and run.stats.counts[:, 0].tolist() == [1, 1]
+    assert run.stats.sums[:, 1].tolist() == [3, 2] and run.queue.stop
+
+
+def test_a_nan_game_poisons_its_own_entry_only():
+    run = Q.QueueRun(1, 2, 1, pose_threshold=0.5)
+    pose_game(run, [0.1, 0.2, np.nan])                   # the NaN frame is the last: the history the restart empties holds it
+    pose_game(run, [0.3, 0.4])
+    ps = run.stats.pose_sums
+    assert np.isnan(ps[0, [0, 1, 2, 3, 6]]).all() and ps[0, 4:6].tolist() == [2, 1]
+    assert np.isfinite(ps[1]).all() and ps[1, 4:].tolist() == [1, 0, 0.4]
+    np.testing.assert_allclose(ps[1, 2], 0.1, rtol=1e-12)
+    assert run.stats.success.tolist() == [0, 1] and run.stats.counts[:, 0].tolist() == [1, 1]
+    assert np.isnan(run.stats.sums[0, 6]) and np.isfinite(run.stats.sums[1]).all()
+
+
+@pytest.mark.parametrize("nan_round", [0, 1])
+def test_a_nan_in_either_round_makes_the_motions_largest_error_nan(nan_round):
+    run = Q.QueueRun(1, 2, 2, pose_threshold=0.5)       # entries 0..3: motions 0 1 0 1, all on env 0
+    for q in range(4):
+        pose_game(run, [0.1 * (q + 1), np.nan if q == 2 * nan_round else 0.05])
+    ps, success = run.per_motion_pose()
+    assert np.isnan(ps[0, 6]) and ps[1, 6] == 0.4 and success.tolist() == [1, 2]
+    assert ps[:, 4].tolist() == [2, 2] and np.isnan(ps[0, 2]) and np.isfinite(ps[1]).all()
+    counts, _ = run.per_motion()
+    assert counts[:, 0].tolist() == [2, 2]
+
+
+def test_queue_fold_of_the_largest_error_with_nan_inf_and_ties():
+    run = Q.QueueRun(1, 3, 3, pose_threshold=0.5)       # only the fold is used: R = 3, M = 3
+    col = np.array([np.inf, -np.inf, -np.inf,            # round 0
+                    1.0, 2.0, -np.inf,                   # round 1
+                    np.nan, 2.0, -np.inf])               # round 2
+    rows = np.zeros((9, 7))
+    rows[:, 0], rows[:, 6] = np.arange(9.0), col
+    for f in (V.queue_fold(rows, 3, 3, max_col=6), run.fold(rows, max_col=6)):
+        assert np.isnan(f[0, 6]) and f[1, 6] == 2.0 and f[2, 6] == -np.inf
+        assert f[:, 0].tolist() == [0.0 + 3.0 + 6.0, 1.0 + 4.0 + 7.0, 2.0 + 5.0 + 8.0]
+    rows[6, 6] = 0.5                                     # no NaN: +Inf wins
+    assert V.queue_fold(rows, 3, 3, max_col=6)[0, 6] == run.fold(rows, max_col=6)[0, 6] == np.inf
+    rows[0, 6] = np.nan                                  # a NaN in the first round survives the later ones
+    assert np.isnan(V.queue_fold(rows, 3, 3, max_col=6)[0, 6]) and np.isnan(run.fold(rows, max_col=6)[0, 6])
+
+
 # ---------------------------------------------------------------------------------------------------------- cfg refusals
 def qcfg(N=4, flat=None, test=True, **over):
     cfg = im_cfg(N, flat, **dict(dict(b200_motion_queue=True), **over))
