@@ -388,6 +388,65 @@ int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream);
 /* sizeof(b200_im_motion_queue_t) as the library was built; the binding refuses a library whose size differs from its own */
 int32_t b200env_im_motion_queue_desc_size(void);
 
+/* The training resample of HumanoidSMPLIM (cfg.env.b200_resample_motions; an addition, the reference draws each env's motion once):
+ * before a reset, every env e < n with mask[e] != 0 and progress_buf[e] > 0 (it played at least one step) draws a new motion from the
+ * distribution whose running sum is cdf [M] (b200env_motion_weights writes it; it need not end at 1):
+ *   u = (bits(seed', c, e) >> 11) * 2^-53, with bits = splitmix64(splitmix64(seed' ^ c * 0xD1B54A32D192ED03) + e) as in
+ *   b200env_reset_masked, c = *counter, and seed' = splitmix64(seed ^ 0x6D6F74696F6E6964) (seed is the caller's seed, the one the
+ *   masked reset takes; the constant is "motionid" in ASCII), so the draw shares no key with the masked reset's or the transforms';
+ *   the new motion m is the smallest with cdf[m] > u * cdf[M - 1], clamped to M - 1 (a motion with no weight is not drawn);
+ *   motion_ids[e] = m, motion_bodies[e] = lib_motion_bodies[m], and env_asset[e] = motion_asset[m] when both are given.
+ * Counts (tries and fails, both or neither): before the draw, tries[old] += 1 and fails[old] += (terminate_buf[e] != 0) for the motion
+ * old = motion_ids[e] the env just finished; integer atomics, so the counts do not depend on the order.  Every other env is untouched.
+ * One thread per env; the last CTA advances *counter by 1 and re-arms the done ticket ([1], zero before the first call).  The caller
+ * then re-points the handle's assets (b200env_set_env_assets) and resets the masked envs.  Returns -1 on a NULL required pointer or
+ * one pointer of a pair, -2 before any launch when n or num_motions is not positive or shape_dim lies outside [0, 32]. */
+typedef struct b200_resample_motions {
+  int32_t n;                       /* envs */
+  int32_t num_motions;             /* M */
+  int32_t shape_dim;               /* columns of motion_bodies */
+  int32_t pad_;
+  uint64_t seed;
+  const uint8_t* mask;             /* [n] */
+  const int64_t* progress_buf;     /* [n] */
+  const int64_t* terminate_buf;    /* [n] */
+  const double* cdf;               /* [M] */
+  const float* lib_motion_bodies;  /* [M, shape_dim] */
+  int64_t* motion_ids;             /* [n] */
+  float* motion_bodies;            /* [n, shape_dim] */
+  int64_t* counter;                /* [1] */
+  uint32_t* done;                  /* [1] */
+  int64_t* tries;                  /* [M] or NULL */
+  int64_t* fails;                  /* [M] or NULL */
+  const int32_t* motion_asset;     /* [M] or NULL */
+  int32_t* env_asset;              /* [n] or NULL */
+} b200_resample_motions_t;
+int b200env_resample_motions(const b200_resample_motions_t* d, void* stream);
+/* sizeof(b200_resample_motions_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_resample_motions_desc_size(void);
+
+/* The motion distribution of the training resample, rebuilt from the failure counts (cfg.env.b200_hard_motion_share = h), in one CTA
+ * with no host synchronisation.  b_m = base[m] (double), or 1 when base is NULL.  With h > 0: for every motion with tries[m] > 0,
+ * rate[m] = fails[m] / tries[m] (double); the others keep theirs; then tries and fails are zeroed.  Then
+ *   p_m = (1 - h) b_m / S_b + h b_m rate[m] / S_br, with S_b = sum b, S_br = sum b rate, or p_m = b_m / S_b when S_br = 0 or h = 0,
+ * and cdf[m] = p_0 + ... + p_m, written in place.  The sums and the scan run in double in a fixed order (each thread a run of
+ * consecutive motions, then a tree over the threads), so every call on the same inputs writes the same bits.  tries, fails and rate
+ * may be NULL when h = 0 (the base distribution).  Returns -1 on a NULL cdf, or a NULL count or rate with h > 0; -2 before any
+ * launch when num_motions is not positive or h is not a finite number in [0, 1]. */
+typedef struct b200_motion_weights {
+  int32_t num_motions;             /* M */
+  int32_t pad_;
+  double h;
+  const float* base;               /* [M] or NULL (uniform) */
+  int64_t* tries;                  /* [M] */
+  int64_t* fails;                  /* [M] */
+  double* rate;                    /* [M] */
+  double* cdf;                     /* [M] */
+} b200_motion_weights_t;
+int b200env_motion_weights(const b200_motion_weights_t* d, void* stream);
+/* sizeof(b200_motion_weights_t) as the library was built; the binding refuses a library whose size differs from its own */
+int32_t b200env_motion_weights_desc_size(void);
+
 /* One recorded frame of HumanoidSMPLIMVis._sync_ref_motion (embodied_pose/env/tasks/humanoid_smpl_im_vis.py:128-152) for every listed
  * env: the qpos the reference's MuJoCo viewer shows, without the viewer.  One warp per recorded env i (row env_ids[i]); frame
  * f = *frame.  With nq = 7 + nd and J = nd / 3, row (i, f) of qpos [n_rec, cap, 2, nq] gets

@@ -321,6 +321,24 @@ class ImMotionQueue(C.Structure):
     _nullable_, _defaults_ = ("games", "env_flags", "motion_asset", "env_asset"), ("pad_",)
 
 
+class ResampleMotions(C.Structure):
+    """b200_resample_motions_t: the training resample of the finished envs' motions (b200env_resample_motions)"""
+    _fields_ = [
+        ("n", C.c_int32), ("num_motions", C.c_int32), ("shape_dim", C.c_int32), ("pad_", C.c_int32), ("seed", C.c_uint64),
+        ("mask", U8P), ("progress_buf", I64P), ("terminate_buf", I64P), ("cdf", F64P), ("lib_motion_bodies", F32P), ("motion_ids", I64P),
+        ("motion_bodies", F32P), ("counter", I64P), ("done", U32P), ("tries", I64P), ("fails", I64P), ("motion_asset", I32P),
+        ("env_asset", I32P),
+    ]
+    _nullable_, _defaults_ = ("tries", "fails", "motion_asset", "env_asset"), ("pad_",)
+
+
+class MotionWeights(C.Structure):
+    """b200_motion_weights_t: the resample's motion distribution rebuilt from the failure counts (b200env_motion_weights)"""
+    _fields_ = [("num_motions", C.c_int32), ("pad_", C.c_int32), ("h", C.c_double), ("base", F32P), ("tries", I64P), ("fails", I64P),
+                ("rate", F64P), ("cdf", F64P)]
+    _nullable_, _defaults_ = ("base", "tries", "fails", "rate"), ("pad_",)
+
+
 class SetEnvAssets(C.Structure):
     """b200_set_env_assets_t: the assets of a mixed-plan handle's envs, re-pointed on the device (b200env_set_env_assets)"""
     _fields_ = [("n", C.c_int32), ("pad_", C.c_int32), ("env_asset", I32P), ("error", I32P)]
@@ -726,6 +744,10 @@ SIGNATURES = {
     "b200env_play_stats_desc_size": (_i32, []),
     "b200env_im_motion_queue": (C.c_int, [_p, _p]),
     "b200env_im_motion_queue_desc_size": (_i32, []),
+    "b200env_resample_motions": (C.c_int, [_p, _p]),
+    "b200env_resample_motions_desc_size": (_i32, []),
+    "b200env_motion_weights": (C.c_int, [_p, _p]),
+    "b200env_motion_weights_desc_size": (_i32, []),
     "b200env_im_motion_queue_stats": (C.c_int, [_p, _p]),
     "b200env_im_motion_queue_stats_desc_size": (_i32, []),
     "b200env_im_record": (C.c_int, [_p, _p]),

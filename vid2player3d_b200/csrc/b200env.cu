@@ -2495,6 +2495,140 @@ __global__ void __launch_bounds__(QUEUE_THREADS) im_motion_queue_kernel(b200_im_
   if (tid == 0 && !stopped) d.cursor[0] = min(cursor + base, d.queue_len);
 }
 
+// b200env_resample_motions: one thread per env, a binary search of the CDF.  COUNT: the finished motion's tries / fails; ASSET: the
+// new motion's asset.  The seed is re-keyed so the draw shares no key with the masked reset or the transforms (include/b200env.h)
+#define RESAMPLE_THREADS 256
+__device__ __forceinline__ uint64_t resample_seed(uint64_t seed) { return splitmix64(seed ^ 0x6D6F74696F6E6964ull); }
+
+template <bool COUNT, bool ASSET>
+__global__ void __launch_bounds__(RESAMPLE_THREADS) resample_motions_kernel(b200_resample_motions_t d) {
+  const int64_t e = (int64_t)blockIdx.x * RESAMPLE_THREADS + threadIdx.x;
+  if (e < d.n && d.mask[e] && d.progress_buf[e] > 0) {
+    if constexpr (COUNT) {
+      const int64_t old = d.motion_ids[e];
+      atomicAdd(reinterpret_cast<unsigned long long*>(d.tries + old), 1ull);
+      if (d.terminate_buf[e] != 0) atomicAdd(reinterpret_cast<unsigned long long*>(d.fails + old), 1ull);
+    }
+    const int M = d.num_motions;
+    const double u = (double)(counter_bits(resample_seed(d.seed), (uint64_t)d.counter[0], (uint64_t)e) >> 11) * 0x1p-53;
+    const double x = u * d.cdf[M - 1];
+    int lo = 0, hi = M - 1;                              // the smallest m < M - 1 with cdf[m] > x, else M - 1
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (d.cdf[mid] > x) hi = mid;
+      else lo = mid + 1;
+    }
+    d.motion_ids[e] = lo;
+    for (int k = 0; k < d.shape_dim; k++) d.motion_bodies[e * d.shape_dim + k] = d.lib_motion_bodies[(int64_t)lo * d.shape_dim + k];
+    if constexpr (ASSET) d.env_asset[e] = d.motion_asset[lo];
+  }
+  last_block_advance(d.counter, d.done, 1);
+}
+
+// b200env_motion_weights: one CTA.  Thread t owns the runs [tile + t ITEMS, tile + (t + 1) ITEMS) of every tile; its sums run over its
+// runs in tile order and the threads' partials meet in a fixed tree, so the bits do not depend on scheduling
+#define WEIGHTS_THREADS 1024
+#define WEIGHTS_ITEMS 4
+static_assert(WEIGHTS_THREADS == 32 * 32, "the block sum and scan take one warp of warp totals");
+
+__device__ __forceinline__ double weights_block_sum(double v, double* s_warp) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  if (lane == 0) s_warp[warp] = v;
+  __syncthreads();
+  if (warp == 0) {
+    double w = s_warp[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) w += __shfl_down_sync(0xffffffffu, w, o);
+    if (lane == 0) s_warp[32] = w;
+  }
+  __syncthreads();
+  const double total = s_warp[32];
+  __syncthreads();                                       // s_warp is rewritten by the next call
+  return total;
+}
+
+// the sum of v over the threads before this one (block order); *total: the sum over all
+__device__ __forceinline__ double weights_block_exclusive(double v, double* s_warp, double* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const double y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  double exc = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) exc = 0.0;
+  if (lane == 31) s_warp[warp] = inc;
+  __syncthreads();
+  if (warp == 0) {
+    double w = s_warp[lane];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const double y = __shfl_up_sync(0xffffffffu, w, o);
+      if (lane >= o) w += y;
+    }
+    s_warp[lane] = w;                                    // inclusive warp totals
+  }
+  __syncthreads();
+  const double before = warp ? s_warp[warp - 1] + exc : exc;
+  *total = s_warp[31];
+  __syncthreads();
+  return before;
+}
+
+__global__ void __launch_bounds__(WEIGHTS_THREADS) motion_weights_kernel(b200_motion_weights_t d) {
+  __shared__ double s_warp[33];
+  const int M = d.num_motions;
+  const bool hard = d.h > 0.0;
+  double sb = 0.0, sbr = 0.0;
+  for (int t0 = 0; t0 < M; t0 += WEIGHTS_THREADS * WEIGHTS_ITEMS) {
+    const int m0 = t0 + threadIdx.x * WEIGHTS_ITEMS;
+#pragma unroll
+    for (int k = 0; k < WEIGHTS_ITEMS; k++) {
+      const int m = m0 + k;
+      if (m >= M) break;
+      const double b = d.base ? (double)d.base[m] : 1.0;
+      sb += b;
+      if (hard) {
+        const int64_t tries = d.tries[m];
+        double r = d.rate[m];
+        if (tries > 0) {
+          r = (double)d.fails[m] / (double)tries;
+          d.rate[m] = r;
+          d.tries[m] = 0;
+          d.fails[m] = 0;
+        }
+        sbr += b * r;
+      }
+    }
+  }
+  const double s_b = weights_block_sum(sb, s_warp);
+  const double s_br = hard ? weights_block_sum(sbr, s_warp) : 0.0;
+  const bool mix = hard && s_br > 0.0;
+  double carry = 0.0;
+  for (int t0 = 0; t0 < M; t0 += WEIGHTS_THREADS * WEIGHTS_ITEMS) {
+    const int m0 = t0 + threadIdx.x * WEIGHTS_ITEMS;
+    double run[WEIGHTS_ITEMS], acc = 0.0;
+#pragma unroll
+    for (int k = 0; k < WEIGHTS_ITEMS; k++) {
+      const int m = m0 + k;
+      if (m < M) {
+        const double b = d.base ? (double)d.base[m] : 1.0;
+        acc += mix ? (1.0 - d.h) * b / s_b + d.h * b * d.rate[m] / s_br : b / s_b;
+      }
+      run[k] = acc;
+    }
+    double tile_total;
+    const double before = carry + weights_block_exclusive(acc, s_warp, &tile_total);
+#pragma unroll
+    for (int k = 0; k < WEIGHTS_ITEMS; k++)
+      if (m0 + k < M) d.cdf[m0 + k] = before + run[k];
+    carry += tile_total;
+  }
+}
+
 // b200env_set_env_assets: one thread per env re-points its entry of the mixed plan's asset-header table; a bad index keeps the old
 // entry and records the first env that had one
 #define SET_ASSET_THREADS 256
@@ -3453,6 +3587,44 @@ int b200env_im_motion_queue(const b200_im_motion_queue_t* d, void* stream) {
 }
 
 int32_t b200env_im_motion_queue_desc_size(void) { return (int32_t)sizeof(b200_im_motion_queue_t); }
+
+int b200env_resample_motions(const b200_resample_motions_t* d, void* stream) {
+  if (!d || !d->mask || !d->progress_buf || !d->terminate_buf || !d->cdf || !d->lib_motion_bodies || !d->motion_ids || !d->motion_bodies ||
+      !d->counter || !d->done)
+    return fail(-1, "b200env_resample_motions: null argument%s");
+  if (!d->tries != !d->fails) return fail(-1, "b200env_resample_motions: tries and fails must be both set or both NULL%s");
+  if (!d->motion_asset != !d->env_asset)
+    return fail(-1, "b200env_resample_motions: motion_asset and env_asset must be both set or both NULL%s");
+  if (d->n <= 0 || d->num_motions <= 0) return fail(-2, "b200env_resample_motions: n and num_motions must be positive%s");
+  if (d->shape_dim < 0 || d->shape_dim > 32) return fail(-2, "b200env_resample_motions: shape_dim must lie in [0, 32]%s");
+  const int grid = (d->n + RESAMPLE_THREADS - 1) / RESAMPLE_THREADS;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d->tries && d->env_asset)
+    resample_motions_kernel<true, true><<<grid, RESAMPLE_THREADS, 0, st>>>(*d);
+  else if (d->tries)
+    resample_motions_kernel<true, false><<<grid, RESAMPLE_THREADS, 0, st>>>(*d);
+  else if (d->env_asset)
+    resample_motions_kernel<false, true><<<grid, RESAMPLE_THREADS, 0, st>>>(*d);
+  else
+    resample_motions_kernel<false, false><<<grid, RESAMPLE_THREADS, 0, st>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int32_t b200env_resample_motions_desc_size(void) { return (int32_t)sizeof(b200_resample_motions_t); }
+
+int b200env_motion_weights(const b200_motion_weights_t* d, void* stream) {
+  if (!d || !d->cdf) return fail(-1, "b200env_motion_weights: null argument%s");
+  if (d->num_motions <= 0) return fail(-2, "b200env_motion_weights: num_motions must be positive%s");
+  if (!(d->h >= 0.0 && d->h <= 1.0)) return fail(-2, "b200env_motion_weights: h must be a finite number in [0, 1]%s");
+  if (d->h > 0.0 && (!d->tries || !d->fails || !d->rate))
+    return fail(-1, "b200env_motion_weights: h > 0 needs tries, fails and rate%s");
+  motion_weights_kernel<<<1, WEIGHTS_THREADS, 0, (cudaStream_t)stream>>>(*d);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int32_t b200env_motion_weights_desc_size(void) { return (int32_t)sizeof(b200_motion_weights_t); }
 
 int b200env_im_record(const b200_im_record_t* d, void* stream) {
   if (!d || !d->env_ids || !d->rigid_body_state || !d->dof_state || !d->p_dof_pos || !d->p_rb_pos || !d->p_rb_rot || !d->reset_buf ||

@@ -32,6 +32,8 @@ def lib():
                         (abi.PlayStats, L.b200env_play_stats_desc_size()), (abi.ImMotionQueue, L.b200env_im_motion_queue_desc_size()),
                         (abi.ImMotionQueueStats, L.b200env_im_motion_queue_stats_desc_size()),
                         (abi.SetEnvAssets, L.b200env_set_env_assets_desc_size()),
+                        (abi.ResampleMotions, L.b200env_resample_motions_desc_size()),
+                        (abi.MotionWeights, L.b200env_motion_weights_desc_size()),
                         (abi.V2PBallStats, L.b200v2p_eval_ball_stats_desc_size()),
                         (abi.V2PRallyStats, L.b200v2p_eval_rally_stats_desc_size())):
             if size != C.sizeof(S):    # these descriptors grow by appended fields within one version
@@ -139,6 +141,19 @@ def im_motion_queue(scalars, tensors):
     """one assignment of the motion queue on the device (include/b200env.h: b200env_im_motion_queue); the fields of abi.ImMotionQueue"""
     d = fill(abi.ImMotionQueue, scalars, tensors)
     _check(lib().b200env_im_motion_queue(C.byref(d), _stream()))
+
+
+def resample_motions(scalars, tensors):
+    """new motions for the masked envs that played a step, drawn on the device (include/b200env.h: b200env_resample_motions); the
+    fields of abi.ResampleMotions"""
+    d = fill(abi.ResampleMotions, scalars, tensors)
+    _check(lib().b200env_resample_motions(C.byref(d), _stream()))
+
+
+def motion_weights(scalars, tensors):
+    """the resample's motion CDF rebuilt on the device (include/b200env.h: b200env_motion_weights); the fields of abi.MotionWeights"""
+    d = fill(abi.MotionWeights, scalars, tensors)
+    _check(lib().b200env_motion_weights(C.byref(d), _stream()))
 
 
 def plan_assets(env_asset, num_assets, envs_per_batch=ENVS_PER_BATCH, mixed=False):

@@ -44,11 +44,39 @@ def resolve_test_motion_file(cfg):
     return path
 
 
+def motion_resample_share(cfg, test_task=False):
+    """cfg.env.b200_resample_motions -> None when off, else the share h of the draws weighted by the motions' failure rates
+    (cfg.env.b200_hard_motion_share, default 0).  Refuses the key in a test run (args.test, or test_task: HumanoidSMPLIMVis), with
+    b200_motion_queue or motion_id, and h that is not a finite number in [0, 1] or is given without the key."""
+    env = cfg["env"]
+    if not env.get("b200_resample_motions", False):
+        if "b200_hard_motion_share" in env:
+            raise ValueError("b200_hard_motion_share weights the motions b200_resample_motions draws: set b200_resample_motions: True")
+        return None
+    args = cfg.get("args", None)
+    if test_task or (args is not None and getattr(args, "test", False)):
+        raise ValueError("b200_resample_motions draws training motions: a test run keeps each env's motion (or takes them from "
+                         "b200_motion_queue)")
+    if env.get("b200_motion_queue", False):
+        raise ValueError("b200_resample_motions and b200_motion_queue both choose a finished env's next motion: set one of them")
+    if "motion_id" in env:
+        raise ValueError("b200_resample_motions draws from the whole library, motion_id pins every env to one motion: set one of them")
+    h = env.get("b200_hard_motion_share", 0.0)
+    if isinstance(h, bool) or not isinstance(h, (int, float, np.integer, np.floating)) or not 0.0 <= float(h) <= 1.0:
+        raise ValueError(f"b200_hard_motion_share must be a finite number in [0, 1], got {h!r}")
+    return float(h)
+
+
 class HumanoidSMPLIM(BaseTask):
+    _test_task = False      # HumanoidSMPLIMVis: the test run's task
+    _rs = None              # the training resample's device state (cfg.env.b200_resample_motions), set by _bind
+    _asset_error = None     # [1] int32 error word of b200env_set_env_assets when envs change body on the device
+
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         self.cfg = cfg
         self.args = cfg.get('args', None)
         env = cfg["env"]
+        self._resample_share = motion_resample_share(cfg, self._test_task)
         self.sim_params = sim_params
         self.physics_engine = physics_engine
         self.sim_dt = float(_sim_param(sim_params, "dt", 1.0 / 60.0))
@@ -237,6 +265,8 @@ class HumanoidSMPLIM(BaseTask):
             self._env = native.Env(self._model_struct, self._verts, self._cfg_struct, self.num_envs, self.device_id)
         else:
             self._env = native.Env(structs, verts, self._cfg_struct, self.num_envs, self.device_id, env_asset=self._env_asset)
+            if self._resample_share is not None and len(models) > 1:
+                self._env.fix_mixed_plan()     # a resampled env takes its new motion's body
         self._key_body_ids = torch.tensor(list(self._cfg_struct.key_body)[:self._cfg_struct.num_key], device=self.device)
         self._contact_body_ids = torch.tensor([i for i in range(self.num_bodies) if self._cfg_struct.contact_body[i]],
                                               device=self.device)
@@ -301,6 +331,8 @@ class HumanoidSMPLIM(BaseTask):
             t["dof_force"] = self.dof_force_tensor
         self._env.bind(t, actors_per_env=1, bodies_per_env=B, num_obs=self.num_obs)
         self._env.set_motion_lib(self._ml_t, nbl)
+        if self._resample_share is not None:
+            self._rs = self._resample_buffers()
         self.extras["terminate"] = self._terminate_buf
         self.extras["sub_rewards"] = self._sub_rewards
         self.extras["sub_rewards_names"] = self._sub_rewards_names
@@ -321,12 +353,57 @@ class HumanoidSMPLIM(BaseTask):
             ids[:] = env['motion_id']
         return ids.contiguous()
 
+    def _resample_buffers(self):
+        """the training resample's device state: the CDF of the base distribution (b_m = motion_lengths[m] under
+        motion_weights_from_length, else uniform, as _sample_motion_ids draws), the draw counter and its done ticket, the mask of an
+        id-list reset; with b200_hard_motion_share > 0 the counts and the rates (r_m = 1 at the start); with several bodies each
+        motion's and each env's asset"""
+        N, M, dev = self.num_envs, self._motion_lib.num_motions(), self.device
+        i64 = lambda n: torch.zeros(n, device=dev, dtype=torch.long)  # noqa: E731
+        base = self._ml_t["motion_lengths"] if self.cfg["env"].get("motion_weights_from_length", False) else None
+        rs = dict(base=base, cdf=torch.zeros(M, device=dev, dtype=torch.float64), counter=i64(1),
+                  done=torch.zeros(1, device=dev, dtype=torch.int32), id_mask=torch.zeros(N, device=dev, dtype=torch.bool))
+        if self._resample_share > 0:
+            rs.update(tries=i64(M), fails=i64(M), rate=torch.ones(M, device=dev, dtype=torch.float64))
+        native.motion_weights(dict(num_motions=M, h=0.0), dict(base=base, cdf=rs["cdf"]))
+        if len(getattr(self, "_asset_models", ())) > 1:
+            i32 = lambda a: torch.as_tensor(a, dtype=torch.int32, device=dev)  # noqa: E731
+            rs.update(motion_asset=i32(self._motion_asset), env_asset=i32(self._env_asset))
+            self._asset_error = torch.zeros(1, device=dev, dtype=torch.int32)
+        return rs
+
+    def _resample_motions(self, mask):
+        """the masked envs that played a step draw their next motion (and body) on the device, before their reset"""
+        rs = self._rs
+        native.resample_motions(dict(n=self.num_envs, num_motions=self._motion_lib.num_motions(),
+                                     shape_dim=self._reset_ref_motion_bodies.shape[1], seed=int(self.cfg.get("seed", 10))),
+                                dict(rs, mask=mask, progress_buf=self.progress_buf, terminate_buf=self._terminate_buf,
+                                     lib_motion_bodies=self._ml_t["motion_bodies"], motion_ids=self._reset_ref_motion_ids,
+                                     motion_bodies=self._reset_ref_motion_bodies))
+        if "env_asset" in rs:                  # the new bodies, read by the next physics launch
+            self._env.set_env_assets(rs["env_asset"], self._asset_error)
+
+    def _check_asset_error(self):
+        """the host's check of b200env_set_env_assets' error word, at its sync points"""
+        if self._asset_error is not None:
+            e = int(self._asset_error)
+            if e:
+                raise ValueError(f"b200env_set_env_assets: env {e - 1} was given an asset index outside the handle's "
+                                 f"{len(self._asset_models)} assets; its body was left unchanged")
+
     # ------------------------------------------------------------------ Task surface
     def register_model(self, model):
         self.model = model
 
     def pre_epoch(self, epoch):
-        return
+        """with cfg.env.b200_resample_motions: reads the asset error word (the agent has just read its losses on the host, so this waits
+        for no work), then, with b200_hard_motion_share > 0, rebuilds the resample's distribution from the last epoch's counts in one
+        launch, in place, with no host synchronisation (include/b200env.h: b200env_motion_weights)"""
+        if self._rs is None:
+            return
+        self._check_asset_error()
+        if self._resample_share > 0:
+            native.motion_weights(dict(num_motions=self._motion_lib.num_motions(), h=self._resample_share), self._rs)
 
     def step(self, actions):
         """BaseTask.step (base_task.py:147-165) = pre_physics_step + _physics_step + post_physics_step,
@@ -339,7 +416,13 @@ class HumanoidSMPLIM(BaseTask):
         if env_ids is None:
             env_ids = torch.arange(self.num_envs, device=self.device, dtype=torch.long)
         if len(env_ids) > 0:
-            self._reset_actors(env_ids.to(self.device, dtype=torch.long).contiguous())
+            env_ids = env_ids.to(self.device, dtype=torch.long).contiguous()
+            if self._rs is not None:
+                mask = self._rs["id_mask"]
+                mask.zero_()
+                mask[env_ids] = True
+                self._resample_motions(mask)
+            self._reset_actors(env_ids)
 
     def _reset_actors(self, env_ids):
         """:470-480, :638-651"""
@@ -402,7 +485,9 @@ class HumanoidSMPLIM(BaseTask):
         of the same distribution as the torch.rand / torch.bernoulli draws of `reset(env_ids)`.  With cfg.env.transform_specs only under
         cfg.env.b200_device_transforms (the window launch applies them, drawing at the same counter); otherwise the transforms are torch
         ops on the reset rows: use `reset(env_ids)` there.  step: a device step counter ([1] int64) the policy reads its context slot
-        from; each window then starts step % context_length frames earlier, so the next slot read is the new game's first frame."""
+        from; each window then starts step % context_length frames earlier, so the next slot read is the new game's first frame.
+        With cfg.env.b200_resample_motions the masked envs that played a step first draw their next motion (and body) on the device,
+        as `reset(env_ids)` does for its ids."""
         if self._transform_specs is not None and self._xf_program is None:
             raise ValueError("reset_masked: cfg.env.transform_specs transforms the context window in torch - use reset(env_ids), "
                              "or set cfg.env.b200_device_transforms")
@@ -412,6 +497,8 @@ class HumanoidSMPLIM(BaseTask):
             raise ValueError(f"Unsupported state initialization strategy: {self._state_init}")
         sample_time, ref_prob = modes[self._state_init]
         truncate = self.context_length * self.dt if self.truncate_time else 0.0
+        if self._rs is not None:
+            self._resample_motions(mask)
         self._context_buffers()
         self._env.reset_masked(mask, sample_time, truncate, ref_prob, self.cfg.get("seed", 10), self._reset_rng,
                                self._initial_humanoid_root_states, self._initial_dof_pos, self._initial_dof_vel, self._reset_ref_motion_times,

@@ -203,6 +203,8 @@ def queue_fold(rows, R, M, max_col=None):
 
 class HumanoidSMPLIMVis(HumanoidSMPLIM):
     _q = None               # the motion queue's device state (cfg.env.b200_motion_queue), set by set_policy
+    _test_task = True       # refuses cfg.env.b200_resample_motions
+
     def __init__(self, cfg, sim_params, physics_engine, device_type, device_id, headless):
         if not headless:
             raise ValueError("HumanoidSMPLIMVis: there is no MuJoCo viewer; run headless")
@@ -340,16 +342,9 @@ class HumanoidSMPLIMVis(HumanoidSMPLIM):
             return {}
         dev, i32 = self.device, torch.int32
         start = torch.as_tensor(self._env_asset, dtype=i32, device=dev)
+        self._asset_error = torch.zeros(1, device=dev, dtype=i32)     # read by _check_asset_error at the run's sync points
         return dict(motion_asset=torch.as_tensor(self._motion_asset, dtype=i32, device=dev), env_asset=start.clone(), start_env_asset=start,
-                    asset_error=torch.zeros(1, device=dev, dtype=i32))
-
-    def _check_asset_error(self):
-        """the host's check of b200env_set_env_assets' error word, at the run's sync points"""
-        if self._q is not None and "asset_error" in self._q:
-            e = int(self._q["asset_error"])
-            if e:
-                raise ValueError(f"b200env_set_env_assets: env {e - 1} was given an asset index outside the handle's "
-                                 f"{len(self._asset_models)} assets; its body was left unchanged")
+                    asset_error=self._asset_error)
 
     def render_vis(self, init=False):
         """without b200_record_qpos the reference's headless branch: nothing.  With it: one frame of the recorded envs (init: after a
